@@ -72,7 +72,8 @@ typedef enum { STK_OPT_ADAM = 0, STK_OPT_ADAMW = 1, STK_OPT_SGD = 2 } stk_optim_
 
 /* flags of stk_grad_reduce */
 #define STK_RF_FINAL 1u        /* last bucket of this optimizer step: finish norm / found_inf (cross-rank exchange) */
-#define STK_RF_ZERO_INPUT 2u   /* zero the local gradient bucket (and accumulator) after it has been consumed */
+#define STK_RF_ZERO_INPUT 2u   /* zero the local gradient bucket after it has been consumed (the accumulator is left as it
+                                  is: the next stk_grad_accumulate with first != 0 overwrites it) */
 #define STK_RF_UNSCALE 4u      /* multiply by 1/loss_scale (device scaler state) and test for inf/nan */
 
 typedef struct {

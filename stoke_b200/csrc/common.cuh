@@ -162,6 +162,17 @@ __device__ __forceinline__ float f16hi(uint32_t u) { return __half2float(__ushor
 
 __device__ __forceinline__ bool finitef(float x) { return (__float_as_uint(x) & 0x7f800000u) != 0x7f800000u; }
 
+// max that propagates NaN (max.NaN.f32, sm_80+), like torch's max / amax: fmaxf returns the non-NaN operand, which would
+// turn the inf-norm of a gradient holding a NaN into a finite number.  Same result as fmaxf when neither input is NaN.
+__device__ __forceinline__ float fmax_nan(float a, float b) {
+  float r;
+  asm("max.NaN.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b));
+  return r;
+}
+// clamps that keep NaN, like torch.clamp (comparisons with NaN are false, so NaN falls through unchanged)
+__device__ __forceinline__ float clamp_max_nan(float x, float hi) { return x > hi ? hi : x; }
+__device__ __forceinline__ float clamp_nan(float x, float lo, float hi) { return x < lo ? lo : (x > hi ? hi : x); }
+
 // ---- NVLS: multimem accesses on a multicast mapping (one address = the same offset in every rank's buffer; the NVSwitch
 // reduces the W copies on a load and replicates a store).  SASS: LDGMC.E.ADD.* / STG on the multicast address. -------------
 __device__ __forceinline__ uint4 mm_ld_reduce_bf16x8(const void* mc) {  // sum over ranks of 8 bf16, fp32 accumulation
@@ -200,7 +211,7 @@ __device__ __forceinline__ float warp_reduce(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) {
     float w = __shfl_xor_sync(0xffffffffu, v, o);
-    v = kMax ? fmaxf(v, w) : v + w;
+    v = kMax ? fmax_nan(v, w) : v + w;
   }
   return v;
 }

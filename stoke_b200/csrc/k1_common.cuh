@@ -171,16 +171,16 @@ __device__ __forceinline__ void reduce_tail(const ReduceParams& p, float part, b
       for (unsigned b = lane; b < gridDim.x; b += 32) {
         const RankScalars* slot = &p.pads.p[p.rank]->blk_scal[r][b];
         const float y = ld_relaxed_sys_f32(&slot->norm_partial);
-        x = mx ? fmaxf(x, y) : x + y;
+        x = mx ? fmax_nan(x, y) : x + y;
         inf |= ld_relaxed_sys_u32(&slot->found_inf);
       }
       x = mx ? warp_reduce<true>(x) : warp_reduce<false>(x);
-      total = mx ? fmaxf(total, x) : total + x;
+      total = mx ? fmax_nan(total, x) : total + x;
     }
     inf = __any_sync(0xffffffffu, inf != 0);
     if (lane == 0) {
       float run = p.accum->norm_partial;   // running over the buckets of this optimizer step (global values)
-      run = mx ? fmaxf(run, total) : run + total;
+      run = mx ? fmax_nan(run, total) : run + total;
       unsigned run_inf = p.accum->found_inf | (inf ? 1u : 0u);
       p.accum->blocks_done = 0;
       if (p.flags & STK_RF_FINAL) {
@@ -220,7 +220,7 @@ __device__ __forceinline__ void reduce_tail(const ReduceParams& p, float part, b
     if (p.norm_kind != STK_NORM_NONE) {
       const float a = lane < gsize ? __ldcg(&p.blk_partial[(grp << 6) + lane]) : 0.f;
       const float b = lane + 32 < gsize ? __ldcg(&p.blk_partial[(grp << 6) + 32 + lane]) : 0.f;
-      x = mx ? warp_reduce<true>(fmaxf(a, b)) : warp_reduce<false>(a + b);
+      x = mx ? warp_reduce<true>(fmax_nan(a, b)) : warp_reduce<false>(a + b);
     }
     last = 0;
     if (lane == 0) {
@@ -240,13 +240,13 @@ __device__ __forceinline__ void reduce_tail(const ReduceParams& p, float part, b
     float x = 0.f;
     for (unsigned i = lane; i < ngroups; i += 32) {  // fixed lane/iteration order -> deterministic
       const float y = __ldcg(&p.grp_partial[i]);
-      x = mx ? fmaxf(x, y) : x + y;
+      x = mx ? fmax_nan(x, y) : x + y;
     }
     tot = mx ? warp_reduce<true>(x) : warp_reduce<false>(x);
   }
   if (lane == 0) {
     float run = p.accum->norm_partial;
-    run = (p.norm_kind == STK_NORM_INF) ? fmaxf(run, tot) : run + tot;
+    run = (p.norm_kind == STK_NORM_INF) ? fmax_nan(run, tot) : run + tot;
     p.accum->norm_partial = run;
     p.accum->blocks_done = 0;
     __threadfence();

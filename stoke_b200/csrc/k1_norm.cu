@@ -120,7 +120,7 @@ __global__ void __launch_bounds__(kNormThreads) k_grad_norm(const NormParams p) 
         bad |= !finitef(x);
         x *= inv_scale;
         if (p.norm_kind == STK_NORM_L2) part = fmaf(x, x, part);
-        else if (p.norm_kind == STK_NORM_INF) part = fmaxf(part, fabsf(x));
+        else if (p.norm_kind == STK_NORM_INF) part = fmax_nan(part, fabsf(x));
         else if (p.norm_kind == STK_NORM_P) part += __powf(fabsf(x), p.norm_p);
       }
     }
@@ -129,8 +129,9 @@ __global__ void __launch_bounds__(kNormThreads) k_grad_norm(const NormParams p) 
   const float blk = mx ? block_reduce<true>(part, s_red) : block_reduce<false>(part, s_red);
   const int any_bad = __syncthreads_or(bad ? 1 : 0);
   if (threadIdx.x == 0) {
-    // sign bit of the partial carries the block's inf/nan verdict (partials are >= 0 for every norm kind)
-    p.blk_partial[blockIdx.x] = any_bad ? -1.f - fminf(blk, 3.0e38f) : blk;
+    // the sign bit of the partial carries the block's inf/nan verdict (partials are +0, positive, +inf or NaN for every
+    // norm kind); setting the bit keeps the magnitude, so an inf or NaN partial reaches the finisher as it is
+    p.blk_partial[blockIdx.x] = any_bad ? __uint_as_float(__float_as_uint(blk) | 0x80000000u) : blk;
   }
 }
 
@@ -141,23 +142,23 @@ __global__ void __launch_bounds__(1024) k_grad_norm_finish(const NormParams p, u
   bool bad = false;
   for (unsigned b = threadIdx.x; b < nblocks; b += blockDim.x) {
     float y = __ldcg(&p.blk_partial[b]);
-    if (y < 0.f) {
+    if (__float_as_uint(y) & 0x80000000u) {
       bad = true;
-      y = -1.f - y;
+      y = fabsf(y);
     }
-    x = mx ? fmaxf(x, y) : x + y;
+    x = mx ? fmax_nan(x, y) : x + y;
   }
   const float tot = mx ? block_reduce<true>(x, s_red) : block_reduce<false>(x, s_red);
   const int any_bad = __syncthreads_or(bad ? 1 : 0);
   if (threadIdx.x == 0) {
     float run = p.accum->norm_partial;
-    run = mx ? fmaxf(run, tot) : run + tot;
+    run = mx ? fmax_nan(run, tot) : run + tot;
     uint32_t inf = p.accum->found_inf | (any_bad ? 1u : 0u);
     if (p.flags & STK_RF_FINAL) {
+      // an inf / nan gradient gives what torch's clip_grad_norm_ returns: NaN if any element is NaN, else inf
       float norm = run;
       if (p.norm_kind == STK_NORM_L2) norm = sqrtf(run);
       else if (p.norm_kind == STK_NORM_P) norm = powf(run, 1.f / p.norm_p);
-      if (inf) norm = __int_as_float(0x7f800000);  // an inf/nan gradient: torch's total_norm is inf (or nan) too
       p.scaler->grad_norm = norm;
       // the inf gate belongs to the loss scaler (GradScaler.step); without one the reference steps regardless
       p.scaler->found_inf = (inf && (p.flags & STK_RF_UNSCALE)) ? 1 : 0;
@@ -174,12 +175,13 @@ __global__ void __launch_bounds__(256) k_grad_scale(float* __restrict__ grad, si
   const size_t v = size_t(blockIdx.x) * blockDim.x + threadIdx.x;
   if (v >= nvec) return;
   float coef = 1.f;
-  if (clip_kind == STK_CLIP_NORM) coef = fminf(max_norm / (scaler->grad_norm + 1e-6f), 1.0f);
+  // a NaN norm gives a NaN coefficient and NaN gradients, as torch.clamp does in clip_grad_norm_
+  if (clip_kind == STK_CLIP_NORM) coef = clamp_max_nan(max_norm / (scaler->grad_norm + 1e-6f), 1.0f);
   f8 g = ld_stream_f8(grad + v * 8);
 #pragma unroll
   for (int i = 0; i < 8; ++i) {
     if (clip_kind == STK_CLIP_NORM) g.v[i] *= coef;
-    else g.v[i] = fminf(fmaxf(g.v[i], -clip_value), clip_value);
+    else g.v[i] = clamp_nan(g.v[i], -clip_value, clip_value);
   }
   st_stream_f8(grad + v * 8, g.v);
 }

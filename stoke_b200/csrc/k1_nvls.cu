@@ -77,7 +77,7 @@ __global__ void __launch_bounds__(kNvlsThreads, 1) k_grad_reduce_nvls(const Redu
           y *= inv_scale;
           x[u][i] = y;
           if (p.norm_kind == STK_NORM_L2) part = fmaf(y, y, part);
-          else if (p.norm_kind == STK_NORM_INF) part = fmaxf(part, fabsf(y));
+          else if (p.norm_kind == STK_NORM_INF) part = fmax_nan(part, fabsf(y));
           else if (p.norm_kind == STK_NORM_P) part += __powf(fabsf(y), p.norm_p);
         }
       }

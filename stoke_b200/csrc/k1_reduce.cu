@@ -118,7 +118,7 @@ __global__ void __launch_bounds__(W_T == 1 ? 256 : 512, W_T == 1 ? 6 : 1) k_grad
           x *= inv_scale;
           s[i] = x;
           if (p.norm_kind == STK_NORM_L2) part = fmaf(x, x, part);
-          else if (p.norm_kind == STK_NORM_INF) part = fmaxf(part, fabsf(x));
+          else if (p.norm_kind == STK_NORM_INF) part = fmax_nan(part, fabsf(x));
           else if (p.norm_kind == STK_NORM_P) part += __powf(fabsf(x), p.norm_p);
         }
         if (OUT_DT == STK_BF16 && p.norm_kind != STK_NORM_NONE) { /* norm is of the fp32 value, before rounding */ }

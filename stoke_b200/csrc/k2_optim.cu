@@ -212,7 +212,9 @@ __global__ void __launch_bounds__(256) k_optim_step(const OptimParams p) {
   const bool skip_all = s_skip != 0;
   const bool first_step = s_first != 0;
   float coef = 1.f;
-  if (p.clip_kind == STK_CLIP_NORM) coef = fminf(p.clip_max_norm / (p.scaler->grad_norm + 1e-6f), 1.0f);
+  // clamps keep NaN like torch.clamp: a NaN norm (a NaN gradient without a loss scaler) makes every gradient NaN, as
+  // clip_grad_norm_ does, and clip by value passes a NaN element through
+  if (p.clip_kind == STK_CLIP_NORM) coef = clamp_max_nan(p.clip_max_norm / (p.scaler->grad_norm + 1e-6f), 1.0f);
   const float cv = p.clip_value;
   const float inv_scale = s_inv_scale;
 
@@ -244,7 +246,7 @@ __global__ void __launch_bounds__(256) k_optim_step(const OptimParams p) {
             gg *= inv_scale;
           }
           if (p.clip_kind == STK_CLIP_NORM) gg *= coef;
-          else if (p.clip_kind == STK_CLIP_VALUE) gg = fminf(fmaxf(gg, -cv), cv);
+          else if (p.clip_kind == STK_CLIP_VALUE) gg = clamp_nan(gg, -cv, cv);
           if (h.maximize) gg = -gg;
           float ww = w[k][e];
           if (KIND == STK_OPT_ADAM || KIND == STK_OPT_ADAMW) {

@@ -249,6 +249,42 @@ def test_amp_scaler_skip_backoff_growth():
     assert _rel(path.gather_master().cpu(), _oracle_flat(path, oracle.weights())) < TOL
 
 
+@pytest.mark.parametrize("route", ["local", "main"])
+@pytest.mark.parametrize("clip", [("norm", 1.0, 2.0), ("norm", 1.0, float("inf")), ("value", 0.3)])
+@pytest.mark.parametrize("bad", ["nan", "inf"])
+def test_nonfinite_gradient_without_scaler_matches_torch(route, clip, bad):
+    """fp32 / bf16 training has no loss scaler, so a step with a NaN or inf gradient is not skipped: it does to the
+    weights what clip_grad_norm_ / clip_grad_value_ + Adam do in torch.  A NaN norm makes every gradient NaN, an inf norm
+    zeroes the finite ones, clip by value keeps a NaN.  Both world-1 routes must agree with the oracle on which weights
+    are NaN and on the finite ones."""
+    from engine_oracle import OracleEngine
+
+    kw = {"lr": 1e-3}
+    net, init, opt = _make(torch.optim.Adam, kw, None, clip, 1, route=route)
+    path = opt.path
+    oracle = OracleEngine(init, 1, torch.optim.Adam, kw, clip=clip)
+    for step in range(3):
+        grads = _inject(path, step, 0, torch.float32)
+        if step == 1:
+            path.grad_views[2].view(-1)[5] = float(bad)
+            grads[2].view(-1)[5] = float(bad)
+        oracle.micro_step([grads])
+        path.after_backward(sync=True, unscale=False)
+        opt.step()
+        oracle.step()
+        if clip[0] == "norm":
+            got_norm, ref_norm = path.engine.scaler_get(path.state_id).grad_norm, float(oracle.last_total_norm)
+            assert (math.isnan(got_norm) and math.isnan(ref_norm)) or got_norm == ref_norm == math.inf or \
+                abs(got_norm - ref_norm) <= 1e-5 * ref_norm
+        got = torch.cat([t.reshape(-1) for t in path.unflatten(path.gather_master().cpu())])
+        ref = torch.cat([w.reshape(-1) for w in oracle.weights()])
+        assert torch.equal(torch.isnan(got), torch.isnan(ref)), f"step {step}: NaN pattern differs"
+        fin = ~torch.isnan(ref)
+        if bool(fin.any()):
+            assert _rel(got[fin], ref[fin]) < TOL
+    opt.close()
+
+
 @pytest.mark.parametrize("name", ["noclip", "clipnorm", "clipvalue"])
 def test_cfg1_through_stoke_api_vs_reference_fixture(golden_dir, name):
     """BASELINE configs[0] end to end through ``Stoke`` on the GPU (fp32) against the fixture produced by the unmodified
