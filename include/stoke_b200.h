@@ -158,11 +158,6 @@ int stk_comm_poll(stk_ctx* ctx);
 #define STK_OPT_COOP_LAUNCH 4   /* 1 (default): cross-rank kernels use cooperative launches (co-residency enforced) */
 #define STK_OPT_NVLS_MAX_BLOCKS 5 /* grid bound of the multimem flavour alone (0: same as STK_OPT_K1_MAX_BLOCKS) */
 #define STK_OPT_K2_AG_MC 6      /* 1: the sharded step publishes its shard with multimem.st when the parameter buffer is bound */
-#define STK_OPT_K1_ONE_SHOT_KB 7 /* all-reduce buckets of at most this many KiB of input take the ONE-SHOT form: every rank reads
-                                    the whole bucket from all W peers and reduces all of it itself (W x the loads, but no peer
-                                    stores, no store-completion fence, no cross-rank partial exchange: the small-message
-                                    latency path).  Default 0 = always two-shot (the one-shot form measured 3-5 us SLOWER at W = 2:
-                                    21.5 vs 18.2 us at 64 KiB; not measured at W = 8).  Same results (rank-order fp32 sums). */
 int stk_option_set(stk_ctx* ctx, int key, int value);
 int stk_option_get(stk_ctx* ctx, int key, int* value);
 
@@ -171,7 +166,7 @@ int stk_option_get(stk_ctx* ctx, int key, int* value);
  * duration and the launch count since the last read, and clears the list. */
 int stk_profile_enable(stk_ctx* ctx, int on);
 int stk_profile_read(stk_ctx* ctx, int kind, double* ms_total, int* launches);
-/* K1 only: time between its start and end barriers (the NVLink data phase) taken with the device timer by block 0 --
+/* cross-rank K1 only: time between its start and end barriers (the NVLink data phase) taken with the device timer by block 0 --
  * excludes the wait for the slowest rank to arrive, which host-side events include; ms_zero_tail (may be NULL) receives
  * the time block 0 then spent zeroing its part of the local bucket (HBM work).  Synchronises `stream`. */
 int stk_profile_read_k1_device(stk_ctx* ctx, double* ms_total, int* launches, double* ms_zero_tail, void* stream);

@@ -88,12 +88,11 @@ def depth_norm_pass(n: int, calls: int = 1) -> int:
 
 
 def depth_reduce_w1(n: int, calls: int = 1) -> int:
-    """The same for stk_grad_reduce at world 1 (k_grad_reduce<1> + its two-level ticket): 16 in the thread (2 vectors of
-    8) + 5 + 5 (warp, then warp 0 over the 8 warps) + 1 + 5 (pair, then warp over a group of 64 blocks) + ceil(groups /
-    32) + 5 (last group over the group partials) + one per call."""
+    """The same for stk_grad_reduce at world 1 (k_grad_reduce<1> + k_grad_norm_finish): 16 in the thread (2 vectors of 8)
+    + 10 in the block tree (5 shuffle levels in the warp, 5 across the 8 warps' partials) + ceil(blocks / 1024) in the
+    finisher's thread + 10 in the finisher's tree + one per call for the running total over calls."""
     blocks = max(1, -(-(n // 8) // 512))
-    groups = -(-blocks // 64)
-    return 16 + 10 + 6 + -(-groups // 32) + 5 + calls
+    return 16 + 10 + -(-blocks // 1024) + 10 + calls
 
 
 def norm_bound(x: torch.Tensor, e_x: torch.Tensor, norm_type: float, depth: int) -> float:

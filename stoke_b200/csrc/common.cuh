@@ -159,6 +159,17 @@ __device__ __forceinline__ float f16lo(uint32_t u) {
   return __half2float(__ushort_as_half((unsigned short)(u & 0xffffu)));
 }
 __device__ __forceinline__ float f16hi(uint32_t u) { return __half2float(__ushort_as_half((unsigned short)(u >> 16))); }
+// the 8 bf16 or f16 values of one 16-byte vector, in memory order
+template <int DT16>
+__device__ __forceinline__ void unpack16(const uint4& u, float (&f)[8]) {
+  static_assert(DT16 == STK_BF16 || DT16 == STK_F16, "unpack16 takes a 16-bit type");
+  const uint32_t w4[4] = {u.x, u.y, u.z, u.w};
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    f[2 * j] = (DT16 == STK_BF16) ? bf16lo(w4[j]) : f16lo(w4[j]);
+    f[2 * j + 1] = (DT16 == STK_BF16) ? bf16hi(w4[j]) : f16hi(w4[j]);
+  }
+}
 
 __device__ __forceinline__ bool finitef(float x) { return (__float_as_uint(x) & 0x7f800000u) != 0x7f800000u; }
 

@@ -15,22 +15,13 @@ int stk_fail(stk_ctx* ctx, int code, const std::string& msg) {
 
 int stk_grow_partials(stk_ctx* c, size_t blocks, cudaStream_t s) {
   if (blocks <= c->blk_partial_cap) return STK_OK;
-  const size_t groups = blocks / 64 + 1;
-  float *bp = nullptr, *gp = nullptr;
-  uint32_t* gc = nullptr;
+  float* bp = nullptr;
   STK_CUDA(c, cudaMalloc(&bp, sizeof(float) * blocks));
-  STK_CUDA(c, cudaMalloc(&gp, sizeof(float) * groups));
-  STK_CUDA(c, cudaMalloc(&gc, sizeof(uint32_t) * groups));
-  STK_CUDA(c, cudaMemset(gc, 0, sizeof(uint32_t) * groups));
   if (c->blk_partial_dev) {
-    STK_CUDA(c, cudaStreamSynchronize(s));  // a previous launch may still use the old arrays
+    STK_CUDA(c, cudaStreamSynchronize(s));  // a previous launch may still use the old array
     cudaFree(c->blk_partial_dev);
-    cudaFree(c->grp_partial_dev);
-    cudaFree(c->grp_count_dev);
   }
   c->blk_partial_dev = bp;
-  c->grp_partial_dev = gp;
-  c->grp_count_dev = gc;
   c->blk_partial_cap = blocks;
   return STK_OK;
 }
@@ -69,7 +60,6 @@ int stk_ctx_create(int rank, int world, int device, unsigned flags, stk_ctx** ou
   if (const char* v = std::getenv("STK_COOP_LAUNCH")) c->coop_launch = std::atoi(v) != 0;
   if (const char* v = std::getenv("STK_NVLS_MAX_BLOCKS")) c->nvls_max_blocks = std::atoi(v);
   if (const char* v = std::getenv("STK_K2_AG")) c->k2_ag_mc = std::strcmp(v, "mc") == 0;
-  if (const char* v = std::getenv("STK_K1_ONE_SHOT_KB")) c->one_shot_bytes = size_t(std::max(0, std::atoi(v))) << 10;
   // memory back end: VMM (needed for NVLS multicast) when there are peers and the driver supports it
   bool mc = false;
   const bool vmm = stk_vmm_available(device, &mc);
@@ -139,8 +129,6 @@ int stk_ctx_destroy(stk_ctx* c) {
     if (ev) cudaEventDestroy(ev);
   if (c->loss_ring) cudaFreeHost(c->loss_ring);
   cudaFree(c->blk_partial_dev);
-  cudaFree(c->grp_partial_dev);
-  cudaFree(c->grp_count_dev);
   cudaFree(c->prof_ns_dev);
   cudaFreeHost(c->host_scratch);
   delete c;
@@ -446,10 +434,6 @@ int stk_option_set(stk_ctx* c, int key, int value) {
     case STK_OPT_K2_AG_MC:
       c->k2_ag_mc = value != 0;
       return STK_OK;
-    case STK_OPT_K1_ONE_SHOT_KB:
-      STK_REQUIRE(c, value >= 0, "stk_option_set: one-shot threshold must be >= 0 KiB");
-      c->one_shot_bytes = size_t(value) << 10;
-      return STK_OK;
     default:
       return stk_fail(c, STK_ERR_INVALID, "stk_option_set: unknown key");
   }
@@ -465,7 +449,6 @@ int stk_option_get(stk_ctx* c, int key, int* value) {
     case STK_OPT_COOP_LAUNCH: *value = c->coop_launch; return STK_OK;
     case STK_OPT_NVLS_MAX_BLOCKS: *value = c->nvls_max_blocks; return STK_OK;
     case STK_OPT_K2_AG_MC: *value = c->k2_ag_mc; return STK_OK;
-    case STK_OPT_K1_ONE_SHOT_KB: *value = (int)(c->one_shot_bytes >> 10); return STK_OK;
     default: return stk_fail(c, STK_ERR_INVALID, "stk_option_get: unknown key");
   }
 }

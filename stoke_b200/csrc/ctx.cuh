@@ -13,7 +13,7 @@
 struct StepAccum {          // per-optimizer-step accumulators on the device (local shard)
   float norm_partial;       // running sum / max over the buckets reduced so far
   uint32_t found_inf;
-  uint32_t blocks_done;     // last-block detection counter (self-resetting)
+  uint32_t blocks_done;     // last-block detection counter of the cross-rank K1 (self-resetting)
   uint32_t pad_;
 };
 
@@ -59,8 +59,6 @@ struct stk_ctx {
   int k1_max_blocks = 0;        // 0: one block per SM
   int coop_launch = 1;
   int nvls_max_blocks = 0;      // grid bound of the multimem flavour (0: like the other flavours)
-  size_t one_shot_bytes = 0;    // all-reduce buckets up to this many input bytes take the one-shot form (0 = never, the default:
-                                // the two-shot form is the default until the one-shot form is shown faster on H100 systems)
   int k2_ag_mc = 0;             // sharded step publishes its shard with multimem.st (one store replicated by the switch)
   // device state
   std::vector<StepState> states;      // [0] is created with the context
@@ -68,8 +66,6 @@ struct stk_ctx {
   stk_scaler_state_t* scaler_dev = nullptr;   // == states[cur_state]
   StepAccum* accum_dev = nullptr;
   float* blk_partial_dev = nullptr;   // [blk_partial_cap] per-block norm partials of K1
-  float* grp_partial_dev = nullptr;   // [blk_partial_cap / 64 + 1] per-group partials (two-level ticket)
-  uint32_t* grp_count_dev = nullptr;  // [blk_partial_cap / 64 + 1] group tickets (self-resetting)
   size_t blk_partial_cap = 0;
   // optional launch timing (stk_profile_*): CUDA-event pairs recorded around the kernel launch, on the launch stream
   bool profiling = false;

@@ -112,28 +112,12 @@ __global__ void __launch_bounds__(kBulkThreads, 1) k_grad_reduce_bulk(const Redu
 #pragma unroll
       for (int r = 0; r < WMAX; ++r)
         if (r < W) {  // rank order, fp32
-          const uint32_t w4[4] = {raw[r].x, raw[r].y, raw[r].z, raw[r].w};
+          float f[8];
+          unpack16<IN_DT>(raw[r], f);
 #pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            if (IN_DT == STK_BF16) {
-              x[2 * j] += bf16lo(w4[j]);
-              x[2 * j + 1] += bf16hi(w4[j]);
-            } else {
-              x[2 * j] += f16lo(w4[j]);
-              x[2 * j + 1] += f16hi(w4[j]);
-            }
-          }
+          for (int i = 0; i < 8; ++i) x[i] += f[i];
         }
-#pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        float y = x[i] * mul;
-        bad |= !finitef(y);
-        y *= inv_scale;
-        x[i] = y;
-        if (p.norm_kind == STK_NORM_L2) part = fmaf(y, y, part);
-        else if (p.norm_kind == STK_NORM_INF) part = fmax_nan(part, fabsf(y));
-        else if (p.norm_kind == STK_NORM_P) part += __powf(fabsf(y), p.norm_p);
-      }
+      fold8(x, mul, inv_scale, p.norm_kind, p.norm_p, part, bad);
 #pragma unroll
       for (int d = 0; d < WMAX; ++d)
         if (d < p.n_dst) {
@@ -142,7 +126,7 @@ __global__ void __launch_bounds__(kBulkThreads, 1) k_grad_reduce_bulk(const Redu
         }
     }
   }
-  reduce_tail<IN_DT, W_T>(p, part, bad, t_begin);
+  cross_rank_tail<IN_DT, W_T>(p, part, bad, t_begin);
 }
 
 template <int IN_DT, int OUT_DT>

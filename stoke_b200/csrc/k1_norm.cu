@@ -2,11 +2,13 @@
 // reduced gradients for the stock-optimizer route.
 //
 //   k_grad_norm  : reads the raw gradient bucket ONCE (2 B/element for bf16), accumulates sum g^2 | max |g| | sum |g|^p and the
-//                  inf/nan flag of x = (g [+ acc]) * mul / scale, finishes them into the state (grad_norm, found_inf).  Writes
-//                  nothing: the fused optimizer step (k_optim_step, raw route) reads the bucket a second time -- from L2 when
-//                  the bucket fits (loads here carry an L2 evict_last policy; H100's L2 is 50 MB) --
-//                  and zeroes it.  Replaces the W == 1 form of k_grad_reduce on the training path: 2 + 30 B/element through
-//                  HBM instead of 8 + 30 (no fp32 main-grad round trip).
+//                  inf/nan flag of x = (g [+ acc]) * mul / scale, one partial per block.  Writes nothing else: the fused
+//                  optimizer step (k_optim_step, raw route) reads the bucket a second time -- from L2 when the bucket fits
+//                  (loads here carry an L2 evict_last policy; H100's L2 is 50 MB) -- and zeroes it.  Replaces the W == 1
+//                  form of k_grad_reduce on the training path: 2 + 30 B/element through HBM instead of 8 + 30 (no fp32
+//                  main-grad round trip).
+//   k_grad_norm_finish : one block behind k_grad_norm or the W == 1 k_grad_reduce: folds their block partials and
+//                  finishes them into the state (grad_norm, found_inf).
 //   k_grad_scale : grad *= clip coefficient, or clamp (clip_grad_norm_'s scaling pass / clip_grad_value_,
 //                  torch/nn/utils/clip_grad.py) for optimizers the fused step does not cover.
 #include <cstdlib>
@@ -39,7 +41,6 @@ struct NormParams {
                      // read of the bucket then partly hits L2: on H100 (50 MB L2) at ResNet-50 size (51 MB bf16 bucket) K2 is
                      // 7 us faster and this pass 2 us slower than without the hint (bench.py, H100 80GB HBM3 at 400 W)
   stk_scaler_state_t* scaler;
-  StepAccum* accum;
   float* blk_partial;
 };
 
@@ -65,14 +66,7 @@ struct RawVec16 {
     const uint4* q = reinterpret_cast<const uint4*>(base) + v;
     u = keep ? ld16_keep(q, pol) : ld_stream16(q);
   }
-  __device__ void unpack(float (&f)[8]) const {
-    const uint32_t w4[4] = {u.x, u.y, u.z, u.w};
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      f[2 * j] = (DT16 == STK_BF16) ? bf16lo(w4[j]) : f16lo(w4[j]);
-      f[2 * j + 1] = (DT16 == STK_BF16) ? bf16hi(w4[j]) : f16hi(w4[j]);
-    }
-  }
+  __device__ void unpack(float (&f)[8]) const { unpack16<DT16>(u, f); }
 };
 template <>
 struct RawVec<STK_BF16> : RawVec16<STK_BF16> {};
@@ -85,10 +79,9 @@ constexpr int kNormUnroll = 8;  // 8 independent 16-byte loads per thread: 32 KB
 // One-shot blocks (one tile of kNormThreads * kNormUnroll vectors each, the shape that streams best on this part,
 // tools/membench.cu): load, reduce, write ONE partial, retire -- no ticket, no fence, no block waits on an atomic.  The
 // partials are folded by k_grad_norm_finish, a single block launched right behind on the same stream (stream order is the
-// only synchronisation), in a fixed order -> run-to-run deterministic.
+// only synchronisation), in a fixed order -> run-to-run deterministic.  k_grad_reduce at world 1 ends the same way.
 template <int IN_DT, bool HAS_ACC>
 __global__ void __launch_bounds__(kNormThreads) k_grad_norm(const NormParams p) {
-  __shared__ float s_red[32];
   const uint64_t pol = policy_evict_last();
   float inv_scale = 1.f;
   if (p.flags & STK_RF_UNSCALE) inv_scale = (float)(1.0 / (double)p.scaler->scale);
@@ -114,34 +107,21 @@ __global__ void __launch_bounds__(kNormThreads) k_grad_norm(const NormParams p) 
 #pragma unroll
         for (int i = 0; i < 8; ++i) g[i] += a[i];
       }
-#pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        float x = g[i] * mul;
-        bad |= !finitef(x);
-        x *= inv_scale;
-        if (p.norm_kind == STK_NORM_L2) part = fmaf(x, x, part);
-        else if (p.norm_kind == STK_NORM_INF) part = fmax_nan(part, fabsf(x));
-        else if (p.norm_kind == STK_NORM_P) part += __powf(fabsf(x), p.norm_p);
-      }
+      fold8(g, mul, inv_scale, p.norm_kind, p.norm_p, part, bad);
     }
   }
-  const bool mx = p.norm_kind == STK_NORM_INF;
-  const float blk = mx ? block_reduce<true>(part, s_red) : block_reduce<false>(part, s_red);
-  const int any_bad = __syncthreads_or(bad ? 1 : 0);
-  if (threadIdx.x == 0) {
-    // the sign bit of the partial carries the block's inf/nan verdict (partials are +0, positive, +inf or NaN for every
-    // norm kind); setting the bit keeps the magnitude, so an inf or NaN partial reaches the finisher as it is
-    p.blk_partial[blockIdx.x] = any_bad ? __uint_as_float(__float_as_uint(blk) | 0x80000000u) : blk;
-  }
+  store_block_partial(p.blk_partial, p.norm_kind, part, bad);
 }
 
-__global__ void __launch_bounds__(1024) k_grad_norm_finish(const NormParams p, unsigned nblocks) {
+// Folds the partials of k_grad_norm or of the world-1 k_grad_reduce (sign bit: the block saw inf/nan) in a fixed order and
+// applies the bucket to the step accumulators.
+__global__ void __launch_bounds__(1024) k_grad_norm_finish(const FinishParams f, unsigned nblocks) {
   __shared__ float s_red[32];
-  const bool mx = p.norm_kind == STK_NORM_INF;
+  const bool mx = f.norm_kind == STK_NORM_INF;
   float x = 0.f;
   bool bad = false;
   for (unsigned b = threadIdx.x; b < nblocks; b += blockDim.x) {
-    float y = __ldcg(&p.blk_partial[b]);
+    float y = __ldcg(&f.blk_partial[b]);
     if (__float_as_uint(y) & 0x80000000u) {
       bad = true;
       y = fabsf(y);
@@ -150,24 +130,12 @@ __global__ void __launch_bounds__(1024) k_grad_norm_finish(const NormParams p, u
   }
   const float tot = mx ? block_reduce<true>(x, s_red) : block_reduce<false>(x, s_red);
   const int any_bad = __syncthreads_or(bad ? 1 : 0);
-  if (threadIdx.x == 0) {
-    float run = p.accum->norm_partial;
-    run = mx ? fmax_nan(run, tot) : run + tot;
-    uint32_t inf = p.accum->found_inf | (any_bad ? 1u : 0u);
-    if (p.flags & STK_RF_FINAL) {
-      // an inf / nan gradient gives what torch's clip_grad_norm_ returns: NaN if any element is NaN, else inf
-      float norm = run;
-      if (p.norm_kind == STK_NORM_L2) norm = sqrtf(run);
-      else if (p.norm_kind == STK_NORM_P) norm = powf(run, 1.f / p.norm_p);
-      p.scaler->grad_norm = norm;
-      // the inf gate belongs to the loss scaler (GradScaler.step); without one the reference steps regardless
-      p.scaler->found_inf = (inf && (p.flags & STK_RF_UNSCALE)) ? 1 : 0;
-      run = 0.f;
-      inf = 0;
-    }
-    p.accum->norm_partial = run;
-    p.accum->found_inf = inf;
-  }
+  if (threadIdx.x == 0) finish_bucket(f, tot, any_bad != 0);
+}
+
+cudaError_t launch_norm_finish(const FinishParams& f, unsigned nblocks, cudaStream_t s) {
+  k_grad_norm_finish<<<1, 1024, 0, s>>>(f, nblocks);
+  return cudaGetLastError();
 }
 
 __global__ void __launch_bounds__(256) k_grad_scale(float* __restrict__ grad, size_t nvec, int clip_kind, float max_norm,
@@ -217,7 +185,6 @@ int stk_grad_norm(stk_ctx* c, const void* grad, int grad_dtype, const float* acc
     p.keep_l2 = keep;
   }
   p.scaler = c->scaler_dev;
-  p.accum = c->accum_dev;
   const size_t tile = size_t(kNormThreads) * kNormUnroll;
   size_t want = (p.nvec + tile - 1) / tile;
   if (want < 1) want = 1;
@@ -236,8 +203,7 @@ int stk_grad_norm(stk_ctx* c, const void* grad, int grad_dtype, const float* acc
   p.blk_partial = c->blk_partial_dev;
   ProfScope prof(c, 3, s);
   kern<<<grid, kNormThreads, 0, s>>>(p);
-  k_grad_norm_finish<<<1, 1024, 0, s>>>(p, grid);
-  STK_CUDA(c, cudaGetLastError());
+  STK_CUDA(c, launch_norm_finish({p.blk_partial, c->accum_dev, p.scaler, p.norm_p, p.norm_kind, p.flags}, grid, s));
   return STK_OK;
 }
 

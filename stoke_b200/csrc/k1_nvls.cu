@@ -53,12 +53,7 @@ __global__ void __launch_bounds__(kNvlsThreads, 1) k_grad_reduce_nvls(const Redu
           x[u][4] = b.x; x[u][5] = b.y; x[u][6] = b.z; x[u][7] = b.w;
         } else {
           const uint4 r = (IN_DT == STK_BF16) ? mm_ld_reduce_bf16x8(gmc + v * kInBytes) : mm_ld_reduce_f16x8(gmc + v * kInBytes);
-          const uint32_t w4[4] = {r.x, r.y, r.z, r.w};
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            x[u][2 * j] = (IN_DT == STK_BF16) ? bf16lo(w4[j]) : f16lo(w4[j]);
-            x[u][2 * j + 1] = (IN_DT == STK_BF16) ? bf16hi(w4[j]) : f16hi(w4[j]);
-          }
+          unpack16<IN_DT>(r, x[u]);
         }
       } else {
 #pragma unroll
@@ -69,18 +64,7 @@ __global__ void __launch_bounds__(kNvlsThreads, 1) k_grad_reduce_nvls(const Redu
     for (int u = 0; u < U; ++u) {
       const size_t v = v0 + u * stride;
       const bool active = v < p.vec_end;
-      if (active) {
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          float y = x[u][i] * mul;
-          bad |= !finitef(y);
-          y *= inv_scale;
-          x[u][i] = y;
-          if (p.norm_kind == STK_NORM_L2) part = fmaf(y, y, part);
-          else if (p.norm_kind == STK_NORM_INF) part = fmax_nan(part, fabsf(y));
-          else if (p.norm_kind == STK_NORM_P) part += __powf(fabsf(y), p.norm_p);
-        }
-      }
+      if (active) fold8(x[u], mul, inv_scale, p.norm_kind, p.norm_p, part, bad);
       if (all) {  // uniform
         if constexpr (OUT_DT == STK_F32) {
           // multimem.st moves at most 16 bytes per thread; two 16-byte stores per thread at a 32-byte thread stride would
@@ -120,7 +104,7 @@ __global__ void __launch_bounds__(kNvlsThreads, 1) k_grad_reduce_nvls(const Redu
       }
     }
   }
-  reduce_tail<IN_DT, 0>(p, part, bad, t_begin);
+  cross_rank_tail<IN_DT, 0>(p, part, bad, t_begin);
 }
 
 template <int IN_DT, int OUT_DT>

@@ -3,7 +3,8 @@
 //   k_grad_accumulate : acc (+)= float(grad)                      (local micro-steps under no_sync; HBM-bound)
 //   k_grad_reduce     : main = (sum over ranks of grad [+ acc]) * mul * inv_scale   for the shard this rank owns,
 //                       pushed to every rank (all-reduce) or kept (reduce-scatter); fused inf/nan test and
-//                       norm partial (sum g^2 | max |g| | sum |g|^p); last block finishes them across ranks.
+//                       norm partial (sum g^2 | max |g| | sum |g|^p); across ranks the last block finishes them, at
+//                       world 1 k_grad_norm_finish (k1_norm.cu) does, launched right behind.
 //
 // Replaces, in one pass: DDP bucket copy-in (/W), NCCL all-reduce, bucket copy-out, GradScaler.unscale_, and the two
 // reduction passes of clip_grad_norm_ (see include/stoke_b200.h for reference file:line).
@@ -45,20 +46,20 @@ struct Unroll {
   static constexpr int value = W == 1 ? 2 : (W == 2 ? 2 : 1);
 };
 
-// W_T: compile-time world size (1, 2, 4, 8) or 0 = runtime p.world
+// W_T: compile-time world size (1, 2, 4, 8) or 0 = runtime p.world (the other cross-rank sizes; never 1)
 template <int IN_DT, int OUT_DT, int W_T>
 __global__ void __launch_bounds__(W_T == 1 ? 256 : 512, W_T == 1 ? 6 : 1) k_grad_reduce(const ReduceParams p) {
   const int W = W_T ? W_T : p.world;
   constexpr int U = Unroll<W_T>::value;
   constexpr int WMAX = W_T ? W_T : kMaxWorld;
   const bool has_acc = p.acc.p[0] != nullptr;
-  const bool zero_in = (p.flags & STK_RF_ZERO_INPUT) && W == 1;
+  const bool zero_in = W_T == 1 && (p.flags & STK_RF_ZERO_INPUT);  // cross-rank: zeroed in the tail, after the end barrier
 
-  if (W > 1 && !block_barrier_all_ranks(p.pads, p.rank, W, 0, p.epoch)) return;  // peer missing: error word set
+  if (W_T != 1 && !block_barrier_all_ranks(p.pads, p.rank, W, 0, p.epoch)) return;  // peer missing: error word set
   // device-side timing of the data phase (after the start barrier = after the slowest rank has arrived, up to the end
   // barrier): the NVLink time of this launch without the cross-rank launch skew that host-side events include
   unsigned long long t_begin = 0;
-  if (p.prof_ns && blockIdx.x == 0 && threadIdx.x == 0) t_begin = globaltimer_ns();
+  if (W_T != 1 && p.prof_ns && blockIdx.x == 0 && threadIdx.x == 0) t_begin = globaltimer_ns();
 
   float inv_scale = 1.f;
   if (p.flags & STK_RF_UNSCALE) inv_scale = (float)(1.0 / (double)p.scaler->scale);
@@ -109,19 +110,13 @@ __global__ void __launch_bounds__(W_T == 1 ? 256 : 512, W_T == 1 ? 6 : 1) k_grad
         float s[8];
 #pragma unroll
         for (int i = 0; i < 8; ++i) {
-          float x = g[u][0][i];
+          s[i] = g[u][0][i];
 #pragma unroll
           for (int r = 1; r < WMAX; ++r)
-            if (r < W) x += g[u][r][i];
-          x *= mul;
-          bad |= !finitef(x);
-          x *= inv_scale;
-          s[i] = x;
-          if (p.norm_kind == STK_NORM_L2) part = fmaf(x, x, part);
-          else if (p.norm_kind == STK_NORM_INF) part = fmax_nan(part, fabsf(x));
-          else if (p.norm_kind == STK_NORM_P) part += __powf(fabsf(x), p.norm_p);
+            if (r < W) s[i] += g[u][r][i];
         }
-        if (OUT_DT == STK_BF16 && p.norm_kind != STK_NORM_NONE) { /* norm is of the fp32 value, before rounding */ }
+        // the norm is of the fp32 value, before a bf16 output rounds it
+        fold8(s, mul, inv_scale, p.norm_kind, p.norm_p, part, bad);
 #pragma unroll
         for (int d = 0; d < WMAX; ++d)
           if (d < p.n_dst) {
@@ -134,7 +129,8 @@ __global__ void __launch_bounds__(W_T == 1 ? 256 : 512, W_T == 1 ? 6 : 1) k_grad
     }
   }
 
-  reduce_tail<IN_DT, W_T>(p, part, bad, t_begin);
+  if constexpr (W_T == 1) store_block_partial(p.blk_partial, p.norm_kind, part, bad);
+  else cross_rank_tail<IN_DT, W_T>(p, part, bad, t_begin);
 }
 
 template <int IN_DT, int OUT_DT>
@@ -148,7 +144,11 @@ static cudaError_t launch_reduce(stk_ctx* c, const ReduceParams& p, int grid, bo
   if (!coop) cfg.numAttrs = 0;
   ProfScope prof(c, 0, s);
   switch (p.world) {
-    case 1: return cudaLaunchKernelEx(&cfg, k_grad_reduce<IN_DT, OUT_DT, 1>, p);
+    case 1: {
+      // the block partials are folded by k_grad_norm_finish, behind the kernel on the same stream (as stk_grad_norm does)
+      const cudaError_t e = cudaLaunchKernelEx(&cfg, k_grad_reduce<IN_DT, OUT_DT, 1>, p);
+      return e != cudaSuccess ? e : launch_norm_finish(finish_params(p), (unsigned)grid, s);
+    }
     case 2: return cudaLaunchKernelEx(&cfg, k_grad_reduce<IN_DT, OUT_DT, 2>, p);
     case 4: return cudaLaunchKernelEx(&cfg, k_grad_reduce<IN_DT, OUT_DT, 4>, p);
     case 8: return cudaLaunchKernelEx(&cfg, k_grad_reduce<IN_DT, OUT_DT, 8>, p);
@@ -207,9 +207,6 @@ int stk_grad_reduce(stk_ctx* c, int mode, void* const* grad_ptrs, int grad_dtype
   p.pads = c->pads;
   p.scaler = c->scaler_dev;
   p.accum = c->accum_dev;
-  p.blk_partial = c->blk_partial_dev;
-  p.grp_partial = c->grp_partial_dev;
-  p.grp_count = c->grp_count_dev;
   p.prof_ns = c->profiling ? c->prof_ns_dev : nullptr;
   size_t b = 0, e = 0;
   stk_shard_range(n, W, c->rank, &b, &e);
@@ -229,39 +226,26 @@ int stk_grad_reduce(stk_ctx* c, int mode, void* const* grad_ptrs, int grad_dtype
   p.aux_epoch = (flags & STK_RF_FINAL) ? ++c->aux_epoch[0] : c->aux_epoch[0];
 
   // grid: identical on every rank (depends on n and W only).  Cross-rank kernels spin on peers, so every block must be
-  // resident: one 512-thread block per SM, cooperative launch.
+  // resident: one 512-thread block per SM, cooperative launch.  World 1: one block per chunk of U * 256 vectors, each
+  // leaving one norm partial for k_grad_norm_finish.
   const size_t nvec_shard = p.vec_per_shard;
   const int U = W == 1 ? 2 : (W == 2 ? 2 : 1);
   const size_t threads = W == 1 ? 256 : 512;
-  size_t want = (nvec_shard + threads * U - 1) / (threads * U);
+  const size_t want = (nvec_shard + threads * U - 1) / (threads * U);
   int grid;
   const size_t cap = c->k1_max_blocks > 0 ? (size_t)std::min(c->k1_max_blocks, c->sm_count) : (size_t)c->sm_count;
   if (W > 1) grid = (int)std::max<size_t>(1, std::min<size_t>(want, cap));
-  else grid = (int)std::max<size_t>(1, want);  // one-shot: every block does one chunk
+  else grid = (int)std::max<size_t>(1, want);
   {
     int rc = stk_grow_partials(c, (size_t)grid, s);
     if (rc != STK_OK) return rc;
     p.blk_partial = c->blk_partial_dev;
-    p.grp_partial = c->grp_partial_dev;
-    p.grp_count = c->grp_count_dev;
   }
   const bool coop = W > 1;
-  // Small all-reduce buckets: one-shot form.  Every rank sums the whole bucket from all W peers in rank order (bit-identical
-  // on every rank by construction) and stores only locally; its own norm partials are already global.
-  const size_t in_bytes = n * (grad_dtype == STK_F32 ? 4 : 2);
-  if (coop && mode == STK_REDUCE_ALL && c->one_shot_bytes > 0 && in_bytes <= c->one_shot_bytes) {
-    p.one_shot = 1;
-    p.vec_begin = 0;
-    p.vec_end = p.vec_total;
-    p.vec_per_shard = p.vec_total;
-    p.n_dst = 1;
-    want = (p.vec_total + threads * U - 1) / (threads * U);
-    grid = (int)std::max<size_t>(1, std::min<size_t>(want, cap));
-  }
   if (coop && grid > kMaxReduceBlocks) grid = kMaxReduceBlocks;
 
   cudaError_t err = cudaErrorNotSupported;
-  if (coop && c->k1_algo == 2 && acc_ptrs == nullptr && !p.one_shot) {
+  if (coop && c->k1_algo == 2 && acc_ptrs == nullptr) {
     // multimem flavour: needs the multicast mappings of the gradient bucket and (all-reduce) of the output bucket
     p.grad_mc = stk_mc_lookup(c, grad_ptrs[c->rank]);
     p.out_mc = (mode == STK_REDUCE_ALL) ? stk_mc_lookup(c, out_ptrs[c->rank]) : nullptr;
@@ -277,7 +261,7 @@ int stk_grad_reduce(stk_ctx* c, int mode, void* const* grad_ptrs, int grad_dtype
     }
   }
   if (err == cudaSuccess) return STK_OK;
-  if (coop && c->k1_algo >= 1 && !p.one_shot) {
+  if (coop && c->k1_algo >= 1) {
     err = launch_reduce_bulk(c, p, grad_dtype, out_dtype, grid, s);
     if (err != cudaSuccess && err != cudaErrorNotSupported)
       return stk_fail(c, STK_ERR_CUDA, std::string("k_grad_reduce_bulk launch: ") + cudaGetErrorString(err));

@@ -181,7 +181,9 @@ REDUCE_CASES = [  # n, in dtype, out dtype, accumulator, zero input, norm p, los
     (262_136, BF16, F32, False, True, 2.0, None, 3),
     (262_152, F32, BF16, False, True, math.inf, None, 2),
     (262_152, F16, F32, True, True, 1.0, 2.0**16, 1),
-    (25_557_040, BF16, F32, False, True, 2.0, None, 1),   # more than 32 ticket groups
+    (25_557_040, BF16, F32, False, True, 2.0, None, 1),   # 6240 blocks: every finisher thread folds several partials
+    (4_194_304, BF16, F32, False, True, 2.0, None, 1),    # 1024 blocks: one partial per finisher thread
+    (4_194_312, BF16, F32, False, True, 2.0, None, 1),    # 1025 blocks: the finisher's thread 0 folds two partials
 ]
 
 
