@@ -279,6 +279,15 @@ int stk_barrier(stk_ctx* ctx, void* stream);
 /* every rank copies bytes from ptrs[root] to ptrs[rank] (peer pull) with start/end barriers */
 int stk_bcast(stk_ctx* ctx, void* const* ptrs, size_t bytes, int root, void* stream);
 
+/* ---- model forward ------------------------------------------------------------------------------------------------- */
+/* Training-mode BatchNorm apply + optional residual add + ReLU over a bf16 channels-last (NHWC) tensor of `numel` elements
+ * and `channels` channels (multiple of 8, numel < 2^31, every pointer 16-byte aligned), from statistics torch reduced
+ * (torch.batch_norm_update_stats: fp32 mean and biased var):
+ *   out = relu(bf16(bf16(weight * (x - mean) * invstd + bias) + residual)),  save_invstd[c] = rsqrtf(var[c] + eps)
+ * with every intermediate rounded as the unfused torch ops round it (bit-identical to them).  residual may be NULL. */
+int stk_bn_act(stk_ctx* ctx, const void* x, const void* residual, const float* mean, const float* var, const void* weight,
+               const void* bias, double eps, void* out, float* save_invstd, size_t numel, size_t channels, void* stream);
+
 /* ---- sampler (stoke/data.py) ---------------------------------------------------------------------------------------- */
 /* torch.randperm(n, generator=g) for each n in lens[0..k) drawn from ONE mt19937 seeded with `seed` (host, bit-exact
  * with torch's CPU generator); out receives the k permutations back to back as int32. */

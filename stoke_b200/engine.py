@@ -307,6 +307,15 @@ class Engine:
         self._check(self.lib.stk_loss_sync_wait(self.ctx, ticket, C.byref(out)))
         return out.value
 
+    def bn_act(self, x: torch.Tensor, residual: Optional[torch.Tensor], mean: torch.Tensor, var: torch.Tensor,
+               weight: torch.Tensor, bias: torch.Tensor, eps: float, out: torch.Tensor, save_invstd: torch.Tensor):
+        """``out = relu(bn(x) [+ residual])`` over a bf16 channels-last tensor from torch's fp32 batch statistics; writes
+        ``save_invstd`` (``stk_bn_act``).  ``fuse.py`` checks dtypes, layout and alignment before calling."""
+        self._check(self.lib.stk_bn_act(self.ctx, x.data_ptr(), residual.data_ptr() if residual is not None else None,
+                                        mean.data_ptr(), var.data_ptr(), weight.data_ptr(), bias.data_ptr(), float(eps),
+                                        out.data_ptr(), save_invstd.data_ptr(), x.numel(), x.shape[1], self._stream()))
+        self.launches += 1
+
     def barrier(self):
         self._check(self.lib.stk_barrier(self.ctx, self._stream()))
         self.launches += 1 if self.world > 1 else 0

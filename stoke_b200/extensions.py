@@ -78,6 +78,12 @@ class B200DataParallel(torch.nn.Module):
         self._buf_flat = None
         self._buf_bytes = 0
         self.require_backward_grad_sync = True
+        self._run = None
+
+    def set_forward(self, fn):
+        """Calls ``fn`` (``fuse.FusedForward`` over ``self.module``: not a module, so ``parameters()`` and
+        ``state_dict()`` stay the user module's) in place of ``self.module``."""
+        self._run = fn
 
     def _flatten_buffers(self):
         bufs = [b for b in self.module.buffers() if b is not None and b.numel() > 0]
@@ -103,7 +109,7 @@ class B200DataParallel(torch.nn.Module):
                 self._flatten_buffers()
             if self._broadcast_buffers:
                 self._engine.bcast(self._buf_flat, self._buf_bytes, root=0)
-        return self.module(*args, **kwargs)
+        return (self.module if self._run is None else self._run)(*args, **kwargs)
 
     @contextmanager
     def no_sync(self):

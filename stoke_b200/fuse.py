@@ -1,0 +1,223 @@
+# -*- coding: utf-8 -*-
+"""BatchNorm2d -> [add] -> ReLU in one pass for bf16 channels-last training (``stk_bn_act``, csrc/bn_act.cu).
+
+``fuse_bn_act(module, engine)`` traces ``module`` with ``torch.fx`` into a ``GraphModule`` that shares every submodule,
+parameter and buffer with ``module``, in which each ``BatchNorm2d -> ReLU`` and ``BatchNorm2d -> add -> ReLU`` chain
+(every intermediate with that single user) is one ``BnAct`` call.  It returns a ``FusedForward``, which runs that graph
+only for calls it is a faithful trace of (training mode, required arguments only, no hooks) and ``module`` itself for
+every other call, or None when tracing or rewriting fails or nothing matches; the caller then keeps running ``module``.
+
+What stays torch's: the forward statistics and the running-statistics update (``torch.batch_norm_update_stats``, the
+reduction the native training forward runs) and the whole backward (``threshold_backward`` +
+``native_batch_norm_backward``, the calls autograd makes for the unfused chain).  Only the elementwise apply / add / ReLU
+moves into the kernel, which rounds every intermediate as the unfused ops do, so the results are bit-identical to them.
+Each call falls back to the unfused torch ops when the kernel does not cover its inputs (eval mode, no running statistics,
+not bf16, not channels-last, misaligned, C % 8 != 0, 2^31 elements or more, a CPU tensor), so the same inputs give the
+same results whether or not the model was rewritten.
+"""
+import inspect
+import operator
+from typing import Optional
+
+import torch
+import torch.nn.functional as F
+
+_RELU_FNS = (F.relu, torch.relu)
+_ADD_FNS = (operator.add, operator.iadd, torch.add)
+
+
+def _momentum(bn: torch.nn.BatchNorm2d) -> float:
+    """The running-statistics bookkeeping of ``_BatchNorm.forward`` in training mode: bumps ``num_batches_tracked`` and
+    returns the averaging factor (a cumulative average when ``momentum`` is None)."""
+    factor = 0.0 if bn.momentum is None else bn.momentum
+    if bn.num_batches_tracked is not None:
+        bn.num_batches_tracked.add_(1)
+        factor = 1.0 / float(bn.num_batches_tracked) if bn.momentum is None else bn.momentum
+    return factor
+
+
+def _aligned(*ts) -> bool:
+    return all(t.data_ptr() % 16 == 0 for t in ts)
+
+
+def _covered(bn: torch.nn.BatchNorm2d, x: torch.Tensor, r: Optional[torch.Tensor]) -> bool:
+    if not (bn.training and bn.track_running_stats and bn.running_mean is not None and bn.running_var is not None):
+        return False
+    w, b = bn.weight, bn.bias
+    if w is None or b is None or w.dtype != torch.bfloat16 or b.dtype != torch.bfloat16:
+        return False
+    if not (x.is_cuda and x.dtype == torch.bfloat16 and x.dim() == 4 and x.is_contiguous(memory_format=torch.channels_last)):
+        return False
+    n, c = x.numel(), x.shape[1]
+    if c % 8 or n // c < 2 or n >= 2 ** 31 or not (w.is_contiguous() and b.is_contiguous() and _aligned(x, w, b)):
+        return False
+    if r is not None and not (r.shape == x.shape and r.dtype == x.dtype and r.device == x.device
+                              and r.is_contiguous(memory_format=torch.channels_last) and _aligned(r)):
+        return False
+    return True
+
+
+class _BnActFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, x, weight, bias, residual, bn, engine):
+        momentum = _momentum(bn)
+        mean, var = torch.batch_norm_update_stats(x, bn.running_mean, bn.running_var, momentum)
+        out = torch.empty_like(x)
+        invstd = torch.empty_like(mean)
+        engine.bn_act(x, residual, mean, var, weight, bias, bn.eps, out, invstd)
+        ctx.save_for_backward(x, weight, out, mean, invstd)
+        ctx.bn = bn
+        ctx.has_residual = residual is not None
+        return out
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        x, weight, out, mean, invstd = ctx.saved_tensors
+        bn = ctx.bn
+        g = torch.ops.aten.threshold_backward(grad_out, out, 0)
+        mask = [ctx.needs_input_grad[0], ctx.needs_input_grad[1], ctx.needs_input_grad[2]]
+        dx, dw, db = torch.ops.aten.native_batch_norm_backward(g, x, weight, bn.running_mean, bn.running_var, mean, invstd,
+                                                              True, bn.eps, mask)
+        dr = g if ctx.has_residual and ctx.needs_input_grad[3] else None
+        return dx, dw, db, dr, None, None
+
+
+class BnAct(torch.nn.Module):
+    """``relu(bn(x) [+ residual])``: one ``stk_bn_act`` launch when the kernel covers the inputs, the unfused torch ops
+    otherwise (``inplace``: the add was ``out += residual``, which keeps ``out``'s dtype).  Holds a reference to the
+    user's BatchNorm2d (shared, not copied)."""
+
+    def __init__(self, bn: torch.nn.BatchNorm2d, engine, inplace: bool = False):
+        super().__init__()
+        self.bn = bn
+        self._engine = engine
+        self._inplace = inplace
+
+    def forward(self, x, residual=None):
+        if _covered(self.bn, x, residual):
+            return _BnActFn.apply(x, self.bn.weight, self.bn.bias, residual, self.bn, self._engine)
+        y = self.bn(x)
+        if residual is not None:
+            if self._inplace:
+                y += residual
+            else:
+                y = y + residual
+        return torch.relu(y)
+
+
+class _InplaceProxy(torch.fx.Proxy):
+    """Records ``a += b`` as ``operator.iadd`` (plain fx rebinds the name to ``a + b``, which drops the mutation and, for
+    mixed dtypes, changes the result's dtype)."""
+
+
+for _op in ("iadd", "isub", "imul", "itruediv"):
+    setattr(_InplaceProxy, f"__{_op}__",
+            lambda self, other, _f=getattr(operator, _op): self.tracer.create_proxy("call_function", _f, (self, other), {}))
+
+
+class _Tracer(torch.fx.Tracer):
+    def proxy(self, node):
+        return _InplaceProxy(node, self)
+
+
+class FusedForward:
+    """Calls the rewritten graph in place of ``module`` when the call is one the graph is a faithful trace of, and
+    ``module`` itself otherwise.  The graph was traced in training mode with every optional argument at its default, and
+    it inlines containers, so it is used only when every submodule is in training mode, the call passes exactly the
+    required arguments positionally, and no module or global hook is registered."""
+
+    def __init__(self, module: torch.nn.Module, gm: torch.fx.GraphModule, n_required: int, sites: int):
+        self.module, self.graph_module, self.fused_sites = module, gm, sites
+        self._n_required = n_required
+        self._modules = list(module.modules())
+
+    def _graph_applies(self, args, kwargs) -> bool:
+        if kwargs or len(args) != self._n_required:
+            return False
+        g = torch.nn.modules.module
+        if any(getattr(g, h, None) for h in _GLOBAL_HOOKS):
+            return False
+        return all(m.training and not (m._forward_hooks or m._forward_pre_hooks or m._backward_hooks
+                                       or m._backward_pre_hooks) for m in self._modules)
+
+    def __call__(self, *args, **kwargs):
+        if self._graph_applies(args, kwargs):
+            return self.graph_module(*args)
+        return self.module(*args, **kwargs)
+
+
+_GLOBAL_HOOKS = ("_global_forward_hooks", "_global_forward_pre_hooks", "_global_backward_hooks",
+                 "_global_backward_pre_hooks")
+
+
+def _is_relu(gm: torch.fx.GraphModule, node: torch.fx.Node) -> bool:
+    if node.op == "call_module":
+        return type(gm.get_submodule(node.target)) is torch.nn.ReLU
+    return node.op == "call_function" and node.target in _RELU_FNS
+
+
+def _single_bn_input(gm: torch.fx.GraphModule, node) -> bool:
+    """``node`` is a BatchNorm2d call on one tensor whose only user is the next node of the chain."""
+    return (isinstance(node, torch.fx.Node) and node.op == "call_module" and len(node.users) == 1
+            and type(gm.get_submodule(node.target)) is torch.nn.BatchNorm2d and len(node.args) == 1 and not node.kwargs)
+
+
+def _trace(module: torch.nn.Module):
+    """(graph module traced in training mode with every optional argument at its default, number of required
+    arguments); the module's training flags are restored afterwards."""
+    params = list(inspect.signature(module.forward).parameters.values())
+    if any(p.kind in (p.VAR_POSITIONAL, p.VAR_KEYWORD, p.KEYWORD_ONLY) for p in params):
+        raise TypeError("only positional forward arguments are traced")
+    required = [p for p in params if p.default is p.empty]   # positional: the ones with defaults come last
+    flags = [(m, m.training) for m in module.modules()]
+    module.train()
+    try:
+        graph = _Tracer().trace(module, concrete_args={p.name: p.default for p in params[len(required):]})
+    finally:
+        for m, t in flags:
+            m.training = t
+    return torch.fx.GraphModule(module, graph), len(required)
+
+
+def _rewrite(gm: torch.fx.GraphModule, engine) -> int:
+    sites = 0
+    for relu in list(gm.graph.nodes):
+        if not _is_relu(gm, relu) or not relu.args:
+            continue
+        src, residual, inplace = relu.args[0], None, False
+        if (isinstance(src, torch.fx.Node) and src.op == "call_function" and src.target in _ADD_FNS and len(src.users) == 1
+                and len(src.args) == 2 and not src.kwargs and all(isinstance(a, torch.fx.Node) for a in src.args)):
+            a, b = src.args
+            inplace = src.target is operator.iadd
+            # an out-of-place add takes the BatchNorm on either side (two-operand float addition is commutative); `+=`
+            # only on the left, where the tensor it mutates is the BatchNorm output nothing else sees
+            bn_node, residual = (a, b) if _single_bn_input(gm, a) or inplace else (b, a)
+            if bn_node is residual:
+                continue
+            chain = [relu, src]
+        else:
+            bn_node, chain = src, [relu]
+        if not _single_bn_input(gm, bn_node):
+            continue
+        name = bn_node.target.replace(".", "_") + "_act"
+        gm.add_submodule(name, BnAct(gm.get_submodule(bn_node.target), engine, inplace))
+        with gm.graph.inserting_before(relu):
+            fused = gm.graph.call_module(name, (bn_node.args[0],) + ((residual,) if residual is not None else ()))
+        relu.replace_all_uses_with(fused)
+        for n in chain + [bn_node]:
+            gm.graph.erase_node(n)
+        sites += 1
+    return sites
+
+
+def fuse_bn_act(module: torch.nn.Module, engine) -> Optional[FusedForward]:
+    try:
+        gm, n_required = _trace(module)
+        sites = _rewrite(gm, engine)
+        if sites == 0:
+            return None
+        gm.graph.lint()
+        gm.recompile()
+    except Exception:  # noqa: BLE001 -- a model fx cannot trace or rewrite runs unchanged
+        return None
+    return FusedForward(module, gm, n_required, sites)

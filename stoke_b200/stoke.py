@@ -23,6 +23,7 @@ from .data import BucketedDistributedSampler, StokeDataLoader
 from .distributed import RunnerDistEnum
 from .extensions import B200DataParallel, RunnerOptimizerEnum
 from .fp16 import RunnerFP16Enum
+from .fuse import fuse_bn_act
 from .io_ops import RunnerIOEnum
 from .status import StokeStatus
 from .utils import ParamNormalize, zero_optimizer_grads
@@ -90,6 +91,15 @@ class Stoke:
             self._optimizer = self._runner.build_optimizer(optimizer=optimizer["optimizer"],
                                                            optimizer_kwargs=optimizer["optimizer_kwargs"],
                                                            model=self._model)
+        self._forward = self._model
+        if self._status.is_fp16_bf16:
+            # BatchNorm2d -> [add] -> ReLU chains run as one kernel pass in training (fuse.py); the user's module is left
+            # as it is and runs every call the rewritten graph does not apply to
+            fused = fuse_bn_act(self.model_access, self._runner.engine)
+            if fused is not None and isinstance(self._model, B200DataParallel):
+                self._model.set_forward(fused)
+            elif fused is not None:
+                self._forward = fused
         self.reset_tracking()
         self._status.set_post_init_values(world_size=self.world_size)
         if self._verbose:
@@ -132,7 +142,7 @@ class Stoke:
     # ---- the four calls ----------------------------------------------------------------------------------------------
     def model(self, *args, **kwargs):
         with self._runner.model_context:
-            return self._model(*args, **kwargs)
+            return self._forward(*args, **kwargs)
 
     def loss(self, *args, **kwargs):
         with self._runner.loss_context:
