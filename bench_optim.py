@@ -1,0 +1,148 @@
+# -*- coding: utf-8 -*-
+"""NAdam, RAdam and Adamax on the fused step, on one GPU, at ResNet-50 size (25.6 M elements) and BERT-base size
+(109.5 M elements), with Adam as the yardstick:
+
+  k_optim_step[raw]    the world-1 route: the step reads and zeroes the raw bf16 bucket and writes the bf16 model copy
+                       (30 B/element algorithmic: read g 2, p m v 12; write p m v 12, bf16 copy 2, zeroing 2), with the
+                       step prologue in front of it
+  k_optim_step[main]   fp32 model, fp32 main gradients (28 B/element: read g p m v 16, write p m v 12)
+  optimizer step       gradient pass + step, the fused route (k_grad_norm + prologue + k_optim_step) against
+                       B200StockOptimizer (K1 main-gradient reduce + the class's own torch update on fp32 views + the cast
+                       into the bf16 model), same class, same gradients, timed in alternating rounds in the same run
+
+    python bench_optim.py [--out optim.json] [--iters 30]
+
+Timing as bench_kernels.py: CUDA events on the launch stream, medians; ResNet-50-sized kernel rows are preceded by an L2 flush
+write.  The card's name and power limit are read in the same run and written with the numbers.
+"""
+import argparse
+import json
+import os
+import subprocess
+import sys
+
+import torch
+
+ROOT = os.path.dirname(os.path.abspath(__file__))
+sys.path.insert(0, ROOT)
+
+
+def card():
+    info = {"name": torch.cuda.get_device_name(0), "power_limit_w": None}
+    try:
+        out = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader,nounits", "-i", "0"],
+                             capture_output=True, text=True, timeout=30).stdout.strip()
+        info["power_limit_w"] = float(out.splitlines()[0])
+    except (OSError, ValueError, IndexError, subprocess.SubprocessError):
+        pass
+    return info
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--out", default=None)
+    ap.add_argument("--iters", type=int, default=30)
+    ap.add_argument("--rounds", type=int, default=4)
+    args = ap.parse_args()
+    if not torch.cuda.is_available():
+        raise SystemExit("bench_optim.py needs a GPU")
+    from stoke_b200 import _lib
+    from stoke_b200.engine import ClipSpec, get_engine
+    from stoke_b200.optim import B200FusedOptimizer, B200StockOptimizer
+
+    torch.cuda.set_device(0)
+    eng = get_engine(0)
+    peak = 3350.0   # H100 SXM data sheet, HBM3
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")
+    rows = []
+    gpu = card()
+    print(json.dumps({"card": gpu}), flush=True)
+
+    def measure(fn, iters, flush_l2):
+        ms = []
+        for _ in range(iters):
+            if flush_l2:
+                flush.fill_(1)
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record()
+            fn()
+            e1.record()
+            torch.cuda.synchronize()
+            ms.append(e0.elapsed_time(e1))
+        return ms
+
+    def report(row):
+        rows.append(row)
+        print(json.dumps(row), flush=True)
+
+    class Flat(torch.nn.Module):
+        def __init__(self, n):
+            super().__init__()
+            self.w = torch.nn.Parameter(torch.zeros(n))
+
+    classes = (("adam", torch.optim.Adam, {"lr": 1e-3}), ("nadam", torch.optim.NAdam, {"lr": 2e-3}),
+               ("radam", torch.optim.RAdam, {"lr": 1e-3}), ("adamax", torch.optim.Adamax, {"lr": 2e-3}))
+    clip = ClipSpec(_lib.CLIP_NORM, max_norm=1.0, norm_type=2.0)
+    for size_name, n in (("resnet50_25.6M", 25_557_032), ("bert_base_109.5M", 109_483_778)):
+        flush_l2 = n < 60_000_000
+        for tag, cls, kw in classes:
+            # ---- the kernel alone, both gradient sources ----
+            for route, lp, per in (("local", torch.bfloat16, 30), ("main", None, 28)):
+                net = Flat(n).cuda()
+                opt = B200FusedOptimizer(net, cls, kw, engine=eng, route=route, clip=clip, lp_dtype=lp)
+                path = opt.path
+                path.g_flat.copy_((torch.randn(path.n, device="cuda") * 1e-3).to(path.g_flat.dtype))
+                if route == "main":
+                    path.main_flat.copy_(torch.randn(path.n, device="cuda") * 1e-3)
+                step = lambda: opt.step()   # noqa: E731 -- prologue + k_optim_step + epilogue
+                measure(step, 5, False)
+                ms = sorted(measure(step, args.iters, flush_l2))
+                med = ms[len(ms) // 2]
+                nbytes = path.n * per
+                report({"row": f"k_optim_step[{'raw' if route == 'local' else 'main'},{tag}] (+prologue, epilogue)",
+                        "size": size_name, "us_median": med * 1e3, "us_min": ms[0] * 1e3, "bytes_per_elem": per,
+                        "achieved_gbs": nbytes / (med * 1e-3) / 1e9, "frac_of_hbm_peak": nbytes / (med * 1e-3) / 1e9 / peak,
+                        "l2_flush_between_launches": flush_l2})
+                opt.close()
+                del opt, path, net
+                torch.cuda.empty_cache()
+            # ---- the whole optimizer step: fused route vs the stock-optimizer route, alternating ----
+            nets = {"fused": Flat(n).cuda(), "stock": Flat(n).cuda()}
+            opts = {"fused": B200FusedOptimizer(nets["fused"], cls, kw, engine=eng, clip=clip, lp_dtype=torch.bfloat16),
+                    "stock": B200StockOptimizer(nets["stock"], cls, kw, engine=eng, clip=clip, lp_dtype=torch.bfloat16)}
+            grads = (torch.randn(opts["fused"].path.n, device="cuda") * 1e-3).to(torch.bfloat16)
+
+            def whole(o):
+                def run():
+                    o.path.g_flat.copy_(grads)   # the same gradients into each route's bucket (2 B/elem, both routes)
+                    o.path.after_backward(sync=True, unscale=False)
+                    o.step()
+                return run
+
+            runs = {k: whole(o) for k, o in opts.items()}
+            for k in runs:
+                measure(runs[k], 3, False)
+            times = {"fused": [], "stock": []}
+            per_round = max(1, args.iters // args.rounds)
+            for _ in range(args.rounds):
+                for k in ("fused", "stock"):
+                    times[k] += measure(runs[k], per_round, flush_l2)
+            med = {}
+            for k, ms in times.items():
+                ms.sort()
+                med[k] = ms[len(ms) // 2]
+            report({"row": f"optimizer_step[{tag}] fused vs stock (grad copy + gradient pass + step)", "size": size_name,
+                    "fused_us_median": med["fused"] * 1e3, "stock_us_median": med["stock"] * 1e3,
+                    "stock_over_fused": med["stock"] / med["fused"], "rounds": args.rounds,
+                    "l2_flush_between_launches": flush_l2})
+            for o in opts.values():
+                o.close()
+            del opts, nets, runs
+            torch.cuda.empty_cache()
+    if args.out:
+        with open(args.out, "w") as f:
+            json.dump({"card": gpu, "peak_hbm_gbs": peak, "rows": rows}, f, indent=1)
+
+
+if __name__ == "__main__":
+    main()

@@ -34,6 +34,7 @@
  *   stk_loss_sync_begin/_wait        detach_and_sync_loss without the per-micro-step host synchronisation
  *   stk_optim_range_prologue         torch's per-parameter `state[p]["step"]` (torch/optim/adam.py: a parameter whose grad is None
  *                                    is not stepped and keeps its own count) for models with sometimes-unused parameters
+ *   stk_optim_step_prologue          the same for every kind, plus NAdam's `state[p]["mu_product"]` (torch/optim/nadam.py)
  */
 #ifndef STOKE_B200_H
 #define STOKE_B200_H
@@ -68,7 +69,12 @@ typedef enum {
 
 typedef enum { STK_NORM_NONE = 0, STK_NORM_L2 = 1, STK_NORM_INF = 2, STK_NORM_P = 3 } stk_norm_kind;
 typedef enum { STK_CLIP_NONE = 0, STK_CLIP_NORM = 1, STK_CLIP_VALUE = 2 } stk_clip_kind;
-typedef enum { STK_OPT_ADAM = 0, STK_OPT_ADAMW = 1, STK_OPT_SGD = 2 } stk_optim_kind;
+typedef enum {
+  STK_OPT_ADAM = 0, STK_OPT_ADAMW = 1, STK_OPT_SGD = 2,
+  STK_OPT_NADAM = 3,   /* torch.optim.NAdam (torch/optim/nadam.py, _single_tensor_nadam) */
+  STK_OPT_RADAM = 4,   /* torch.optim.RAdam (torch/optim/radam.py, _single_tensor_radam) */
+  STK_OPT_ADAMAX = 5   /* torch.optim.Adamax (torch/optim/adamax.py, _single_tensor_adamax); exp_avg_sq holds exp_inf */
+} stk_optim_kind;
 
 /* flags of stk_grad_reduce */
 #define STK_RF_FINAL 1u        /* last bucket of this optimizer step: finish norm / found_inf (cross-rank exchange) */
@@ -100,7 +106,7 @@ typedef struct {
 
 typedef struct {
   int kind;               /* stk_optim_kind */
-  double lr, beta1, beta2, eps, weight_decay;   /* Adam / AdamW */
+  double lr, beta1, beta2, eps, weight_decay;   /* Adam / AdamW / NAdam / RAdam / Adamax */
   double momentum, dampening;                   /* SGD */
   int nesterov;
   int maximize;
@@ -108,6 +114,13 @@ typedef struct {
   double clip_max_norm;   /* STK_CLIP_NORM: max_norm (norm kind / p were given to stk_grad_reduce) */
   double clip_value;      /* STK_CLIP_VALUE */
 } stk_optim_hyper_t;
+
+/* Per-group hyper-parameters of the NAdam / RAdam kinds that stk_optim_hyper_t has no field for (one entry per group,
+ * same order as the stk_optim_hyper_t array).  A NULL array means every field is 0. */
+typedef struct {
+  double momentum_decay;        /* NAdam: momentum_decay (psi): mu_t = beta1 (1 - 0.5 * 0.96^(t psi)), torch/optim/nadam.py */
+  int decoupled_weight_decay;   /* NAdam / RAdam: 1 = param *= 1 - lr wd before the update (AdamW-style); 0 = L2, grad += wd param */
+} stk_optim_hyper_ext_t;
 
 /* ---- library / context -------------------------------------------------------------------------------------------- */
 int stk_version(void);
@@ -251,9 +264,15 @@ typedef struct {
   size_t grid_n;   /* cross-rank (lp_world > 1) launches: the LARGEST n_local over the ranks, identical on every rank, so that
                       every rank launches the same grid (the block barriers pair block b with block b); 0: n_local */
   const float* range_bc;  /* DEVICE, 4 floats per range {step_size, bias_correction2_sqrt, first_step, 0} written by
-                             stk_optim_range_prologue: per-PARAMETER step counts (torch keeps `step` per parameter, so a
+                             stk_optim_range_prologue (NAdam / RAdam / Adamax: the layout of stk_optim_step_prologue,
+                             which writes it for every kind): per-PARAMETER step counts (torch keeps `step` per parameter, so a
                              parameter that skipped some steps has its own bias corrections); NULL: the optimizer-wide
                              counter of the selected state is used for every range */
+  const stk_optim_hyper_ext_t* hyper_ext;  /* n_groups entries or NULL (all zero): NAdam / RAdam extras */
+  const float* group_bc;  /* DEVICE, 4 floats per GROUP written by stk_optim_step_prologue with n_ranges = 0; used where
+                             range_bc is NULL.  NADAM / RADAM / ADAMAX need group_bc or range_bc: their per-step scalars
+                             (NAdam's come from mu_product, which only the prologue advances) are formed once by the
+                             prologue, not in every block.  Ignored by ADAM / ADAMW / SGD */
 } stk_optim_args_t;
 int stk_optim_step_ex(stk_ctx* ctx, const stk_optim_args_t* args, void* stream);
 /* Per-range step bookkeeping for stk_optim_step_ex (call it right before, same stream): for every range j computes the
@@ -262,6 +281,27 @@ int stk_optim_step_ex(stk_ctx* ctx, const stk_optim_args_t* args, void* stream);
  * All three arrays live in device memory. */
 int stk_optim_range_prologue(stk_ctx* ctx, const stk_optim_hyper_t* hyper, int n_groups, int n_ranges,
                              const uint8_t* range_group, int32_t* range_steps, float* range_bc, void* stream);
+/* Step bookkeeping for every kind, NAdam's mu_product included (call it right before stk_optim_step_ex, same stream).
+ * n_ranges > 0: per range j, like stk_optim_range_prologue: the scalars of step t = range_steps[j] + 1 with the group
+ *   hyper[range_group[j] & 0x7f] go to bc[4j..4j+3] (pass bc as the step's range_bc), and unless bit 7 is set or the
+ *   selected state says found_inf, range_steps[j] and mu_product[j] advance.
+ * n_ranges = 0: per group g, with t = the selected state's optimizer-wide counter + 1: bc[4g..4g+3] (pass bc as the
+ *   step's group_bc) and, unless found_inf, mu_product[g] advances.  range_group and range_steps are not read.
+ * The four floats per entry, computed in double from torch's python-scalar formulas and stored as fp32:
+ *   ADAM / ADAMW / SGD: {lr / bc1, sqrt(bc2), t == 1, 0}     (the values stk_optim_range_prologue writes)
+ *   NADAM:  {c_g, c_m, bc2, 0}: param += c_g grad / denom + c_m exp_avg / denom, denom = sqrt(exp_avg_sq / bc2) + eps,
+ *           c_g = -lr (1 - mu_t) / (1 - P_t), c_m = -lr mu_{t+1} / (1 - P_t mu_{t+1}), P_t = fp32(P_{t-1} * fp32(mu_t))
+ *           is the advanced mu_product (torch: mu_product *= mu, then .item())
+ *   RADAM:  {c, rectified, 0, 0}: rho_t = rho_inf - 2 t beta2^t / bc2 > 5 -> rectified = 1,
+ *           c = lr rect sqrt(bc2) / bc1, param -= c exp_avg / (sqrt(exp_avg_sq) + eps); else rectified = 0,
+ *           c = lr / bc1, param -= c exp_avg
+ *   ADAMAX: {lr / bc1, 0, 0, 0}: param -= (lr / bc1) exp_avg / exp_inf
+ * with bc1 = 1 - beta1^t, bc2 = 1 - beta2^t.  mu_product (fp32, one per range or per group, torch initialises it to 1)
+ * is read and written only for STK_OPT_NADAM and may be NULL for the other kinds; hyper_ext may be NULL (all zero).
+ * All pointers but hyper / hyper_ext are device memory; bc must be 16-byte aligned. */
+int stk_optim_step_prologue(stk_ctx* ctx, const stk_optim_hyper_t* hyper, const stk_optim_hyper_ext_t* hyper_ext,
+                            int n_groups, int n_ranges, const uint8_t* range_group, int32_t* range_steps,
+                            float* mu_product, float* bc, void* stream);
 
 /* scaler.update(), opt_steps/skipped_steps bookkeeping, reset of the per-step accumulators */
 int stk_step_epilogue(stk_ctx* ctx, void* stream);

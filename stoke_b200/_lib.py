@@ -14,7 +14,7 @@ F32, BF16, F16 = 0, 1, 2
 REDUCE_ALL, REDUCE_SCATTER = 0, 1
 NORM_NONE, NORM_L2, NORM_INF, NORM_P = 0, 1, 2, 3
 CLIP_NONE, CLIP_NORM, CLIP_VALUE = 0, 1, 2
-OPT_ADAM, OPT_ADAMW, OPT_SGD = 0, 1, 2
+OPT_ADAM, OPT_ADAMW, OPT_SGD, OPT_NADAM, OPT_RADAM, OPT_ADAMAX = 0, 1, 2, 3, 4, 5
 RF_FINAL, RF_ZERO_INPUT, RF_UNSCALE = 1, 2, 4
 OPT_K1_ALGO, OPT_MEM_MODE, OPT_K1_MAX_BLOCKS, OPT_COOP_LAUNCH, OPT_NVLS_MAX_BLOCKS, OPT_K2_AG_MC = 1, 2, 3, 4, 5, 6
 K1_ALGO_LDG, K1_ALGO_BULK, K1_ALGO_NVLS = 0, 1, 2
@@ -48,6 +48,10 @@ class OptimHyper(C.Structure):
                 ("clip_max_norm", C.c_double), ("clip_value", C.c_double)]
 
 
+class OptimHyperExt(C.Structure):
+    _fields_ = [("momentum_decay", C.c_double), ("decoupled_weight_decay", C.c_int)]
+
+
 class OptimArgs(C.Structure):
     _fields_ = [("hyper", C.POINTER(OptimHyper)), ("n_groups", C.c_int), ("master", C.c_void_p), ("exp_avg", C.c_void_p),
                 ("exp_avg_sq", C.c_void_p), ("grad", C.c_void_p), ("grad_dtype", C.c_int), ("grad_raw", C.c_int),
@@ -55,7 +59,8 @@ class OptimArgs(C.Structure):
                 ("lp_ptrs", C.POINTER(C.c_void_p)), ("lp_world", C.c_int), ("lp_dtype", C.c_int), ("lp_offset", C.c_size_t),
                 ("n_seg", C.c_int), ("seg_local", C.POINTER(C.c_size_t)), ("seg_global", C.POINTER(C.c_size_t)),
                 ("n_ranges", C.c_int), ("range_end_vec", C.c_void_p), ("range_group", C.c_void_p),
-                ("grid_n", C.c_size_t), ("range_bc", C.c_void_p)]
+                ("grid_n", C.c_size_t), ("range_bc", C.c_void_p), ("hyper_ext", C.POINTER(OptimHyperExt)),
+                ("group_bc", C.c_void_p)]
 
 
 class SamplerPlan(C.Structure):
@@ -107,6 +112,8 @@ _SIGNATURES = {
                                  C.c_size_t, _P]),
     "stk_optim_step_ex": (C.c_int, [_P, C.POINTER(OptimArgs), _P]),
     "stk_optim_range_prologue": (C.c_int, [_P, C.POINTER(OptimHyper), C.c_int, C.c_int, _P, _P, _P, _P]),
+    "stk_optim_step_prologue": (C.c_int, [_P, C.POINTER(OptimHyper), C.POINTER(OptimHyperExt), C.c_int, C.c_int, _P, _P,
+                                          _P, _P, _P]),
     "stk_step_epilogue": (C.c_int, [_P, _P]),
     "stk_loss_sync": (C.c_int, [_P, _P, C.c_int, C.POINTER(C.c_double), _P]),
     "stk_loss_sync_begin": (C.c_int, [_P, _P, C.c_int, C.POINTER(C.c_int64), _P]),

@@ -1,10 +1,12 @@
-// k2_optim.cu -- K2: single-pass fused optimizer step (Adam / AdamW / SGD-momentum), plus the step epilogue.
+// k2_optim.cu -- K2: single-pass fused optimizer step (Adam / AdamW / SGD-momentum / NAdam / RAdam / Adamax), plus the
+// step prologue (per-parameter step counts, NAdam's mu_product) and epilogue.
 //
 // One sweep over (grad, master, exp_avg, exp_avg_sq) does what the reference spreads over clip_grad_norm_'s scaling pass /
 // clip_grad_value_, GradScaler.step's inf gate, the ~7 foreach kernels of torch.optim.Adam and (mixed precision) the
 // fp32 -> bf16 parameter cast; in sharded (OSS / ZeRO-1) mode the updated low-precision shard is stored straight into
 // every rank's parameter buffer, which is the parameter all-gather (K3).  HBM bytes per element: read g,p,m,v (16) +
-// write p,m,v (12) [+ 2 for the bf16 copy] = 28 / 30.  The clip coefficient, the skip decision and the bias corrections
+// write p,m,v (12) [+ 2 for the bf16 copy] = 28 / 30, for every kind but SGD (NAdam, RAdam and Adamax keep two fp32 state
+// tensors like Adam; Adamax's exp_inf lives in the exp_avg_sq buffer).  The clip coefficient, the skip decision and the bias corrections
 // come from device memory, so there is no host synchronisation anywhere on the step.
 //
 // Gradient sources:  MAIN  -- fp32 reduced / unscaled gradients written by K1 (cross-rank routes), indexed like the state;
@@ -15,8 +17,9 @@
 // table over the flat index space selecting the parameter group (per-group lr / betas / eps / weight decay ...) or skipping
 // parameters that received no gradient this step (torch skips `p.grad is None`, torch/optim/optimizer.py).
 //
-// Arithmetic follows torch/optim/adam.py (_single_tensor_adam, the path torch takes on CPU -- the oracle) and
-// torch/optim/sgd.py (_single_tensor_sgd); the clip follows torch/nn/utils/clip_grad.py:165-174 (coef = max_norm /
+// Arithmetic follows torch/optim/adam.py (_single_tensor_adam, the path torch takes on CPU -- the oracle),
+// torch/optim/sgd.py (_single_tensor_sgd), nadam.py (_single_tensor_nadam), radam.py (_single_tensor_radam) and adamax.py
+// (_single_tensor_adamax); the clip follows torch/nn/utils/clip_grad.py:165-174 (coef = max_norm /
 // (total_norm + 1e-6), clamped to 1) and :291-292 (clamp).
 #include <cstdlib>
 
@@ -27,10 +30,14 @@ namespace stk {
 struct GroupHyperD {   // host-side doubles, converted exactly like torch converts python scalars
   double lr, beta1, beta2, eps, weight_decay, momentum, dampening;
   int nesterov, maximize;
+  double momentum_decay;  // NAdam
+  int decoupled;          // NAdam / RAdam: decoupled weight decay
 };
 struct GroupHyperS {   // what the inner loop reads (shared memory, one entry per parameter group)
   float step_size, bc2_sqrt, b2, eps, wd, one_m_b1, one_m_b2, lr, one_m_damp, decay_mul, mom;
   int nesterov, maximize;
+  float c0, c1, c2;  // NAdam / RAdam / Adamax: the per-step scalars (layout of stk_optim_step_prologue)
+  int decoupled;
 };
 
 struct OptimParams {
@@ -64,7 +71,37 @@ struct OptimParams {
   const uint32_t* range_end;                 // device, ascending, vector units (global)
   const uint8_t* range_group;                // device; bit 7: skip
   const float4* range_bc;                    // device, optional: per-range {step_size, bc2_sqrt, first_step, 0}
+  const float4* group_bc;                    // device: per-group scalars of the NAdam / RAdam / Adamax kinds
 };
+
+__host__ __device__ constexpr bool is_new_kind(int kind) { return kind == STK_OPT_NADAM || kind == STK_OPT_RADAM || kind == STK_OPT_ADAMAX; }
+
+// Per-step scalars of the NAdam / RAdam / Adamax update of step t (the float4 layout documented at stk_optim_step_prologue),
+// in double from the python-scalar formulas of torch's single-tensor functions.  *mu_prod: NAdam's mu_product before the
+// step on entry, after it on return (fp32, like torch's tensor).
+__device__ __forceinline__ float4 new_kind_scalars(int kind, const GroupHyperD& h, double t, float* mu_prod) {
+  const double bc1 = 1.0 - pow(h.beta1, t);
+  const double bc2 = 1.0 - pow(h.beta2, t);
+  if (kind == STK_OPT_NADAM) {  // torch/optim/nadam.py: mu, mu_next, mu_product *= mu, the two addcdiv_ values
+    const double mu = h.beta1 * (1.0 - 0.5 * pow(0.96, t * h.momentum_decay));
+    const double mu_next = h.beta1 * (1.0 - 0.5 * pow(0.96, (t + 1.0) * h.momentum_decay));
+    const float prod = __fmul_rn(*mu_prod, (float)mu);  // fp32 tensor times a python float
+    *mu_prod = prod;
+    const double prod_next = (double)prod * mu_next;
+    return make_float4((float)(-h.lr * (1.0 - mu) / (1.0 - (double)prod)), (float)(-h.lr * mu_next / (1.0 - prod_next)),
+                       (float)bc2, 0.f);
+  }
+  if (kind == STK_OPT_RADAM) {  // torch/optim/radam.py: rho_inf, rho_t, rect, the rectified and the plain update
+    const double rho_inf = 2.0 / (1.0 - h.beta2) - 1.0;
+    const double rho_t = rho_inf - 2.0 * t * pow(h.beta2, t) / bc2;
+    if (rho_t > 5.0) {
+      const double rect = sqrt((rho_t - 4.0) * (rho_t - 2.0) * rho_inf / ((rho_inf - 4.0) * (rho_inf - 2.0) * rho_t));
+      return make_float4((float)(h.lr * rect * sqrt(bc2) / bc1), 1.f, 0.f, 0.f);
+    }
+    return make_float4((float)(h.lr / bc1), 0.f, 0.f, 0.f);
+  }
+  return make_float4((float)(h.lr / bc1), 0.f, 0.f, 0.f);  // Adamax: clr = lr / bias_correction
+}
 
 // local vector index -> global vector index
 __device__ __forceinline__ size_t to_global(const OptimParams& p, size_t i) {
@@ -206,6 +243,14 @@ __global__ void __launch_bounds__(256) k_optim_step(const OptimParams p) {
     o.mom = (float)h.momentum;
     o.nesterov = h.nesterov;
     o.maximize = h.maximize;
+    o.c0 = o.c1 = o.c2 = 0.f;
+    if (is_new_kind(KIND) && p.group_bc != nullptr) {  // stk_optim_step_prologue's values (nullptr: range_bc has them)
+      const float4 c = p.group_bc[threadIdx.x];
+      o.c0 = c.x;
+      o.c1 = c.y;
+      o.c2 = c.z;
+    }
+    o.decoupled = h.decoupled;
     s_g[threadIdx.x] = o;
   }
   __syncthreads();
@@ -229,9 +274,15 @@ __global__ void __launch_bounds__(256) k_optim_step(const OptimParams p) {
     GroupHyperS h = s_g[rb & 0x7f];
     bool first_here = first_step;
     if (p.range_bc != nullptr) {  // per-parameter step counts (torch's `state[p]["step"]`)
-      h.step_size = bc.x;
-      h.bc2_sqrt = bc.y;
-      first_here = bc.z != 0.f;
+      if constexpr (is_new_kind(KIND)) {
+        h.c0 = bc.x;
+        h.c1 = bc.y;
+        h.c2 = bc.z;
+      } else {
+        h.step_size = bc.x;
+        h.bc2_sqrt = bc.y;
+        first_here = bc.z != 0.f;
+      }
     }
     const bool skip = skip_all || (rb & 0x80u);
     if (!skip) {
@@ -260,6 +311,35 @@ __global__ void __launch_bounds__(256) k_optim_step(const OptimParams p) {
             ww = ww - h.step_size * (mm / denom);                    // addcdiv_(exp_avg, denom, value=-step_size)
             m[k][e] = mm;
             v[k][e] = vv;
+          } else if (KIND == STK_OPT_NADAM || KIND == STK_OPT_RADAM) {
+            if (h.wd != 0.f) {
+              if (h.decoupled) ww *= h.decay_mul;                    // param.mul_(1 - lr * wd)
+              else gg = fmaf(ww, h.wd, gg);                          // grad.add(param, alpha=wd)
+            }
+            float mm = m[k][e];
+            mm = fmaf(h.one_m_b1, gg - mm, mm);                      // exp_avg.lerp_(grad, 1 - beta1)
+            float vv = v[k][e] * h.b2;
+            vv = fmaf(h.one_m_b2 * gg, gg, vv);                      // mul_(beta2).addcmul_(grad, grad, value=1-beta2)
+            if (KIND == STK_OPT_NADAM) {
+              const float denom = sqrtf(vv / h.c2) + h.eps;          // exp_avg_sq.div(bc2).sqrt().add_(eps)
+              ww = fmaf(h.c0, gg / denom, ww);                       // addcdiv_(grad, denom, value=c_g)
+              ww = fmaf(h.c1, mm / denom, ww);                       // addcdiv_(exp_avg, denom, value=c_m)
+            } else if (h.c1 != 0.f) {                                // rho_t > 5: rectified adaptive step
+              ww = ww - h.c0 * (mm / (sqrtf(vv) + h.eps));
+            } else {                                                 // unrectified: SGD with momentum
+              ww = ww - h.c0 * mm;
+            }
+            m[k][e] = mm;
+            v[k][e] = vv;
+          } else if (KIND == STK_OPT_ADAMAX) {
+            if (h.wd != 0.f) gg = fmaf(ww, h.wd, gg);               // grad.add(param, alpha=wd)
+            float mm = m[k][e];
+            mm = fmaf(h.one_m_b1, gg - mm, mm);                      // exp_avg.lerp_(grad, 1 - beta1)
+            // torch.maximum(exp_inf.mul_(beta2), grad.abs().add_(eps)): NaN-propagating, unlike fmaxf
+            const float uu = fmax_nan(v[k][e] * h.b2, fabsf(gg) + h.eps);
+            ww = ww - h.c0 * (mm / uu);                              // addcdiv_(exp_avg, exp_inf, value=-clr)
+            m[k][e] = mm;
+            v[k][e] = uu;
           } else {  // SGD
             if (h.wd != 0.f) gg = fmaf(ww, h.wd, gg);
             if (h.mom != 0.f) {
@@ -325,6 +405,43 @@ __global__ void k_range_prologue(const RangePrologueParams p) {
   if (!(b & 0x80u) && p.scaler->found_inf == 0) p.range_steps[j] = done + 1;
 }
 
+struct StepPrologueParams {
+  GroupHyperD g[STK_MAX_GROUPS];
+  int n_groups, n_ranges, kind;
+  const uint8_t* range_group;
+  int32_t* range_steps;
+  float* mu_product;
+  float4* bc;
+  const stk_scaler_state_t* scaler;
+};
+
+// one thread per range (n_ranges > 0) or per group (n_ranges == 0): the scalars of that entry's NEXT step and, unless it is
+// skipped or the step is (found_inf), the advance of its step count and of NAdam's mu_product
+__global__ void k_step_prologue(const StepPrologueParams p) {
+  const int j = blockIdx.x * blockDim.x + threadIdx.x;
+  const bool per_range = p.n_ranges > 0;
+  if (j >= (per_range ? p.n_ranges : p.n_groups)) return;
+  const unsigned b = per_range ? (unsigned)p.range_group[j] : (unsigned)j;
+  const GroupHyperD& h = p.g[b & 0x7f];
+  const int64_t done = per_range ? (int64_t)p.range_steps[j] : p.scaler->opt_steps;
+  const double t = (double)(done + 1);
+  const bool advance = !(b & 0x80u) && p.scaler->found_inf == 0;
+  float4 o;
+  if (is_new_kind(p.kind)) {
+    float mu = p.kind == STK_OPT_NADAM ? p.mu_product[j] : 1.f;
+    o = new_kind_scalars(p.kind, h, t, &mu);
+    if (p.kind == STK_OPT_NADAM && advance) p.mu_product[j] = mu;
+  } else {  // the values of k_range_prologue
+    o = make_float4(0.f, 1.f, done == 0 ? 1.f : 0.f, 0.f);
+    if (p.kind != STK_OPT_SGD) {
+      o.x = (float)(h.lr / (1.0 - pow(h.beta1, t)));
+      o.y = (float)sqrt(1.0 - pow(h.beta2, t));
+    }
+  }
+  p.bc[j] = o;
+  if (per_range && advance) p.range_steps[j] = (int32_t)(done + 1);
+}
+
 // scaler.update() (torch/amp/grad_scaler.py:549-556 -> _amp_update_scale_), step counters, per-step accumulator reset
 __global__ void k_step_epilogue(stk_scaler_state_t* st, StepAccum* acc) {
   if (threadIdx.x != 0 || blockIdx.x != 0) return;
@@ -353,6 +470,16 @@ __global__ void k_step_epilogue(stk_scaler_state_t* st, StepAccum* acc) {
 }  // namespace stk
 
 using namespace stk;
+
+static void fill_groups(GroupHyperD* o, const stk_optim_hyper_t* h, const stk_optim_hyper_ext_t* ext, int n) {
+  for (int gi = 0; gi < n; ++gi) {
+    o[gi].lr = h[gi].lr; o[gi].beta1 = h[gi].beta1; o[gi].beta2 = h[gi].beta2; o[gi].eps = h[gi].eps;
+    o[gi].weight_decay = h[gi].weight_decay; o[gi].momentum = h[gi].momentum; o[gi].dampening = h[gi].dampening;
+    o[gi].nesterov = h[gi].nesterov; o[gi].maximize = h[gi].maximize;
+    o[gi].momentum_decay = ext ? ext[gi].momentum_decay : 0.0;
+    o[gi].decoupled = ext ? (ext[gi].decoupled_weight_decay != 0) : 0;
+  }
+}
 
 static size_t g_grid_nvec = 0;  // set under the context lock by stk_optim_step_ex (cross-rank launches only)
 
@@ -408,7 +535,10 @@ int stk_optim_step_ex(stk_ctx* c, const stk_optim_args_t* a, void* stream) {
   STK_REQUIRE(c, a->n_groups >= 1 && a->n_groups <= STK_MAX_GROUPS, "stk_optim_step_ex: n_groups must be in [1, 8]");
   STK_REQUIRE(c, a->n_local % 8 == 0, "stk_optim_step_ex: n_local must be a multiple of 8");
   const stk_optim_hyper_t* h = a->hyper;
-  STK_REQUIRE(c, h->kind >= STK_OPT_ADAM && h->kind <= STK_OPT_SGD, "stk_optim_step_ex: bad optimizer kind");
+  STK_REQUIRE(c, h->kind >= STK_OPT_ADAM && h->kind <= STK_OPT_ADAMAX, "stk_optim_step_ex: bad optimizer kind");
+  STK_REQUIRE(c, h->kind <= STK_OPT_SGD || a->group_bc || (a->n_ranges > 0 && a->range_bc),
+              "stk_optim_step_ex: NAdam / RAdam / Adamax need the scalars of stk_optim_step_prologue (group_bc or range_bc)");
+  STK_REQUIRE(c, (reinterpret_cast<uintptr_t>(a->group_bc) & 15) == 0, "stk_optim_step_ex: group_bc must be 16-byte aligned");
   STK_REQUIRE(c, h->kind == STK_OPT_SGD || (a->exp_avg && a->exp_avg_sq), "stk_optim_step_ex: Adam needs exp_avg and exp_avg_sq");
   bool any_mom = false;
   for (int gi = 0; gi < a->n_groups; ++gi) {
@@ -487,16 +617,13 @@ int stk_optim_step_ex(stk_ctx* c, const stk_optim_args_t* a, void* stream) {
   p.grad_mul = (float)a->grad_mul;
   p.unscale = 0;
   p.n_groups = a->n_groups;
-  for (int gi = 0; gi < a->n_groups; ++gi) {
-    GroupHyperD& o = p.g[gi];
-    o.lr = h[gi].lr; o.beta1 = h[gi].beta1; o.beta2 = h[gi].beta2; o.eps = h[gi].eps; o.weight_decay = h[gi].weight_decay;
-    o.momentum = h[gi].momentum; o.dampening = h[gi].dampening; o.nesterov = h[gi].nesterov; o.maximize = h[gi].maximize;
-  }
+  fill_groups(p.g, h, a->hyper_ext, a->n_groups);
   p.any_mom = any_mom ? 1 : 0;
   p.n_ranges = a->n_ranges;
   p.range_end = a->range_end_vec;
   p.range_group = a->range_group;
   p.range_bc = a->n_ranges > 0 ? reinterpret_cast<const float4*>(a->range_bc) : nullptr;
+  p.group_bc = reinterpret_cast<const float4*>(a->group_bc);
   if (a->grad_raw) {
     // 1/loss_scale is applied when the scaler is live; the device flag decides (enabled), so no host read
     p.unscale = 1;
@@ -516,6 +643,9 @@ int stk_optim_step_ex(stk_ctx* c, const stk_optim_args_t* a, void* stream) {
   switch (h->kind) {
     case STK_OPT_ADAM: err = launch_optim<STK_OPT_ADAM>(c, p, a->lp_dtype, a->grad_dtype, raw, pair_ok, s); break;
     case STK_OPT_ADAMW: err = launch_optim<STK_OPT_ADAMW>(c, p, a->lp_dtype, a->grad_dtype, raw, pair_ok, s); break;
+    case STK_OPT_NADAM: err = launch_optim<STK_OPT_NADAM>(c, p, a->lp_dtype, a->grad_dtype, raw, pair_ok, s); break;
+    case STK_OPT_RADAM: err = launch_optim<STK_OPT_RADAM>(c, p, a->lp_dtype, a->grad_dtype, raw, pair_ok, s); break;
+    case STK_OPT_ADAMAX: err = launch_optim<STK_OPT_ADAMAX>(c, p, a->lp_dtype, a->grad_dtype, raw, pair_ok, s); break;
     default: err = launch_optim<STK_OPT_SGD>(c, p, a->lp_dtype, a->grad_dtype, raw, pair_ok, s); break;
   }
   if (err == cudaErrorNotSupported)
@@ -550,14 +680,12 @@ int stk_optim_range_prologue(stk_ctx* c, const stk_optim_hyper_t* h, int n_group
   STK_REQUIRE(c, n_groups >= 1 && n_groups <= STK_MAX_GROUPS, "stk_optim_range_prologue: n_groups must be in [1, 8]");
   STK_REQUIRE(c, n_ranges >= 1, "stk_optim_range_prologue: no ranges");
   STK_REQUIRE(c, (reinterpret_cast<uintptr_t>(range_bc) & 15) == 0, "stk_optim_range_prologue: range_bc must be 16-byte aligned");
+  STK_REQUIRE(c, h->kind >= STK_OPT_ADAM && h->kind <= STK_OPT_SGD,
+              "stk_optim_range_prologue: NAdam / RAdam / Adamax take stk_optim_step_prologue");
   std::lock_guard<std::mutex> lk(c->mu);
   DeviceGuard g(c->device);
   RangePrologueParams p{};
-  for (int gi = 0; gi < n_groups; ++gi) {
-    GroupHyperD& o = p.g[gi];
-    o.lr = h[gi].lr; o.beta1 = h[gi].beta1; o.beta2 = h[gi].beta2; o.eps = h[gi].eps; o.weight_decay = h[gi].weight_decay;
-    o.momentum = h[gi].momentum; o.dampening = h[gi].dampening; o.nesterov = h[gi].nesterov; o.maximize = h[gi].maximize;
-  }
+  fill_groups(p.g, h, nullptr, n_groups);
   p.n_ranges = n_ranges;
   p.kind = h->kind;
   p.range_group = range_group;
@@ -565,6 +693,34 @@ int stk_optim_range_prologue(stk_ctx* c, const stk_optim_hyper_t* h, int n_group
   p.range_bc = reinterpret_cast<float4*>(range_bc);
   p.scaler = c->scaler_dev;
   k_range_prologue<<<(n_ranges + 127) / 128, 128, 0, reinterpret_cast<cudaStream_t>(stream)>>>(p);
+  STK_CUDA(c, cudaGetLastError());
+  return STK_OK;
+}
+
+int stk_optim_step_prologue(stk_ctx* c, const stk_optim_hyper_t* h, const stk_optim_hyper_ext_t* ext, int n_groups,
+                            int n_ranges, const uint8_t* range_group, int32_t* range_steps, float* mu_product, float* bc,
+                            void* stream) {
+  STK_REQUIRE(c, c && h && bc, "stk_optim_step_prologue: NULL argument");
+  STK_REQUIRE(c, n_groups >= 1 && n_groups <= STK_MAX_GROUPS, "stk_optim_step_prologue: n_groups must be in [1, 8]");
+  STK_REQUIRE(c, n_ranges >= 0, "stk_optim_step_prologue: negative n_ranges");
+  STK_REQUIRE(c, n_ranges == 0 || (range_group && range_steps), "stk_optim_step_prologue: range arrays are NULL");
+  STK_REQUIRE(c, h->kind >= STK_OPT_ADAM && h->kind <= STK_OPT_ADAMAX, "stk_optim_step_prologue: bad optimizer kind");
+  STK_REQUIRE(c, h->kind != STK_OPT_NADAM || mu_product, "stk_optim_step_prologue: NAdam needs mu_product");
+  STK_REQUIRE(c, (reinterpret_cast<uintptr_t>(bc) & 15) == 0, "stk_optim_step_prologue: bc must be 16-byte aligned");
+  std::lock_guard<std::mutex> lk(c->mu);
+  DeviceGuard g(c->device);
+  StepPrologueParams p{};
+  fill_groups(p.g, h, ext, n_groups);
+  p.n_groups = n_groups;
+  p.n_ranges = n_ranges;
+  p.kind = h->kind;
+  p.range_group = range_group;
+  p.range_steps = range_steps;
+  p.mu_product = mu_product;
+  p.bc = reinterpret_cast<float4*>(bc);
+  p.scaler = c->scaler_dev;
+  const int n = n_ranges > 0 ? n_ranges : n_groups;
+  k_step_prologue<<<(n + 127) / 128, 128, 0, reinterpret_cast<cudaStream_t>(stream)>>>(p);
   STK_CUDA(c, cudaGetLastError());
   return STK_OK;
 }

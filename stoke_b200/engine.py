@@ -423,7 +423,8 @@ class GradPath:
                  clip: Optional[ClipSpec] = None, sharded: bool = False, lp_dtype: Optional[torch.dtype] = None,
                  module: Optional[torch.nn.Module] = None, sync_init: bool = True, needs_second_moment: bool = True,
                  needs_first_moment: bool = True, bucket_mb: Optional[float] = None, state_id: Optional[int] = None,
-                 route: Optional[str] = None, group_of: Optional[Sequence[int]] = None, overlap: bool = True):
+                 route: Optional[str] = None, group_of: Optional[Sequence[int]] = None, overlap: bool = True,
+                 mu_product: bool = False):
         self.engine = engine
         self.params = [p for p in params if p.requires_grad]
         if not self.params:
@@ -538,6 +539,12 @@ class GradPath:
         self._range_skip_live = False   # the device table currently carries skip bits
         self._range_steps = None        # int32 per parameter once per-parameter step counts are on (enable_per_param_steps)
         self._range_bc = None
+        # NAdam's mu_product (torch keeps it per parameter as fp32 state): one per group, one per parameter once per-parameter
+        # step counts are on; stk_optim_step_prologue advances it on the device.  group_bc: the prologue's per-group scalars.
+        n_grp = max(self.group_of) + 1
+        self._group_mu = torch.ones(n_grp, dtype=torch.float32, device=dev) if mu_product else None
+        self._range_mu = None
+        self._group_bc = torch.zeros(n_grp, 4, dtype=torch.float32, device=dev)
         self._touched = np.ones(len(self.params), dtype=bool)
         self._track_touched = False
 
@@ -716,14 +723,20 @@ class GradPath:
             self._range_skip_live = skip
         return len(self.params), self._range_end.data_ptr(), self._range_group.data_ptr()
 
-    def enable_per_param_steps(self, steps: Optional[Sequence[int]] = None):
-        """Switches the fused step to per-parameter step counts (one synchronisation to read the optimizer-wide count)."""
+    def enable_per_param_steps(self, steps: Optional[Sequence[int]] = None, mu_products: Optional[Sequence[float]] = None):
+        """Switches the fused step to per-parameter step counts (one synchronisation to read the optimizer-wide count).
+        NAdam's mu_product goes per parameter too: ``mu_products``, or each parameter's group value."""
         dev = self._range_end.device
         if steps is None:
             done = int(self.engine.scaler_get(self.state_id).opt_steps)
             steps = [done] * len(self.params)
         self._range_steps = torch.tensor(list(steps), dtype=torch.int32, device=dev)
         self._range_bc = torch.zeros(len(self.params), 4, dtype=torch.float32, device=dev)
+        if self._group_mu is not None:
+            if mu_products is not None:
+                self._range_mu = torch.tensor(list(mu_products), dtype=torch.float32, device=dev)
+            else:
+                self._range_mu = self._group_mu[torch.tensor(self.group_of, dtype=torch.long, device=dev)].contiguous()
 
     def param_steps(self) -> List[int]:
         """Steps taken by every parameter (what torch reports as ``state[p]["step"]``)."""
@@ -731,8 +744,21 @@ class GradPath:
             return [int(self.engine.scaler_get(self.state_id).opt_steps)] * len(self.params)
         return [int(v) for v in self._range_steps.cpu().tolist()]
 
-    def optimizer_step(self, hypers):
-        """One fused K2 launch (+ the one-thread epilogue).  ``hypers``: one ``OptimHyper`` or a list (one per group)."""
+    def param_mu_products(self) -> List[float]:
+        """NAdam's mu_product of every parameter (torch's ``state[p]["mu_product"]``); synchronises."""
+        if self._range_mu is not None:
+            return [float(v) for v in self._range_mu.cpu().tolist()]
+        mus = self._group_mu.cpu().tolist()
+        return [float(mus[g]) for g in self.group_of]
+
+    def set_group_mu_products(self, mus: Sequence[float]):
+        """Sets NAdam's per-group mu_product (checkpoint load while step counts are optimizer-wide)."""
+        self._group_mu.copy_(torch.tensor(list(mus), dtype=torch.float32))
+
+    def optimizer_step(self, hypers, exts=None):
+        """One fused K2 launch (+ the one-thread epilogue).  ``hypers``: one ``OptimHyper`` or a list (one per group).
+        ``exts``: per-group ``OptimHyperExt`` of the NAdam / RAdam / Adamax kinds, whose per-step scalars (and NAdam's
+        mu_product) stk_optim_step_prologue forms on the device before the step."""
         e = self.engine
         e.state_select(self.state_id)
         if isinstance(hypers, _lib.OptimHyper):
@@ -775,7 +801,22 @@ class GradPath:
             a.lp_ptrs, a.lp_world, a.lp_dtype = None, 0, _lib.F32
         nr, rend, rgrp = self._ranges_for_step()
         a.n_ranges, a.range_end_vec, a.range_group = nr, rend, rgrp
-        if nr and self._range_steps is not None:
+        if exts is not None:
+            xarr = (_lib.OptimHyperExt * ng)(*exts)
+            keep.append(xarr)
+            a.hyper_ext = xarr
+            per_range = bool(nr) and self._range_steps is not None
+            mu = self._range_mu if per_range else self._group_mu
+            bc = self._range_bc if per_range else self._group_bc
+            e._check(e.lib.stk_optim_step_prologue(e.ctx, harr, xarr, ng, nr if per_range else 0, rgrp if per_range else None,
+                                                   self._range_steps.data_ptr() if per_range else None,
+                                                   mu.data_ptr() if mu is not None else None, bc.data_ptr(), e._stream()))
+            e.launches += 1
+            if per_range:
+                a.range_bc = bc.data_ptr()
+            else:
+                a.group_bc = bc.data_ptr()
+        elif nr and self._range_steps is not None:
             e._check(e.lib.stk_optim_range_prologue(e.ctx, harr, ng, nr, rgrp, self._range_steps.data_ptr(),
                                                     self._range_bc.data_ptr(), e._stream()))
             e.launches += 1

@@ -4,11 +4,14 @@
 ``B200FusedOptimizer`` -- a ``torch.optim.Optimizer`` (so LR schedulers and ``param_groups`` edits work, README.md:241-250
 of the reference) whose ``step()`` is the single fused K2 launch over the flat fp32 master / moment buffers; its sharded
 flavour is the ZeRO-1 analogue of fairscale ``OSS`` (/root/reference/stoke/extensions.py:109-141): same ``clip_grad_norm`` /
-``consolidate_state_dict`` surface.  Adam, AdamW and SGD(-momentum), up to 8 parameter groups (per-group lr / betas / eps /
-weight decay / momentum ... selected inside the kernel by element range).
+``consolidate_state_dict`` surface.  Adam, AdamW, SGD(-momentum), NAdam, RAdam and Adamax, up to 8 parameter groups
+(per-group lr / betas / eps / weight decay / momentum ... selected inside the kernel by element range).  NAdam, RAdam and
+Adamax keep two fp32 state tensors per parameter like Adam (Adamax's ``exp_inf`` in the second-moment buffer); their
+per-step scalars, and NAdam's ``mu_product``, are formed on the device by ``stk_optim_step_prologue``.
 
 ``B200StockOptimizer`` -- every other ``torch.optim`` class (the reference instantiates whatever class the user passes,
-stoke/extensions.py:53-78) and the options the fused step does not cover (amsgrad, more than 8 groups): the gradient path
+stoke/extensions.py:53-78) and the options the fused step does not cover (amsgrad, capturable, differentiable, more than 8
+groups): the gradient path
 is still the engine's (K1 reduce with fused cast / unscale / inf test / norm, the clip applied by ``k_grad_scale``); the
 update itself is the stock optimizer stepping on per-parameter fp32 views of the flat master / main-grad buffers.
 """
@@ -19,7 +22,13 @@ import torch
 from . import _lib
 from .engine import ClipSpec, Engine, GradPath
 
-_KINDS = {torch.optim.Adam: _lib.OPT_ADAM, torch.optim.AdamW: _lib.OPT_ADAMW, torch.optim.SGD: _lib.OPT_SGD}
+_KINDS = {torch.optim.Adam: _lib.OPT_ADAM, torch.optim.AdamW: _lib.OPT_ADAMW, torch.optim.SGD: _lib.OPT_SGD,
+          torch.optim.NAdam: _lib.OPT_NADAM, torch.optim.RAdam: _lib.OPT_RADAM, torch.optim.Adamax: _lib.OPT_ADAMAX}
+_EXT_KINDS = (_lib.OPT_NADAM, _lib.OPT_RADAM, _lib.OPT_ADAMAX)   # per-step scalars from stk_optim_step_prologue
+# torch's per-parameter state keys of the two fp32 buffers M and V
+_STATE_KEYS = {_lib.OPT_ADAM: ("exp_avg", "exp_avg_sq"), _lib.OPT_ADAMW: ("exp_avg", "exp_avg_sq"),
+               _lib.OPT_NADAM: ("exp_avg", "exp_avg_sq"), _lib.OPT_RADAM: ("exp_avg", "exp_avg_sq"),
+               _lib.OPT_ADAMAX: ("exp_avg", "exp_inf")}
 _STOCK_ONLY_TRUE = ("amsgrad", "capturable", "differentiable")
 
 
@@ -79,7 +88,7 @@ class B200FusedOptimizer(torch.optim.Optimizer):
                  bucket_mb: Optional[float] = None):
         if optim_cls not in _KINDS:
             raise NotImplementedError(
-                f"Stoke -- the fused step covers torch.optim.Adam, AdamW and SGD; got {getattr(optim_cls, '__name__', optim_cls)}"
+                f"Stoke -- the fused step covers torch.optim.Adam, AdamW, SGD, NAdam, RAdam and Adamax; got {getattr(optim_cls, '__name__', optim_cls)}"
                 f" (use B200StockOptimizer / build_optimizer, which routes other classes to the stock-optimizer path)")
         params, group_of, extra, kw = _group_layout(module, optim_kwargs)
         if len(extra) > _lib.MAX_GROUPS:
@@ -91,14 +100,17 @@ class B200FusedOptimizer(torch.optim.Optimizer):
                 if g.get(k):
                     raise NotImplementedError(f"Stoke -- optimizer option {k}=True is not covered by the fused step")
         self._kind = _KINDS[optim_cls]
-        if probe.defaults.get("decoupled_weight_decay"):  # torch >= 2.6: AdamW is Adam(decoupled_weight_decay=True)
+        # torch >= 2.6: AdamW is Adam(decoupled_weight_decay=True).  NAdam and RAdam carry the same flag as a per-group option
+        # of their own update (hyper_ext), so it does not change their kind.
+        if self._kind == _lib.OPT_ADAM and probe.defaults.get("decoupled_weight_decay"):
             self._kind = _lib.OPT_ADAMW
         self._torch_cls = optim_cls
         sgd = self._kind == _lib.OPT_SGD
         any_mom = any(g.get("momentum", 0) != 0 for g in probe.param_groups)
         self.path = GradPath(engine, params, grad_accum=grad_accum, clip=clip, sharded=sharded, lp_dtype=lp_dtype,
                              module=module, needs_second_moment=not sgd, needs_first_moment=(not sgd) or any_mom,
-                             state_id=state_id, route=route, group_of=group_of, bucket_mb=bucket_mb)
+                             state_id=state_id, route=route, group_of=group_of, bucket_mb=bucket_mb,
+                             mu_product=self._kind == _lib.OPT_NADAM)
         by_group: List[List[torch.nn.Parameter]] = [[] for _ in extra]
         for p, gi in zip(params, group_of):
             by_group[gi].append(p)
@@ -130,11 +142,22 @@ class B200FusedOptimizer(torch.optim.Optimizer):
     def _hypers(self) -> List[_lib.OptimHyper]:
         return [self._hyper_of(g) for g in self.param_groups]
 
+    def _exts(self) -> Optional[List[_lib.OptimHyperExt]]:
+        if self._kind not in _EXT_KINDS:
+            return None
+        out = []
+        for g in self.param_groups:
+            x = _lib.OptimHyperExt()
+            x.momentum_decay = float(g.get("momentum_decay", 0.0))
+            x.decoupled_weight_decay = int(bool(g.get("decoupled_weight_decay", False)))
+            out.append(x)
+        return out
+
     @torch.no_grad()
     def step(self, closure=None):
         if closure is not None:
             raise NotImplementedError("Stoke -- closures are not supported by the fused step")
-        self.path.optimizer_step(self._hypers())
+        self.path.optimizer_step(self._hypers(), self._exts())
 
     def zero_grad(self, set_to_none: bool = True):
         """No-op: the gradient bucket is zeroed by the kernel that consumes it, and ``param.grad`` must stay a view of that
@@ -166,13 +189,19 @@ class B200FusedOptimizer(torch.optim.Optimizer):
         ms = path.unflatten(m) if m is not None else None
         vs = path.unflatten(v) if v is not None else None
         steps = path.param_steps() if path._range_steps is not None else [int(st.opt_steps)] * len(path.params)
+        mus = path.param_mu_products() if self._kind == _lib.OPT_NADAM else None
         for i in range(len(path.params)):
             j = self._sd_index[i]
             if self._kind == _lib.OPT_SGD:
                 # torch creates the buffer on the first step; before that (or without momentum) it is None
                 state[j] = {"momentum_buffer": ms[i].clone() if ms is not None and steps[i] > 0 else None}
             else:
-                state[j] = {"step": torch.tensor(float(steps[i])), "exp_avg": ms[i].clone(), "exp_avg_sq": vs[i].clone()}
+                k_m, k_v = _STATE_KEYS[self._kind]
+                state[j] = {"step": torch.tensor(float(steps[i]))}
+                if mus is not None:   # torch/optim/nadam.py: a 0-dim fp32 tensor
+                    state[j]["mu_product"] = torch.tensor(mus[i], dtype=torch.float32)
+                state[j][k_m] = ms[i].clone()
+                state[j][k_v] = vs[i].clone()
         groups, start = [], 0
         for g in self.param_groups:
             d = {k: val for k, val in g.items() if k != "params"}
@@ -209,16 +238,30 @@ class B200FusedOptimizer(torch.optim.Optimizer):
         if self._kind == _lib.OPT_SGD:
             put(path.m_flat, "momentum_buffer")
         else:
-            put(path.m_flat, "exp_avg")
-            put(path.v_flat, "exp_avg_sq")
+            k_m, k_v = _STATE_KEYS[self._kind]
+            put(path.m_flat, k_m)
+            put(path.v_flat, k_v)
             per_param = [int(float(state[self._sd_index[i]]["step"])) if self._sd_index[i] in state and "step" in state[self._sd_index[i]]
                          else None for i in range(n)]
             known = [v for v in per_param if v is not None]
             if "b200_opt_steps" not in sd and known:
                 steps = max(known)
-            if known and (len(set(known)) > 1 or len(known) < n):
+            mus = None
+            if self._kind == _lib.OPT_NADAM:
+                # a parameter torch never stepped has no state yet: its mu_product is torch's initial 1.0
+                mus = [float(state[self._sd_index[i]]["mu_product"]) if "mu_product" in state.get(self._sd_index[i], {})
+                       else 1.0 for i in range(n)]
+            groups_differ = mus is not None and any(
+                len({mus[i] for i in range(n) if self._group_of[i] == gi}) > 1 for gi in range(len(self.param_groups)))
+            if known and (len(set(known)) > 1 or len(known) < n) or groups_differ or (
+                    mus is not None and path._range_steps is not None):
                 # parameters stepped a different number of times (some were unused for a while): keep torch's per-parameter counts
-                path.enable_per_param_steps([steps if v is None else v for v in per_param])
+                path.enable_per_param_steps([steps if v is None else v for v in per_param], mu_products=mus)
+            elif mus is not None:
+                first = {}
+                for i in range(n):
+                    first.setdefault(self._group_of[i], mus[i])
+                path.set_group_mu_products([first.get(gi, 1.0) for gi in range(len(self.param_groups))])
         if "b200_master" in sd:
             master = sd["b200_master"].to(device=dev, dtype=torch.float32)
             if path.master_flat is not path.p_flat:
