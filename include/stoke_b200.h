@@ -328,6 +328,24 @@ int stk_bcast(stk_ctx* ctx, void* const* ptrs, size_t bytes, int root, void* str
 int stk_bn_act(stk_ctx* ctx, const void* x, const void* residual, const float* mean, const float* var, const void* weight,
                const void* bias, double eps, void* out, float* save_invstd, size_t numel, size_t channels, void* stream);
 
+/* ---- model backward ------------------------------------------------------------------------------------------------ */
+/* Backward of stk_bn_act: the ReLU's threshold_backward followed by torch's training-mode BatchNorm backward, with the
+ * coverage of stk_bn_act (bf16 channels-last, channels % 8 == 0, numel < 2^31, every pointer 16-byte aligned).
+ *   g = !(out <= 0) ? grad : +0;  sum_dy = sum g,  sum_dy_xmu = sum g * (x - mean)  (per channel over R = numel / channels)
+ *   grad_bias = bf16(sum_dy),  grad_weight = bf16(sum_dy_xmu * invstd)
+ *   grad_x = bf16(((g - sum_dy * n) - (x - mean) * (invstd * invstd * sum_dy_xmu * n)) * (weight * invstd)),  n = float(1.0 / R)
+ * out != NULL: a site with a residual; the mask comes from out and g is written to grad_residual.  out == NULL: the mask
+ * comes from y = bf16(weight * (x - mean) * invstd + bias), the formula stk_bn_act applies (relu(y) <= 0 iff y <= 0);
+ * grad_residual is unused.  grad_x may be NULL (no elementwise pass).
+ * Order contract: the two sums add in the order of torch's batch_norm_backward_reduce_channels_last_kernel as launched by
+ * flexible_launch_configs(R, channels, coop) with MAX_BLOCK_SIZE 512 (a function of R and channels only), so all four
+ * outputs are bit-identical to threshold_backward + native_batch_norm_backward on channels-last bf16 inputs.
+ * workspace: 2 * (1 + 128) * channels floats (the two sums, then per-block partials); no initialisation needed. */
+int stk_bn_act_backward(stk_ctx* ctx, const void* grad, const void* x, const void* out, const float* mean,
+                        const float* invstd, const void* weight, const void* bias, void* grad_x, void* grad_weight,
+                        void* grad_bias, void* grad_residual, float* workspace, size_t numel, size_t channels,
+                        void* stream);
+
 /* ---- sampler (stoke/data.py) ---------------------------------------------------------------------------------------- */
 /* torch.randperm(n, generator=g) for each n in lens[0..k) drawn from ONE mt19937 seeded with `seed` (host, bit-exact
  * with torch's CPU generator); out receives the k permutations back to back as int32. */

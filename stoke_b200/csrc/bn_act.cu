@@ -19,6 +19,12 @@ constexpr int kBnThreads = 256;
 __device__ __forceinline__ uint16_t bf16_bits(float f) { return __bfloat16_as_ushort(__float2bfloat16_rn(f)); }
 __device__ __forceinline__ float bf16_val(uint16_t u) { return __uint_as_float(uint32_t(u) << 16); }
 
+// The BatchNorm apply y = bf16(w * (x - mean) * invstd + b), as torch's channels-last transform kernel rounds it.  The
+// forward writes it and the backward recomputes the ReLU mask !(y <= 0) from it, so the two cannot disagree.
+__device__ __forceinline__ uint16_t bn_apply(float x, float m, float is, float w, float b) {
+  return bf16_bits(__fmaf_rn(__fmul_rn(w, __fsub_rn(x, m)), is, b));
+}
+
 // Thread t owns channel group t % G (G = C / 8) and walks rows t / G, t / G + T / G, ...: T (the active thread count) is a
 // multiple of G, so the per-channel parameters stay in registers for the whole loop.
 template <bool kResidual>
@@ -54,7 +60,7 @@ __global__ void __launch_bounds__(kBnThreads) k_bn_act(const __nv_bfloat16* __re
     uint16_t o[8];
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
-      uint16_t z = bf16_bits(w[j] * (xf[j] - m[j]) * is[j] + b[j]);
+      uint16_t z = bn_apply(xf[j], m[j], is[j], w[j], b[j]);
       if (kResidual) z = bf16_bits(bf16_val(z) + rf[j]);
       const float zf = bf16_val(z);
       o[j] = isnan(zf) ? z : bf16_bits(fmaxf(zf, 0.f));
@@ -62,6 +68,252 @@ __global__ void __launch_bounds__(kBnThreads) k_bn_act(const __nv_bfloat16* __re
     ov[v] = make_uint4(o[0] | uint32_t(o[1]) << 16, o[2] | uint32_t(o[3]) << 16, o[4] | uint32_t(o[5]) << 16,
                        o[6] | uint32_t(o[7]) << 16);
   }
+}
+
+// ---- backward ------------------------------------------------------------------------------------------------------
+// The ReLU's threshold_backward g = !(out <= 0) ? grad : +0 is folded into the two passes of torch's channels-last
+// BatchNorm backward (batch_norm_backward_reduce_channels_last_kernel, batch_norm_backward_elemt_channels_last_kernel),
+// whose sums are reproduced in torch's order, so every result is bit-identical to the unfused chain.  The mask comes
+// from out (sites with a residual, where g is also written: it is the residual's gradient) or from bn_apply(x) (sites
+// without one, where relu(y) <= 0 exactly when y <= 0).  Bytes per element: 4 + 6 without the residual, 8 + 6 with it;
+// the unfused chain moves 16.
+constexpr int kBwdThreads = 256;
+constexpr int kChains = 4;   // torch's ELEMENTS_PER_ITER: accumulators per virtual thread
+
+// 16-byte vector of 8 bf16 grads with the elements whose mask is off replaced by +0 (bits kept, NaN payloads included)
+__device__ __forceinline__ uint4 mask_grad(const uint4& g, const bool (&pass)[8]) {
+  const uint32_t m[4] = {(pass[0] ? 0xffffu : 0u) | (pass[1] ? 0xffff0000u : 0u), (pass[2] ? 0xffffu : 0u) | (pass[3] ? 0xffff0000u : 0u),
+                         (pass[4] ? 0xffffu : 0u) | (pass[5] ? 0xffff0000u : 0u), (pass[6] ? 0xffffu : 0u) | (pass[7] ? 0xffff0000u : 0u)};
+  return make_uint4(g.x & m[0], g.y & m[1], g.z & m[2], g.w & m[3]);
+}
+
+__device__ __forceinline__ void load8(const float* __restrict__ p, float (&f)[8]) {
+  const float4 a = __ldg(reinterpret_cast<const float4*>(p)), b = __ldg(reinterpret_cast<const float4*>(p + 4));
+  f[0] = a.x; f[1] = a.y; f[2] = a.z; f[3] = a.w; f[4] = b.x; f[5] = b.y; f[6] = b.z; f[7] = b.w;
+}
+
+// sum_dy = sum g and sum_dy_xmu = sum g * (x - mean) per channel, in torch's order.  torch runs a (block_x, block_y) x
+// (grid_x, grid_y) grid; for one channel, virtual thread (ty, by) keeps kChains accumulators, chain j adding rows
+// m0 + (kChains * i + j) * S, i < loops (S = block_y * grid_y, m0 = by * block_y + ty; rows past the end add g = x = 0),
+// as acc += g and acc = fma(g, x - mean, acc).  The chains are folded 0 += 1, 2, 3, then halved over ty (offsets
+// block_y / 2 .. 1).  Here one real thread runs one chain of one virtual thread for 8 channels; a block holds every ty
+// of its by for kBwdThreads / (kChains * block_y) channel groups.  With grid_y == 1 the block's sums are final;
+// otherwise they go to the workspace partials and k_bn_bwd_finish adds them.
+template <bool kResidual>
+__global__ void __launch_bounds__(kBwdThreads) k_bn_bwd_reduce(const uint4* __restrict__ grad, const uint4* __restrict__ x,
+                                                               const uint4* __restrict__ out, const float* __restrict__ mean,
+                                                               const float* __restrict__ invstd,
+                                                               const __nv_bfloat16* __restrict__ weight,
+                                                               const __nv_bfloat16* __restrict__ bias, uint4* __restrict__ g_out,
+                                                               float* __restrict__ ws, __nv_bfloat16* __restrict__ dweight,
+                                                               __nv_bfloat16* __restrict__ dbias, uint32_t rows,
+                                                               uint32_t groups, uint32_t block_y, uint32_t loops) {
+  __shared__ float4 sh[kBwdThreads][4];   // per thread: 8 sums of g, then 8 sums of g * (x - mean)
+  const uint32_t t = threadIdx.x, gb = kBwdThreads / (kChains * block_y);
+  const uint32_t cgl = t % gb, j = t / gb % kChains, ty = t / (gb * kChains);
+  const uint32_t cg = blockIdx.x * gb + cgl, c0 = cg * 8, channels = groups * 8;
+  const bool live = cg < groups;
+  float sdy[8], sxm[8];
+#pragma unroll
+  for (int k = 0; k < 8; ++k) sdy[k] = sxm[k] = 0.f;
+  if (live) {
+    float m[8], is[8], w[8], b[8];
+    if (!kResidual) {
+      load8(invstd + c0, is);
+      unpack16<STK_BF16>(__ldg(reinterpret_cast<const uint4*>(weight + c0)), w);
+      unpack16<STK_BF16>(__ldg(reinterpret_cast<const uint4*>(bias + c0)), b);
+    }
+    load8(mean + c0, m);
+    const uint32_t stride = block_y * gridDim.y, m0 = blockIdx.y * block_y + ty;
+#pragma unroll 2
+    for (uint32_t i = 0; i < loops; ++i) {
+      const uint32_t row = m0 + (kChains * i + j) * stride;
+      const bool in = row < rows;
+      const size_t v = size_t(row) * groups + cg;
+      const uint4 zero = make_uint4(0, 0, 0, 0);
+      const uint4 gv = in ? __ldg(grad + v) : zero, xv = in ? __ldg(x + v) : zero;
+      float xf[8], gf[8], mf[8];
+      unpack16<STK_BF16>(xv, xf);
+      bool pass[8];
+      if (kResidual) {
+        unpack16<STK_BF16>(in ? __ldg(out + v) : zero, mf);
+#pragma unroll
+        for (int k = 0; k < 8; ++k) pass[k] = !(mf[k] <= 0.f);
+      } else {
+#pragma unroll
+        for (int k = 0; k < 8; ++k) pass[k] = !(bf16_val(bn_apply(xf[k], m[k], is[k], w[k], b[k])) <= 0.f);
+      }
+      const uint4 g = mask_grad(gv, pass);
+      if (kResidual && in) g_out[v] = g;
+      unpack16<STK_BF16>(g, gf);
+#pragma unroll
+      for (int k = 0; k < 8; ++k) {
+        sdy[k] = __fadd_rn(sdy[k], gf[k]);
+        sxm[k] = __fmaf_rn(gf[k], __fsub_rn(xf[k], m[k]), sxm[k]);
+      }
+    }
+  }
+  sh[t][0] = make_float4(sdy[0], sdy[1], sdy[2], sdy[3]);
+  sh[t][1] = make_float4(sdy[4], sdy[5], sdy[6], sdy[7]);
+  sh[t][2] = make_float4(sxm[0], sxm[1], sxm[2], sxm[3]);
+  sh[t][3] = make_float4(sxm[4], sxm[5], sxm[6], sxm[7]);
+  __syncthreads();
+  // fold the chains, then halve over ty; thread (cgl, ty) of chain 0 owns the slot of that virtual thread
+  const bool owner = j == 0;
+  float s[16];
+  if (owner) {
+    const float* p = reinterpret_cast<const float*>(sh[t]);
+#pragma unroll
+    for (int k = 0; k < 16; ++k) s[k] = p[k];
+#pragma unroll
+    for (int q = 1; q < kChains; ++q) {
+      const float* r = reinterpret_cast<const float*>(sh[t + q * gb]);
+#pragma unroll
+      for (int k = 0; k < 16; ++k) s[k] = __fadd_rn(s[k], r[k]);
+    }
+  }
+  __syncthreads();
+  for (uint32_t off = block_y / 2; off > 0; off >>= 1) {
+    if (owner && ty < 2 * off) {
+      float* p = reinterpret_cast<float*>(sh[t]);
+#pragma unroll
+      for (int k = 0; k < 16; ++k) p[k] = s[k];
+    }
+    __syncthreads();
+    if (owner && ty < off) {
+      const float* r = reinterpret_cast<const float*>(sh[t + off * gb * kChains]);
+#pragma unroll
+      for (int k = 0; k < 16; ++k) s[k] = __fadd_rn(s[k], r[k]);
+    }
+    __syncthreads();
+  }
+  if (!(owner && ty == 0 && live)) return;
+  if (gridDim.y == 1) {
+    float is[8];
+    load8(invstd + c0, is);
+    uint16_t dw[8], db[8];
+#pragma unroll
+    for (int k = 0; k < 8; ++k) {
+      ws[c0 + k] = s[k];
+      ws[channels + c0 + k] = s[8 + k];
+      db[k] = bf16_bits(s[k]);
+      dw[k] = bf16_bits(__fmul_rn(s[8 + k], is[k]));
+    }
+    *reinterpret_cast<uint4*>(dbias + c0) = make_uint4(db[0] | uint32_t(db[1]) << 16, db[2] | uint32_t(db[3]) << 16,
+                                                       db[4] | uint32_t(db[5]) << 16, db[6] | uint32_t(db[7]) << 16);
+    *reinterpret_cast<uint4*>(dweight + c0) = make_uint4(dw[0] | uint32_t(dw[1]) << 16, dw[2] | uint32_t(dw[3]) << 16,
+                                                         dw[4] | uint32_t(dw[5]) << 16, dw[6] | uint32_t(dw[7]) << 16);
+  } else {
+    float* pdy = ws + 2 * channels + size_t(blockIdx.y) * channels + c0;
+    float* pxm = pdy + size_t(gridDim.y) * channels;
+#pragma unroll
+    for (int k = 0; k < 8; ++k) {
+      pdy[k] = s[k];
+      pxm[k] = s[8 + k];
+    }
+  }
+}
+
+// torch's cross-block finish: thread ty adds the partials of blocks ty, ty + block_y, ... from +0, then the halving
+// tree over ty.  One thread per (channel, ty).
+__global__ void __launch_bounds__(kBwdThreads) k_bn_bwd_finish(float* __restrict__ ws, const float* __restrict__ invstd,
+                                                               __nv_bfloat16* __restrict__ dweight,
+                                                               __nv_bfloat16* __restrict__ dbias, uint32_t channels,
+                                                               uint32_t block_y, uint32_t grid_y) {
+  __shared__ float sh[2][kBwdThreads];
+  const uint32_t t = threadIdx.x, cb = kBwdThreads / block_y, ty = t / cb, c = blockIdx.x * cb + t % cb;
+  const bool live = c < channels;
+  const float* pdy = ws + 2 * channels;
+  const float* pxm = pdy + size_t(grid_y) * channels;
+  float dy = 0.f, xm = 0.f;
+  if (live)
+    for (uint32_t y = ty; y < grid_y; y += block_y) {
+      dy = __fadd_rn(dy, pdy[size_t(y) * channels + c]);
+      xm = __fadd_rn(xm, pxm[size_t(y) * channels + c]);
+    }
+  for (uint32_t off = block_y / 2; off > 0; off >>= 1) {
+    sh[0][t] = dy;
+    sh[1][t] = xm;
+    __syncthreads();
+    if (ty < off) {
+      dy = __fadd_rn(dy, sh[0][t + off * cb]);
+      xm = __fadd_rn(xm, sh[1][t + off * cb]);
+    }
+    __syncthreads();
+  }
+  if (ty != 0 || !live) return;
+  ws[c] = dy;
+  ws[channels + c] = xm;
+  dbias[c] = __float2bfloat16_rn(dy);
+  dweight[c] = __float2bfloat16_rn(__fmul_rn(xm, invstd[c]));
+}
+
+// dx = bf16(((g - sum_dy * n) - (x - mean) * k1) * k2), k1 = invstd * invstd * sum_dy_xmu * n, k2 = w * invstd,
+// n = float(1.0 / rows): torch's channels-last elementwise backward, whose SASS contracts both subtractions with their
+// products (FFMA -sum_dy * n + g; FADD x - mean; FFMA -k1 * (x - mean) + t; FMUL k2).  Thread layout as in k_bn_act.
+template <bool kResidual>
+__global__ void __launch_bounds__(kBnThreads) k_bn_bwd_elemt(const uint4* __restrict__ grad, const uint4* __restrict__ x,
+                                                            const float* __restrict__ mean, const float* __restrict__ invstd,
+                                                            const __nv_bfloat16* __restrict__ weight,
+                                                            const __nv_bfloat16* __restrict__ bias,
+                                                            const float* __restrict__ ws, uint4* __restrict__ dx, float n,
+                                                            uint32_t nvec, uint32_t groups, uint32_t active) {
+  const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= active) return;
+  const uint32_t c0 = (t % groups) * 8, channels = groups * 8;
+  float m[8], is[8], w[8], b[8], sdy[8], k1[8], k2[8];
+  {
+    float sxm[8];
+    load8(mean + c0, m);
+    load8(invstd + c0, is);
+    load8(ws + c0, sdy);
+    load8(ws + channels + c0, sxm);
+    unpack16<STK_BF16>(__ldg(reinterpret_cast<const uint4*>(weight + c0)), w);
+    if (!kResidual) unpack16<STK_BF16>(__ldg(reinterpret_cast<const uint4*>(bias + c0)), b);
+#pragma unroll
+    for (int k = 0; k < 8; ++k) {
+      k1[k] = __fmul_rn(__fmul_rn(__fmul_rn(is[k], is[k]), sxm[k]), n);
+      k2[k] = __fmul_rn(w[k], is[k]);
+    }
+  }
+  for (uint32_t v = t; v < nvec; v += active) {
+    float xf[8], gf[8];
+    unpack16<STK_BF16>(__ldg(x + v), xf);
+    uint4 g = __ldg(grad + v);
+    if (!kResidual) {
+      bool pass[8];
+#pragma unroll
+      for (int k = 0; k < 8; ++k) pass[k] = !(bf16_val(bn_apply(xf[k], m[k], is[k], w[k], b[k])) <= 0.f);
+      g = mask_grad(g, pass);
+    }
+    unpack16<STK_BF16>(g, gf);
+    uint16_t o[8];
+#pragma unroll
+    for (int k = 0; k < 8; ++k)
+      o[k] = bf16_bits(__fmul_rn(__fmaf_rn(-__fsub_rn(xf[k], m[k]), k1[k], __fmaf_rn(-sdy[k], n, gf[k])), k2[k]));
+    dx[v] = make_uint4(o[0] | uint32_t(o[1]) << 16, o[2] | uint32_t(o[3]) << 16, o[4] | uint32_t(o[5]) << 16,
+                       o[6] | uint32_t(o[7]) << 16);
+  }
+}
+
+// torch's flexible_launch_configs(rows, channels, coop = true) with MAX_BLOCK_SIZE 512, as the channels-last backward
+// reduce launches it: the only inputs of its summation order besides the row count.
+struct BnBwdConfig {
+  uint32_t block_y, grid_y, loops;
+};
+
+static uint32_t last_pow2(uint32_t n) {
+  uint32_t p = 1;
+  while (p <= n / 2) p *= 2;
+  return p;
+}
+
+static BnBwdConfig bn_bwd_config(uint32_t rows, uint32_t channels) {
+  const uint32_t block_x = std::min(last_pow2(channels), 32u);
+  const uint32_t block_y = std::min(last_pow2((rows + 15) / 16), 512u / block_x);
+  uint32_t grid_y = std::min((rows + block_y * 16 - 1) / (block_y * 16), 128u);
+  if (grid_y < 8) grid_y = 1;
+  return {block_y, grid_y, 1 + (rows - 1) / (block_y * grid_y * kChains)};
 }
 
 }  // namespace stk
@@ -93,6 +345,58 @@ int stk_bn_act(stk_ctx* c, const void* x, const void* residual, const float* mea
                                                static_cast<__nv_bfloat16*>(out), save_invstd, nvec, groups, active,
                                                uint32_t(channels));
   STK_CUDA(c, cudaGetLastError());
+  return STK_OK;
+}
+
+int stk_bn_act_backward(stk_ctx* c, const void* grad, const void* x, const void* out, const float* mean, const float* invstd,
+                        const void* weight, const void* bias, void* grad_x, void* grad_weight, void* grad_bias,
+                        void* grad_residual, float* workspace, size_t numel, size_t channels, void* stream) {
+  STK_REQUIRE(c, c && grad && x && mean && invstd && weight && grad_weight && grad_bias && workspace,
+              "stk_bn_act_backward: NULL argument");
+  STK_REQUIRE(c, out ? grad_residual != nullptr : bias != nullptr,
+              "stk_bn_act_backward: a residual site needs grad_residual, a site without one needs bias");
+  STK_REQUIRE(c, channels > 0 && channels % 8 == 0 && numel % channels == 0 && numel >= channels,
+              "stk_bn_act_backward: channels must be a positive multiple of 8 dividing numel");
+  STK_REQUIRE(c, numel < (size_t(1) << 31), "stk_bn_act_backward: numel must be below 2^31");
+  const uintptr_t align = uintptr_t(grad) | uintptr_t(x) | uintptr_t(out) | uintptr_t(mean) | uintptr_t(invstd) |
+                          uintptr_t(weight) | uintptr_t(bias) | uintptr_t(grad_x) | uintptr_t(grad_weight) |
+                          uintptr_t(grad_bias) | uintptr_t(grad_residual) | uintptr_t(workspace);
+  STK_REQUIRE(c, align % 16 == 0, "stk_bn_act_backward: every tensor must be 16-byte aligned");
+  DeviceGuard g(c->device);
+  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+  const uint32_t rows = uint32_t(numel / channels), groups = uint32_t(channels / 8);
+  const BnBwdConfig cfg = bn_bwd_config(rows, uint32_t(channels));
+  const bool res = out != nullptr;
+  const uint32_t gb = kBwdThreads / (kChains * cfg.block_y);   // block_y <= 512 / 8 since channels >= 8
+  const dim3 grid((groups + gb - 1) / gb, cfg.grid_y);
+  auto reduce = res ? k_bn_bwd_reduce<true> : k_bn_bwd_reduce<false>;
+  auto bf = [](const void* p) { return static_cast<const __nv_bfloat16*>(p); };
+  reduce<<<grid, kBwdThreads, 0, s>>>(static_cast<const uint4*>(grad), static_cast<const uint4*>(x),
+                                      static_cast<const uint4*>(out), mean, invstd, bf(weight), bf(bias),
+                                      static_cast<uint4*>(grad_residual), workspace,
+                                      static_cast<__nv_bfloat16*>(grad_weight), static_cast<__nv_bfloat16*>(grad_bias),
+                                      rows, groups, cfg.block_y, cfg.loops);
+  STK_CUDA(c, cudaGetLastError());
+  if (cfg.grid_y > 1) {
+    const uint32_t cb = kBwdThreads / cfg.block_y;
+    k_bn_bwd_finish<<<unsigned((channels + cb - 1) / cb), kBwdThreads, 0, s>>>(
+        workspace, invstd, static_cast<__nv_bfloat16*>(grad_weight), static_cast<__nv_bfloat16*>(grad_bias),
+        uint32_t(channels), cfg.block_y, cfg.grid_y);
+    STK_CUDA(c, cudaGetLastError());
+  }
+  if (grad_x) {
+    const uint32_t nvec = uint32_t(numel / 8);
+    auto elemt = res ? k_bn_bwd_elemt<true> : k_bn_bwd_elemt<false>;
+    const size_t resident = size_t(blocks_per_sm(c, elemt, kBnThreads)) * c->sm_count;
+    size_t blocks = std::min(resident, (size_t(nvec) + kBnThreads - 1) / kBnThreads);
+    blocks = std::max(blocks, (size_t(groups) + kBnThreads - 1) / kBnThreads);
+    const uint32_t active = uint32_t(blocks * kBnThreads / groups * groups);
+    elemt<<<unsigned(blocks), kBnThreads, 0, s>>>(static_cast<const uint4*>(res ? grad_residual : grad),
+                                                  static_cast<const uint4*>(x), mean, invstd, bf(weight), bf(bias),
+                                                  workspace, static_cast<uint4*>(grad_x), float(1.0 / double(rows)),
+                                                  nvec, groups, active);
+    STK_CUDA(c, cudaGetLastError());
+  }
   return STK_OK;
 }
 

@@ -39,6 +39,24 @@ ALIGN_ELEMS = layout.ALIGN_ELEMS  # every parameter starts on a 16-element bound
 DEFAULT_BUCKET_MB = 25.0  # DDPConfig.bucket_cap_mb of the reference (stoke/configs.py:178-188)
 
 
+def bn_backward_grid(rows: int, channels: int) -> Tuple[int, int, int]:
+    """(block_y, grid_y, loops) of torch's channels-last BatchNorm backward reduce over ``rows`` x ``channels``
+    (``flexible_launch_configs`` with ``coop``, MAX_BLOCK_SIZE 512), which fix its summation order; ``stk_bn_act_backward``
+    derives the same numbers in C."""
+    def last_pow2(n):
+        return 1 << (n.bit_length() - 1)
+
+    block_y = min(last_pow2(-(-rows // 16)), 512 // min(last_pow2(channels), 32))
+    grid_y = min(-(-rows // (block_y * 16)), 128)
+    grid_y = 1 if grid_y < 8 else grid_y
+    return block_y, grid_y, 1 + (rows - 1) // (block_y * grid_y * 4)
+
+
+def _bn_bwd_launches(rows: int, channels: int, grad_x: bool) -> int:
+    """reduce, the cross-block finish when the reduce has more than one block per channel, the elementwise pass"""
+    return 1 + (bn_backward_grid(rows, channels)[1] > 1) + bool(grad_x)
+
+
 class DeviceBuffer:
     """A device allocation owned by the library, mapped into every peer (VMM / CUDA IPC) when world > 1."""
 
@@ -315,6 +333,22 @@ class Engine:
                                         mean.data_ptr(), var.data_ptr(), weight.data_ptr(), bias.data_ptr(), float(eps),
                                         out.data_ptr(), save_invstd.data_ptr(), x.numel(), x.shape[1], self._stream()))
         self.launches += 1
+
+    def bn_act_backward(self, grad: torch.Tensor, x: torch.Tensor, out: Optional[torch.Tensor], mean: torch.Tensor,
+                        invstd: torch.Tensor, weight: torch.Tensor, bias: Optional[torch.Tensor],
+                        grad_x: Optional[torch.Tensor], grad_weight: torch.Tensor, grad_bias: torch.Tensor,
+                        grad_residual: Optional[torch.Tensor]):
+        """Backward of ``bn_act`` (``stk_bn_act_backward``): the ReLU mask comes from ``out`` at a site with a residual
+        (``grad_residual`` receives the masked gradient) and from ``x``, ``weight``, ``bias`` otherwise (``out`` None);
+        ``grad_x`` None skips the elementwise pass.  ``fuse.py`` checks dtypes, layout and alignment before calling."""
+        c = x.shape[1]
+        ws = torch.empty(2 * (1 + 128) * c, dtype=torch.float32, device=x.device)
+        ptr = lambda t: t.data_ptr() if t is not None else None  # noqa: E731
+        self._check(self.lib.stk_bn_act_backward(self.ctx, grad.data_ptr(), x.data_ptr(), ptr(out), mean.data_ptr(),
+                                                 invstd.data_ptr(), weight.data_ptr(), ptr(bias), ptr(grad_x),
+                                                 grad_weight.data_ptr(), grad_bias.data_ptr(), ptr(grad_residual),
+                                                 ws.data_ptr(), x.numel(), c, self._stream()))
+        self.launches += _bn_bwd_launches(x.numel() // c, c, grad_x is not None)
 
     def barrier(self):
         self._check(self.lib.stk_barrier(self.ctx, self._stream()))

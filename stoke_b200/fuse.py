@@ -8,9 +8,12 @@ only for calls it is a faithful trace of (training mode, required arguments only
 every other call, or None when tracing or rewriting fails or nothing matches; the caller then keeps running ``module``.
 
 What stays torch's: the forward statistics and the running-statistics update (``torch.batch_norm_update_stats``, the
-reduction the native training forward runs) and the whole backward (``threshold_backward`` +
-``native_batch_norm_backward``, the calls autograd makes for the unfused chain).  Only the elementwise apply / add / ReLU
-moves into the kernel, which rounds every intermediate as the unfused ops do, so the results are bit-identical to them.
+reduction the native training forward runs).  The forward's elementwise apply / add / ReLU is one kernel, which rounds
+every intermediate as the unfused ops do.  The backward (``stk_bn_act_backward``) folds the ReLU's ``threshold_backward``
+into the two passes of torch's channels-last ``native_batch_norm_backward`` and adds its per-channel sums in torch's
+order, so every result is bit-identical to the calls autograd makes for the unfused chain.  It takes the gradient when
+torch's BatchNorm backward would run its channels-last kernels on it (``threshold_backward``'s output is channels-last;
+another layout is made channels-last first) and it is bf16 and aligned; otherwise it runs those calls.
 Each call falls back to the unfused torch ops when the kernel does not cover its inputs (eval mode, no running statistics,
 not bf16, not channels-last, misaligned, C % 8 != 0, 2^31 elements or more, a CPU tensor), so the same inputs give the
 same results whether or not the model was rewritten.
@@ -57,6 +60,22 @@ def _covered(bn: torch.nn.BatchNorm2d, x: torch.Tensor, r: Optional[torch.Tensor
     return True
 
 
+def _grad_covered(grad: torch.Tensor, x: torch.Tensor) -> bool:
+    """The backward kernel takes ``grad`` when torch would run its channels-last BatchNorm backward on it."""
+    return (grad.dtype == torch.bfloat16 and grad.device == x.device and grad.shape == x.shape
+            and grad.is_contiguous(memory_format=torch.channels_last) and _aligned(grad))
+
+
+def _mask_output_channels_last(grad: torch.Tensor, x: torch.Tensor) -> bool:
+    """Whether ``threshold_backward(grad, out)`` (``out`` laid out like ``x``) returns a channels-last tensor, which is
+    what decides whether torch's BatchNorm backward runs its channels-last kernels.  Asked of the op's meta kernel, which
+    lays the output out as every backend does.  A gradient arriving expanded (the average pool's backward) gets one."""
+    def meta(t):
+        return torch.empty_strided(t.shape, t.stride(), dtype=t.dtype, device="meta")
+
+    return torch.ops.aten.threshold_backward(meta(grad), meta(x), 0).is_contiguous(memory_format=torch.channels_last)
+
+
 class _BnActFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x, weight, bias, residual, bn, engine):
@@ -65,20 +84,35 @@ class _BnActFn(torch.autograd.Function):
         out = torch.empty_like(x)
         invstd = torch.empty_like(mean)
         engine.bn_act(x, residual, mean, var, weight, bias, bn.eps, out, invstd)
-        ctx.save_for_backward(x, weight, out, mean, invstd)
-        ctx.bn = bn
+        # the ReLU mask: out at a site with a residual, else recomputed from x and the parameters (bias saved instead)
+        ctx.save_for_backward(x, weight, out if residual is not None else bias, mean, invstd)
+        ctx.bn, ctx.engine = bn, engine
         ctx.has_residual = residual is not None
         return out
 
     @staticmethod
     def backward(ctx, grad_out):
-        x, weight, out, mean, invstd = ctx.saved_tensors
-        bn = ctx.bn
+        x, weight, out_or_bias, mean, invstd = ctx.saved_tensors
+        bn, res = ctx.bn, ctx.has_residual
+        need_x, need_w, need_b, need_r = ctx.needs_input_grad[:4]
+        if (grad_out.dtype == torch.bfloat16 and grad_out.shape == x.shape
+                and not grad_out.is_contiguous(memory_format=torch.channels_last) and _mask_output_channels_last(grad_out, x)):
+            grad_out = grad_out.contiguous(memory_format=torch.channels_last)   # same values, so the same g
+        if _grad_covered(grad_out, x):
+            dx = torch.empty_like(x) if need_x else None
+            dw, db = torch.empty_like(weight), torch.empty_like(weight)
+            dr = torch.empty_like(x) if res else None
+            ctx.engine.bn_act_backward(grad_out, x, out_or_bias if res else None, mean, invstd, weight,
+                                       None if res else out_or_bias, dx, dw, db, dr)
+            return dx, dw if need_w else None, db if need_b else None, dr if need_r else None, None, None
+        # relu(y) <= 0 exactly when y <= 0, so without a residual y = batch_norm_elemt(x) (the transform the forward
+        # kernel reproduces) gives threshold_backward the same mask as out
+        out = out_or_bias if res else torch.batch_norm_elemt(x, weight, out_or_bias, mean, invstd, bn.eps)
         g = torch.ops.aten.threshold_backward(grad_out, out, 0)
-        mask = [ctx.needs_input_grad[0], ctx.needs_input_grad[1], ctx.needs_input_grad[2]]
+        mask = [need_x, need_w, need_b]
         dx, dw, db = torch.ops.aten.native_batch_norm_backward(g, x, weight, bn.running_mean, bn.running_var, mean, invstd,
                                                               True, bn.eps, mask)
-        dr = g if ctx.has_residual and ctx.needs_input_grad[3] else None
+        dr = g if res and need_r else None
         return dx, dw, db, dr, None, None
 
 
