@@ -35,6 +35,8 @@
  *   stk_optim_range_prologue         torch's per-parameter `state[p]["step"]` (torch/optim/adam.py: a parameter whose grad is None
  *                                    is not stepped and keeps its own count) for models with sometimes-unused parameters
  *   stk_optim_step_prologue          the same for every kind, plus NAdam's `state[p]["mu_product"]` (torch/optim/nadam.py)
+ *   stk_adafactor_plan / _step       torch.optim.Adafactor's step (torch/optim/_adafactor.py _single_tensor_adafactor) plus
+ *                                    the clip and the GradScaler.step gate, without its two .item() per parameter
  */
 #ifndef STOKE_B200_H
 #define STOKE_B200_H
@@ -305,6 +307,69 @@ int stk_optim_step_prologue(stk_ctx* ctx, const stk_optim_hyper_t* hyper, const 
 
 /* scaler.update(), opt_steps/skipped_steps bookkeeping, reset of the per-step accumulators */
 int stk_step_epilogue(stk_ctx* ctx, void* stream);
+
+/* ---- Adafactor: fused step of torch.optim.Adafactor ------------------------------------------------------------------
+ * Replaces torch/optim/_adafactor.py _single_tensor_adafactor (its per-parameter python loop with two .item() host
+ * synchronisations), plus clip_grad_norm_ / clip_grad_value_'s scaling and GradScaler.step's inf gate, like stk_optim_step.
+ * Per parameter with a gradient, t = its own step count after the increment:
+ *   b2hat = t^beta2_decay, rho = min(lr, 1/sqrt(t)), alpha = max(eps2, ||w|| / sqrt(numel)) * rho   (norm BEFORE decay)
+ *   w *= 1 - lr * weight_decay                                             (weight_decay != 0)
+ *   dim >= 2: row_var = lerp(row_var, mean_c g^2, b2hat), col_var = lerp(col_var, mean_r g^2, b2hat) over the last two dims
+ *             (leading dims are a batch), v = row_var[r] col_var[c] / clamp_min(mean_r row_var, eps1)
+ *   dim <= 1: variance = lerp(variance, g^2, b2hat), v = variance
+ *   u = g rsqrt(clamp_min(v, eps1^2)),  w += (-alpha / max(1, ||u|| / (sqrt(numel) d))) u
+ * with python's max / min (a NaN norm gives eps2 and 1) and eps1 "None" = fp32 epsilon (the masters are fp32).
+ * Deterministic: every sum adds in an order fixed by the shapes (per-block / per-chunk partials folded in index order by a
+ * finisher), no floating-point atomics.  Nothing is synchronised; the launches go to `stream` in order. */
+typedef struct {
+  uint64_t offset;        /* first element of the parameter in the flat master / gradient / lp buffers */
+  uint64_t state;         /* first element of its state in the state buffer */
+  int32_t numel;          /* 1 .. 2^31 - 1 */
+  int32_t factored;       /* 1 (dim >= 2): row_var [B*R] then col_var [B*C] at `state`, torch's contiguous [..., R, 1] and
+                             [..., 1, C]; 0 (dim <= 1): variance [numel] */
+  int32_t size[4];        /* logical sizes (B0, B1, R, C), left-padded with 1; B = B0 * B1 */
+  int32_t stride[4];      /* element strides of those dims in the flat buffers; the parameter must be dense (any order) */
+  /* filled by stk_adafactor_plan */
+  int32_t contiguous, tile0, b0, pad_;
+  int64_t line0, out0, rm0;
+} stk_adafactor_param_t;
+
+typedef struct {          /* totals of a plan (filled by stk_adafactor_plan) */
+  int32_t n_params, n_tiles, n_b, pad_;
+  int64_t n_line, n_out, n_rm;
+  size_t workspace_bytes; /* device workspace stk_adafactor_step needs (no initialisation) */
+} stk_adafactor_plan_t;
+
+typedef struct {          /* one per parameter group */
+  double lr, beta2_decay, eps1, eps2, d, weight_decay;
+  int eps1_none;          /* 1: eps=(None, eps2): fp32 epsilon */
+  int maximize;
+} stk_adafactor_hyper_t;
+
+typedef struct {
+  const stk_adafactor_hyper_t* hyper; int n_groups;   /* host array, <= STK_MAX_GROUPS */
+  int clip_kind; double clip_max_norm, clip_value;
+  const stk_adafactor_param_t* params;  /* DEVICE copy of the planned table */
+  const stk_adafactor_plan_t* plan;     /* host */
+  const uint8_t* param_group;  /* DEVICE, one per parameter: group index, bit 7 = no gradient this step (not stepped) */
+  int32_t* steps;              /* DEVICE, one per parameter: steps taken; advanced here unless skipped or found_inf */
+  float* master;               /* fp32 masters (flat indexing) */
+  float* state;                /* fp32 state buffer */
+  void* workspace;             /* plan->workspace_bytes, 16-byte aligned */
+  const void* grad; int grad_dtype; int grad_raw;  /* raw = 1: model-dtype bucket (bf16 | f32) scaled by grad_mul and
+                                                      1/loss_scale, ZEROED after the step (also when skipped);
+                                                      raw = 0: fp32 reduced main gradients */
+  const float* acc; double grad_mul;  /* raw route: optional fp32 accumulator, multiplier */
+  void* lp; int lp_dtype;      /* low-precision parameter copy written after the update (bf16 | f32), or NULL */
+} stk_adafactor_args_t;
+
+/* Validates `params_host[0..n)` (offset, state, numel, factored, size, stride filled by the caller) and fills their plan
+ * fields and the totals.  Host only. */
+int stk_adafactor_plan(stk_adafactor_param_t* params_host, int n_params, stk_adafactor_plan_t* plan_out);
+/* One Adafactor step: eight stream-ordered launches (||w||^2 partials, per-parameter scalars and step counts, row / column
+ * sums of g^2, their lerp, row means, ||u||^2 partials, the per-parameter coefficient, the update).  Reads the selected
+ * scaler state (found_inf skips every parameter and leaves state and counts unchanged; the raw bucket is still zeroed). */
+int stk_adafactor_step(stk_ctx* ctx, const stk_adafactor_args_t* args, void* stream);
 
 /* ---- small collectives on the signal pads -------------------------------------------------------------------------- */
 /* mean over ranks of *loss_dev (float32/bf16/f16 scalar) -> *out_host (pinned, mapped) ; synchronises `stream` */

@@ -63,6 +63,31 @@ class OptimArgs(C.Structure):
                 ("group_bc", C.c_void_p)]
 
 
+class AdafactorParam(C.Structure):
+    _fields_ = [("offset", C.c_uint64), ("state", C.c_uint64), ("numel", C.c_int32), ("factored", C.c_int32),
+                ("size", C.c_int32 * 4), ("stride", C.c_int32 * 4), ("contiguous", C.c_int32), ("tile0", C.c_int32),
+                ("b0", C.c_int32), ("pad_", C.c_int32), ("line0", C.c_int64), ("out0", C.c_int64), ("rm0", C.c_int64)]
+
+
+class AdafactorPlan(C.Structure):
+    _fields_ = [("n_params", C.c_int32), ("n_tiles", C.c_int32), ("n_b", C.c_int32), ("pad_", C.c_int32),
+                ("n_line", C.c_int64), ("n_out", C.c_int64), ("n_rm", C.c_int64), ("workspace_bytes", C.c_size_t)]
+
+
+class AdafactorHyper(C.Structure):
+    _fields_ = [("lr", C.c_double), ("beta2_decay", C.c_double), ("eps1", C.c_double), ("eps2", C.c_double),
+                ("d", C.c_double), ("weight_decay", C.c_double), ("eps1_none", C.c_int), ("maximize", C.c_int)]
+
+
+class AdafactorArgs(C.Structure):
+    _fields_ = [("hyper", C.POINTER(AdafactorHyper)), ("n_groups", C.c_int), ("clip_kind", C.c_int),
+                ("clip_max_norm", C.c_double), ("clip_value", C.c_double), ("params", C.c_void_p),
+                ("plan", C.POINTER(AdafactorPlan)), ("param_group", C.c_void_p), ("steps", C.c_void_p),
+                ("master", C.c_void_p), ("state", C.c_void_p), ("workspace", C.c_void_p), ("grad", C.c_void_p),
+                ("grad_dtype", C.c_int), ("grad_raw", C.c_int), ("acc", C.c_void_p), ("grad_mul", C.c_double),
+                ("lp", C.c_void_p), ("lp_dtype", C.c_int)]
+
+
 class SamplerPlan(C.Structure):
     _fields_ = [("n", C.c_int64), ("buckets", C.c_int64), ("batch_size", C.c_int64), ("world", C.c_int64),
                 ("rank", C.c_int64), ("drop_last", C.c_int32), ("allow_bucket_overlap", C.c_int32),
@@ -115,6 +140,8 @@ _SIGNATURES = {
     "stk_optim_step_prologue": (C.c_int, [_P, C.POINTER(OptimHyper), C.POINTER(OptimHyperExt), C.c_int, C.c_int, _P, _P,
                                           _P, _P, _P]),
     "stk_step_epilogue": (C.c_int, [_P, _P]),
+    "stk_adafactor_plan": (C.c_int, [C.POINTER(AdafactorParam), C.c_int, C.POINTER(AdafactorPlan)]),
+    "stk_adafactor_step": (C.c_int, [_P, C.POINTER(AdafactorArgs), _P]),
     "stk_loss_sync": (C.c_int, [_P, _P, C.c_int, C.POINTER(C.c_double), _P]),
     "stk_loss_sync_begin": (C.c_int, [_P, _P, C.c_int, C.POINTER(C.c_int64), _P]),
     "stk_loss_sync_wait": (C.c_int, [_P, C.c_int64, C.POINTER(C.c_double)]),

@@ -458,7 +458,7 @@ class GradPath:
                  module: Optional[torch.nn.Module] = None, sync_init: bool = True, needs_second_moment: bool = True,
                  needs_first_moment: bool = True, bucket_mb: Optional[float] = None, state_id: Optional[int] = None,
                  route: Optional[str] = None, group_of: Optional[Sequence[int]] = None, overlap: bool = True,
-                 mu_product: bool = False):
+                 mu_product: bool = False, adafactor: bool = False):
         self.engine = engine
         self.params = [p for p in params if p.requires_grad]
         if not self.params:
@@ -608,9 +608,37 @@ class GradPath:
         for idx, p in enumerate(self.params):
             self._hooks.append(p.register_post_accumulate_grad_hook(self._make_hook(ref, idx)))
         self._closed = False
+        self.adafactor = bool(adafactor)
+        if self.adafactor:
+            self._adafactor_setup()
         torch.cuda.synchronize(engine.device)
         if W > 1:
             torch.distributed.barrier(group=engine.group)
+
+    def _adafactor_setup(self):
+        """State, descriptor table and workspace of the fused Adafactor step, built once.  The state is one flat fp32 buffer:
+        per parameter row_var then col_var (dim >= 2) or variance (dim <= 1), in torch's layouts.  Step counts are kept per
+        parameter on the device from the start (torch's ``state[p]["step"]``; every Adafactor scalar is per parameter)."""
+        if self.sharded:
+            raise ValueError("Stoke -- the fused Adafactor step needs whole parameters on one rank (no sharded route)")
+        dev = self._range_end.device
+        descs = (_lib.AdafactorParam * len(self.params))()
+        self.af_layouts = []
+        off = 0
+        for i, (p, o) in enumerate(zip(self.params, self.offsets)):
+            lay = layout.adafactor_layout(p.shape, p.stride())
+            d = descs[i]
+            d.offset, d.state, d.numel, d.factored = o, off, lay["numel"], int(lay["factored"])
+            d.size[:] = lay["size"]
+            d.stride[:] = lay["stride"]
+            self.af_layouts.append(dict(lay, offset=off))
+            off += lay["state"]
+        self.af_plan = _lib.AdafactorPlan()
+        check(self.engine.lib.stk_adafactor_plan(descs, len(descs), C.byref(self.af_plan)))
+        self._af_desc = torch.frombuffer(bytearray(C.string_at(descs, C.sizeof(descs))), dtype=torch.uint8).to(dev)
+        self.af_state = torch.zeros(max(off, 1), dtype=torch.float32, device=dev)
+        self._af_ws = torch.empty(max(int(self.af_plan.workspace_bytes), 16), dtype=torch.uint8, device=dev)
+        self._range_steps = torch.zeros(len(self.params), dtype=torch.int32, device=dev)
 
     # -- layout helpers -----------------------------------------------------------------------------------------------
     @staticmethod
@@ -861,6 +889,52 @@ class GradPath:
         self._raw_has_acc = False
         e.comm_poll()  # a peer that went missing during this step surfaces here (no synchronisation)
 
+    def adafactor_step(self, hypers: Sequence[_lib.AdafactorHyper]):
+        """One fused Adafactor step (``stk_adafactor_step``: eight launches over the descriptor table), then the epilogue.
+        ``hypers``: one ``AdafactorHyper`` per group.  Parameters without a gradient in this window are skipped through
+        the skip bits of the range table; their step counts and state do not move."""
+        e = self.engine
+        e.state_select(self.state_id)
+        ng = len(hypers)
+        if ng > _lib.MAX_GROUPS:
+            raise NotImplementedError(f"Stoke -- the fused step handles up to {_lib.MAX_GROUPS} parameter groups")
+        harr = (_lib.AdafactorHyper * ng)(*hypers)
+        a = _lib.AdafactorArgs()
+        a.hyper, a.n_groups = harr, ng
+        a.clip_kind, a.clip_max_norm, a.clip_value = self.clip.kind, self.clip.max_norm, self.clip.clip_value
+        a.params, a.plan = self._af_desc.data_ptr(), C.pointer(self.af_plan)
+        self._ranges_for_step()   # refreshes the skip bits of the per-parameter group table
+        a.param_group, a.steps = self._range_group.data_ptr(), self._range_steps.data_ptr()
+        a.master, a.state, a.workspace = self.master_ptr, self.af_state.data_ptr(), self._af_ws.data_ptr()
+        if self.route == "local":
+            a.grad, a.grad_dtype, a.grad_raw, a.grad_mul = self.G.ptr, _DT[self.model_dtype], 1, 1.0
+            a.acc = self.ACC.ptr if self._raw_has_acc else None
+        else:
+            a.grad, a.grad_dtype, a.grad_raw = self.MAIN.ptr, _lib.F32, 0
+        if self.low_precision:
+            a.lp, a.lp_dtype = self.P.ptr, _DT[self.model_dtype]
+        e._check(e.lib.stk_adafactor_step(e.ctx, C.byref(a), e._stream()))
+        e.launches += 8 if self.af_plan.n_line else 5
+        e.step_epilogue()
+        self._track_touched = False
+        self._raw_has_acc = False
+        e.comm_poll()
+
+    def adafactor_state_views(self) -> List[Tuple[torch.Tensor, ...]]:
+        """Per parameter, views of the state buffer in torch's shapes: (row_var [..., R, 1], col_var [..., 1, C]) or
+        (variance,) shaped like the parameter."""
+        out = []
+        for p, lay in zip(self.params, self.af_layouts):
+            o = lay["offset"]
+            if lay["factored"]:
+                B, R, C_ = lay["B"], lay["R"], lay["C"]
+                lead = list(p.shape[:-2])
+                out.append((self.af_state[o: o + B * R].view(lead + [R, 1]),
+                            self.af_state[o + B * R: o + B * R + B * C_].view(lead + [1, C_])))
+            else:
+                out.append((self.af_state[o: o + lay["numel"]].view(p.shape),))
+        return out
+
     # -- inspection (tests, checkpoints) ----------------------------------------------------------------------------------
     def gather_master(self) -> torch.Tensor:
         """Full fp32 master vector (all-gathered across shards when sharded)."""
@@ -905,6 +979,7 @@ class GradPath:
                 p.grad = None
         self.grad_views = []
         self.p_flat = self.g_flat = self.main_flat = self.m_flat = self.v_flat = self.master_flat = None
+        self.af_state = self._af_ws = self._af_desc = None
         for b in self._bufs:
             try:
                 e.free(b)

@@ -67,3 +67,32 @@ def plan_segments(buckets: Sequence[Tuple[int, int]], world: int, sharded: bool,
         segs_by_rank.append(out)
         n_local.append(lo)
     return segs_by_rank, n_local
+
+
+ADAFACTOR_MAX_DIM = 4  # stk_adafactor_param_t carries four logical dims; a larger parameter keeps the stock route
+
+
+def adafactor_layout(shape: Sequence[int], stride: Sequence[int]) -> dict:
+    """How the fused Adafactor step sees one parameter of logical ``shape`` laid out with element ``stride``:
+    ``factored`` (dim >= 2: torch factors g^2 over the last two dims, leading dims are a batch), the sizes and strides
+    left-padded with 1 to four dims (B0, B1, R, C), and ``state``, the fp32 elements of its state (row_var [..., R, 1] then
+    col_var [..., 1, C]; or variance, one per element).  Raises ValueError for more than four dims or a layout that is not
+    dense (overlapping or with holes)."""
+    shape, stride = [int(s) for s in shape], [int(s) for s in stride]
+    if len(shape) > ADAFACTOR_MAX_DIM:
+        raise ValueError(f"Stoke -- fused Adafactor handles parameters of up to {ADAFACTOR_MAX_DIM} dims, got {len(shape)}")
+    numel = 1
+    for s in shape:
+        numel *= s
+    expect = 1
+    for s, st in sorted(((s, st) for s, st in zip(shape, stride) if s != 1), key=lambda x: x[1]):
+        if st != expect:
+            raise ValueError("Stoke -- fused Adafactor needs dense parameters")
+        expect *= s
+    pad = ADAFACTOR_MAX_DIM - len(shape)
+    size4 = [1] * pad + shape
+    stride4 = [numel] * pad + stride
+    factored = len(shape) >= 2
+    B, R, C = size4[0] * size4[1], size4[2], size4[3]
+    return {"factored": factored, "size": size4, "stride": stride4, "numel": numel, "B": B, "R": R, "C": C,
+            "state": B * R + B * C if factored else numel}

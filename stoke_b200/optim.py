@@ -8,6 +8,11 @@ flavour is the ZeRO-1 analogue of fairscale ``OSS`` (/root/reference/stoke/exten
 (per-group lr / betas / eps / weight decay / momentum ... selected inside the kernel by element range).  NAdam, RAdam and
 Adamax keep two fp32 state tensors per parameter like Adam (Adamax's ``exp_inf`` in the second-moment buffer); their
 per-step scalars, and NAdam's ``mu_product``, are formed on the device by ``stk_optim_step_prologue``.
+``torch.optim.Adafactor`` takes its own fused entry point, ``stk_adafactor_step`` (per-parameter reductions: row / column
+means of g^2, the parameter's RMS, the update's RMS), with per-parameter step counts on the device and torch's
+state_dict layout (``row_var`` / ``col_var`` or ``variance``).  Its state is never sharded: the reductions need whole
+parameters on one rank, so at world > 1 (``fairscale_oss=True`` included) it runs replicated on the all-reduce route,
+every rank taking the same deterministic step on the same gradients, as the stock route is replicated too.
 
 ``B200StockOptimizer`` -- every other ``torch.optim`` class (the reference instantiates whatever class the user passes,
 stoke/extensions.py:53-78) and the options the fused step does not cover (amsgrad, capturable, differentiable, more than 8
@@ -19,7 +24,7 @@ from typing import Dict, List, Optional, Type
 
 import torch
 
-from . import _lib
+from . import _lib, layout
 from .engine import ClipSpec, Engine, GradPath
 
 _KINDS = {torch.optim.Adam: _lib.OPT_ADAM, torch.optim.AdamW: _lib.OPT_ADAMW, torch.optim.SGD: _lib.OPT_SGD,
@@ -30,6 +35,10 @@ _STATE_KEYS = {_lib.OPT_ADAM: ("exp_avg", "exp_avg_sq"), _lib.OPT_ADAMW: ("exp_a
                _lib.OPT_NADAM: ("exp_avg", "exp_avg_sq"), _lib.OPT_RADAM: ("exp_avg", "exp_avg_sq"),
                _lib.OPT_ADAMAX: ("exp_avg", "exp_inf")}
 _STOCK_ONLY_TRUE = ("amsgrad", "capturable", "differentiable")
+# torch.optim.Adafactor (torch >= 2.5) runs on its own entry point, stk_adafactor_step, not as a kind of K2
+_ADAFACTOR = "adafactor"
+if hasattr(torch.optim, "Adafactor"):
+    _KINDS[torch.optim.Adafactor] = _ADAFACTOR
 
 
 def _module_params(module: torch.nn.Module):
@@ -78,6 +87,12 @@ def fused_supported(optim_cls, optim_kwargs: Dict, module: torch.nn.Module) -> b
         merged = dict(kw, **g)
         if any(merged.get(k) for k in _STOCK_ONLY_TRUE):
             return False
+    if _KINDS[optim_cls] == _ADAFACTOR:
+        try:   # up to four dims, dense (channels-last included)
+            for p in _module_params(module):
+                layout.adafactor_layout(p.shape, p.stride())
+        except ValueError:
+            return False
     return True
 
 
@@ -88,7 +103,7 @@ class B200FusedOptimizer(torch.optim.Optimizer):
                  bucket_mb: Optional[float] = None):
         if optim_cls not in _KINDS:
             raise NotImplementedError(
-                f"Stoke -- the fused step covers torch.optim.Adam, AdamW, SGD, NAdam, RAdam and Adamax; got {getattr(optim_cls, '__name__', optim_cls)}"
+                f"Stoke -- the fused step covers torch.optim.Adam, AdamW, SGD, NAdam, RAdam, Adamax and Adafactor; got {getattr(optim_cls, '__name__', optim_cls)}"
                 f" (use B200StockOptimizer / build_optimizer, which routes other classes to the stock-optimizer path)")
         params, group_of, extra, kw = _group_layout(module, optim_kwargs)
         if len(extra) > _lib.MAX_GROUPS:
@@ -107,10 +122,16 @@ class B200FusedOptimizer(torch.optim.Optimizer):
         self._torch_cls = optim_cls
         sgd = self._kind == _lib.OPT_SGD
         any_mom = any(g.get("momentum", 0) != 0 for g in probe.param_groups)
+        ada = self._kind == _ADAFACTOR
+        if ada and engine.world > 1:
+            # Adafactor's per-parameter reductions need whole parameters on one rank: its state is replicated (also under
+            # fairscale_oss) and every rank runs the same deterministic step on the same all-reduced fp32 gradients
+            route = "allreduce"
         self.path = GradPath(engine, params, grad_accum=grad_accum, clip=clip, sharded=sharded, lp_dtype=lp_dtype,
-                             module=module, needs_second_moment=not sgd, needs_first_moment=(not sgd) or any_mom,
-                             state_id=state_id, route=route, group_of=group_of, bucket_mb=bucket_mb,
-                             mu_product=self._kind == _lib.OPT_NADAM)
+                             module=module, needs_second_moment=not (sgd or ada),
+                             needs_first_moment=not (sgd or ada) or any_mom, state_id=state_id, route=route,
+                             group_of=group_of, bucket_mb=bucket_mb, mu_product=self._kind == _lib.OPT_NADAM,
+                             adafactor=ada)
         by_group: List[List[torch.nn.Parameter]] = [[] for _ in extra]
         for p, gi in zip(params, group_of):
             by_group[gi].append(p)
@@ -121,6 +142,16 @@ class B200FusedOptimizer(torch.optim.Optimizer):
         engine.scaler_set(state=self.path.state_id, opt_steps=0, skipped_steps=0, found_inf=0, growth_tracker=0)
 
     # -- the step -------------------------------------------------------------------------------------------------------
+    @staticmethod
+    def _adafactor_hyper_of(g) -> _lib.AdafactorHyper:
+        h = _lib.AdafactorHyper()
+        eps1, eps2 = g["eps"]
+        h.lr, h.beta2_decay, h.eps2, h.d = float(g["lr"]), float(g["beta2_decay"]), float(eps2), float(g["d"])
+        h.weight_decay = float(g["weight_decay"])
+        h.eps1_none, h.eps1 = int(eps1 is None), float(eps1 if eps1 is not None else 0.0)
+        h.maximize = int(bool(g.get("maximize", False)))
+        return h
+
     def _hyper_of(self, g) -> _lib.OptimHyper:
         h = _lib.OptimHyper()
         h.kind = self._kind
@@ -157,6 +188,9 @@ class B200FusedOptimizer(torch.optim.Optimizer):
     def step(self, closure=None):
         if closure is not None:
             raise NotImplementedError("Stoke -- closures are not supported by the fused step")
+        if self._kind == _ADAFACTOR:
+            self.path.adafactor_step([self._adafactor_hyper_of(g) for g in self.param_groups])
+            return
         self.path.optimizer_step(self._hypers(), self._exts())
 
     def zero_grad(self, set_to_none: bool = True):
@@ -181,8 +215,51 @@ class B200FusedOptimizer(torch.optim.Optimizer):
             return None
         return self.path._gather_shards(flat) if self.path.sharded else flat
 
+    def _groups_sd(self):
+        groups, start = [], 0
+        for g in self.param_groups:
+            d = {k: val for k, val in g.items() if k != "params"}
+            d["params"] = list(range(start, start + len(g["params"])))
+            start += len(g["params"])
+            groups.append(d)
+        return groups
+
+    def _adafactor_state_dict(self):
+        """torch's format: a parameter that was never stepped has no entry (torch creates its state at its first gradient)."""
+        path = self.path
+        st = path.engine.scaler_get(path.state_id)
+        steps = path.param_steps()
+        state = {}
+        for i, views in enumerate(path.adafactor_state_views()):
+            if steps[i] == 0:
+                continue
+            keys = ("row_var", "col_var") if len(views) == 2 else ("variance",)
+            state[self._sd_index[i]] = dict({"step": torch.tensor(float(steps[i]))},
+                                            **{k: v.clone() for k, v in zip(keys, views)})
+        return {"state": state, "param_groups": self._groups_sd(), "b200_master": path.gather_master(),
+                "b200_opt_steps": int(st.opt_steps)}
+
+    def _adafactor_load_state_dict(self, sd):
+        path = self.path
+        dev = path.p_flat.device
+        state = sd["state"]
+        steps = []
+        for i, views in enumerate(path.adafactor_state_views()):
+            src = state.get(self._sd_index[i], {})
+            keys = ("row_var", "col_var") if len(views) == 2 else ("variance",)
+            for k, v in zip(keys, views):
+                if k in src:
+                    v.copy_(src[k].to(device=dev, dtype=torch.float32).reshape(v.shape))
+                else:
+                    v.zero_()
+            steps.append(int(float(src["step"])) if "step" in src else 0)
+        path._range_steps.copy_(torch.tensor(steps, dtype=torch.int32))
+        return int(sd.get("b200_opt_steps", max(steps)))
+
     def state_dict(self):
         path = self.path
+        if self._kind == _ADAFACTOR:
+            return self._adafactor_state_dict()
         st = path.engine.scaler_get(path.state_id)
         m, v, master = self._full(path.m_flat), self._full(path.v_flat), path.gather_master()
         state = {}
@@ -202,13 +279,8 @@ class B200FusedOptimizer(torch.optim.Optimizer):
                     state[j]["mu_product"] = torch.tensor(mus[i], dtype=torch.float32)
                 state[j][k_m] = ms[i].clone()
                 state[j][k_v] = vs[i].clone()
-        groups, start = [], 0
-        for g in self.param_groups:
-            d = {k: val for k, val in g.items() if k != "params"}
-            d["params"] = list(range(start, start + len(g["params"])))
-            start += len(g["params"])
-            groups.append(d)
-        return {"state": state, "param_groups": groups, "b200_master": master, "b200_opt_steps": int(st.opt_steps)}
+        return {"state": state, "param_groups": self._groups_sd(), "b200_master": master,
+                "b200_opt_steps": int(st.opt_steps)}
 
     def load_state_dict(self, sd):
         """Accepts this class's own export and a plain ``torch.optim`` state dict written by the reference
@@ -223,6 +295,8 @@ class B200FusedOptimizer(torch.optim.Optimizer):
         dev = path.p_flat.device
         n = len(path.params)
         state = sd["state"]
+        if self._kind == _ADAFACTOR:
+            steps = self._adafactor_load_state_dict(sd)
 
         def put(local_dst, key):
             if local_dst is None:
@@ -235,7 +309,9 @@ class B200FusedOptimizer(torch.optim.Optimizer):
                     views[i].copy_(src.to(device=dev, dtype=torch.float32))
             path.scatter_local(full, local_dst)
 
-        if self._kind == _lib.OPT_SGD:
+        if self._kind == _ADAFACTOR:
+            pass
+        elif self._kind == _lib.OPT_SGD:
             put(path.m_flat, "momentum_buffer")
         else:
             k_m, k_v = _STATE_KEYS[self._kind]
