@@ -1,16 +1,18 @@
 # -*- coding: utf-8 -*-
-"""NAdam, RAdam and Adamax on the fused step, on one GPU, at ResNet-50 size (25.6 M elements) and BERT-base size
-(109.5 M elements), with Adam as the yardstick:
+"""torch.optim classes on the fused step, on one GPU, at ResNet-50 size (25.6 M elements) and BERT-base size
+(109.5 M elements), with Adam as the yardstick.  By default Adam, NAdam, RAdam and Adamax; ``--kinds`` picks others, e.g.
+``--kinds adadelta,rprop,asgd``:
 
   k_optim_step[raw]    the world-1 route: the step reads and zeroes the raw bf16 bucket and writes the bf16 model copy
                        (30 B/element algorithmic: read g 2, p m v 12; write p m v 12, bf16 copy 2, zeroing 2), with the
-                       step prologue in front of it
-  k_optim_step[main]   fp32 model, fp32 main gradients (28 B/element: read g p m v 16, write p m v 12)
+                       step prologue in front of it.  ASGD keeps one state tensor and, while mu == 1 (torch's default
+                       t0 = 1e6), writes it without reading it: 18 B/element
+  k_optim_step[main]   fp32 model, fp32 main gradients (28 B/element: read g p m v 16, write p m v 12; ASGD 16)
   optimizer step       gradient pass + step, the fused route (k_grad_norm + prologue + k_optim_step) against
                        B200StockOptimizer (K1 main-gradient reduce + the class's own torch update on fp32 views + the cast
                        into the bf16 model), same class, same gradients, timed in alternating rounds in the same run
 
-    python bench_optim.py [--out optim.json] [--iters 30]
+    python bench_optim.py [--out optim.json] [--iters 30] [--kinds adam,nadam,radam,adamax]
 
 Timing as bench_kernels.py: CUDA events on the launch stream, medians; ResNet-50-sized kernel rows are preceded by an L2 flush
 write.  The card's name and power limit are read in the same run and written with the numbers.
@@ -38,12 +40,24 @@ def card():
     return info
 
 
+CLASSES = {"adam": (torch.optim.Adam, {"lr": 1e-3}), "nadam": (torch.optim.NAdam, {"lr": 2e-3}),
+           "radam": (torch.optim.RAdam, {"lr": 1e-3}), "adamax": (torch.optim.Adamax, {"lr": 2e-3}),
+           "adadelta": (torch.optim.Adadelta, {"lr": 1.0}), "rprop": (torch.optim.Rprop, {"lr": 1e-2}),
+           "asgd": (torch.optim.ASGD, {"lr": 1e-2})}
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--out", default=None)
     ap.add_argument("--iters", type=int, default=30)
     ap.add_argument("--rounds", type=int, default=4)
+    ap.add_argument("--kinds", default="adam,nadam,radam,adamax",
+                    help="comma-separated: " + ",".join(CLASSES))
     args = ap.parse_args()
+    kinds = [k.strip() for k in args.kinds.split(",") if k.strip()]
+    unknown = [k for k in kinds if k not in CLASSES]
+    if unknown:
+        raise SystemExit(f"bench_optim.py: unknown kinds {unknown} (known: {', '.join(CLASSES)})")
     if not torch.cuda.is_available():
         raise SystemExit("bench_optim.py needs a GPU")
     from stoke_b200 import _lib
@@ -80,14 +94,14 @@ def main():
             super().__init__()
             self.w = torch.nn.Parameter(torch.zeros(n))
 
-    classes = (("adam", torch.optim.Adam, {"lr": 1e-3}), ("nadam", torch.optim.NAdam, {"lr": 2e-3}),
-               ("radam", torch.optim.RAdam, {"lr": 1e-3}), ("adamax", torch.optim.Adamax, {"lr": 2e-3}))
+    classes = [(k,) + CLASSES[k] for k in kinds]
     clip = ClipSpec(_lib.CLIP_NORM, max_norm=1.0, norm_type=2.0)
     for size_name, n in (("resnet50_25.6M", 25_557_032), ("bert_base_109.5M", 109_483_778)):
         flush_l2 = n < 60_000_000
         for tag, cls, kw in classes:
             # ---- the kernel alone, both gradient sources ----
-            for route, lp, per in (("local", torch.bfloat16, 30), ("main", None, 28)):
+            one_state = tag == "asgd"   # one state tensor, written without being read while mu == 1
+            for route, lp, per in (("local", torch.bfloat16, 18 if one_state else 30), ("main", None, 16 if one_state else 28)):
                 net = Flat(n).cuda()
                 opt = B200FusedOptimizer(net, cls, kw, engine=eng, route=route, clip=clip, lp_dtype=lp)
                 path = opt.path

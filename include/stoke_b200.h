@@ -35,6 +35,7 @@
  *   stk_optim_range_prologue         torch's per-parameter `state[p]["step"]` (torch/optim/adam.py: a parameter whose grad is None
  *                                    is not stepped and keeps its own count) for models with sometimes-unused parameters
  *   stk_optim_step_prologue          the same for every kind, plus NAdam's `state[p]["mu_product"]` (torch/optim/nadam.py)
+ *                                    and ASGD's `state[p]["eta"]` / `["mu"]` (torch/optim/asgd.py) without `.item()`
  *   stk_adafactor_plan / _step       torch.optim.Adafactor's step (torch/optim/_adafactor.py _single_tensor_adafactor) plus
  *                                    the clip and the GradScaler.step gate, without its two .item() per parameter
  */
@@ -75,7 +76,10 @@ typedef enum {
   STK_OPT_ADAM = 0, STK_OPT_ADAMW = 1, STK_OPT_SGD = 2,
   STK_OPT_NADAM = 3,   /* torch.optim.NAdam (torch/optim/nadam.py, _single_tensor_nadam) */
   STK_OPT_RADAM = 4,   /* torch.optim.RAdam (torch/optim/radam.py, _single_tensor_radam) */
-  STK_OPT_ADAMAX = 5   /* torch.optim.Adamax (torch/optim/adamax.py, _single_tensor_adamax); exp_avg_sq holds exp_inf */
+  STK_OPT_ADAMAX = 5,  /* torch.optim.Adamax (torch/optim/adamax.py, _single_tensor_adamax); exp_avg_sq holds exp_inf */
+  STK_OPT_ADADELTA = 6,  /* torch.optim.Adadelta (_single_tensor_adadelta); exp_avg = square_avg, exp_avg_sq = acc_delta */
+  STK_OPT_RPROP = 7,   /* torch.optim.Rprop (_single_tensor_rprop); exp_avg = prev, exp_avg_sq = step_size */
+  STK_OPT_ASGD = 8     /* torch.optim.ASGD (_single_tensor_asgd); exp_avg = ax, no exp_avg_sq */
 } stk_optim_kind;
 
 /* flags of stk_grad_reduce */
@@ -117,11 +121,16 @@ typedef struct {
   double clip_value;      /* STK_CLIP_VALUE */
 } stk_optim_hyper_t;
 
-/* Per-group hyper-parameters of the NAdam / RAdam kinds that stk_optim_hyper_t has no field for (one entry per group,
- * same order as the stk_optim_hyper_t array).  A NULL array means every field is 0. */
+/* Per-group hyper-parameters of the kinds after SGD that stk_optim_hyper_t has no field for (one entry per group, same
+ * order as the stk_optim_hyper_t array).  A NULL array means every field is 0.  stk_optim_hyper_t's lr, eps, weight_decay
+ * and maximize apply to every kind that has them (Adadelta: lr, eps, weight_decay; Rprop: lr; ASGD: lr, weight_decay). */
 typedef struct {
   double momentum_decay;        /* NAdam: momentum_decay (psi): mu_t = beta1 (1 - 0.5 * 0.96^(t psi)), torch/optim/nadam.py */
   int decoupled_weight_decay;   /* NAdam / RAdam: 1 = param *= 1 - lr wd before the update (AdamW-style); 0 = L2, grad += wd param */
+  double rho;                   /* Adadelta: rho */
+  double etaminus, etaplus;     /* Rprop: etas */
+  double step_size_min, step_size_max;  /* Rprop: step_sizes */
+  double lambd, alpha, t0;      /* ASGD */
 } stk_optim_hyper_ext_t;
 
 /* ---- library / context -------------------------------------------------------------------------------------------- */
@@ -270,11 +279,12 @@ typedef struct {
                              which writes it for every kind): per-PARAMETER step counts (torch keeps `step` per parameter, so a
                              parameter that skipped some steps has its own bias corrections); NULL: the optimizer-wide
                              counter of the selected state is used for every range */
-  const stk_optim_hyper_ext_t* hyper_ext;  /* n_groups entries or NULL (all zero): NAdam / RAdam extras */
+  const stk_optim_hyper_ext_t* hyper_ext;  /* n_groups entries or NULL (all zero): the extras of the kinds after SGD */
   const float* group_bc;  /* DEVICE, 4 floats per GROUP written by stk_optim_step_prologue with n_ranges = 0; used where
-                             range_bc is NULL.  NADAM / RADAM / ADAMAX need group_bc or range_bc: their per-step scalars
-                             (NAdam's come from mu_product, which only the prologue advances) are formed once by the
-                             prologue, not in every block.  Ignored by ADAM / ADAMW / SGD */
+                             range_bc is NULL.  Every kind after SGD needs group_bc or range_bc: their per-step scalars
+                             (NAdam's and ASGD's come from scalar state that only the prologue advances) are formed once
+                             by the prologue, not in every block.  Ignored by ADAM / ADAMW / SGD.  ASGD takes no
+                             exp_avg_sq */
 } stk_optim_args_t;
 int stk_optim_step_ex(stk_ctx* ctx, const stk_optim_args_t* args, void* stream);
 /* Per-range step bookkeeping for stk_optim_step_ex (call it right before, same stream): for every range j computes the
@@ -283,12 +293,13 @@ int stk_optim_step_ex(stk_ctx* ctx, const stk_optim_args_t* args, void* stream);
  * All three arrays live in device memory. */
 int stk_optim_range_prologue(stk_ctx* ctx, const stk_optim_hyper_t* hyper, int n_groups, int n_ranges,
                              const uint8_t* range_group, int32_t* range_steps, float* range_bc, void* stream);
-/* Step bookkeeping for every kind, NAdam's mu_product included (call it right before stk_optim_step_ex, same stream).
+/* Step bookkeeping for every kind, including the per-entry scalar state of NAdam and ASGD (call it right before
+ * stk_optim_step_ex, same stream).
  * n_ranges > 0: per range j, like stk_optim_range_prologue: the scalars of step t = range_steps[j] + 1 with the group
  *   hyper[range_group[j] & 0x7f] go to bc[4j..4j+3] (pass bc as the step's range_bc), and unless bit 7 is set or the
- *   selected state says found_inf, range_steps[j] and mu_product[j] advance.
+ *   selected state says found_inf, range_steps[j] and entry j's scalar state advance.
  * n_ranges = 0: per group g, with t = the selected state's optimizer-wide counter + 1: bc[4g..4g+3] (pass bc as the
- *   step's group_bc) and, unless found_inf, mu_product[g] advances.  range_group and range_steps are not read.
+ *   step's group_bc) and, unless found_inf, entry g's scalar state advances.  range_group and range_steps are not read.
  * The four floats per entry, computed in double from torch's python-scalar formulas and stored as fp32:
  *   ADAM / ADAMW / SGD: {lr / bc1, sqrt(bc2), t == 1, 0}     (the values stk_optim_range_prologue writes)
  *   NADAM:  {c_g, c_m, bc2, 0}: param += c_g grad / denom + c_m exp_avg / denom, denom = sqrt(exp_avg_sq / bc2) + eps,
@@ -298,8 +309,14 @@ int stk_optim_range_prologue(stk_ctx* ctx, const stk_optim_hyper_t* hyper, int n
  *           c = lr rect sqrt(bc2) / bc1, param -= c exp_avg / (sqrt(exp_avg_sq) + eps); else rectified = 0,
  *           c = lr / bc1, param -= c exp_avg
  *   ADAMAX: {lr / bc1, 0, 0, 0}: param -= (lr / bc1) exp_avg / exp_inf
- * with bc1 = 1 - beta1^t, bc2 = 1 - beta2^t.  mu_product (fp32, one per range or per group, torch initialises it to 1)
- * is read and written only for STK_OPT_NADAM and may be NULL for the other kinds; hyper_ext may be NULL (all zero).
+ *   ADADELTA, RPROP: {0, 0, t == 1, 0}: Rprop's first step seeds step_size with the lr passed now (torch: full_like(p, lr)
+ *           at the parameter's first step) and takes prev as 0; the exp_avg_sq buffer is not used then
+ *   ASGD:   {-eta, 1 - lambd eta, mu, 0} with the STORED fp32 eta and mu (the lr and 1 at t == 1, torch's lazy
+ *           initialisation): param = param (1 - lambd eta) - eta grad; ax = param if mu == 1 (ax not read), else
+ *           ax + (param - ax) mu.  Then eta = lr / (1 + lambd lr t)^alpha and mu = 1 / max(1, t - t0), as fp32
+ * with bc1 = 1 - beta1^t, bc2 = 1 - beta2^t.  The scalar state `mu_product` (fp32, torch keeps it per parameter) holds per
+ * range or per group: NADAM one float, mu_product (torch initialises it to 1); ASGD two floats, {eta, mu}.  It is read and
+ * written only for those two kinds and may be NULL for the others; hyper_ext may be NULL (all zero).
  * All pointers but hyper / hyper_ext are device memory; bc must be 16-byte aligned. */
 int stk_optim_step_prologue(stk_ctx* ctx, const stk_optim_hyper_t* hyper, const stk_optim_hyper_ext_t* hyper_ext,
                             int n_groups, int n_ranges, const uint8_t* range_group, int32_t* range_steps,

@@ -15,6 +15,7 @@ REDUCE_ALL, REDUCE_SCATTER = 0, 1
 NORM_NONE, NORM_L2, NORM_INF, NORM_P = 0, 1, 2, 3
 CLIP_NONE, CLIP_NORM, CLIP_VALUE = 0, 1, 2
 OPT_ADAM, OPT_ADAMW, OPT_SGD, OPT_NADAM, OPT_RADAM, OPT_ADAMAX = 0, 1, 2, 3, 4, 5
+OPT_ADADELTA, OPT_RPROP, OPT_ASGD = 6, 7, 8
 RF_FINAL, RF_ZERO_INPUT, RF_UNSCALE = 1, 2, 4
 OPT_K1_ALGO, OPT_MEM_MODE, OPT_K1_MAX_BLOCKS, OPT_COOP_LAUNCH, OPT_NVLS_MAX_BLOCKS, OPT_K2_AG_MC = 1, 2, 3, 4, 5, 6
 K1_ALGO_LDG, K1_ALGO_BULK, K1_ALGO_NVLS = 0, 1, 2
@@ -49,7 +50,9 @@ class OptimHyper(C.Structure):
 
 
 class OptimHyperExt(C.Structure):
-    _fields_ = [("momentum_decay", C.c_double), ("decoupled_weight_decay", C.c_int)]
+    _fields_ = [("momentum_decay", C.c_double), ("decoupled_weight_decay", C.c_int), ("rho", C.c_double),
+                ("etaminus", C.c_double), ("etaplus", C.c_double), ("step_size_min", C.c_double),
+                ("step_size_max", C.c_double), ("lambd", C.c_double), ("alpha", C.c_double), ("t0", C.c_double)]
 
 
 class OptimArgs(C.Structure):

@@ -1,12 +1,14 @@
-// k2_optim.cu -- K2: single-pass fused optimizer step (Adam / AdamW / SGD-momentum / NAdam / RAdam / Adamax), plus the
-// step prologue (per-parameter step counts, NAdam's mu_product) and epilogue.
+// k2_optim.cu -- K2: single-pass fused optimizer step (Adam / AdamW / SGD-momentum / NAdam / RAdam / Adamax / Adadelta /
+// Rprop / ASGD), plus the step prologue (per-parameter step counts, NAdam's mu_product, ASGD's eta and mu) and epilogue.
 //
 // One sweep over (grad, master, exp_avg, exp_avg_sq) does what the reference spreads over clip_grad_norm_'s scaling pass /
 // clip_grad_value_, GradScaler.step's inf gate, the ~7 foreach kernels of torch.optim.Adam and (mixed precision) the
 // fp32 -> bf16 parameter cast; in sharded (OSS / ZeRO-1) mode the updated low-precision shard is stored straight into
 // every rank's parameter buffer, which is the parameter all-gather (K3).  HBM bytes per element: read g,p,m,v (16) +
-// write p,m,v (12) [+ 2 for the bf16 copy] = 28 / 30, for every kind but SGD (NAdam, RAdam and Adamax keep two fp32 state
-// tensors like Adam; Adamax's exp_inf lives in the exp_avg_sq buffer).  The clip coefficient, the skip decision and the bias corrections
+// write p,m,v (12) [+ 2 for the bf16 copy] = 28 / 30, for every kind but SGD and ASGD (NAdam, RAdam, Adamax, Adadelta and
+// Rprop keep two fp32 state tensors like Adam; Adamax's exp_inf, Adadelta's acc_delta and Rprop's step_size live in the
+// exp_avg_sq buffer).  ASGD keeps one (ax, in exp_avg): read g,p,ax + write p,ax = 20 / 22, and 16 / 18 while mu == 1,
+// when ax is written without being read.  The clip coefficient, the skip decision and the bias corrections
 // come from device memory, so there is no host synchronisation anywhere on the step.
 //
 // Gradient sources:  MAIN  -- fp32 reduced / unscaled gradients written by K1 (cross-rank routes), indexed like the state;
@@ -18,8 +20,9 @@
 // parameters that received no gradient this step (torch skips `p.grad is None`, torch/optim/optimizer.py).
 //
 // Arithmetic follows torch/optim/adam.py (_single_tensor_adam, the path torch takes on CPU -- the oracle),
-// torch/optim/sgd.py (_single_tensor_sgd), nadam.py (_single_tensor_nadam), radam.py (_single_tensor_radam) and adamax.py
-// (_single_tensor_adamax); the clip follows torch/nn/utils/clip_grad.py:165-174 (coef = max_norm /
+// torch/optim/sgd.py (_single_tensor_sgd), nadam.py (_single_tensor_nadam), radam.py (_single_tensor_radam), adamax.py
+// (_single_tensor_adamax), adadelta.py (_single_tensor_adadelta), rprop.py (_single_tensor_rprop) and asgd.py
+// (_single_tensor_asgd); the clip follows torch/nn/utils/clip_grad.py:165-174 (coef = max_norm /
 // (total_norm + 1e-6), clamped to 1) and :291-292 (clamp).
 #include <cstdlib>
 
@@ -32,12 +35,17 @@ struct GroupHyperD {   // host-side doubles, converted exactly like torch conver
   int nesterov, maximize;
   double momentum_decay;  // NAdam
   int decoupled;          // NAdam / RAdam: decoupled weight decay
+  double rho;                                    // Adadelta
+  double etaminus, etaplus, step_size_min, step_size_max;  // Rprop
+  double lambd, alpha, t0;                       // ASGD
 };
 struct GroupHyperS {   // what the inner loop reads (shared memory, one entry per parameter group)
   float step_size, bc2_sqrt, b2, eps, wd, one_m_b1, one_m_b2, lr, one_m_damp, decay_mul, mom;
   int nesterov, maximize;
-  float c0, c1, c2;  // NAdam / RAdam / Adamax: the per-step scalars (layout of stk_optim_step_prologue)
+  float c0, c1, c2;  // the kinds of stk_optim_step_prologue: the per-step scalars (its layout)
   int decoupled;
+  float rho, one_m_rho;                         // Adadelta
+  float etaminus, etaplus, ss_min, ss_max;      // Rprop
 };
 
 struct OptimParams {
@@ -74,19 +82,38 @@ struct OptimParams {
   const float4* group_bc;                    // device: per-group scalars of the NAdam / RAdam / Adamax kinds
 };
 
-__host__ __device__ constexpr bool is_new_kind(int kind) { return kind == STK_OPT_NADAM || kind == STK_OPT_RADAM || kind == STK_OPT_ADAMAX; }
+// the kinds whose per-step scalars come from stk_optim_step_prologue (group_bc / range_bc), not from the kernel itself
+__host__ __device__ constexpr bool is_new_kind(int kind) { return kind >= STK_OPT_NADAM && kind <= STK_OPT_ASGD; }
+// floats of per-entry scalar state the prologue carries (the stk_optim_step_prologue `mu_product` array)
+__host__ __device__ constexpr int scalar_state_width(int kind) {
+  return kind == STK_OPT_NADAM ? 1 : (kind == STK_OPT_ASGD ? 2 : 0);
+}
 
-// Per-step scalars of the NAdam / RAdam / Adamax update of step t (the float4 layout documented at stk_optim_step_prologue),
-// in double from the python-scalar formulas of torch's single-tensor functions.  *mu_prod: NAdam's mu_product before the
-// step on entry, after it on return (fp32, like torch's tensor).
-__device__ __forceinline__ float4 new_kind_scalars(int kind, const GroupHyperD& h, double t, float* mu_prod) {
+// Per-step scalars of the update of step t of the prologue's kinds (the float4 layout documented at
+// stk_optim_step_prologue), in double from the python-scalar formulas of torch's single-tensor functions.  st: the entry's
+// scalar state before the step on entry, after it on return (fp32, like torch's tensors): NAdam's mu_product; ASGD's
+// {eta, mu}.
+__device__ __forceinline__ float4 new_kind_scalars(int kind, const GroupHyperD& h, double t, float* st) {
+  if (kind == STK_OPT_ADADELTA || kind == STK_OPT_RPROP)  // Rprop: step_size = full_like(p, lr) at the first step
+    return make_float4(0.f, 0.f, t == 1.0 ? 1.f : 0.f, 0.f);
+  if (kind == STK_OPT_ASGD) {  // torch/optim/asgd.py: the update uses the STORED eta and mu, then both advance
+    float eta = st[0], mu = st[1];
+    if (t == 1.0) {  // lazy state initialisation: eta = lr (fp32 tensor), mu = 1
+      eta = (float)h.lr;
+      mu = 1.f;
+    }
+    const float4 o = make_float4(-eta, (float)(1.0 - h.lambd * (double)eta), mu, 0.f);
+    st[0] = (float)(h.lr / pow(1.0 + h.lambd * h.lr * t, h.alpha));  // lr / ((1 + lambd lr step) ** alpha)
+    st[1] = (float)(t - h.t0 > 1.0 ? 1.0 / (t - h.t0) : 1.0);      // 1 / max(1, step - t0)
+    return o;
+  }
   const double bc1 = 1.0 - pow(h.beta1, t);
   const double bc2 = 1.0 - pow(h.beta2, t);
   if (kind == STK_OPT_NADAM) {  // torch/optim/nadam.py: mu, mu_next, mu_product *= mu, the two addcdiv_ values
     const double mu = h.beta1 * (1.0 - 0.5 * pow(0.96, t * h.momentum_decay));
     const double mu_next = h.beta1 * (1.0 - 0.5 * pow(0.96, (t + 1.0) * h.momentum_decay));
-    const float prod = __fmul_rn(*mu_prod, (float)mu);  // fp32 tensor times a python float
-    *mu_prod = prod;
+    const float prod = __fmul_rn(*st, (float)mu);  // fp32 tensor times a python float
+    *st = prod;
     const double prod_next = (double)prod * mu_next;
     return make_float4((float)(-h.lr * (1.0 - mu) / (1.0 - (double)prod)), (float)(-h.lr * mu_next / (1.0 - prod_next)),
                        (float)bc2, 0.f);
@@ -168,8 +195,11 @@ __device__ __forceinline__ void store_lp(const OptimParams& p, size_t gv, const 
 // PERSIST = false: one-shot launch, VPT vectors per thread (local step; tools/membench.cu compares it with a persistent
 // grid-stride loop).  PERSIST = true: co-resident grid-stride loop, required when the kernel
 // pushes its shard to peers and therefore carries the cross-rank block barriers (sharded / OSS step).
+// ASGD asks for two co-resident blocks per SM: left to itself, ptxas caps its paired sharded form at 80 registers and
+// spills (its conditional ax load); with the bound it takes 84 and none spills.  A minimum of 0 is no minimum: the other
+// kinds compile exactly as with __launch_bounds__(256).
 template <int KIND, int LP_DT, bool PERSIST, int VPT, int GRAD, bool RAW>
-__global__ void __launch_bounds__(256) k_optim_step(const OptimParams p) {
+__global__ void __launch_bounds__(256, KIND == STK_OPT_ASGD ? 2 : 0) k_optim_step(const OptimParams p) {
   __shared__ GroupHyperS s_g[STK_MAX_GROUPS];
   __shared__ int s_skip, s_first;
   __shared__ float s_inv_scale;
@@ -178,6 +208,7 @@ __global__ void __launch_bounds__(256) k_optim_step(const OptimParams p) {
   if (PERSIST && p.prof_ns && blockIdx.x == 0 && threadIdx.x == 0) t_begin = globaltimer_ns();
 
   const bool use_m = (KIND != STK_OPT_SGD) || p.m != nullptr;
+  constexpr bool kHasV = KIND != STK_OPT_SGD && KIND != STK_OPT_ASGD;  // ASGD: one state tensor (ax, in p.m)
   const size_t stride = PERSIST ? size_t(gridDim.x) * blockDim.x * VPT : 0;
   size_t i = (size_t(blockIdx.x) * blockDim.x + threadIdx.x) * VPT;
 
@@ -196,8 +227,8 @@ __global__ void __launch_bounds__(256) k_optim_step(const OptimParams p) {
         if constexpr (RAW) InVec<GRAD>::load(p.grad, gv + k, g[k]);
         else InVec<STK_F32>::load(p.grad, i + k, g[k]);
         InVec<STK_F32>::load(p.master, i + k, w[k]);
-        if (use_m) InVec<STK_F32>::load(p.m, i + k, m[k]);
-        if (KIND != STK_OPT_SGD) InVec<STK_F32>::load(p.v, i + k, v[k]);
+        if (use_m && KIND != STK_OPT_ASGD) InVec<STK_F32>::load(p.m, i + k, m[k]);  // ASGD: ax only when mu != 1
+        if (kHasV) InVec<STK_F32>::load(p.v, i + k, v[k]);
       }
     if constexpr (RAW) {
       if (p.acc != nullptr) {
@@ -251,6 +282,16 @@ __global__ void __launch_bounds__(256) k_optim_step(const OptimParams p) {
       o.c2 = c.z;
     }
     o.decoupled = h.decoupled;
+    if constexpr (KIND == STK_OPT_ADADELTA) {
+      o.rho = (float)h.rho;
+      o.one_m_rho = (float)(1.0 - h.rho);
+    }
+    if constexpr (KIND == STK_OPT_RPROP) {
+      o.etaminus = (float)h.etaminus;
+      o.etaplus = (float)h.etaplus;
+      o.ss_min = (float)h.step_size_min;
+      o.ss_max = (float)h.step_size_max;
+    }
     s_g[threadIdx.x] = o;
   }
   __syncthreads();
@@ -289,6 +330,9 @@ __global__ void __launch_bounds__(256) k_optim_step(const OptimParams p) {
 #pragma unroll
       for (int k = 0; k < VPT; ++k) {
         if (k >= nv) continue;
+        if constexpr (KIND == STK_OPT_ASGD) {  // ax is only read when it is averaged (torch: mu.item() != 1)
+          if (h.c2 != 1.f) InVec<STK_F32>::load(p.m, i + k, m[k]);
+        }
 #pragma unroll
         for (int e = 0; e < 8; ++e) {
           float gg = g[k][e];
@@ -340,6 +384,37 @@ __global__ void __launch_bounds__(256) k_optim_step(const OptimParams p) {
             ww = ww - h.c0 * (mm / uu);                              // addcdiv_(exp_avg, exp_inf, value=-clr)
             m[k][e] = mm;
             v[k][e] = uu;
+          } else if (KIND == STK_OPT_ADADELTA) {
+            if (h.wd != 0.f) gg = fmaf(ww, h.wd, gg);               // grad.add(param, alpha=wd)
+            const float sq = fmaf(h.one_m_rho * gg, gg, m[k][e] * h.rho);  // square_avg.mul_(rho).addcmul_(g, g, 1-rho)
+            // delta = acc_delta.add(eps).sqrt_().div_(square_avg.add(eps).sqrt_()).mul_(grad)
+            const float dl = sqrtf(v[k][e] + h.eps) / sqrtf(sq + h.eps) * gg;
+            v[k][e] = fmaf(h.one_m_rho * dl, dl, v[k][e] * h.rho);  // acc_delta.mul_(rho).addcmul_(delta, delta, 1-rho)
+            m[k][e] = sq;
+            ww = fmaf(-h.lr, dl, ww);                                // param.add_(delta, alpha=-lr)
+          } else if (KIND == STK_OPT_RPROP) {
+            // first step: prev = zeros, step_size = full_like(p, lr) with the lr in force now; V is not used then
+            const bool first = h.c2 != 0.f;
+            const float prev = first ? 0.f : m[k][e];
+            float ss = first ? h.lr : v[k][e];
+            const float x = gg * prev;                               // grad.mul(prev).sign(): the fp32 product's sign
+            float f = (float)((x > 0.f) - (x < 0.f));                // torch.sign: NaN and +-0 give 0
+            if (f > 0.f) f = h.etaplus;                              // sign[sign.gt(0)] = etaplus
+            if (f < 0.f) f = h.etaminus;                             // sign[sign.lt(0)] = etaminus
+            if (f == 0.f) f = 1.f;                                   // sign[sign.eq(0)] = 1
+            ss = ss * f;                                             // step_size.mul_(sign).clamp_(min, max), NaN kept
+            ss = ss < h.ss_min ? h.ss_min : ss;
+            ss = ss > h.ss_max ? h.ss_max : ss;
+            if (f == h.etaminus) gg = 0.f;                           // grad[sign.eq(etaminus)] = 0
+            const float sg = (float)((gg > 0.f) - (gg < 0.f));
+            ww = ww - sg * ss;                                       // param.addcmul_(grad.sign(), step_size, value=-1)
+            m[k][e] = gg;                                            // prev.copy_(grad)
+            v[k][e] = ss;
+          } else if (KIND == STK_OPT_ASGD) {
+            if (h.wd != 0.f) gg = fmaf(ww, h.wd, gg);               // grad.add(param, alpha=wd)
+            ww = fmaf(h.c0, gg, __fmul_rn(ww, h.c1));                // param.mul_(1 - lambd eta).add_(grad, alpha=-eta)
+            // ax.add_(param.sub(ax).mul_(mu)), or ax.copy_(param) while mu == 1
+            m[k][e] = h.c2 == 1.f ? ww : __fadd_rn(m[k][e], __fmul_rn(ww - m[k][e], h.c2));
           } else {  // SGD
             if (h.wd != 0.f) gg = fmaf(ww, h.wd, gg);
             if (h.mom != 0.f) {
@@ -357,7 +432,7 @@ __global__ void __launch_bounds__(256) k_optim_step(const OptimParams p) {
         if (k < nv) {
           st_stream_f8(p.master + (i + k) * 8, w[k]);
           if (use_m && (KIND != STK_OPT_SGD || p.any_mom)) st_stream_f8(p.m + (i + k) * 8, m[k]);
-          if (KIND != STK_OPT_SGD) st_stream_f8(p.v + (i + k) * 8, v[k]);
+          if (kHasV) st_stream_f8(p.v + (i + k) * 8, v[k]);
         }
       store_lp<LP_DT, VPT>(p, gv, w, nv);
     }
@@ -416,7 +491,8 @@ struct StepPrologueParams {
 };
 
 // one thread per range (n_ranges > 0) or per group (n_ranges == 0): the scalars of that entry's NEXT step and, unless it is
-// skipped or the step is (found_inf), the advance of its step count and of NAdam's mu_product
+// skipped or the step is (found_inf), the advance of its step count and of its scalar state (NAdam's mu_product, ASGD's
+// eta and mu)
 __global__ void k_step_prologue(const StepPrologueParams p) {
   const int j = blockIdx.x * blockDim.x + threadIdx.x;
   const bool per_range = p.n_ranges > 0;
@@ -428,9 +504,12 @@ __global__ void k_step_prologue(const StepPrologueParams p) {
   const bool advance = !(b & 0x80u) && p.scaler->found_inf == 0;
   float4 o;
   if (is_new_kind(p.kind)) {
-    float mu = p.kind == STK_OPT_NADAM ? p.mu_product[j] : 1.f;
-    o = new_kind_scalars(p.kind, h, t, &mu);
-    if (p.kind == STK_OPT_NADAM && advance) p.mu_product[j] = mu;
+    const int w = scalar_state_width(p.kind);
+    float st[2] = {1.f, 1.f};
+    for (int k = 0; k < w; ++k) st[k] = p.mu_product[j * w + k];
+    o = new_kind_scalars(p.kind, h, t, st);
+    if (advance)
+      for (int k = 0; k < w; ++k) p.mu_product[j * w + k] = st[k];
   } else {  // the values of k_range_prologue
     o = make_float4(0.f, 1.f, done == 0 ? 1.f : 0.f, 0.f);
     if (p.kind != STK_OPT_SGD) {
@@ -478,6 +557,14 @@ static void fill_groups(GroupHyperD* o, const stk_optim_hyper_t* h, const stk_op
     o[gi].nesterov = h[gi].nesterov; o[gi].maximize = h[gi].maximize;
     o[gi].momentum_decay = ext ? ext[gi].momentum_decay : 0.0;
     o[gi].decoupled = ext ? (ext[gi].decoupled_weight_decay != 0) : 0;
+    o[gi].rho = ext ? ext[gi].rho : 0.0;
+    o[gi].etaminus = ext ? ext[gi].etaminus : 0.0;
+    o[gi].etaplus = ext ? ext[gi].etaplus : 0.0;
+    o[gi].step_size_min = ext ? ext[gi].step_size_min : 0.0;
+    o[gi].step_size_max = ext ? ext[gi].step_size_max : 0.0;
+    o[gi].lambd = ext ? ext[gi].lambd : 0.0;
+    o[gi].alpha = ext ? ext[gi].alpha : 0.0;
+    o[gi].t0 = ext ? ext[gi].t0 : 0.0;
   }
 }
 
@@ -535,11 +622,12 @@ int stk_optim_step_ex(stk_ctx* c, const stk_optim_args_t* a, void* stream) {
   STK_REQUIRE(c, a->n_groups >= 1 && a->n_groups <= STK_MAX_GROUPS, "stk_optim_step_ex: n_groups must be in [1, 8]");
   STK_REQUIRE(c, a->n_local % 8 == 0, "stk_optim_step_ex: n_local must be a multiple of 8");
   const stk_optim_hyper_t* h = a->hyper;
-  STK_REQUIRE(c, h->kind >= STK_OPT_ADAM && h->kind <= STK_OPT_ADAMAX, "stk_optim_step_ex: bad optimizer kind");
+  STK_REQUIRE(c, h->kind >= STK_OPT_ADAM && h->kind <= STK_OPT_ASGD, "stk_optim_step_ex: bad optimizer kind");
   STK_REQUIRE(c, h->kind <= STK_OPT_SGD || a->group_bc || (a->n_ranges > 0 && a->range_bc),
-              "stk_optim_step_ex: NAdam / RAdam / Adamax need the scalars of stk_optim_step_prologue (group_bc or range_bc)");
+              "stk_optim_step_ex: the kinds after SGD need the scalars of stk_optim_step_prologue (group_bc or range_bc)");
   STK_REQUIRE(c, (reinterpret_cast<uintptr_t>(a->group_bc) & 15) == 0, "stk_optim_step_ex: group_bc must be 16-byte aligned");
-  STK_REQUIRE(c, h->kind == STK_OPT_SGD || (a->exp_avg && a->exp_avg_sq), "stk_optim_step_ex: Adam needs exp_avg and exp_avg_sq");
+  STK_REQUIRE(c, h->kind == STK_OPT_SGD || (a->exp_avg && (a->exp_avg_sq || h->kind == STK_OPT_ASGD)),
+              "stk_optim_step_ex: this kind needs exp_avg and exp_avg_sq (ASGD: exp_avg)");
   bool any_mom = false;
   for (int gi = 0; gi < a->n_groups; ++gi) {
     STK_REQUIRE(c, h[gi].kind == h->kind, "stk_optim_step_ex: all groups must use the same optimizer kind");
@@ -646,6 +734,9 @@ int stk_optim_step_ex(stk_ctx* c, const stk_optim_args_t* a, void* stream) {
     case STK_OPT_NADAM: err = launch_optim<STK_OPT_NADAM>(c, p, a->lp_dtype, a->grad_dtype, raw, pair_ok, s); break;
     case STK_OPT_RADAM: err = launch_optim<STK_OPT_RADAM>(c, p, a->lp_dtype, a->grad_dtype, raw, pair_ok, s); break;
     case STK_OPT_ADAMAX: err = launch_optim<STK_OPT_ADAMAX>(c, p, a->lp_dtype, a->grad_dtype, raw, pair_ok, s); break;
+    case STK_OPT_ADADELTA: err = launch_optim<STK_OPT_ADADELTA>(c, p, a->lp_dtype, a->grad_dtype, raw, pair_ok, s); break;
+    case STK_OPT_RPROP: err = launch_optim<STK_OPT_RPROP>(c, p, a->lp_dtype, a->grad_dtype, raw, pair_ok, s); break;
+    case STK_OPT_ASGD: err = launch_optim<STK_OPT_ASGD>(c, p, a->lp_dtype, a->grad_dtype, raw, pair_ok, s); break;
     default: err = launch_optim<STK_OPT_SGD>(c, p, a->lp_dtype, a->grad_dtype, raw, pair_ok, s); break;
   }
   if (err == cudaErrorNotSupported)
@@ -681,7 +772,7 @@ int stk_optim_range_prologue(stk_ctx* c, const stk_optim_hyper_t* h, int n_group
   STK_REQUIRE(c, n_ranges >= 1, "stk_optim_range_prologue: no ranges");
   STK_REQUIRE(c, (reinterpret_cast<uintptr_t>(range_bc) & 15) == 0, "stk_optim_range_prologue: range_bc must be 16-byte aligned");
   STK_REQUIRE(c, h->kind >= STK_OPT_ADAM && h->kind <= STK_OPT_SGD,
-              "stk_optim_range_prologue: NAdam / RAdam / Adamax take stk_optim_step_prologue");
+              "stk_optim_range_prologue: the kinds after SGD take stk_optim_step_prologue");
   std::lock_guard<std::mutex> lk(c->mu);
   DeviceGuard g(c->device);
   RangePrologueParams p{};
@@ -704,8 +795,9 @@ int stk_optim_step_prologue(stk_ctx* c, const stk_optim_hyper_t* h, const stk_op
   STK_REQUIRE(c, n_groups >= 1 && n_groups <= STK_MAX_GROUPS, "stk_optim_step_prologue: n_groups must be in [1, 8]");
   STK_REQUIRE(c, n_ranges >= 0, "stk_optim_step_prologue: negative n_ranges");
   STK_REQUIRE(c, n_ranges == 0 || (range_group && range_steps), "stk_optim_step_prologue: range arrays are NULL");
-  STK_REQUIRE(c, h->kind >= STK_OPT_ADAM && h->kind <= STK_OPT_ADAMAX, "stk_optim_step_prologue: bad optimizer kind");
-  STK_REQUIRE(c, h->kind != STK_OPT_NADAM || mu_product, "stk_optim_step_prologue: NAdam needs mu_product");
+  STK_REQUIRE(c, h->kind >= STK_OPT_ADAM && h->kind <= STK_OPT_ASGD, "stk_optim_step_prologue: bad optimizer kind");
+  STK_REQUIRE(c, scalar_state_width(h->kind) == 0 || mu_product,
+              "stk_optim_step_prologue: NAdam and ASGD need their scalar state (mu_product)");
   STK_REQUIRE(c, (reinterpret_cast<uintptr_t>(bc) & 15) == 0, "stk_optim_step_prologue: bc must be 16-byte aligned");
   std::lock_guard<std::mutex> lk(c->mu);
   DeviceGuard g(c->device);

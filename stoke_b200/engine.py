@@ -458,7 +458,7 @@ class GradPath:
                  module: Optional[torch.nn.Module] = None, sync_init: bool = True, needs_second_moment: bool = True,
                  needs_first_moment: bool = True, bucket_mb: Optional[float] = None, state_id: Optional[int] = None,
                  route: Optional[str] = None, group_of: Optional[Sequence[int]] = None, overlap: bool = True,
-                 mu_product: bool = False, adafactor: bool = False):
+                 scalar_state: int = 0, adafactor: bool = False):
         self.engine = engine
         self.params = [p for p in params if p.requires_grad]
         if not self.params:
@@ -573,11 +573,13 @@ class GradPath:
         self._range_skip_live = False   # the device table currently carries skip bits
         self._range_steps = None        # int32 per parameter once per-parameter step counts are on (enable_per_param_steps)
         self._range_bc = None
-        # NAdam's mu_product (torch keeps it per parameter as fp32 state): one per group, one per parameter once per-parameter
-        # step counts are on; stk_optim_step_prologue advances it on the device.  group_bc: the prologue's per-group scalars.
+        # Per-entry scalar state, `scalar_state` fp32 values per entry (torch keeps them per parameter as 0-dim fp32 tensors):
+        # NAdam's mu_product (1) or ASGD's (eta, mu) (2).  One entry per group, one per parameter once per-parameter step
+        # counts are on; stk_optim_step_prologue advances it on the device.  group_bc: the prologue's per-group scalars.
         n_grp = max(self.group_of) + 1
-        self._group_mu = torch.ones(n_grp, dtype=torch.float32, device=dev) if mu_product else None
-        self._range_mu = None
+        self._scal_width = int(scalar_state)
+        self._group_scal = torch.ones(n_grp, self._scal_width, dtype=torch.float32, device=dev) if scalar_state else None
+        self._range_scal = None
         self._group_bc = torch.zeros(n_grp, 4, dtype=torch.float32, device=dev)
         self._touched = np.ones(len(self.params), dtype=bool)
         self._track_touched = False
@@ -785,20 +787,22 @@ class GradPath:
             self._range_skip_live = skip
         return len(self.params), self._range_end.data_ptr(), self._range_group.data_ptr()
 
-    def enable_per_param_steps(self, steps: Optional[Sequence[int]] = None, mu_products: Optional[Sequence[float]] = None):
+    def enable_per_param_steps(self, steps: Optional[Sequence[int]] = None,
+                               scalars: Optional[Sequence[Sequence[float]]] = None):
         """Switches the fused step to per-parameter step counts (one synchronisation to read the optimizer-wide count).
-        NAdam's mu_product goes per parameter too: ``mu_products``, or each parameter's group value."""
+        The per-entry scalar state (NAdam's mu_product, ASGD's eta and mu) goes per parameter too: ``scalars`` (one
+        sequence of ``scalar_state`` floats per parameter), or each parameter's group value."""
         dev = self._range_end.device
         if steps is None:
             done = int(self.engine.scaler_get(self.state_id).opt_steps)
             steps = [done] * len(self.params)
         self._range_steps = torch.tensor(list(steps), dtype=torch.int32, device=dev)
         self._range_bc = torch.zeros(len(self.params), 4, dtype=torch.float32, device=dev)
-        if self._group_mu is not None:
-            if mu_products is not None:
-                self._range_mu = torch.tensor(list(mu_products), dtype=torch.float32, device=dev)
+        if self._group_scal is not None:
+            if scalars is not None:
+                self._range_scal = torch.tensor([list(s) for s in scalars], dtype=torch.float32, device=dev)
             else:
-                self._range_mu = self._group_mu[torch.tensor(self.group_of, dtype=torch.long, device=dev)].contiguous()
+                self._range_scal = self._group_scal[torch.tensor(self.group_of, dtype=torch.long, device=dev)].contiguous()
 
     def param_steps(self) -> List[int]:
         """Steps taken by every parameter (what torch reports as ``state[p]["step"]``)."""
@@ -806,21 +810,21 @@ class GradPath:
             return [int(self.engine.scaler_get(self.state_id).opt_steps)] * len(self.params)
         return [int(v) for v in self._range_steps.cpu().tolist()]
 
-    def param_mu_products(self) -> List[float]:
-        """NAdam's mu_product of every parameter (torch's ``state[p]["mu_product"]``); synchronises."""
-        if self._range_mu is not None:
-            return [float(v) for v in self._range_mu.cpu().tolist()]
-        mus = self._group_mu.cpu().tolist()
-        return [float(mus[g]) for g in self.group_of]
+    def param_scalars(self) -> List[List[float]]:
+        """The scalar state of every parameter (NAdam: [mu_product]; ASGD: [eta, mu]); synchronises."""
+        if self._range_scal is not None:
+            return [[float(x) for x in row] for row in self._range_scal.cpu().tolist()]
+        rows = self._group_scal.cpu().tolist()
+        return [[float(x) for x in rows[g]] for g in self.group_of]
 
-    def set_group_mu_products(self, mus: Sequence[float]):
-        """Sets NAdam's per-group mu_product (checkpoint load while step counts are optimizer-wide)."""
-        self._group_mu.copy_(torch.tensor(list(mus), dtype=torch.float32))
+    def set_group_scalars(self, rows: Sequence[Sequence[float]]):
+        """Sets the per-group scalar state (checkpoint load while step counts are optimizer-wide)."""
+        self._group_scal.copy_(torch.tensor([list(r) for r in rows], dtype=torch.float32))
 
     def optimizer_step(self, hypers, exts=None):
         """One fused K2 launch (+ the one-thread epilogue).  ``hypers``: one ``OptimHyper`` or a list (one per group).
-        ``exts``: per-group ``OptimHyperExt`` of the NAdam / RAdam / Adamax kinds, whose per-step scalars (and NAdam's
-        mu_product) stk_optim_step_prologue forms on the device before the step."""
+        ``exts``: per-group ``OptimHyperExt`` of the kinds after SGD, whose per-step scalars (and the scalar state of
+        NAdam and ASGD) stk_optim_step_prologue forms on the device before the step."""
         e = self.engine
         e.state_select(self.state_id)
         if isinstance(hypers, _lib.OptimHyper):
@@ -868,7 +872,7 @@ class GradPath:
             keep.append(xarr)
             a.hyper_ext = xarr
             per_range = bool(nr) and self._range_steps is not None
-            mu = self._range_mu if per_range else self._group_mu
+            mu = self._range_scal if per_range else self._group_scal
             bc = self._range_bc if per_range else self._group_bc
             e._check(e.lib.stk_optim_step_prologue(e.ctx, harr, xarr, ng, nr if per_range else 0, rgrp if per_range else None,
                                                    self._range_steps.data_ptr() if per_range else None,

@@ -4,10 +4,13 @@
 ``B200FusedOptimizer`` -- a ``torch.optim.Optimizer`` (so LR schedulers and ``param_groups`` edits work, README.md:241-250
 of the reference) whose ``step()`` is the single fused K2 launch over the flat fp32 master / moment buffers; its sharded
 flavour is the ZeRO-1 analogue of fairscale ``OSS`` (/root/reference/stoke/extensions.py:109-141): same ``clip_grad_norm`` /
-``consolidate_state_dict`` surface.  Adam, AdamW, SGD(-momentum), NAdam, RAdam and Adamax, up to 8 parameter groups
-(per-group lr / betas / eps / weight decay / momentum ... selected inside the kernel by element range).  NAdam, RAdam and
-Adamax keep two fp32 state tensors per parameter like Adam (Adamax's ``exp_inf`` in the second-moment buffer); their
-per-step scalars, and NAdam's ``mu_product``, are formed on the device by ``stk_optim_step_prologue``.
+``consolidate_state_dict`` surface.  Adam, AdamW, SGD(-momentum), NAdam, RAdam, Adamax, Adadelta, Rprop and ASGD, up to 8
+parameter groups (per-group lr / betas / eps / weight decay / momentum ... selected inside the kernel by element range).
+NAdam, RAdam, Adamax, Adadelta and Rprop keep two fp32 state tensors per parameter like Adam (Adamax's ``exp_inf``,
+Adadelta's ``acc_delta`` and Rprop's ``step_size`` in the second-moment buffer); ASGD keeps one (``ax``).  Their per-step
+scalars, NAdam's ``mu_product`` and ASGD's ``eta`` / ``mu`` are formed on the device by ``stk_optim_step_prologue``, so
+none of them reads a scalar back to the host (torch's single-tensor ASGD calls ``.item()`` three times per parameter).
+Adadelta, Rprop and ASGD create their state lazily like torch: a parameter never stepped has no ``state_dict`` entry.
 ``torch.optim.Adafactor`` takes its own fused entry point, ``stk_adafactor_step`` (per-parameter reductions: row / column
 means of g^2, the parameter's RMS, the update's RMS), with per-parameter step counts on the device and torch's
 state_dict layout (``row_var`` / ``col_var`` or ``variance``).  Its state is never sharded: the reductions need whole
@@ -28,12 +31,19 @@ from . import _lib, layout
 from .engine import ClipSpec, Engine, GradPath
 
 _KINDS = {torch.optim.Adam: _lib.OPT_ADAM, torch.optim.AdamW: _lib.OPT_ADAMW, torch.optim.SGD: _lib.OPT_SGD,
-          torch.optim.NAdam: _lib.OPT_NADAM, torch.optim.RAdam: _lib.OPT_RADAM, torch.optim.Adamax: _lib.OPT_ADAMAX}
-_EXT_KINDS = (_lib.OPT_NADAM, _lib.OPT_RADAM, _lib.OPT_ADAMAX)   # per-step scalars from stk_optim_step_prologue
-# torch's per-parameter state keys of the two fp32 buffers M and V
+          torch.optim.NAdam: _lib.OPT_NADAM, torch.optim.RAdam: _lib.OPT_RADAM, torch.optim.Adamax: _lib.OPT_ADAMAX,
+          torch.optim.Adadelta: _lib.OPT_ADADELTA, torch.optim.Rprop: _lib.OPT_RPROP, torch.optim.ASGD: _lib.OPT_ASGD}
+# per-step scalars from stk_optim_step_prologue
+_EXT_KINDS = (_lib.OPT_NADAM, _lib.OPT_RADAM, _lib.OPT_ADAMAX, _lib.OPT_ADADELTA, _lib.OPT_RPROP, _lib.OPT_ASGD)
+# element-wise classes whose state torch creates at a parameter's first step (no state_dict entry before it)
+_LAZY_KINDS = (_lib.OPT_ADADELTA, _lib.OPT_RPROP, _lib.OPT_ASGD)
+# torch's per-parameter state keys of the two fp32 buffers M and V (None: no V buffer)
 _STATE_KEYS = {_lib.OPT_ADAM: ("exp_avg", "exp_avg_sq"), _lib.OPT_ADAMW: ("exp_avg", "exp_avg_sq"),
                _lib.OPT_NADAM: ("exp_avg", "exp_avg_sq"), _lib.OPT_RADAM: ("exp_avg", "exp_avg_sq"),
-               _lib.OPT_ADAMAX: ("exp_avg", "exp_inf")}
+               _lib.OPT_ADAMAX: ("exp_avg", "exp_inf"), _lib.OPT_ADADELTA: ("square_avg", "acc_delta"),
+               _lib.OPT_RPROP: ("prev", "step_size"), _lib.OPT_ASGD: ("ax", None)}
+# per-entry scalar state carried by the step prologue: NAdam's mu_product, ASGD's (eta, mu), torch's 0-dim fp32 tensors
+_SCALAR_KEYS = {_lib.OPT_NADAM: ("mu_product",), _lib.OPT_ASGD: ("eta", "mu")}
 _STOCK_ONLY_TRUE = ("amsgrad", "capturable", "differentiable")
 # torch.optim.Adafactor (torch >= 2.5) runs on its own entry point, stk_adafactor_step, not as a kind of K2
 _ADAFACTOR = "adafactor"
@@ -103,7 +113,7 @@ class B200FusedOptimizer(torch.optim.Optimizer):
                  bucket_mb: Optional[float] = None):
         if optim_cls not in _KINDS:
             raise NotImplementedError(
-                f"Stoke -- the fused step covers torch.optim.Adam, AdamW, SGD, NAdam, RAdam, Adamax and Adafactor; got {getattr(optim_cls, '__name__', optim_cls)}"
+                f"Stoke -- the fused step covers torch.optim.Adam, AdamW, SGD, NAdam, RAdam, Adamax, Adadelta, Rprop, ASGD and Adafactor; got {getattr(optim_cls, '__name__', optim_cls)}"
                 f" (use B200StockOptimizer / build_optimizer, which routes other classes to the stock-optimizer path)")
         params, group_of, extra, kw = _group_layout(module, optim_kwargs)
         if len(extra) > _lib.MAX_GROUPS:
@@ -128,9 +138,9 @@ class B200FusedOptimizer(torch.optim.Optimizer):
             # fairscale_oss) and every rank runs the same deterministic step on the same all-reduced fp32 gradients
             route = "allreduce"
         self.path = GradPath(engine, params, grad_accum=grad_accum, clip=clip, sharded=sharded, lp_dtype=lp_dtype,
-                             module=module, needs_second_moment=not (sgd or ada),
+                             module=module, needs_second_moment=not (sgd or ada or self._kind == _lib.OPT_ASGD),
                              needs_first_moment=not (sgd or ada) or any_mom, state_id=state_id, route=route,
-                             group_of=group_of, bucket_mb=bucket_mb, mu_product=self._kind == _lib.OPT_NADAM,
+                             group_of=group_of, bucket_mb=bucket_mb, scalar_state=len(_SCALAR_KEYS.get(self._kind, ())),
                              adafactor=ada)
         by_group: List[List[torch.nn.Parameter]] = [[] for _ in extra]
         for p, gi in zip(params, group_of):
@@ -162,8 +172,10 @@ class B200FusedOptimizer(torch.optim.Optimizer):
             h.momentum = float(g.get("momentum", 0.0))
             h.dampening = float(g.get("dampening", 0.0))
             h.nesterov = int(bool(g.get("nesterov", False)))
-        else:
+        elif "betas" in g:
             h.beta1, h.beta2 = (float(b) for b in g["betas"])
+            h.eps = float(g["eps"])
+        elif "eps" in g:   # Adadelta
             h.eps = float(g["eps"])
         return h
 
@@ -181,6 +193,10 @@ class B200FusedOptimizer(torch.optim.Optimizer):
             x = _lib.OptimHyperExt()
             x.momentum_decay = float(g.get("momentum_decay", 0.0))
             x.decoupled_weight_decay = int(bool(g.get("decoupled_weight_decay", False)))
+            x.rho = float(g.get("rho", 0.0))
+            x.etaminus, x.etaplus = (float(e) for e in g.get("etas", (0.0, 0.0)))
+            x.step_size_min, x.step_size_max = (float(e) for e in g.get("step_sizes", (0.0, 0.0)))
+            x.lambd, x.alpha, x.t0 = float(g.get("lambd", 0.0)), float(g.get("alpha", 0.0)), float(g.get("t0", 0.0))
             out.append(x)
         return out
 
@@ -256,17 +272,74 @@ class B200FusedOptimizer(torch.optim.Optimizer):
         path._range_steps.copy_(torch.tensor(steps, dtype=torch.int32))
         return int(sd.get("b200_opt_steps", max(steps)))
 
+    def _lazy_state_dict(self):
+        """Adadelta / Rprop / ASGD in torch's format: ``step`` and the class's state tensors (ASGD: ``eta`` and ``mu`` as
+        0-dim fp32 tensors too); a parameter that was never stepped has no entry (torch creates its state at its first
+        gradient)."""
+        path = self.path
+        st = path.engine.scaler_get(path.state_id)
+        k_m, k_v = _STATE_KEYS[self._kind]
+        ms = path.unflatten(self._full(path.m_flat))
+        vs = path.unflatten(self._full(path.v_flat)) if k_v is not None else None
+        steps = path.param_steps()
+        scal = path.param_scalars() if self._kind in _SCALAR_KEYS else None
+        state = {}
+        for i in range(len(path.params)):
+            if steps[i] == 0:
+                continue
+            d = {"step": torch.tensor(float(steps[i]))}
+            if scal is not None:
+                for key, val in zip(_SCALAR_KEYS[self._kind], scal[i]):
+                    d[key] = torch.tensor(val, dtype=torch.float32)
+            d[k_m] = ms[i].clone()
+            if k_v is not None:
+                d[k_v] = vs[i].clone()
+            state[self._sd_index[i]] = d
+        return {"state": state, "param_groups": self._groups_sd(), "b200_master": path.gather_master(),
+                "b200_opt_steps": int(st.opt_steps)}
+
+    def _lazy_load_state_dict(self, sd, put) -> int:
+        """Adadelta / Rprop / ASGD: a parameter without an entry has taken no step (torch's lazy state), so its step
+        count is 0 and its first fused step initialises it as torch would.  Step counts that differ between parameters, or
+        ASGD scalars that differ within a group, switch to per-parameter bookkeeping."""
+        path = self.path
+        n = len(path.params)
+        state = sd["state"]
+        k_m, k_v = _STATE_KEYS[self._kind]
+        put(path.m_flat, k_m)
+        if k_v is not None:
+            put(path.v_flat, k_v)
+        srcs = [state.get(self._sd_index[i], {}) for i in range(n)]
+        per_param = [int(float(src["step"])) if "step" in src else 0 for src in srcs]
+        keys = _SCALAR_KEYS.get(self._kind, ())
+        # the placeholder of a parameter without state is never read: the prologue initialises it at the first step
+        scal = [[float(src[k]) if k in src else 1.0 for k in keys] for src in srcs]
+        groups_differ = any(len({tuple(scal[i]) for i in range(n) if self._group_of[i] == gi and per_param[i] > 0}) > 1
+                            for gi in range(len(self.param_groups)))
+        # one optimizer-wide count serves every parameter only if each took exactly that many steps
+        wide = int(sd.get("b200_opt_steps", per_param[0]))
+        if len(set(per_param)) > 1 or per_param[0] != wide or groups_differ or path._range_steps is not None:
+            path.enable_per_param_steps(per_param, scalars=scal if keys else None)
+        elif keys:
+            first = {}
+            for i in range(n):
+                first.setdefault(self._group_of[i], scal[i])
+            path.set_group_scalars([first.get(gi, [1.0] * len(keys)) for gi in range(len(self.param_groups))])
+        return int(sd.get("b200_opt_steps", max(per_param)))
+
     def state_dict(self):
         path = self.path
         if self._kind == _ADAFACTOR:
             return self._adafactor_state_dict()
+        if self._kind in _LAZY_KINDS:
+            return self._lazy_state_dict()
         st = path.engine.scaler_get(path.state_id)
         m, v, master = self._full(path.m_flat), self._full(path.v_flat), path.gather_master()
         state = {}
         ms = path.unflatten(m) if m is not None else None
         vs = path.unflatten(v) if v is not None else None
         steps = path.param_steps() if path._range_steps is not None else [int(st.opt_steps)] * len(path.params)
-        mus = path.param_mu_products() if self._kind == _lib.OPT_NADAM else None
+        mus = [r[0] for r in path.param_scalars()] if self._kind == _lib.OPT_NADAM else None
         for i in range(len(path.params)):
             j = self._sd_index[i]
             if self._kind == _lib.OPT_SGD:
@@ -311,6 +384,8 @@ class B200FusedOptimizer(torch.optim.Optimizer):
 
         if self._kind == _ADAFACTOR:
             pass
+        elif self._kind in _LAZY_KINDS:
+            steps = self._lazy_load_state_dict(sd, put)
         elif self._kind == _lib.OPT_SGD:
             put(path.m_flat, "momentum_buffer")
         else:
@@ -332,12 +407,13 @@ class B200FusedOptimizer(torch.optim.Optimizer):
             if known and (len(set(known)) > 1 or len(known) < n) or groups_differ or (
                     mus is not None and path._range_steps is not None):
                 # parameters stepped a different number of times (some were unused for a while): keep torch's per-parameter counts
-                path.enable_per_param_steps([steps if v is None else v for v in per_param], mu_products=mus)
+                path.enable_per_param_steps([steps if v is None else v for v in per_param],
+                                            scalars=None if mus is None else [[mu] for mu in mus])
             elif mus is not None:
                 first = {}
                 for i in range(n):
                     first.setdefault(self._group_of[i], mus[i])
-                path.set_group_mu_products([first.get(gi, 1.0) for gi in range(len(self.param_groups))])
+                path.set_group_scalars([[first.get(gi, 1.0)] for gi in range(len(self.param_groups))])
         if "b200_master" in sd:
             master = sd["b200_master"].to(device=dev, dtype=torch.float32)
             if path.master_flat is not path.p_flat:
