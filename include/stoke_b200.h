@@ -402,27 +402,49 @@ int stk_barrier(stk_ctx* ctx, void* stream);
 int stk_bcast(stk_ctx* ctx, void* const* ptrs, size_t bytes, int root, void* stream);
 
 /* ---- model forward ------------------------------------------------------------------------------------------------- */
-/* Training-mode BatchNorm apply + optional residual add + ReLU over a bf16 channels-last (NHWC) tensor of `numel` elements
- * and `channels` channels (multiple of 8, numel < 2^31, every pointer 16-byte aligned), from statistics torch reduced
- * (torch.batch_norm_update_stats: fp32 mean and biased var):
- *   out = relu(bf16(bf16(weight * (x - mean) * invstd + bias) + residual)),  save_invstd[c] = rsqrtf(var[c] + eps)
- * with every intermediate rounded as the unfused torch ops round it (bit-identical to them).  residual may be NULL. */
+/* The activation that follows the BatchNorm, as torch 2.11's CUDA kernels evaluate it on a bf16 input (fp32 opmath, one
+ * rounding to bf16): relu (clamp_min(0)), silu (x / (1 + expf(-x))), hardswish (x * min(max(x + 3, 0), 6) * (1/6)),
+ * relu6 (hardtanh(x, 0, 6) = clamp(x, 0, 6)).  relu and relu6 keep a NaN's bits. */
+enum { STK_ACT_RELU = 0, STK_ACT_SILU = 1, STK_ACT_HARDSWISH = 2, STK_ACT_RELU6 = 3 };
+
+/* Training-mode BatchNorm apply + optional residual add + activation `act` (STK_ACT_*) over a bf16 channels-last (NHWC)
+ * tensor of `numel` elements and `channels` channels (multiple of 8, numel < 2^31, every pointer 16-byte aligned), from
+ * statistics torch reduced (torch.batch_norm_update_stats: fp32 mean and biased var):
+ *   out = act(bf16(bf16(weight * (x - mean) * invstd + bias) + residual)),  save_invstd[c] = rsqrtf(var[c] + eps)
+ * with every intermediate rounded as the unfused torch ops round it (bit-identical to them).  residual may be NULL, and
+ * must be NULL unless act is STK_ACT_RELU. */
+int stk_bn_act_ex(stk_ctx* ctx, int act, const void* x, const void* residual, const float* mean, const float* var,
+                  const void* weight, const void* bias, double eps, void* out, float* save_invstd, size_t numel,
+                  size_t channels, void* stream);
+/* stk_bn_act_ex with act = STK_ACT_RELU */
 int stk_bn_act(stk_ctx* ctx, const void* x, const void* residual, const float* mean, const float* var, const void* weight,
                const void* bias, double eps, void* out, float* save_invstd, size_t numel, size_t channels, void* stream);
 
 /* ---- model backward ------------------------------------------------------------------------------------------------ */
-/* Backward of stk_bn_act: the ReLU's threshold_backward followed by torch's training-mode BatchNorm backward, with the
- * coverage of stk_bn_act (bf16 channels-last, channels % 8 == 0, numel < 2^31, every pointer 16-byte aligned).
- *   g = !(out <= 0) ? grad : +0;  sum_dy = sum g,  sum_dy_xmu = sum g * (x - mean)  (per channel over R = numel / channels)
+/* Backward of stk_bn_act_ex: the activation's backward followed by torch's training-mode BatchNorm backward, with the
+ * coverage of stk_bn_act_ex (bf16 channels-last, channels % 8 == 0, numel < 2^31, every pointer 16-byte aligned).
+ *   g = act_backward(grad, y);  sum_dy = sum g,  sum_dy_xmu = sum g * (x - mean)  (per channel over R = numel / channels)
  *   grad_bias = bf16(sum_dy),  grad_weight = bf16(sum_dy_xmu * invstd)
  *   grad_x = bf16(((g - sum_dy * n) - (x - mean) * (invstd * invstd * sum_dy_xmu * n)) * (weight * invstd)),  n = float(1.0 / R)
- * out != NULL: a site with a residual; the mask comes from out and g is written to grad_residual.  out == NULL: the mask
- * comes from y = bf16(weight * (x - mean) * invstd + bias), the formula stk_bn_act applies (relu(y) <= 0 iff y <= 0);
- * grad_residual is unused.  grad_x may be NULL (no elementwise pass).
+ * act_backward is torch's backward op of the activation, g rounded to bf16 as it rounds it:
+ *   relu       threshold_backward(grad, out, 0) = !(out <= 0) ? grad : +0 (grad's bits kept)
+ *   silu       silu_backward: s = 1 / (1 + expf(-y)); bf16(grad * s * fmaf(y, 1 - s, 1))
+ *   hardswish  hardswish_backward: bf16(y <= -3 ? 0 : y < 3 ? grad * (y / 3 + 0.5) : grad)
+ *   relu6      hardtanh_backward(grad, y, 0, 6): bf16(y <= 0 || y >= 6 ? 0 : grad)
+ * out != NULL (STK_ACT_RELU only): a site with a residual; the mask comes from out and g is written to grad_residual.
+ * out == NULL: y = bf16(weight * (x - mean) * invstd + bias) is recomputed, the formula stk_bn_act_ex applies (relu(y)
+ * <= 0 iff y <= 0); grad_residual is unused.  grad_pre, when not NULL, receives g (2 B/element more; it exists so the
+ * derivative can be tested apart from the sums, and must be NULL for STK_ACT_RELU, whose g keeps grad's bits or is +0).
+ * grad_x may be NULL (no elementwise pass).
  * Order contract: the two sums add in the order of torch's batch_norm_backward_reduce_channels_last_kernel as launched by
  * flexible_launch_configs(R, channels, coop) with MAX_BLOCK_SIZE 512 (a function of R and channels only), so all four
- * outputs are bit-identical to threshold_backward + native_batch_norm_backward on channels-last bf16 inputs.
+ * outputs are bit-identical to act_backward + native_batch_norm_backward on channels-last bf16 inputs.
  * workspace: 2 * (1 + 128) * channels floats (the two sums, then per-block partials); no initialisation needed. */
+int stk_bn_act_backward_ex(stk_ctx* ctx, int act, const void* grad, const void* x, const void* out, const float* mean,
+                           const float* invstd, const void* weight, const void* bias, void* grad_x, void* grad_weight,
+                           void* grad_bias, void* grad_residual, void* grad_pre, float* workspace, size_t numel,
+                           size_t channels, void* stream);
+/* stk_bn_act_backward_ex with act = STK_ACT_RELU and no grad_pre */
 int stk_bn_act_backward(stk_ctx* ctx, const void* grad, const void* x, const void* out, const float* mean,
                         const float* invstd, const void* weight, const void* bias, void* grad_x, void* grad_weight,
                         void* grad_bias, void* grad_residual, float* workspace, size_t numel, size_t channels,

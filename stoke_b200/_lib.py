@@ -16,6 +16,7 @@ NORM_NONE, NORM_L2, NORM_INF, NORM_P = 0, 1, 2, 3
 CLIP_NONE, CLIP_NORM, CLIP_VALUE = 0, 1, 2
 OPT_ADAM, OPT_ADAMW, OPT_SGD, OPT_NADAM, OPT_RADAM, OPT_ADAMAX = 0, 1, 2, 3, 4, 5
 OPT_ADADELTA, OPT_RPROP, OPT_ASGD = 6, 7, 8
+ACT_RELU, ACT_SILU, ACT_HARDSWISH, ACT_RELU6 = 0, 1, 2, 3
 RF_FINAL, RF_ZERO_INPUT, RF_UNSCALE = 1, 2, 4
 OPT_K1_ALGO, OPT_MEM_MODE, OPT_K1_MAX_BLOCKS, OPT_COOP_LAUNCH, OPT_NVLS_MAX_BLOCKS, OPT_K2_AG_MC = 1, 2, 3, 4, 5, 6
 K1_ALGO_LDG, K1_ALGO_BULK, K1_ALGO_NVLS = 0, 1, 2
@@ -152,6 +153,9 @@ _SIGNATURES = {
     "stk_bcast": (C.c_int, [_P, _PP, C.c_size_t, C.c_int, _P]),
     "stk_bn_act": (C.c_int, [_P, _P, _P, _P, _P, _P, _P, C.c_double, _P, _P, C.c_size_t, C.c_size_t, _P]),
     "stk_bn_act_backward": (C.c_int, [_P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, C.c_size_t, C.c_size_t, _P]),
+    "stk_bn_act_ex": (C.c_int, [_P, C.c_int, _P, _P, _P, _P, _P, _P, C.c_double, _P, _P, C.c_size_t, C.c_size_t, _P]),
+    "stk_bn_act_backward_ex": (C.c_int, [_P, C.c_int, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, C.c_size_t,
+                                         C.c_size_t, _P]),
     "stk_randperm": (C.c_int, [C.c_uint64, C.POINTER(C.c_int64), C.c_int, _P]),
     "stk_sampler_plan": (C.c_int, [C.POINTER(SamplerPlan)]),
     "stk_sampler_last_slice": (C.c_int, [C.POINTER(SamplerPlan), C.c_int64, _P]),

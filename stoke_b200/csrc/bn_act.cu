@@ -1,10 +1,10 @@
-// bn_act.cu -- BatchNorm apply (+ residual add) + ReLU in one pass over a bf16 NHWC activation, for training-mode
-// BatchNorm whose statistics torch has already reduced (stk_bn_act in include/stoke_b200.h).
+// bn_act.cu -- BatchNorm apply (+ residual add) + activation in one pass over a bf16 NHWC activation, for training-mode
+// BatchNorm whose statistics torch has already reduced (stk_bn_act_ex in include/stoke_b200.h), and its backward.
 //
 // Purely elementwise.  Every rounding of the unfused torch sequence is kept, so the result is bit-identical to it:
 //   y = bf16(w * (x - mean) * invstd + b)        batch_norm_transform_input_channels_last_kernel (FADD, FMUL, FFMA)
-//   z = bf16(float(y) + float(r))                `out += identity` on bf16 (fp32 add, one rounding)
-//   out = isnan(z) ? z : bf16(fmaxf(z, 0))       relu_ = clamp_min_(0), which keeps a NaN's bits
+//   z = bf16(float(y) + float(r))                `out += identity` on bf16 (fp32 add, one rounding; ReLU only)
+//   out = act(z)                                 torch's CUDA activation kernel on a bf16 input (act_out below)
 //   invstd = rsqrtf(var + eps)                   batch_norm_update_stats_and_invert
 // Bytes per element: x read 2 + out write 2 (+ residual read 2).  The unfused chain moves 8 (15 with the residual).
 #include <algorithm>
@@ -20,14 +20,54 @@ __device__ __forceinline__ uint16_t bf16_bits(float f) { return __bfloat16_as_us
 __device__ __forceinline__ float bf16_val(uint16_t u) { return __uint_as_float(uint32_t(u) << 16); }
 
 // The BatchNorm apply y = bf16(w * (x - mean) * invstd + b), as torch's channels-last transform kernel rounds it.  The
-// forward writes it and the backward recomputes the ReLU mask !(y <= 0) from it, so the two cannot disagree.
+// forward activates it and the backward recomputes the activation's input from it, so the two cannot disagree.
 __device__ __forceinline__ uint16_t bn_apply(float x, float m, float is, float w, float b) {
   return bf16_bits(__fmaf_rn(__fmul_rn(w, __fsub_rn(x, m)), is, b));
 }
 
+// The activation of a bf16 value z, as torch 2.11's CUDA kernel evaluates it: in fp32 (opmath) with one rounding, IEEE
+// division and libdevice expf (the library is built without --use_fast_math, as torch is).
+//   ReLU       relu_ = clamp_min_(0): a NaN keeps its bits
+//   SiLU       x / (1 + exp(-x))
+//   Hardswish  x * min(max(x + 3, 0), 6) * (1/6)   (std::min / std::max; a NaN gives NaN either way)
+//   ReLU6      hardtanh = clamp(x, 0, 6): a NaN keeps its bits, otherwise fminf(fmaxf(x, 0), 6)
+template <int kAct>
+__device__ __forceinline__ uint16_t act_out(uint16_t z) {
+  const float f = bf16_val(z);
+  if (kAct == STK_ACT_RELU) return isnan(f) ? z : bf16_bits(fmaxf(f, 0.f));
+  if (kAct == STK_ACT_SILU) return bf16_bits(__fdiv_rn(f, __fadd_rn(1.f, expf(-f))));
+  if (kAct == STK_ACT_HARDSWISH) {
+    float t = __fadd_rn(f, 3.f);
+    t = t < 0.f ? 0.f : t;
+    t = 6.f < t ? 6.f : t;
+    return bf16_bits(__fmul_rn(__fmul_rn(f, t), 1.0f / 6.0f));
+  }
+  return isnan(f) ? z : bf16_bits(fminf(fmaxf(f, 0.f), 6.f));
+}
+
+// The activation's backward at input y (a bf16 value) for incoming gradient d, in fp32 before torch's rounding to bf16:
+//   SiLU       silu_backward: s = 1 / (1 + exp(-y)); d * s * (1 + y * (1 - s)), the last product-sum contracted (FFMA)
+//   Hardswish  hardswish_backward: y <= -3 ? 0 : y < 3 ? d * (y / 3 + 0.5) : d
+//   ReLU6      hardtanh_backward(d, y, 0, 6): y <= 0 || y >= 6 ? 0 : d
+// (ReLU's threshold_backward keeps the gradient's bits instead; it is mask_grad below.)
+template <int kAct>
+__device__ __forceinline__ float act_grad(float d, float y) {
+  if (kAct == STK_ACT_SILU) {
+    const float s = __fdiv_rn(1.f, __fadd_rn(1.f, expf(-y)));
+    return __fmul_rn(__fmul_rn(d, s), __fmaf_rn(y, __fsub_rn(1.f, s), 1.f));
+  }
+  if (kAct == STK_ACT_HARDSWISH) return y <= -3.f ? 0.f : y < 3.f ? __fmul_rn(d, __fadd_rn(__fdiv_rn(y, 3.f), 0.5f)) : d;
+  return y <= 0.f || y >= 6.f ? 0.f : d;
+}
+
+__device__ __forceinline__ uint4 pack8(const uint16_t (&o)[8]) {
+  return make_uint4(o[0] | uint32_t(o[1]) << 16, o[2] | uint32_t(o[3]) << 16, o[4] | uint32_t(o[5]) << 16,
+                    o[6] | uint32_t(o[7]) << 16);
+}
+
 // Thread t owns channel group t % G (G = C / 8) and walks rows t / G, t / G + T / G, ...: T (the active thread count) is a
 // multiple of G, so the per-channel parameters stay in registers for the whole loop.
-template <bool kResidual>
+template <int kAct, bool kResidual>
 __global__ void __launch_bounds__(kBnThreads) k_bn_act(const __nv_bfloat16* __restrict__ x, const __nv_bfloat16* __restrict__ r,
                                                       const float* __restrict__ mean, const float* __restrict__ var,
                                                       const __nv_bfloat16* __restrict__ weight,
@@ -62,21 +102,19 @@ __global__ void __launch_bounds__(kBnThreads) k_bn_act(const __nv_bfloat16* __re
     for (int j = 0; j < 8; ++j) {
       uint16_t z = bn_apply(xf[j], m[j], is[j], w[j], b[j]);
       if (kResidual) z = bf16_bits(bf16_val(z) + rf[j]);
-      const float zf = bf16_val(z);
-      o[j] = isnan(zf) ? z : bf16_bits(fmaxf(zf, 0.f));
+      o[j] = act_out<kAct>(z);
     }
-    ov[v] = make_uint4(o[0] | uint32_t(o[1]) << 16, o[2] | uint32_t(o[3]) << 16, o[4] | uint32_t(o[5]) << 16,
-                       o[6] | uint32_t(o[7]) << 16);
+    ov[v] = pack8(o);
   }
 }
 
 // ---- backward ------------------------------------------------------------------------------------------------------
-// The ReLU's threshold_backward g = !(out <= 0) ? grad : +0 is folded into the two passes of torch's channels-last
-// BatchNorm backward (batch_norm_backward_reduce_channels_last_kernel, batch_norm_backward_elemt_channels_last_kernel),
-// whose sums are reproduced in torch's order, so every result is bit-identical to the unfused chain.  The mask comes
-// from out (sites with a residual, where g is also written: it is the residual's gradient) or from bn_apply(x) (sites
-// without one, where relu(y) <= 0 exactly when y <= 0).  Bytes per element: 4 + 6 without the residual, 8 + 6 with it;
-// the unfused chain moves 16.
+// The activation's backward g (ReLU's threshold_backward g = !(out <= 0) ? grad : +0, or act_grad) is folded into the
+// two passes of torch's channels-last BatchNorm backward (batch_norm_backward_reduce_channels_last_kernel,
+// batch_norm_backward_elemt_channels_last_kernel), whose sums are reproduced in torch's order, so every result is
+// bit-identical to the unfused chain.  The ReLU mask comes from out at sites with a residual (where g is also written:
+// it is the residual's gradient); every other site recomputes y = bn_apply(x) (relu(y) <= 0 exactly when y <= 0).
+// Bytes per element: 4 + 6 without the residual, 8 + 6 with it; the unfused chain moves 16.
 constexpr int kBwdThreads = 256;
 constexpr int kChains = 4;   // torch's ELEMENTS_PER_ITER: accumulators per virtual thread
 
@@ -85,6 +123,24 @@ __device__ __forceinline__ uint4 mask_grad(const uint4& g, const bool (&pass)[8]
   const uint32_t m[4] = {(pass[0] ? 0xffffu : 0u) | (pass[1] ? 0xffff0000u : 0u), (pass[2] ? 0xffffu : 0u) | (pass[3] ? 0xffff0000u : 0u),
                          (pass[4] ? 0xffffu : 0u) | (pass[5] ? 0xffff0000u : 0u), (pass[6] ? 0xffffu : 0u) | (pass[7] ? 0xffff0000u : 0u)};
   return make_uint4(g.x & m[0], g.y & m[1], g.z & m[2], g.w & m[3]);
+}
+
+// g at a site without a residual, from the activation's input y = bn_apply(x) recomputed per element
+template <int kAct>
+__device__ __forceinline__ uint4 act_backward8(const uint4& gv, const float (&xf)[8], const float (&m)[8], const float (&is)[8],
+                                               const float (&w)[8], const float (&b)[8]) {
+  if (kAct == STK_ACT_RELU) {
+    bool pass[8];
+#pragma unroll
+    for (int k = 0; k < 8; ++k) pass[k] = !(bf16_val(bn_apply(xf[k], m[k], is[k], w[k], b[k])) <= 0.f);
+    return mask_grad(gv, pass);
+  }
+  float d[8];
+  unpack16<STK_BF16>(gv, d);
+  uint16_t o[8];
+#pragma unroll
+  for (int k = 0; k < 8; ++k) o[k] = bf16_bits(act_grad<kAct>(d[k], bf16_val(bn_apply(xf[k], m[k], is[k], w[k], b[k]))));
+  return pack8(o);
 }
 
 __device__ __forceinline__ void load8(const float* __restrict__ p, float (&f)[8]) {
@@ -98,8 +154,10 @@ __device__ __forceinline__ void load8(const float* __restrict__ p, float (&f)[8]
 // as acc += g and acc = fma(g, x - mean, acc).  The chains are folded 0 += 1, 2, 3, then halved over ty (offsets
 // block_y / 2 .. 1).  Here one real thread runs one chain of one virtual thread for 8 channels; a block holds every ty
 // of its by for kBwdThreads / (kChains * block_y) channel groups.  With grid_y == 1 the block's sums are final;
-// otherwise they go to the workspace partials and k_bn_bwd_finish adds them.
-template <bool kResidual>
+// otherwise they go to the workspace partials and k_bn_bwd_finish adds them.  g_out receives g: the residual's gradient
+// (ReLU), or the optional grad_pre of another activation.  ReLU without a residual has no g_out: a run-time checked
+// store there would take its instantiation from 80 to 99 registers.
+template <int kAct, bool kResidual>
 __global__ void __launch_bounds__(kBwdThreads) k_bn_bwd_reduce(const uint4* __restrict__ grad, const uint4* __restrict__ x,
                                                                const uint4* __restrict__ out, const float* __restrict__ mean,
                                                                const float* __restrict__ invstd,
@@ -134,17 +192,21 @@ __global__ void __launch_bounds__(kBwdThreads) k_bn_bwd_reduce(const uint4* __re
       const uint4 gv = in ? __ldg(grad + v) : zero, xv = in ? __ldg(x + v) : zero;
       float xf[8], gf[8], mf[8];
       unpack16<STK_BF16>(xv, xf);
-      bool pass[8];
+      uint4 g;
       if (kResidual) {
+        bool pass[8];
         unpack16<STK_BF16>(in ? __ldg(out + v) : zero, mf);
 #pragma unroll
         for (int k = 0; k < 8; ++k) pass[k] = !(mf[k] <= 0.f);
+        g = mask_grad(gv, pass);
+      } else if (kAct == STK_ACT_RELU || in) {
+        g = act_backward8<kAct>(gv, xf, m, is, w, b);
       } else {
-#pragma unroll
-        for (int k = 0; k < 8; ++k) pass[k] = !(bf16_val(bn_apply(xf[k], m[k], is[k], w[k], b[k])) <= 0.f);
+        // a row past the end adds g = +0 as in torch, whose activation backward never sees it: SiLU's backward of a
+        // zero gradient is NaN where bn_apply(0) overflows to +-inf (0 * s * fma(inf, 1 - s, 1))
+        g = zero;
       }
-      const uint4 g = mask_grad(gv, pass);
-      if (kResidual && in) g_out[v] = g;
+      if ((kResidual || (kAct != STK_ACT_RELU && g_out != nullptr)) && in) g_out[v] = g;
       unpack16<STK_BF16>(g, gf);
 #pragma unroll
       for (int k = 0; k < 8; ++k) {
@@ -251,7 +313,7 @@ __global__ void __launch_bounds__(kBwdThreads) k_bn_bwd_finish(float* __restrict
 // dx = bf16(((g - sum_dy * n) - (x - mean) * k1) * k2), k1 = invstd * invstd * sum_dy_xmu * n, k2 = w * invstd,
 // n = float(1.0 / rows): torch's channels-last elementwise backward, whose SASS contracts both subtractions with their
 // products (FFMA -sum_dy * n + g; FADD x - mean; FFMA -k1 * (x - mean) + t; FMUL k2).  Thread layout as in k_bn_act.
-template <bool kResidual>
+template <int kAct, bool kResidual>
 __global__ void __launch_bounds__(kBnThreads) k_bn_bwd_elemt(const uint4* __restrict__ grad, const uint4* __restrict__ x,
                                                             const float* __restrict__ mean, const float* __restrict__ invstd,
                                                             const __nv_bfloat16* __restrict__ weight,
@@ -280,12 +342,7 @@ __global__ void __launch_bounds__(kBnThreads) k_bn_bwd_elemt(const uint4* __rest
     float xf[8], gf[8];
     unpack16<STK_BF16>(__ldg(x + v), xf);
     uint4 g = __ldg(grad + v);
-    if (!kResidual) {
-      bool pass[8];
-#pragma unroll
-      for (int k = 0; k < 8; ++k) pass[k] = !(bf16_val(bn_apply(xf[k], m[k], is[k], w[k], b[k])) <= 0.f);
-      g = mask_grad(g, pass);
-    }
+    if (!kResidual) g = act_backward8<kAct>(g, xf, m, is, w, b);
     unpack16<STK_BF16>(g, gf);
     uint16_t o[8];
 #pragma unroll
@@ -316,15 +373,30 @@ static BnBwdConfig bn_bwd_config(uint32_t rows, uint32_t channels) {
   return {block_y, grid_y, 1 + (rows - 1) / (block_y * grid_y * kChains)};
 }
 
+// The instantiation of `kernel` for (act, residual): every activation without a residual, and ReLU with one.
+#define STK_BN_KERNEL(kernel, act, res)                                                                              \
+  ((act) == STK_ACT_SILU        ? kernel<STK_ACT_SILU, false>                                                        \
+   : (act) == STK_ACT_HARDSWISH ? kernel<STK_ACT_HARDSWISH, false>                                                   \
+   : (act) == STK_ACT_RELU6     ? kernel<STK_ACT_RELU6, false>                                                       \
+   : (res)                      ? kernel<STK_ACT_RELU, true>                                                         \
+                                : kernel<STK_ACT_RELU, false>)
+
+static bool act_valid(int act, bool residual) {
+  return act >= STK_ACT_RELU && act <= STK_ACT_RELU6 && (act == STK_ACT_RELU || !residual);
+}
+
 }  // namespace stk
 
 using namespace stk;
 
 extern "C" {
 
-int stk_bn_act(stk_ctx* c, const void* x, const void* residual, const float* mean, const float* var, const void* weight,
-               const void* bias, double eps, void* out, float* save_invstd, size_t numel, size_t channels, void* stream) {
+int stk_bn_act_ex(stk_ctx* c, int act, const void* x, const void* residual, const float* mean, const float* var,
+                  const void* weight, const void* bias, double eps, void* out, float* save_invstd, size_t numel,
+                  size_t channels, void* stream) {
   STK_REQUIRE(c, c && x && mean && var && weight && bias && out && save_invstd, "stk_bn_act: NULL argument");
+  STK_REQUIRE(c, act_valid(act, residual != nullptr),
+              "stk_bn_act: act must be an STK_ACT_* kind, and only STK_ACT_RELU takes a residual");
   STK_REQUIRE(c, channels > 0 && channels % 8 == 0 && numel % channels == 0, "stk_bn_act: channels must be a positive multiple of 8 dividing numel");
   STK_REQUIRE(c, numel < (size_t(1) << 31), "stk_bn_act: numel must be below 2^31");
   const uintptr_t align = uintptr_t(x) | uintptr_t(residual) | uintptr_t(mean) | uintptr_t(var) | uintptr_t(weight) |
@@ -333,7 +405,7 @@ int stk_bn_act(stk_ctx* c, const void* x, const void* residual, const float* mea
   DeviceGuard g(c->device);
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
   const uint32_t nvec = uint32_t(numel / 8), groups = uint32_t(channels / 8);
-  auto kern = residual ? k_bn_act<true> : k_bn_act<false>;
+  auto kern = STK_BN_KERNEL(k_bn_act, act, residual != nullptr);
   const size_t resident = size_t(blocks_per_sm(c, kern, kBnThreads)) * c->sm_count;
   // enough threads to cover every channel group once, at most one resident wave, at most one thread per vector
   size_t blocks = std::min(resident, (size_t(nvec) + kBnThreads - 1) / kBnThreads);
@@ -348,19 +420,29 @@ int stk_bn_act(stk_ctx* c, const void* x, const void* residual, const float* mea
   return STK_OK;
 }
 
-int stk_bn_act_backward(stk_ctx* c, const void* grad, const void* x, const void* out, const float* mean, const float* invstd,
-                        const void* weight, const void* bias, void* grad_x, void* grad_weight, void* grad_bias,
-                        void* grad_residual, float* workspace, size_t numel, size_t channels, void* stream) {
+int stk_bn_act(stk_ctx* c, const void* x, const void* residual, const float* mean, const float* var, const void* weight,
+               const void* bias, double eps, void* out, float* save_invstd, size_t numel, size_t channels, void* stream) {
+  return stk_bn_act_ex(c, STK_ACT_RELU, x, residual, mean, var, weight, bias, eps, out, save_invstd, numel, channels,
+                       stream);
+}
+
+int stk_bn_act_backward_ex(stk_ctx* c, int act, const void* grad, const void* x, const void* out, const float* mean,
+                           const float* invstd, const void* weight, const void* bias, void* grad_x, void* grad_weight,
+                           void* grad_bias, void* grad_residual, void* grad_pre, float* workspace, size_t numel,
+                           size_t channels, void* stream) {
   STK_REQUIRE(c, c && grad && x && mean && invstd && weight && grad_weight && grad_bias && workspace,
               "stk_bn_act_backward: NULL argument");
+  STK_REQUIRE(c, act_valid(act, out != nullptr),
+              "stk_bn_act_backward: act must be an STK_ACT_* kind, and only STK_ACT_RELU takes a residual");
   STK_REQUIRE(c, out ? grad_residual != nullptr : bias != nullptr,
               "stk_bn_act_backward: a residual site needs grad_residual, a site without one needs bias");
+  STK_REQUIRE(c, grad_pre == nullptr || act != STK_ACT_RELU, "stk_bn_act_backward: grad_pre is not written for STK_ACT_RELU");
   STK_REQUIRE(c, channels > 0 && channels % 8 == 0 && numel % channels == 0 && numel >= channels,
               "stk_bn_act_backward: channels must be a positive multiple of 8 dividing numel");
   STK_REQUIRE(c, numel < (size_t(1) << 31), "stk_bn_act_backward: numel must be below 2^31");
   const uintptr_t align = uintptr_t(grad) | uintptr_t(x) | uintptr_t(out) | uintptr_t(mean) | uintptr_t(invstd) |
                           uintptr_t(weight) | uintptr_t(bias) | uintptr_t(grad_x) | uintptr_t(grad_weight) |
-                          uintptr_t(grad_bias) | uintptr_t(grad_residual) | uintptr_t(workspace);
+                          uintptr_t(grad_bias) | uintptr_t(grad_residual) | uintptr_t(grad_pre) | uintptr_t(workspace);
   STK_REQUIRE(c, align % 16 == 0, "stk_bn_act_backward: every tensor must be 16-byte aligned");
   DeviceGuard g(c->device);
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
@@ -369,11 +451,11 @@ int stk_bn_act_backward(stk_ctx* c, const void* grad, const void* x, const void*
   const bool res = out != nullptr;
   const uint32_t gb = kBwdThreads / (kChains * cfg.block_y);   // block_y <= 512 / 8 since channels >= 8
   const dim3 grid((groups + gb - 1) / gb, cfg.grid_y);
-  auto reduce = res ? k_bn_bwd_reduce<true> : k_bn_bwd_reduce<false>;
+  auto reduce = STK_BN_KERNEL(k_bn_bwd_reduce, act, res);
   auto bf = [](const void* p) { return static_cast<const __nv_bfloat16*>(p); };
   reduce<<<grid, kBwdThreads, 0, s>>>(static_cast<const uint4*>(grad), static_cast<const uint4*>(x),
                                       static_cast<const uint4*>(out), mean, invstd, bf(weight), bf(bias),
-                                      static_cast<uint4*>(grad_residual), workspace,
+                                      static_cast<uint4*>(res ? grad_residual : grad_pre), workspace,
                                       static_cast<__nv_bfloat16*>(grad_weight), static_cast<__nv_bfloat16*>(grad_bias),
                                       rows, groups, cfg.block_y, cfg.loops);
   STK_CUDA(c, cudaGetLastError());
@@ -386,7 +468,7 @@ int stk_bn_act_backward(stk_ctx* c, const void* grad, const void* x, const void*
   }
   if (grad_x) {
     const uint32_t nvec = uint32_t(numel / 8);
-    auto elemt = res ? k_bn_bwd_elemt<true> : k_bn_bwd_elemt<false>;
+    auto elemt = STK_BN_KERNEL(k_bn_bwd_elemt, act, res);
     const size_t resident = size_t(blocks_per_sm(c, elemt, kBnThreads)) * c->sm_count;
     size_t blocks = std::min(resident, (size_t(nvec) + kBnThreads - 1) / kBnThreads);
     blocks = std::max(blocks, (size_t(groups) + kBnThreads - 1) / kBnThreads);
@@ -398,6 +480,13 @@ int stk_bn_act_backward(stk_ctx* c, const void* grad, const void* x, const void*
     STK_CUDA(c, cudaGetLastError());
   }
   return STK_OK;
+}
+
+int stk_bn_act_backward(stk_ctx* c, const void* grad, const void* x, const void* out, const float* mean, const float* invstd,
+                        const void* weight, const void* bias, void* grad_x, void* grad_weight, void* grad_bias,
+                        void* grad_residual, float* workspace, size_t numel, size_t channels, void* stream) {
+  return stk_bn_act_backward_ex(c, STK_ACT_RELU, grad, x, out, mean, invstd, weight, bias, grad_x, grad_weight, grad_bias,
+                                grad_residual, nullptr, workspace, numel, channels, stream);
 }
 
 }  // extern "C"

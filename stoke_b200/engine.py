@@ -326,28 +326,34 @@ class Engine:
         return out.value
 
     def bn_act(self, x: torch.Tensor, residual: Optional[torch.Tensor], mean: torch.Tensor, var: torch.Tensor,
-               weight: torch.Tensor, bias: torch.Tensor, eps: float, out: torch.Tensor, save_invstd: torch.Tensor):
-        """``out = relu(bn(x) [+ residual])`` over a bf16 channels-last tensor from torch's fp32 batch statistics; writes
-        ``save_invstd`` (``stk_bn_act``).  ``fuse.py`` checks dtypes, layout and alignment before calling."""
-        self._check(self.lib.stk_bn_act(self.ctx, x.data_ptr(), residual.data_ptr() if residual is not None else None,
-                                        mean.data_ptr(), var.data_ptr(), weight.data_ptr(), bias.data_ptr(), float(eps),
-                                        out.data_ptr(), save_invstd.data_ptr(), x.numel(), x.shape[1], self._stream()))
+               weight: torch.Tensor, bias: torch.Tensor, eps: float, out: torch.Tensor, save_invstd: torch.Tensor,
+               act: int = _lib.ACT_RELU):
+        """``out = act(bn(x) [+ residual])`` over a bf16 channels-last tensor from torch's fp32 batch statistics; writes
+        ``save_invstd`` (``stk_bn_act_ex``).  ``act`` is one of ``_lib.ACT_*``; only ReLU takes a residual.  ``fuse.py``
+        checks dtypes, layout and alignment before calling."""
+        self._check(self.lib.stk_bn_act_ex(self.ctx, act, x.data_ptr(), residual.data_ptr() if residual is not None else None,
+                                           mean.data_ptr(), var.data_ptr(), weight.data_ptr(), bias.data_ptr(), float(eps),
+                                           out.data_ptr(), save_invstd.data_ptr(), x.numel(), x.shape[1], self._stream()))
         self.launches += 1
 
     def bn_act_backward(self, grad: torch.Tensor, x: torch.Tensor, out: Optional[torch.Tensor], mean: torch.Tensor,
                         invstd: torch.Tensor, weight: torch.Tensor, bias: Optional[torch.Tensor],
                         grad_x: Optional[torch.Tensor], grad_weight: torch.Tensor, grad_bias: torch.Tensor,
-                        grad_residual: Optional[torch.Tensor]):
-        """Backward of ``bn_act`` (``stk_bn_act_backward``): the ReLU mask comes from ``out`` at a site with a residual
-        (``grad_residual`` receives the masked gradient) and from ``x``, ``weight``, ``bias`` otherwise (``out`` None);
-        ``grad_x`` None skips the elementwise pass.  ``fuse.py`` checks dtypes, layout and alignment before calling."""
+                        grad_residual: Optional[torch.Tensor], act: int = _lib.ACT_RELU,
+                        grad_pre: Optional[torch.Tensor] = None):
+        """Backward of ``bn_act`` (``stk_bn_act_backward_ex``): the ReLU mask comes from ``out`` at a site with a
+        residual (``grad_residual`` receives the masked gradient); otherwise (``out`` None) the activation's input is
+        recomputed from ``x``, ``weight``, ``bias``, and ``grad_pre``, when given, receives the gradient at it (not for
+        ReLU).  ``grad_x`` None skips the elementwise pass.  ``fuse.py`` checks dtypes, layout and alignment before
+        calling."""
         c = x.shape[1]
         ws = torch.empty(2 * (1 + 128) * c, dtype=torch.float32, device=x.device)
         ptr = lambda t: t.data_ptr() if t is not None else None  # noqa: E731
-        self._check(self.lib.stk_bn_act_backward(self.ctx, grad.data_ptr(), x.data_ptr(), ptr(out), mean.data_ptr(),
-                                                 invstd.data_ptr(), weight.data_ptr(), ptr(bias), ptr(grad_x),
-                                                 grad_weight.data_ptr(), grad_bias.data_ptr(), ptr(grad_residual),
-                                                 ws.data_ptr(), x.numel(), c, self._stream()))
+        self._check(self.lib.stk_bn_act_backward_ex(self.ctx, act, grad.data_ptr(), x.data_ptr(), ptr(out),
+                                                    mean.data_ptr(), invstd.data_ptr(), weight.data_ptr(), ptr(bias),
+                                                    ptr(grad_x), grad_weight.data_ptr(), grad_bias.data_ptr(),
+                                                    ptr(grad_residual), ptr(grad_pre), ws.data_ptr(), x.numel(), c,
+                                                    self._stream()))
         self.launches += _bn_bwd_launches(x.numel() // c, c, grad_x is not None)
 
     def barrier(self):

@@ -1,32 +1,51 @@
 # -*- coding: utf-8 -*-
-"""BatchNorm2d -> [add] -> ReLU in one pass for bf16 channels-last training (``stk_bn_act``, csrc/bn_act.cu).
+"""BatchNorm2d -> [add] -> activation in one pass for bf16 channels-last training (``stk_bn_act_ex``, csrc/bn_act.cu).
 
 ``fuse_bn_act(module, engine)`` traces ``module`` with ``torch.fx`` into a ``GraphModule`` that shares every submodule,
-parameter and buffer with ``module``, in which each ``BatchNorm2d -> ReLU`` and ``BatchNorm2d -> add -> ReLU`` chain
-(every intermediate with that single user) is one ``BnAct`` call.  It returns a ``FusedForward``, which runs that graph
-only for calls it is a faithful trace of (training mode, required arguments only, no hooks) and ``module`` itself for
-every other call, or None when tracing or rewriting fails or nothing matches; the caller then keeps running ``module``.
+parameter and buffer with ``module``, in which each ``BatchNorm2d -> act`` and ``BatchNorm2d -> add -> ReLU`` chain
+(every intermediate with that single user) is one ``BnAct`` call.  ``act`` is ReLU, SiLU, Hardswish or ReLU6, as a module
+(``nn.ReLU``, ``nn.SiLU``, ``nn.Hardswish``, ``nn.ReLU6``) or a function (``F.relu`` / ``torch.relu``, ``F.silu``,
+``F.hardswish``, ``F.relu6``), in place or not; a residual add is fused only before a ReLU.  It returns a
+``FusedForward``, which runs that graph only for calls it is a faithful trace of (training mode, required arguments
+only, no hooks) and ``module`` itself for every other call, or None when tracing or rewriting fails or nothing matches;
+the caller then keeps running ``module``.
 
 What stays torch's: the forward statistics and the running-statistics update (``torch.batch_norm_update_stats``, the
-reduction the native training forward runs).  The forward's elementwise apply / add / ReLU is one kernel, which rounds
-every intermediate as the unfused ops do.  The backward (``stk_bn_act_backward``) folds the ReLU's ``threshold_backward``
-into the two passes of torch's channels-last ``native_batch_norm_backward`` and adds its per-channel sums in torch's
-order, so every result is bit-identical to the calls autograd makes for the unfused chain.  It takes the gradient when
-torch's BatchNorm backward would run its channels-last kernels on it (``threshold_backward``'s output is channels-last;
-another layout is made channels-last first) and it is bf16 and aligned; otherwise it runs those calls.
+reduction the native training forward runs).  The forward's elementwise apply / add / activation is one kernel, which
+rounds every intermediate as the unfused ops do.  The backward (``stk_bn_act_backward_ex``) folds the activation's
+backward op (``threshold_backward``, ``silu_backward``, ``hardswish_backward``, ``hardtanh_backward``) into the two
+passes of torch's channels-last ``native_batch_norm_backward`` and adds its per-channel sums in torch's order, so every
+result is bit-identical to the calls autograd makes for the unfused chain.  It takes the gradient when torch's BatchNorm
+backward would run its channels-last kernels on it (the activation backward's output is channels-last; another layout
+is made channels-last first) and it is bf16 and aligned; otherwise it runs those calls.
 Each call falls back to the unfused torch ops when the kernel does not cover its inputs (eval mode, no running statistics,
 not bf16, not channels-last, misaligned, C % 8 != 0, 2^31 elements or more, a CPU tensor), so the same inputs give the
 same results whether or not the model was rewritten.
 """
+import functools
 import inspect
 import operator
-from typing import Optional
+from typing import Dict, Optional
 
 import torch
 import torch.nn.functional as F
 
+from ._lib import ACT_HARDSWISH, ACT_RELU, ACT_RELU6, ACT_SILU
+
 _RELU_FNS = (F.relu, torch.relu)
 _ADD_FNS = (operator.add, operator.iadd, torch.add)
+# the activations other than ReLU, as modules and as functions (whose only other argument is ``inplace``)
+_ACT_MODULES = {torch.nn.SiLU: ACT_SILU, torch.nn.Hardswish: ACT_HARDSWISH, torch.nn.ReLU6: ACT_RELU6}
+_ACT_FNS = {F.silu: ACT_SILU, F.hardswish: ACT_HARDSWISH, F.relu6: ACT_RELU6}
+# the unfused activation of a BnAct built without one
+_DEFAULT_ACT_FN = {ACT_RELU: torch.relu, ACT_SILU: F.silu, ACT_HARDSWISH: F.hardswish, ACT_RELU6: F.relu6}
+# the backward op autograd runs for each activation, as a function of (grad, activation input or ReLU output)
+_ACT_BACKWARD = {
+    ACT_RELU: lambda g, y: torch.ops.aten.threshold_backward(g, y, 0),
+    ACT_SILU: lambda g, y: torch.ops.aten.silu_backward(g, y),
+    ACT_HARDSWISH: lambda g, y: torch.ops.aten.hardswish_backward(g, y),
+    ACT_RELU6: lambda g, y: torch.ops.aten.hardtanh_backward(g, y, 0, 6),
+}
 
 
 def _momentum(bn: torch.nn.BatchNorm2d) -> float:
@@ -66,77 +85,93 @@ def _grad_covered(grad: torch.Tensor, x: torch.Tensor) -> bool:
             and grad.is_contiguous(memory_format=torch.channels_last) and _aligned(grad))
 
 
-def _mask_output_channels_last(grad: torch.Tensor, x: torch.Tensor) -> bool:
-    """Whether ``threshold_backward(grad, out)`` (``out`` laid out like ``x``) returns a channels-last tensor, which is
-    what decides whether torch's BatchNorm backward runs its channels-last kernels.  Asked of the op's meta kernel, which
-    lays the output out as every backend does.  A gradient arriving expanded (the average pool's backward) gets one."""
+def _mask_output_channels_last(grad: torch.Tensor, x: torch.Tensor, act: int = ACT_RELU) -> bool:
+    """Whether the activation's backward op (``threshold_backward(grad, out)``, ``silu_backward(grad, y)``, ...; ``out``
+    and ``y`` laid out like ``x``) returns a channels-last tensor, which is what decides whether torch's BatchNorm
+    backward runs its channels-last kernels.  Asked of a structured op's meta kernel, which is TensorIterator's own
+    layout logic: ``threshold_backward``'s for ReLU (its iterator takes ``out`` first, so an NCHW gradient gives a
+    channels-last output), ``silu_backward``'s for the others.  ``silu_backward``, ``hardswish_backward`` and
+    ``hardtanh_backward`` are all binary TensorIterator ops over (grad, y), so an NCHW gradient gives an NCHW output;
+    the Python meta functions of the latter two lay it out differently from their CUDA kernels, so they are not asked.
+    A gradient arriving expanded (the average pool's backward) gets a channels-last output from all of them."""
     def meta(t):
         return torch.empty_strided(t.shape, t.stride(), dtype=t.dtype, device="meta")
 
-    return torch.ops.aten.threshold_backward(meta(grad), meta(x), 0).is_contiguous(memory_format=torch.channels_last)
+    op = _ACT_BACKWARD[ACT_RELU if act == ACT_RELU else ACT_SILU]
+    return op(meta(grad), meta(x)).is_contiguous(memory_format=torch.channels_last)
 
 
 class _BnActFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, x, weight, bias, residual, bn, engine):
+    def forward(ctx, x, weight, bias, residual, bn, engine, act):
         momentum = _momentum(bn)
         mean, var = torch.batch_norm_update_stats(x, bn.running_mean, bn.running_var, momentum)
         out = torch.empty_like(x)
         invstd = torch.empty_like(mean)
-        engine.bn_act(x, residual, mean, var, weight, bias, bn.eps, out, invstd)
-        # the ReLU mask: out at a site with a residual, else recomputed from x and the parameters (bias saved instead)
+        engine.bn_act(x, residual, mean, var, weight, bias, bn.eps, out, invstd, act)
+        # the ReLU mask: out at a site with a residual; otherwise the activation's input is recomputed from x and the
+        # parameters (bias saved instead)
         ctx.save_for_backward(x, weight, out if residual is not None else bias, mean, invstd)
-        ctx.bn, ctx.engine = bn, engine
+        ctx.bn, ctx.engine, ctx.act = bn, engine, act
         ctx.has_residual = residual is not None
         return out
 
     @staticmethod
     def backward(ctx, grad_out):
         x, weight, out_or_bias, mean, invstd = ctx.saved_tensors
-        bn, res = ctx.bn, ctx.has_residual
+        bn, res, act = ctx.bn, ctx.has_residual, ctx.act
         need_x, need_w, need_b, need_r = ctx.needs_input_grad[:4]
         if (grad_out.dtype == torch.bfloat16 and grad_out.shape == x.shape
-                and not grad_out.is_contiguous(memory_format=torch.channels_last) and _mask_output_channels_last(grad_out, x)):
+                and not grad_out.is_contiguous(memory_format=torch.channels_last)
+                and _mask_output_channels_last(grad_out, x, act)):
             grad_out = grad_out.contiguous(memory_format=torch.channels_last)   # same values, so the same g
         if _grad_covered(grad_out, x):
             dx = torch.empty_like(x) if need_x else None
             dw, db = torch.empty_like(weight), torch.empty_like(weight)
             dr = torch.empty_like(x) if res else None
             ctx.engine.bn_act_backward(grad_out, x, out_or_bias if res else None, mean, invstd, weight,
-                                       None if res else out_or_bias, dx, dw, db, dr)
-            return dx, dw if need_w else None, db if need_b else None, dr if need_r else None, None, None
-        # relu(y) <= 0 exactly when y <= 0, so without a residual y = batch_norm_elemt(x) (the transform the forward
-        # kernel reproduces) gives threshold_backward the same mask as out
+                                       None if res else out_or_bias, dx, dw, db, dr, act)
+            return dx, dw if need_w else None, db if need_b else None, dr if need_r else None, None, None, None
+        # without a residual y = batch_norm_elemt(x) (the transform the forward kernel reproduces) is the activation's
+        # input, which its backward op takes (threshold_backward takes relu's output, but relu(y) <= 0 exactly when y <= 0)
         out = out_or_bias if res else torch.batch_norm_elemt(x, weight, out_or_bias, mean, invstd, bn.eps)
-        g = torch.ops.aten.threshold_backward(grad_out, out, 0)
+        g = _ACT_BACKWARD[act](grad_out, out)
         mask = [need_x, need_w, need_b]
         dx, dw, db = torch.ops.aten.native_batch_norm_backward(g, x, weight, bn.running_mean, bn.running_var, mean, invstd,
                                                               True, bn.eps, mask)
         dr = g if res and need_r else None
-        return dx, dw, db, dr, None, None
+        return dx, dw, db, dr, None, None, None
 
 
 class BnAct(torch.nn.Module):
-    """``relu(bn(x) [+ residual])``: one ``stk_bn_act`` launch when the kernel covers the inputs, the unfused torch ops
-    otherwise (``inplace``: the add was ``out += residual``, which keeps ``out``'s dtype).  Holds a reference to the
-    user's BatchNorm2d (shared, not copied)."""
+    """``act(bn(x) [+ residual])``: one ``stk_bn_act_ex`` launch when the kernel covers the inputs, the unfused torch
+    ops otherwise (``inplace``: the add was ``out += residual``, which keeps ``out``'s dtype).  ``act`` is one of
+    ``_lib.ACT_*``; only ReLU takes a residual.  ``act_fn`` is the unfused activation (the user's module or function),
+    by default ``torch.relu``, ``F.silu``, ``F.hardswish`` or ``F.relu6``.  Holds a reference to the user's BatchNorm2d
+    (shared, not copied)."""
 
-    def __init__(self, bn: torch.nn.BatchNorm2d, engine, inplace: bool = False):
+    def __init__(self, bn: torch.nn.BatchNorm2d, engine, inplace: bool = False, act: int = ACT_RELU, act_fn=None):
         super().__init__()
+        if act not in _DEFAULT_ACT_FN:
+            raise ValueError(f"unknown activation kind {act}")
         self.bn = bn
+        self.act = act
         self._engine = engine
         self._inplace = inplace
+        self._act_fn = act_fn if act_fn is not None else _DEFAULT_ACT_FN[act]
 
     def forward(self, x, residual=None):
+        if residual is not None and self.act != ACT_RELU:
+            raise ValueError("BnAct: only a ReLU site takes a residual")
         if _covered(self.bn, x, residual):
-            return _BnActFn.apply(x, self.bn.weight, self.bn.bias, residual, self.bn, self._engine)
+            return _BnActFn.apply(x, self.bn.weight, self.bn.bias, residual, self.bn, self._engine, self.act)
         y = self.bn(x)
         if residual is not None:
             if self._inplace:
                 y += residual
             else:
                 y = y + residual
-        return torch.relu(y)
+        return self._act_fn(y)
 
 
 class _InplaceProxy(torch.fx.Proxy):
@@ -190,6 +225,24 @@ def _is_relu(gm: torch.fx.GraphModule, node: torch.fx.Node) -> bool:
     return node.op == "call_function" and node.target in _RELU_FNS
 
 
+def _other_act(gm: torch.fx.GraphModule, node: torch.fx.Node):
+    """(kind, unfused activation) when ``node`` is a SiLU, Hardswish or ReLU6 module call, or a call of its function
+    whose only other argument is a constant ``inplace``; None otherwise."""
+    if node.op == "call_module":
+        m = gm.get_submodule(node.target)
+        return (_ACT_MODULES[type(m)], m) if type(m) in _ACT_MODULES else None
+    if node.op != "call_function" or node.target not in _ACT_FNS:
+        return None
+    kwargs = dict(node.kwargs)
+    if len(node.args) == 2 and "inplace" not in kwargs:   # f(input, inplace): bound by name, after the input
+        kwargs["inplace"] = node.args[1]
+    elif len(node.args) != 1:
+        return None
+    if set(kwargs) - {"inplace"} or any(isinstance(a, torch.fx.Node) for a in kwargs.values()):
+        return None
+    return _ACT_FNS[node.target], functools.partial(node.target, **kwargs)
+
+
 def _single_bn_input(gm: torch.fx.GraphModule, node) -> bool:
     """``node`` is a BatchNorm2d call on one tensor whose only user is the next node of the chain."""
     return (isinstance(node, torch.fx.Node) and node.op == "call_module" and len(node.users) == 1
@@ -215,12 +268,16 @@ def _trace(module: torch.nn.Module):
 
 def _rewrite(gm: torch.fx.GraphModule, engine) -> int:
     sites = 0
-    for relu in list(gm.graph.nodes):
-        if not _is_relu(gm, relu) or not relu.args:
+    for relu in list(gm.graph.nodes):   # the activation node (a ReLU, or another kind when `other` is set)
+        is_relu = _is_relu(gm, relu)
+        other = None if is_relu else _other_act(gm, relu)
+        if not (is_relu or other) or not relu.args:
             continue
         src, residual, inplace = relu.args[0], None, False
-        if (isinstance(src, torch.fx.Node) and src.op == "call_function" and src.target in _ADD_FNS and len(src.users) == 1
-                and len(src.args) == 2 and not src.kwargs and all(isinstance(a, torch.fx.Node) for a in src.args)):
+        # a residual add is fused only before a ReLU
+        if (other is None and isinstance(src, torch.fx.Node) and src.op == "call_function" and src.target in _ADD_FNS
+                and len(src.users) == 1 and len(src.args) == 2 and not src.kwargs
+                and all(isinstance(a, torch.fx.Node) for a in src.args)):
             a, b = src.args
             inplace = src.target is operator.iadd
             # an out-of-place add takes the BatchNorm on either side (two-operand float addition is commutative); `+=`
@@ -234,13 +291,35 @@ def _rewrite(gm: torch.fx.GraphModule, engine) -> int:
         if not _single_bn_input(gm, bn_node):
             continue
         name = bn_node.target.replace(".", "_") + "_act"
-        gm.add_submodule(name, BnAct(gm.get_submodule(bn_node.target), engine, inplace))
+        bn = gm.get_submodule(bn_node.target)
+        gm.add_submodule(name, BnAct(bn, engine, inplace) if other is None else BnAct(bn, engine, act=other[0],
+                                                                                         act_fn=other[1]))
         with gm.graph.inserting_before(relu):
             fused = gm.graph.call_module(name, (bn_node.args[0],) + ((residual,) if residual is not None else ()))
         relu.replace_all_uses_with(fused)
         for n in chain + [bn_node]:
             gm.graph.erase_node(n)
         sites += 1
+    return sites
+
+
+def site_shapes(fwd: FusedForward, *example) -> Dict[tuple, int]:
+    """{(act, C, H, W, eps, momentum): number of sites} of a rewritten model: runs its graph once on ``example`` (meta
+    tensors of a model built on the meta device work, and cost no arithmetic) with hooks on the ``BnAct`` modules."""
+    sites: Dict[tuple, int] = {}
+
+    def hook(mod, args, out):
+        _, c, h, w = args[0].shape
+        key = (mod.act, c, h, w, mod.bn.eps, mod.bn.momentum)
+        sites[key] = sites.get(key, 0) + 1
+
+    handles = [m.register_forward_hook(hook) for m in fwd.graph_module.modules() if isinstance(m, BnAct)]
+    try:
+        with torch.no_grad():
+            fwd.graph_module(*example)
+    finally:
+        for h in handles:
+            h.remove()
     return sites
 
 
