@@ -32,10 +32,11 @@
  *   stk_grad_scale                   clip_grad_norm_'s scaling pass / clip_grad_value_ (stoke/fp16.py:184, 233) for the
  *                                    stock-optimizer route (any torch.optim class, stoke/extensions.py:53-78)
  *   stk_loss_sync_begin/_wait        detach_and_sync_loss without the per-micro-step host synchronisation
- *   stk_optim_range_prologue         torch's per-parameter `state[p]["step"]` (torch/optim/adam.py: a parameter whose grad is None
- *                                    is not stepped and keeps its own count) for models with sometimes-unused parameters
- *   stk_optim_step_prologue          the same for every kind, plus NAdam's `state[p]["mu_product"]` (torch/optim/nadam.py)
- *                                    and ASGD's `state[p]["eta"]` / `["mu"]` (torch/optim/asgd.py) without `.item()`
+ *   stk_optim_step_prologue          the per-step scalars of the kinds after SGD; torch's per-parameter `state[p]["step"]`
+ *                                    (torch/optim/adam.py: a parameter whose grad is None is not stepped and keeps its own
+ *                                    count) for models with sometimes-unused parameters; NAdam's `state[p]["mu_product"]`
+ *                                    (torch/optim/nadam.py) and ASGD's `state[p]["eta"]` / `["mu"]` (torch/optim/asgd.py)
+ *                                    without `.item()`
  *   stk_adafactor_plan / _step       torch.optim.Adafactor's step (torch/optim/_adafactor.py _single_tensor_adafactor) plus
  *                                    the clip and the GradScaler.step gate, without its two .item() per parameter
  */
@@ -274,34 +275,26 @@ typedef struct {
   int n_ranges; const uint32_t* range_end_vec; const uint8_t* range_group;  /* DEVICE arrays; ends in units of 8 elements */
   size_t grid_n;   /* cross-rank (lp_world > 1) launches: the LARGEST n_local over the ranks, identical on every rank, so that
                       every rank launches the same grid (the block barriers pair block b with block b); 0: n_local */
-  const float* range_bc;  /* DEVICE, 4 floats per range {step_size, bias_correction2_sqrt, first_step, 0} written by
-                             stk_optim_range_prologue (NAdam / RAdam / Adamax: the layout of stk_optim_step_prologue,
-                             which writes it for every kind): per-PARAMETER step counts (torch keeps `step` per parameter, so a
-                             parameter that skipped some steps has its own bias corrections); NULL: the optimizer-wide
-                             counter of the selected state is used for every range */
+  const float* range_bc;  /* DEVICE, 4 floats per RANGE written by stk_optim_step_prologue with n_ranges > 0: per-PARAMETER
+                             step counts (torch keeps `step` per parameter, so a parameter that skipped some steps has its
+                             own bias corrections); NULL: group_bc */
   const stk_optim_hyper_ext_t* hyper_ext;  /* n_groups entries or NULL (all zero): the extras of the kinds after SGD */
   const float* group_bc;  /* DEVICE, 4 floats per GROUP written by stk_optim_step_prologue with n_ranges = 0; used where
-                             range_bc is NULL.  Every kind after SGD needs group_bc or range_bc: their per-step scalars
-                             (NAdam's and ASGD's come from scalar state that only the prologue advances) are formed once
-                             by the prologue, not in every block.  Ignored by ADAM / ADAMW / SGD.  ASGD takes no
-                             exp_avg_sq */
+                             range_bc is NULL.  NULL: ADAM / ADAMW / SGD form the scalars of the optimizer-wide step
+                             themselves.  Every kind after SGD needs group_bc or range_bc: their per-step scalars (NAdam's
+                             and ASGD's come from scalar state that only the prologue advances) are formed once by the
+                             prologue, not in every block.  ASGD takes no exp_avg_sq */
 } stk_optim_args_t;
 int stk_optim_step_ex(stk_ctx* ctx, const stk_optim_args_t* args, void* stream);
-/* Per-range step bookkeeping for stk_optim_step_ex (call it right before, same stream): for every range j computes the
- * bias corrections of step range_steps[j] + 1 with its group's hyper-parameters into range_bc[4j..4j+3] and, unless the range
- * is skipped this step (bit 7 of range_group[j]) or the selected state says found_inf, increments range_steps[j].
- * All three arrays live in device memory. */
-int stk_optim_range_prologue(stk_ctx* ctx, const stk_optim_hyper_t* hyper, int n_groups, int n_ranges,
-                             const uint8_t* range_group, int32_t* range_steps, float* range_bc, void* stream);
 /* Step bookkeeping for every kind, including the per-entry scalar state of NAdam and ASGD (call it right before
  * stk_optim_step_ex, same stream).
- * n_ranges > 0: per range j, like stk_optim_range_prologue: the scalars of step t = range_steps[j] + 1 with the group
- *   hyper[range_group[j] & 0x7f] go to bc[4j..4j+3] (pass bc as the step's range_bc), and unless bit 7 is set or the
- *   selected state says found_inf, range_steps[j] and entry j's scalar state advance.
+ * n_ranges > 0: per range j: the scalars of step t = range_steps[j] + 1 with the group hyper[range_group[j] & 0x7f] go to
+ *   bc[4j..4j+3] (pass bc as the step's range_bc), and unless the range is skipped this step (bit 7 of range_group[j]) or
+ *   the selected state says found_inf, range_steps[j] and entry j's scalar state advance.
  * n_ranges = 0: per group g, with t = the selected state's optimizer-wide counter + 1: bc[4g..4g+3] (pass bc as the
  *   step's group_bc) and, unless found_inf, entry g's scalar state advances.  range_group and range_steps are not read.
  * The four floats per entry, computed in double from torch's python-scalar formulas and stored as fp32:
- *   ADAM / ADAMW / SGD: {lr / bc1, sqrt(bc2), t == 1, 0}     (the values stk_optim_range_prologue writes)
+ *   ADAM / ADAMW: {lr / bc1, sqrt(bc2), t == 1, 0}
  *   NADAM:  {c_g, c_m, bc2, 0}: param += c_g grad / denom + c_m exp_avg / denom, denom = sqrt(exp_avg_sq / bc2) + eps,
  *           c_g = -lr (1 - mu_t) / (1 - P_t), c_m = -lr mu_{t+1} / (1 - P_t mu_{t+1}), P_t = fp32(P_{t-1} * fp32(mu_t))
  *           is the advanced mu_product (torch: mu_product *= mu, then .item())
@@ -309,18 +302,19 @@ int stk_optim_range_prologue(stk_ctx* ctx, const stk_optim_hyper_t* hyper, int n
  *           c = lr rect sqrt(bc2) / bc1, param -= c exp_avg / (sqrt(exp_avg_sq) + eps); else rectified = 0,
  *           c = lr / bc1, param -= c exp_avg
  *   ADAMAX: {lr / bc1, 0, 0, 0}: param -= (lr / bc1) exp_avg / exp_inf
- *   ADADELTA, RPROP: {0, 0, t == 1, 0}: Rprop's first step seeds step_size with the lr passed now (torch: full_like(p, lr)
- *           at the parameter's first step) and takes prev as 0; the exp_avg_sq buffer is not used then
+ *   SGD, ADADELTA, RPROP: {0, 0, t == 1, 0}: SGD's first step seeds the momentum buffer with the gradient; Rprop's seeds
+ *           step_size with the lr passed now (torch: full_like(p, lr) at the parameter's first step) and takes prev as 0;
+ *           the exp_avg_sq buffer is not used then
  *   ASGD:   {-eta, 1 - lambd eta, mu, 0} with the STORED fp32 eta and mu (the lr and 1 at t == 1, torch's lazy
  *           initialisation): param = param (1 - lambd eta) - eta grad; ax = param if mu == 1 (ax not read), else
  *           ax + (param - ax) mu.  Then eta = lr / (1 + lambd lr t)^alpha and mu = 1 / max(1, t - t0), as fp32
- * with bc1 = 1 - beta1^t, bc2 = 1 - beta2^t.  The scalar state `mu_product` (fp32, torch keeps it per parameter) holds per
+ * with bc1 = 1 - beta1^t, bc2 = 1 - beta2^t.  The scalar state `scalar_state` (fp32, torch keeps it per parameter) holds per
  * range or per group: NADAM one float, mu_product (torch initialises it to 1); ASGD two floats, {eta, mu}.  It is read and
  * written only for those two kinds and may be NULL for the others; hyper_ext may be NULL (all zero).
  * All pointers but hyper / hyper_ext are device memory; bc must be 16-byte aligned. */
 int stk_optim_step_prologue(stk_ctx* ctx, const stk_optim_hyper_t* hyper, const stk_optim_hyper_ext_t* hyper_ext,
                             int n_groups, int n_ranges, const uint8_t* range_group, int32_t* range_steps,
-                            float* mu_product, float* bc, void* stream);
+                            float* scalar_state, float* bc, void* stream);
 
 /* scaler.update(), opt_steps/skipped_steps bookkeeping, reset of the per-step accumulators */
 int stk_step_epilogue(stk_ctx* ctx, void* stream);

@@ -293,7 +293,7 @@ def sgd_bound(w, buf, G, e_g, hyper: Dict, ref_w, ref_buf):
 # ---- per-range bookkeeping and the loss scaler ----------------------------------------------------------------------------
 def bias_corrections(hyper: Dict, done: int) -> Tuple[float, float]:
     """(step_size, sqrt(bias_correction2)) of step done + 1 in float64, as torch/optim/adam.py forms them from python
-    floats, then cast to fp32 (what stk_optim_range_prologue stores).  The kernel must be within 1 fp32 ulp."""
+    floats, then cast to fp32 (what stk_optim_step_prologue stores for Adam).  The kernel must be within 1 fp32 ulp."""
     t = float(done + 1)
     bc1 = 1.0 - hyper["beta1"] ** t
     bc2 = 1.0 - hyper["beta2"] ** t

@@ -140,7 +140,6 @@ _SIGNATURES = {
     "stk_optim_step": (C.c_int, [_P, C.POINTER(OptimHyper), _P, _P, _P, _P, C.c_size_t, _PP, C.c_int, C.c_int,
                                  C.c_size_t, _P]),
     "stk_optim_step_ex": (C.c_int, [_P, C.POINTER(OptimArgs), _P]),
-    "stk_optim_range_prologue": (C.c_int, [_P, C.POINTER(OptimHyper), C.c_int, C.c_int, _P, _P, _P, _P]),
     "stk_optim_step_prologue": (C.c_int, [_P, C.POINTER(OptimHyper), C.POINTER(OptimHyperExt), C.c_int, C.c_int, _P, _P,
                                           _P, _P, _P]),
     "stk_step_epilogue": (C.c_int, [_P, _P]),

@@ -40,9 +40,9 @@ struct GroupHyperD {   // host-side doubles, converted exactly like torch conver
   double lambd, alpha, t0;                       // ASGD
 };
 struct GroupHyperS {   // what the inner loop reads (shared memory, one entry per parameter group)
-  float step_size, bc2_sqrt, b2, eps, wd, one_m_b1, one_m_b2, lr, one_m_damp, decay_mul, mom;
+  float b2, eps, wd, one_m_b1, one_m_b2, lr, one_m_damp, decay_mul, mom;
   int nesterov, maximize;
-  float c0, c1, c2;  // the kinds of stk_optim_step_prologue: the per-step scalars (its layout)
+  float c0, c1, c2;  // the per-step scalars of step_scalars (the layout documented at stk_optim_step_prologue)
   int decoupled;
   float rho, one_m_rho;                         // Adadelta
   float etaminus, etaplus, ss_min, ss_max;      // Rprop
@@ -78,23 +78,21 @@ struct OptimParams {
   int n_ranges;                              // 0: group 0 everywhere
   const uint32_t* range_end;                 // device, ascending, vector units (global)
   const uint8_t* range_group;                // device; bit 7: skip
-  const float4* range_bc;                    // device, optional: per-range {step_size, bc2_sqrt, first_step, 0}
-  const float4* group_bc;                    // device: per-group scalars of the NAdam / RAdam / Adamax kinds
+  const float4* range_bc;                    // device, optional: per-range scalars of stk_optim_step_prologue
+  const float4* group_bc;                    // device, optional: per-group scalars of stk_optim_step_prologue
 };
 
-// the kinds whose per-step scalars come from stk_optim_step_prologue (group_bc / range_bc), not from the kernel itself
-__host__ __device__ constexpr bool is_new_kind(int kind) { return kind >= STK_OPT_NADAM && kind <= STK_OPT_ASGD; }
-// floats of per-entry scalar state the prologue carries (the stk_optim_step_prologue `mu_product` array)
+// floats of per-entry scalar state the prologue carries (the stk_optim_step_prologue `scalar_state` array)
 __host__ __device__ constexpr int scalar_state_width(int kind) {
   return kind == STK_OPT_NADAM ? 1 : (kind == STK_OPT_ASGD ? 2 : 0);
 }
 
-// Per-step scalars of the update of step t of the prologue's kinds (the float4 layout documented at
-// stk_optim_step_prologue), in double from the python-scalar formulas of torch's single-tensor functions.  st: the entry's
-// scalar state before the step on entry, after it on return (fp32, like torch's tensors): NAdam's mu_product; ASGD's
-// {eta, mu}.
-__device__ __forceinline__ float4 new_kind_scalars(int kind, const GroupHyperD& h, double t, float* st) {
-  if (kind == STK_OPT_ADADELTA || kind == STK_OPT_RPROP)  // Rprop: step_size = full_like(p, lr) at the first step
+// Per-step scalars of the update of step t (the float4 layout documented at stk_optim_step_prologue), in double from the
+// python-scalar formulas of torch's single-tensor functions.  st: the entry's scalar state before the step on entry, after
+// it on return (fp32, like torch's tensors): NAdam's mu_product; ASGD's {eta, mu}; not touched for the other kinds.
+__device__ __forceinline__ float4 step_scalars(int kind, const GroupHyperD& h, double t, float* st) {
+  // SGD: the first step seeds the momentum buffer; Rprop: step_size = full_like(p, lr) at the first step
+  if (kind == STK_OPT_SGD || kind == STK_OPT_ADADELTA || kind == STK_OPT_RPROP)
     return make_float4(0.f, 0.f, t == 1.0 ? 1.f : 0.f, 0.f);
   if (kind == STK_OPT_ASGD) {  // torch/optim/asgd.py: the update uses the STORED eta and mu, then both advance
     float eta = st[0], mu = st[1];
@@ -109,6 +107,8 @@ __device__ __forceinline__ float4 new_kind_scalars(int kind, const GroupHyperD& 
   }
   const double bc1 = 1.0 - pow(h.beta1, t);
   const double bc2 = 1.0 - pow(h.beta2, t);
+  if (kind == STK_OPT_ADAM || kind == STK_OPT_ADAMW)  // torch/optim/adam.py:531-547: step_size, bias_correction2_sqrt
+    return make_float4((float)(h.lr / bc1), (float)sqrt(bc2), t == 1.0 ? 1.f : 0.f, 0.f);
   if (kind == STK_OPT_NADAM) {  // torch/optim/nadam.py: mu, mu_next, mu_product *= mu, the two addcdiv_ values
     const double mu = h.beta1 * (1.0 - 0.5 * pow(0.96, t * h.momentum_decay));
     const double mu_next = h.beta1 * (1.0 - 0.5 * pow(0.96, (t + 1.0) * h.momentum_decay));
@@ -195,13 +195,13 @@ __device__ __forceinline__ void store_lp(const OptimParams& p, size_t gv, const 
 // PERSIST = false: one-shot launch, VPT vectors per thread (local step; tools/membench.cu compares it with a persistent
 // grid-stride loop).  PERSIST = true: co-resident grid-stride loop, required when the kernel
 // pushes its shard to peers and therefore carries the cross-rank block barriers (sharded / OSS step).
-// ASGD asks for two co-resident blocks per SM: left to itself, ptxas caps its paired sharded form at 80 registers and
-// spills (its conditional ax load); with the bound it takes 84 and none spills.  A minimum of 0 is no minimum: the other
-// kinds compile exactly as with __launch_bounds__(256).
+// The kinds after SGD ask for two co-resident blocks per SM: left to themselves, ptxas caps ASGD's paired sharded form at
+// 80 registers and NAdam's and RAdam's unpaired sharded forms at 64, and spills (ASGD's conditional ax load); with the
+// bound none spills.  A minimum of 0 is no minimum: Adam, AdamW and SGD compile exactly as with __launch_bounds__(256).
 template <int KIND, int LP_DT, bool PERSIST, int VPT, int GRAD, bool RAW>
-__global__ void __launch_bounds__(256, KIND == STK_OPT_ASGD ? 2 : 0) k_optim_step(const OptimParams p) {
+__global__ void __launch_bounds__(256, KIND >= STK_OPT_NADAM ? 2 : 0) k_optim_step(const OptimParams p) {
   __shared__ GroupHyperS s_g[STK_MAX_GROUPS];
-  __shared__ int s_skip, s_first;
+  __shared__ int s_skip;
   __shared__ float s_inv_scale;
   if (PERSIST && p.cross_rank && !block_barrier_all_ranks(p.pads, p.rank, p.world, 0, p.epoch)) return;
   unsigned long long t_begin = 0;
@@ -247,22 +247,19 @@ __global__ void __launch_bounds__(256, KIND == STK_OPT_ASGD ? 2 : 0) k_optim_ste
 
   if (threadIdx.x == 0) {
     s_skip = p.scaler->found_inf != 0;  // GradScaler.step: no optimizer.step() at all when any grad is inf/nan
-    s_first = (p.scaler->opt_steps == 0) ? 1 : 0;  // SGD: first step seeds the momentum buffer with the gradient
     s_inv_scale = (RAW && p.unscale) ? (float)(1.0 / (double)p.scaler->scale) : 1.f;
   }
   if (threadIdx.x < (unsigned)p.n_groups) {
     const GroupHyperD& h = p.g[threadIdx.x];
     GroupHyperS o;
-    // bias corrections in double, exactly as the python scalars in torch/optim/adam.py:531-547
-    const double t = (double)(p.scaler->opt_steps + 1);
-    o.step_size = 0.f;
-    o.bc2_sqrt = 1.f;
-    if (KIND != STK_OPT_SGD) {
-      const double bc1 = 1.0 - pow(h.beta1, t);
-      const double bc2 = 1.0 - pow(h.beta2, t);
-      o.step_size = (float)(h.lr / bc1);
-      o.bc2_sqrt = (float)sqrt(bc2);
-    }
+    // the per-step scalars: stk_optim_step_prologue's when given; else Adam / AdamW / SGD form the optimizer-wide step's
+    // here (in double, ahead of the rest so that the pow() latency overlaps the loads) and the kinds after SGD take range_bc
+    float4 c = make_float4(0.f, 0.f, 0.f, 0.f);
+    if constexpr (KIND <= STK_OPT_SGD) c = step_scalars(KIND, h, (double)(p.scaler->opt_steps + 1), nullptr);
+    if (p.group_bc != nullptr) c = p.group_bc[threadIdx.x];
+    o.c0 = c.x;
+    o.c1 = c.y;
+    o.c2 = c.z;
     o.b2 = (float)h.beta2;
     o.eps = (float)h.eps;
     o.wd = (float)h.weight_decay;
@@ -274,13 +271,6 @@ __global__ void __launch_bounds__(256, KIND == STK_OPT_ASGD ? 2 : 0) k_optim_ste
     o.mom = (float)h.momentum;
     o.nesterov = h.nesterov;
     o.maximize = h.maximize;
-    o.c0 = o.c1 = o.c2 = 0.f;
-    if (is_new_kind(KIND) && p.group_bc != nullptr) {  // stk_optim_step_prologue's values (nullptr: range_bc has them)
-      const float4 c = p.group_bc[threadIdx.x];
-      o.c0 = c.x;
-      o.c1 = c.y;
-      o.c2 = c.z;
-    }
     o.decoupled = h.decoupled;
     if constexpr (KIND == STK_OPT_ADADELTA) {
       o.rho = (float)h.rho;
@@ -296,7 +286,6 @@ __global__ void __launch_bounds__(256, KIND == STK_OPT_ASGD ? 2 : 0) k_optim_ste
   }
   __syncthreads();
   const bool skip_all = s_skip != 0;
-  const bool first_step = s_first != 0;
   float coef = 1.f;
   // clamps keep NaN like torch.clamp: a NaN norm (a NaN gradient without a loss scaler) makes every gradient NaN, as
   // clip_grad_norm_ does, and clip by value passes a NaN element through
@@ -313,17 +302,10 @@ __global__ void __launch_bounds__(256, KIND == STK_OPT_ASGD ? 2 : 0) k_optim_ste
       if (p.range_bc != nullptr) bc = __ldg(&p.range_bc[rj]);
     }
     GroupHyperS h = s_g[rb & 0x7f];
-    bool first_here = first_step;
     if (p.range_bc != nullptr) {  // per-parameter step counts (torch's `state[p]["step"]`)
-      if constexpr (is_new_kind(KIND)) {
-        h.c0 = bc.x;
-        h.c1 = bc.y;
-        h.c2 = bc.z;
-      } else {
-        h.step_size = bc.x;
-        h.bc2_sqrt = bc.y;
-        first_here = bc.z != 0.f;
-      }
+      h.c0 = bc.x;
+      h.c1 = bc.y;
+      h.c2 = bc.z;
     }
     const bool skip = skip_all || (rb & 0x80u);
     if (!skip) {
@@ -351,8 +333,8 @@ __global__ void __launch_bounds__(256, KIND == STK_OPT_ASGD ? 2 : 0) k_optim_ste
             mm = fmaf(h.one_m_b1, gg - mm, mm);                      // exp_avg.lerp_(grad, 1 - beta1)
             float vv = v[k][e] * h.b2;
             vv = fmaf(h.one_m_b2 * gg, gg, vv);                      // mul_(beta2).addcmul_(grad, grad, value=1-beta2)
-            const float denom = sqrtf(vv) / h.bc2_sqrt + h.eps;
-            ww = ww - h.step_size * (mm / denom);                    // addcdiv_(exp_avg, denom, value=-step_size)
+            const float denom = sqrtf(vv) / h.c1 + h.eps;            // c1 = bias_correction2_sqrt
+            ww = ww - h.c0 * (mm / denom);                           // addcdiv_(exp_avg, denom, value=-step_size)
             m[k][e] = mm;
             v[k][e] = vv;
           } else if (KIND == STK_OPT_NADAM || KIND == STK_OPT_RADAM) {
@@ -418,7 +400,7 @@ __global__ void __launch_bounds__(256, KIND == STK_OPT_ASGD ? 2 : 0) k_optim_ste
           } else {  // SGD
             if (h.wd != 0.f) gg = fmaf(ww, h.wd, gg);
             if (h.mom != 0.f) {
-              const float bb = first_here ? gg : fmaf(m[k][e], h.mom, h.one_m_damp * gg);
+              const float bb = h.c2 != 0.f ? gg : fmaf(m[k][e], h.mom, h.one_m_damp * gg);  // first step: buf = g
               m[k][e] = bb;
               gg = h.nesterov ? fmaf(bb, h.mom, gg) : bb;
             }
@@ -453,72 +435,33 @@ __global__ void __launch_bounds__(256, KIND == STK_OPT_ASGD ? 2 : 0) k_optim_ste
   }
 }
 
-struct RangePrologueParams {
-  GroupHyperD g[STK_MAX_GROUPS];
-  int n_ranges, kind;
-  const uint8_t* range_group;
-  int32_t* range_steps;
-  float4* range_bc;
-  const stk_scaler_state_t* scaler;
-};
-
-// one thread per range: bias corrections of that range's NEXT step (double, like the python scalars of torch/optim/adam.py)
-// and the step count itself (torch increments state[p]["step"] only for parameters that are stepped)
-__global__ void k_range_prologue(const RangePrologueParams p) {
-  const int j = blockIdx.x * blockDim.x + threadIdx.x;
-  if (j >= p.n_ranges) return;
-  const unsigned b = p.range_group[j];
-  const GroupHyperD& h = p.g[b & 0x7f];
-  const int32_t done = p.range_steps[j];
-  const double t = (double)(done + 1);
-  float4 o = make_float4(0.f, 1.f, done == 0 ? 1.f : 0.f, 0.f);
-  if (p.kind != STK_OPT_SGD) {
-    o.x = (float)(h.lr / (1.0 - pow(h.beta1, t)));
-    o.y = (float)sqrt(1.0 - pow(h.beta2, t));
-  }
-  p.range_bc[j] = o;
-  if (!(b & 0x80u) && p.scaler->found_inf == 0) p.range_steps[j] = done + 1;
-}
-
 struct StepPrologueParams {
   GroupHyperD g[STK_MAX_GROUPS];
   int n_groups, n_ranges, kind;
   const uint8_t* range_group;
   int32_t* range_steps;
-  float* mu_product;
+  float* scalar_state;
   float4* bc;
   const stk_scaler_state_t* scaler;
 };
 
 // one thread per range (n_ranges > 0) or per group (n_ranges == 0): the scalars of that entry's NEXT step and, unless it is
-// skipped or the step is (found_inf), the advance of its step count and of its scalar state (NAdam's mu_product, ASGD's
-// eta and mu)
+// skipped or the step is (found_inf), the advance of its step count (torch increments state[p]["step"] only for
+// parameters that are stepped) and of its scalar state (NAdam's mu_product, ASGD's eta and mu)
 __global__ void k_step_prologue(const StepPrologueParams p) {
   const int j = blockIdx.x * blockDim.x + threadIdx.x;
   const bool per_range = p.n_ranges > 0;
   if (j >= (per_range ? p.n_ranges : p.n_groups)) return;
   const unsigned b = per_range ? (unsigned)p.range_group[j] : (unsigned)j;
-  const GroupHyperD& h = p.g[b & 0x7f];
   const int64_t done = per_range ? (int64_t)p.range_steps[j] : p.scaler->opt_steps;
-  const double t = (double)(done + 1);
   const bool advance = !(b & 0x80u) && p.scaler->found_inf == 0;
-  float4 o;
-  if (is_new_kind(p.kind)) {
-    const int w = scalar_state_width(p.kind);
-    float st[2] = {1.f, 1.f};
-    for (int k = 0; k < w; ++k) st[k] = p.mu_product[j * w + k];
-    o = new_kind_scalars(p.kind, h, t, st);
-    if (advance)
-      for (int k = 0; k < w; ++k) p.mu_product[j * w + k] = st[k];
-  } else {  // the values of k_range_prologue
-    o = make_float4(0.f, 1.f, done == 0 ? 1.f : 0.f, 0.f);
-    if (p.kind != STK_OPT_SGD) {
-      o.x = (float)(h.lr / (1.0 - pow(h.beta1, t)));
-      o.y = (float)sqrt(1.0 - pow(h.beta2, t));
-    }
-  }
-  p.bc[j] = o;
-  if (per_range && advance) p.range_steps[j] = (int32_t)(done + 1);
+  const int w = scalar_state_width(p.kind);
+  float st[2] = {1.f, 1.f};
+  for (int k = 0; k < w; ++k) st[k] = p.scalar_state[j * w + k];
+  p.bc[j] = step_scalars(p.kind, p.g[b & 0x7f], (double)(done + 1), st);
+  if (!advance) return;
+  for (int k = 0; k < w; ++k) p.scalar_state[j * w + k] = st[k];
+  if (per_range) p.range_steps[j] = (int32_t)(done + 1);
 }
 
 // scaler.update() (torch/amp/grad_scaler.py:549-556 -> _amp_update_scale_), step counters, per-step accumulator reset
@@ -765,39 +708,16 @@ int stk_optim_step(stk_ctx* c, const stk_optim_hyper_t* h, float* master, float*
   return stk_optim_step_ex(c, &a, stream);
 }
 
-int stk_optim_range_prologue(stk_ctx* c, const stk_optim_hyper_t* h, int n_groups, int n_ranges, const uint8_t* range_group,
-                             int32_t* range_steps, float* range_bc, void* stream) {
-  STK_REQUIRE(c, c && h && range_group && range_steps && range_bc, "stk_optim_range_prologue: NULL argument");
-  STK_REQUIRE(c, n_groups >= 1 && n_groups <= STK_MAX_GROUPS, "stk_optim_range_prologue: n_groups must be in [1, 8]");
-  STK_REQUIRE(c, n_ranges >= 1, "stk_optim_range_prologue: no ranges");
-  STK_REQUIRE(c, (reinterpret_cast<uintptr_t>(range_bc) & 15) == 0, "stk_optim_range_prologue: range_bc must be 16-byte aligned");
-  STK_REQUIRE(c, h->kind >= STK_OPT_ADAM && h->kind <= STK_OPT_SGD,
-              "stk_optim_range_prologue: the kinds after SGD take stk_optim_step_prologue");
-  std::lock_guard<std::mutex> lk(c->mu);
-  DeviceGuard g(c->device);
-  RangePrologueParams p{};
-  fill_groups(p.g, h, nullptr, n_groups);
-  p.n_ranges = n_ranges;
-  p.kind = h->kind;
-  p.range_group = range_group;
-  p.range_steps = range_steps;
-  p.range_bc = reinterpret_cast<float4*>(range_bc);
-  p.scaler = c->scaler_dev;
-  k_range_prologue<<<(n_ranges + 127) / 128, 128, 0, reinterpret_cast<cudaStream_t>(stream)>>>(p);
-  STK_CUDA(c, cudaGetLastError());
-  return STK_OK;
-}
-
 int stk_optim_step_prologue(stk_ctx* c, const stk_optim_hyper_t* h, const stk_optim_hyper_ext_t* ext, int n_groups,
-                            int n_ranges, const uint8_t* range_group, int32_t* range_steps, float* mu_product, float* bc,
+                            int n_ranges, const uint8_t* range_group, int32_t* range_steps, float* scalar_state, float* bc,
                             void* stream) {
   STK_REQUIRE(c, c && h && bc, "stk_optim_step_prologue: NULL argument");
   STK_REQUIRE(c, n_groups >= 1 && n_groups <= STK_MAX_GROUPS, "stk_optim_step_prologue: n_groups must be in [1, 8]");
   STK_REQUIRE(c, n_ranges >= 0, "stk_optim_step_prologue: negative n_ranges");
   STK_REQUIRE(c, n_ranges == 0 || (range_group && range_steps), "stk_optim_step_prologue: range arrays are NULL");
   STK_REQUIRE(c, h->kind >= STK_OPT_ADAM && h->kind <= STK_OPT_ASGD, "stk_optim_step_prologue: bad optimizer kind");
-  STK_REQUIRE(c, scalar_state_width(h->kind) == 0 || mu_product,
-              "stk_optim_step_prologue: NAdam and ASGD need their scalar state (mu_product)");
+  STK_REQUIRE(c, scalar_state_width(h->kind) == 0 || scalar_state,
+              "stk_optim_step_prologue: NAdam and ASGD need their scalar state");
   STK_REQUIRE(c, (reinterpret_cast<uintptr_t>(bc) & 15) == 0, "stk_optim_step_prologue: bc must be 16-byte aligned");
   std::lock_guard<std::mutex> lk(c->mu);
   DeviceGuard g(c->device);
@@ -808,7 +728,7 @@ int stk_optim_step_prologue(stk_ctx* c, const stk_optim_hyper_t* h, const stk_op
   p.kind = h->kind;
   p.range_group = range_group;
   p.range_steps = range_steps;
-  p.mu_product = mu_product;
+  p.scalar_state = scalar_state;
   p.bc = reinterpret_cast<float4*>(bc);
   p.scaler = c->scaler_dev;
   const int n = n_ranges > 0 ? n_ranges : n_groups;

@@ -829,8 +829,9 @@ class GradPath:
 
     def optimizer_step(self, hypers, exts=None):
         """One fused K2 launch (+ the one-thread epilogue).  ``hypers``: one ``OptimHyper`` or a list (one per group).
-        ``exts``: per-group ``OptimHyperExt`` of the kinds after SGD, whose per-step scalars (and the scalar state of
-        NAdam and ASGD) stk_optim_step_prologue forms on the device before the step."""
+        ``exts``: per-group ``OptimHyperExt`` of the kinds after SGD.  stk_optim_step_prologue forms their per-step scalars
+        (and the scalar state of NAdam and ASGD) on the device before the step, and every kind's once step counts are
+        per parameter; the optimizer-wide Adam / AdamW / SGD step forms its own."""
         e = self.engine
         e.state_select(self.state_id)
         if isinstance(hypers, _lib.OptimHyper):
@@ -873,26 +874,22 @@ class GradPath:
             a.lp_ptrs, a.lp_world, a.lp_dtype = None, 0, _lib.F32
         nr, rend, rgrp = self._ranges_for_step()
         a.n_ranges, a.range_end_vec, a.range_group = nr, rend, rgrp
-        if exts is not None:
-            xarr = (_lib.OptimHyperExt * ng)(*exts)
+        per_range = bool(nr) and self._range_steps is not None
+        if exts is not None or per_range:
+            xarr = (_lib.OptimHyperExt * ng)(*exts) if exts is not None else None
             keep.append(xarr)
             a.hyper_ext = xarr
-            per_range = bool(nr) and self._range_steps is not None
-            mu = self._range_scal if per_range else self._group_scal
+            scal = self._range_scal if per_range else self._group_scal
             bc = self._range_bc if per_range else self._group_bc
             e._check(e.lib.stk_optim_step_prologue(e.ctx, harr, xarr, ng, nr if per_range else 0, rgrp if per_range else None,
                                                    self._range_steps.data_ptr() if per_range else None,
-                                                   mu.data_ptr() if mu is not None else None, bc.data_ptr(), e._stream()))
+                                                   scal.data_ptr() if scal is not None else None, bc.data_ptr(),
+                                                   e._stream()))
             e.launches += 1
             if per_range:
                 a.range_bc = bc.data_ptr()
             else:
                 a.group_bc = bc.data_ptr()
-        elif nr and self._range_steps is not None:
-            e._check(e.lib.stk_optim_range_prologue(e.ctx, harr, ng, nr, rgrp, self._range_steps.data_ptr(),
-                                                    self._range_bc.data_ptr(), e._stream()))
-            e.launches += 1
-            a.range_bc = self._range_bc.data_ptr()
         e.optim_step_ex(a)
         e.step_epilogue()
         self._track_touched = False

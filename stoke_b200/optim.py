@@ -38,7 +38,8 @@ _EXT_KINDS = (_lib.OPT_NADAM, _lib.OPT_RADAM, _lib.OPT_ADAMAX, _lib.OPT_ADADELTA
 # element-wise classes whose state torch creates at a parameter's first step (no state_dict entry before it)
 _LAZY_KINDS = (_lib.OPT_ADADELTA, _lib.OPT_RPROP, _lib.OPT_ASGD)
 # torch's per-parameter state keys of the two fp32 buffers M and V (None: no V buffer)
-_STATE_KEYS = {_lib.OPT_ADAM: ("exp_avg", "exp_avg_sq"), _lib.OPT_ADAMW: ("exp_avg", "exp_avg_sq"),
+_STATE_KEYS = {_lib.OPT_SGD: ("momentum_buffer", None),
+               _lib.OPT_ADAM: ("exp_avg", "exp_avg_sq"), _lib.OPT_ADAMW: ("exp_avg", "exp_avg_sq"),
                _lib.OPT_NADAM: ("exp_avg", "exp_avg_sq"), _lib.OPT_RADAM: ("exp_avg", "exp_avg_sq"),
                _lib.OPT_ADAMAX: ("exp_avg", "exp_inf"), _lib.OPT_ADADELTA: ("square_avg", "acc_delta"),
                _lib.OPT_RPROP: ("prev", "step_size"), _lib.OPT_ASGD: ("ax", None)}
@@ -85,6 +86,51 @@ def state_dict_index(group_of: List[int], n_groups: int) -> Dict[int, int]:
     order: torch/optim/optimizer.py ``state_dict``)."""
     order = [i for gi in range(n_groups) for i, g in enumerate(group_of) if g == gi]
     return {flat_i: sd_i for sd_i, flat_i in enumerate(order)}
+
+
+def load_step_counts(kind, entries: List[Dict], group_of: List[int], opt_steps: Optional[int], per_param_on: bool,
+                     momentum: Optional[List[float]] = None):
+    """How a loaded state dict's step counts and scalar state (NAdam's ``mu_product``, ASGD's ``eta`` / ``mu``) go onto
+    the fused step.  ``entries``: torch's state entry of every parameter in flat order (``{}`` where it has none);
+    ``opt_steps``: the checkpoint's ``b200_opt_steps`` (None in a torch-written one); ``per_param_on``: the step already
+    keeps per-parameter counts; ``momentum``: SGD's per-group momentum.
+
+    torch creates a parameter's state at its first step, so a parameter without an entry has taken 0 steps and has the
+    initial scalar state (1.0).  torch's SGD keeps no ``step``: a parameter with a ``momentum_buffer`` has taken
+    ``opt_steps`` steps (1 in a torch-written checkpoint), one without it 0; in a group without momentum the count has no
+    effect and is the optimizer-wide one.
+
+    Returns ``(opt_steps, steps, scalars)``: the optimizer-wide count, then either per-parameter counts and per-parameter
+    scalar state (``steps`` a list) or ``steps = None`` and per-group scalar state.  Counts go per parameter when they
+    are not all the optimizer-wide count, when the scalar state differs within a group, or when ``per_param_on``.
+    ``scalars`` is None for the kinds without scalar state."""
+    def count(e, g):
+        if kind != _lib.OPT_SGD:
+            return int(float(e["step"])) if "step" in e else 0
+        if momentum[g] == 0:
+            return None
+        if e.get("momentum_buffer") is None:
+            return 0
+        return 1 if opt_steps is None else opt_steps
+
+    keys = _SCALAR_KEYS.get(kind, ())
+    steps = [count(e, g) for e, g in zip(entries, group_of)]
+    if opt_steps is None:
+        opt_steps = max([s for s in steps if s is not None], default=0)
+    steps = [opt_steps if s is None else s for s in steps]
+    scal = [[float(e[k]) if k in e else 1.0 for k in keys] for e in entries]
+    n_groups = max(group_of, default=-1) + 1
+    # only stepped parameters' scalars count: an unstepped one forces per-parameter counts through its count of 0
+    groups_differ = any(len({tuple(scal[i]) for i, g in enumerate(group_of) if g == gi and steps[i] > 0}) > 1
+                        for gi in range(n_groups))
+    if per_param_on or groups_differ or any(s != opt_steps for s in steps):
+        return opt_steps, steps, scal if keys else None
+    if not keys:
+        return opt_steps, None, None
+    first = {}
+    for i, g in enumerate(group_of):
+        first.setdefault(g, scal[i])
+    return opt_steps, None, [first.get(gi, [1.0] * len(keys)) for gi in range(n_groups)]
 
 
 def fused_supported(optim_cls, optim_kwargs: Dict, module: torch.nn.Module) -> bool:
@@ -240,10 +286,14 @@ class B200FusedOptimizer(torch.optim.Optimizer):
             groups.append(d)
         return groups
 
+    def _export(self, state):
+        path = self.path
+        return {"state": state, "param_groups": self._groups_sd(), "b200_master": path.gather_master(),
+                "b200_opt_steps": int(path.engine.scaler_get(path.state_id).opt_steps)}
+
     def _adafactor_state_dict(self):
         """torch's format: a parameter that was never stepped has no entry (torch creates its state at its first gradient)."""
         path = self.path
-        st = path.engine.scaler_get(path.state_id)
         steps = path.param_steps()
         state = {}
         for i, views in enumerate(path.adafactor_state_views()):
@@ -252,40 +302,28 @@ class B200FusedOptimizer(torch.optim.Optimizer):
             keys = ("row_var", "col_var") if len(views) == 2 else ("variance",)
             state[self._sd_index[i]] = dict({"step": torch.tensor(float(steps[i]))},
                                             **{k: v.clone() for k, v in zip(keys, views)})
-        return {"state": state, "param_groups": self._groups_sd(), "b200_master": path.gather_master(),
-                "b200_opt_steps": int(st.opt_steps)}
+        return self._export(state)
 
-    def _adafactor_load_state_dict(self, sd):
+    def state_dict(self):
+        """torch's per-parameter format: ``step``, the scalar state (NAdam's ``mu_product``, ASGD's ``eta`` and ``mu``) as
+        0-dim fp32 tensors, then the class's state tensors.  Adadelta, Rprop and ASGD omit a parameter that was never
+        stepped (torch creates their state at its first gradient); the other kinds emit it.  SGD emits only
+        ``momentum_buffer``, None before a parameter's first step or without momentum."""
         path = self.path
-        dev = path.p_flat.device
-        state = sd["state"]
-        steps = []
-        for i, views in enumerate(path.adafactor_state_views()):
-            src = state.get(self._sd_index[i], {})
-            keys = ("row_var", "col_var") if len(views) == 2 else ("variance",)
-            for k, v in zip(keys, views):
-                if k in src:
-                    v.copy_(src[k].to(device=dev, dtype=torch.float32).reshape(v.shape))
-                else:
-                    v.zero_()
-            steps.append(int(float(src["step"])) if "step" in src else 0)
-        path._range_steps.copy_(torch.tensor(steps, dtype=torch.int32))
-        return int(sd.get("b200_opt_steps", max(steps)))
-
-    def _lazy_state_dict(self):
-        """Adadelta / Rprop / ASGD in torch's format: ``step`` and the class's state tensors (ASGD: ``eta`` and ``mu`` as
-        0-dim fp32 tensors too); a parameter that was never stepped has no entry (torch creates its state at its first
-        gradient)."""
-        path = self.path
-        st = path.engine.scaler_get(path.state_id)
+        if self._kind == _ADAFACTOR:
+            return self._adafactor_state_dict()
         k_m, k_v = _STATE_KEYS[self._kind]
-        ms = path.unflatten(self._full(path.m_flat))
+        ms = path.unflatten(self._full(path.m_flat)) if path.m_flat is not None else None
         vs = path.unflatten(self._full(path.v_flat)) if k_v is not None else None
         steps = path.param_steps()
         scal = path.param_scalars() if self._kind in _SCALAR_KEYS else None
         state = {}
         for i in range(len(path.params)):
-            if steps[i] == 0:
+            j = self._sd_index[i]
+            if self._kind == _lib.OPT_SGD:
+                state[j] = {k_m: ms[i].clone() if ms is not None and steps[i] > 0 else None}
+                continue
+            if steps[i] == 0 and self._kind in _LAZY_KINDS:
                 continue
             d = {"step": torch.tensor(float(steps[i]))}
             if scal is not None:
@@ -294,126 +332,45 @@ class B200FusedOptimizer(torch.optim.Optimizer):
             d[k_m] = ms[i].clone()
             if k_v is not None:
                 d[k_v] = vs[i].clone()
-            state[self._sd_index[i]] = d
-        return {"state": state, "param_groups": self._groups_sd(), "b200_master": path.gather_master(),
-                "b200_opt_steps": int(st.opt_steps)}
-
-    def _lazy_load_state_dict(self, sd, put) -> int:
-        """Adadelta / Rprop / ASGD: a parameter without an entry has taken no step (torch's lazy state), so its step
-        count is 0 and its first fused step initialises it as torch would.  Step counts that differ between parameters, or
-        ASGD scalars that differ within a group, switch to per-parameter bookkeeping."""
-        path = self.path
-        n = len(path.params)
-        state = sd["state"]
-        k_m, k_v = _STATE_KEYS[self._kind]
-        put(path.m_flat, k_m)
-        if k_v is not None:
-            put(path.v_flat, k_v)
-        srcs = [state.get(self._sd_index[i], {}) for i in range(n)]
-        per_param = [int(float(src["step"])) if "step" in src else 0 for src in srcs]
-        keys = _SCALAR_KEYS.get(self._kind, ())
-        # the placeholder of a parameter without state is never read: the prologue initialises it at the first step
-        scal = [[float(src[k]) if k in src else 1.0 for k in keys] for src in srcs]
-        groups_differ = any(len({tuple(scal[i]) for i in range(n) if self._group_of[i] == gi and per_param[i] > 0}) > 1
-                            for gi in range(len(self.param_groups)))
-        # one optimizer-wide count serves every parameter only if each took exactly that many steps
-        wide = int(sd.get("b200_opt_steps", per_param[0]))
-        if len(set(per_param)) > 1 or per_param[0] != wide or groups_differ or path._range_steps is not None:
-            path.enable_per_param_steps(per_param, scalars=scal if keys else None)
-        elif keys:
-            first = {}
-            for i in range(n):
-                first.setdefault(self._group_of[i], scal[i])
-            path.set_group_scalars([first.get(gi, [1.0] * len(keys)) for gi in range(len(self.param_groups))])
-        return int(sd.get("b200_opt_steps", max(per_param)))
-
-    def state_dict(self):
-        path = self.path
-        if self._kind == _ADAFACTOR:
-            return self._adafactor_state_dict()
-        if self._kind in _LAZY_KINDS:
-            return self._lazy_state_dict()
-        st = path.engine.scaler_get(path.state_id)
-        m, v, master = self._full(path.m_flat), self._full(path.v_flat), path.gather_master()
-        state = {}
-        ms = path.unflatten(m) if m is not None else None
-        vs = path.unflatten(v) if v is not None else None
-        steps = path.param_steps() if path._range_steps is not None else [int(st.opt_steps)] * len(path.params)
-        mus = [r[0] for r in path.param_scalars()] if self._kind == _lib.OPT_NADAM else None
-        for i in range(len(path.params)):
-            j = self._sd_index[i]
-            if self._kind == _lib.OPT_SGD:
-                # torch creates the buffer on the first step; before that (or without momentum) it is None
-                state[j] = {"momentum_buffer": ms[i].clone() if ms is not None and steps[i] > 0 else None}
-            else:
-                k_m, k_v = _STATE_KEYS[self._kind]
-                state[j] = {"step": torch.tensor(float(steps[i]))}
-                if mus is not None:   # torch/optim/nadam.py: a 0-dim fp32 tensor
-                    state[j]["mu_product"] = torch.tensor(mus[i], dtype=torch.float32)
-                state[j][k_m] = ms[i].clone()
-                state[j][k_v] = vs[i].clone()
-        return {"state": state, "param_groups": self._groups_sd(), "b200_master": master,
-                "b200_opt_steps": int(st.opt_steps)}
+            state[j] = d
+        return self._export(state)
 
     def load_state_dict(self, sd):
         """Accepts this class's own export and a plain ``torch.optim`` state dict written by the reference
         (stoke/io_ops.py:224-236): without ``b200_master`` the fp32 master weights are rebuilt from the model parameters
-        that ``model.load_state_dict`` has just filled (load order of BaseStokeIO.load)."""
+        that ``model.load_state_dict`` has just filled (load order of BaseStokeIO.load).  Step counts and scalar state
+        follow torch's lazy state creation (``load_step_counts``)."""
         path = self.path
         for g, src in zip(self.param_groups, sd["param_groups"]):
             for k, val in src.items():
                 if k != "params":
                     g[k] = val
-        steps = int(sd.get("b200_opt_steps", 0))
         dev = path.p_flat.device
-        n = len(path.params)
-        state = sd["state"]
+        entries = [sd["state"].get(self._sd_index[i], {}) for i in range(len(path.params))]
         if self._kind == _ADAFACTOR:
-            steps = self._adafactor_load_state_dict(sd)
-
-        def put(local_dst, key):
-            if local_dst is None:
-                return
-            full = torch.zeros(path.n, dtype=torch.float32, device=dev)
-            views = path.unflatten(full)
-            for i in range(n):
-                src = state.get(self._sd_index[i], {}).get(key)
-                if src is not None:
-                    views[i].copy_(src.to(device=dev, dtype=torch.float32))
-            path.scatter_local(full, local_dst)
-
-        if self._kind == _ADAFACTOR:
-            pass
-        elif self._kind in _LAZY_KINDS:
-            steps = self._lazy_load_state_dict(sd, put)
-        elif self._kind == _lib.OPT_SGD:
-            put(path.m_flat, "momentum_buffer")
+            for src, views in zip(entries, path.adafactor_state_views()):
+                keys = ("row_var", "col_var") if len(views) == 2 else ("variance",)
+                for k, v in zip(keys, views):
+                    if k in src:
+                        v.copy_(src[k].to(device=dev, dtype=torch.float32).reshape(v.shape))
+                    else:
+                        v.zero_()
         else:
-            k_m, k_v = _STATE_KEYS[self._kind]
-            put(path.m_flat, k_m)
-            put(path.v_flat, k_v)
-            per_param = [int(float(state[self._sd_index[i]]["step"])) if self._sd_index[i] in state and "step" in state[self._sd_index[i]]
-                         else None for i in range(n)]
-            known = [v for v in per_param if v is not None]
-            if "b200_opt_steps" not in sd and known:
-                steps = max(known)
-            mus = None
-            if self._kind == _lib.OPT_NADAM:
-                # a parameter torch never stepped has no state yet: its mu_product is torch's initial 1.0
-                mus = [float(state[self._sd_index[i]]["mu_product"]) if "mu_product" in state.get(self._sd_index[i], {})
-                       else 1.0 for i in range(n)]
-            groups_differ = mus is not None and any(
-                len({mus[i] for i in range(n) if self._group_of[i] == gi}) > 1 for gi in range(len(self.param_groups)))
-            if known and (len(set(known)) > 1 or len(known) < n) or groups_differ or (
-                    mus is not None and path._range_steps is not None):
-                # parameters stepped a different number of times (some were unused for a while): keep torch's per-parameter counts
-                path.enable_per_param_steps([steps if v is None else v for v in per_param],
-                                            scalars=None if mus is None else [[mu] for mu in mus])
-            elif mus is not None:
-                first = {}
-                for i in range(n):
-                    first.setdefault(self._group_of[i], mus[i])
-                path.set_group_scalars([[first.get(gi, 1.0)] for gi in range(len(self.param_groups))])
+            for local_dst, key in zip((path.m_flat, path.v_flat), _STATE_KEYS[self._kind]):
+                if local_dst is None:
+                    continue
+                full = torch.zeros(path.n, dtype=torch.float32, device=dev)
+                for view, src in zip(path.unflatten(full), entries):
+                    if src.get(key) is not None:
+                        view.copy_(src[key].to(device=dev, dtype=torch.float32))
+                path.scatter_local(full, local_dst)
+        steps, per_param, scalars = load_step_counts(self._kind, entries, self._group_of, sd.get("b200_opt_steps"),
+                                                     path._range_steps is not None,
+                                                     [g.get("momentum", 0.0) for g in self.param_groups])
+        if per_param is not None:
+            path.enable_per_param_steps(per_param, scalars)
+        elif scalars is not None:
+            path.set_group_scalars(scalars)
         if "b200_master" in sd:
             master = sd["b200_master"].to(device=dev, dtype=torch.float32)
             if path.master_flat is not path.p_flat:

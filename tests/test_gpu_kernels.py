@@ -475,8 +475,8 @@ def test_optim_step_matches_torch_float64(eng, name):
         a.seg_local, a.seg_global = (sl, sg) if n_seg else (None, None)
         if use_ranges:
             a.n_ranges, a.range_end_vec, a.range_group = len(ends), rend.data_ptr(), rgrp.data_ptr()
-            eng._check(eng.lib.stk_optim_range_prologue(eng.ctx, hyp, len(groups), len(ends), rgrp.data_ptr(),
-                                                        rsteps.data_ptr(), rbc.data_ptr(), eng._stream()))
+            eng._check(eng.lib.stk_optim_step_prologue(eng.ctx, hyp, None, len(groups), len(ends), rgrp.data_ptr(),
+                                                       rsteps.data_ptr(), None, rbc.data_ptr(), eng._stream()))
             a.range_bc = rbc.data_ptr()
         eng.optim_step_ex(a)
         eng.step_epilogue()
@@ -624,8 +624,8 @@ def test_optim_step_matches_torch_float64(eng, name):
         assert controls_hit or kind == "sgd" and not groups[0].get("momentum"), "no negative control ran"
 
 
-# ---- 5. k_range_prologue and k_step_epilogue ------------------------------------------------------------------------------
-def test_range_prologue_bias_corrections(eng):
+# ---- 5. k_step_prologue and k_step_epilogue -------------------------------------------------------------------------------
+def test_step_prologue_per_range_bias_corrections(eng):
     L = _lib()
     groups = [ADAM, {"lr": 1e-3, "beta1": 0.9, "beta2": 0.999, "eps": 1e-8}, dict(ADAM, beta1=0.0)]
     hyp = (L.OptimHyper * 3)(*[_hyper("adam", h, None) for h in groups])
@@ -638,8 +638,8 @@ def test_range_prologue_bias_corrections(eng):
     for found_inf in (0, 1):
         eng.scaler_set(found_inf=found_inf)
         before = rs.cpu().clone()
-        eng._check(eng.lib.stk_optim_range_prologue(eng.ctx, hyp, 3, nr, rgrp.data_ptr(), rs.data_ptr(), rbc.data_ptr(),
-                                                    eng._stream()))
+        eng._check(eng.lib.stk_optim_step_prologue(eng.ctx, hyp, None, 3, nr, rgrp.data_ptr(), rs.data_ptr(), None,
+                                                   rbc.data_ptr(), eng._stream()))
         got = rbc.cpu()
         for j in range(nr):
             ss, c2 = kr.bias_corrections(groups[rgrp_l[j] & 0x7F], int(before[j]))
@@ -648,6 +648,41 @@ def test_range_prologue_bias_corrections(eng):
             assert float(got[j, 2]) == (1.0 if int(before[j]) == 0 else 0.0)
             want = int(before[j]) + (0 if (rgrp_l[j] & 0x80 or found_inf) else 1)
             assert int(rs[j]) == want
+
+
+@pytest.mark.parametrize("kind,h", [("adam", ADAM), ("adamw", dict(ADAM, weight_decay=0.25)), ("sgd", SGD_M)])
+def test_group_bc_from_prologue_matches_in_kernel_scalars(eng, kind, h):
+    """Adam / AdamW / SGD given the prologue's per-group scalars (group_bc) step bit for bit like the optimizer-wide step
+    that forms them itself: master, moments and the bf16 copy, from the first step (SGD: buf = g) on."""
+    L = _lib()
+    n = 4096
+    hyp = (L.OptimHyper * 1)(_hyper(kind, h, None))
+    w0 = _rand(n, F32, seed=5).cuda()
+    runs = []
+    for use_bc in (False, True):
+        M, MM, VV, GG = Buf(n, F32, w0), Buf(n, F32, torch.zeros(n)), Buf(n, F32, torch.zeros(n)), Buf(n, F32)
+        LP = Buf(n, BF16, torch.zeros(n))
+        bc = torch.zeros(1, 4, dtype=torch.float32, device="cuda")
+        lpp = _lib().ptr_array([LP.ptr()])
+        out = []
+        for step in range(3):
+            GG.t.copy_(_rand(n, F32, seed=10 + step).cuda())
+            eng.scaler_set(opt_steps=step, skipped_steps=0, found_inf=0)
+            a = L.OptimArgs()
+            a.hyper, a.n_groups = hyp, 1
+            a.master, a.exp_avg, a.exp_avg_sq = M.ptr(), MM.ptr(), (VV.ptr() if kind != "sgd" else None)
+            a.grad, a.grad_dtype, a.grad_raw, a.n_local = GG.ptr(), L.F32, 0, n
+            a.lp_ptrs, a.lp_world, a.lp_dtype = lpp, 1, L.BF16
+            if use_bc:
+                eng._check(eng.lib.stk_optim_step_prologue(eng.ctx, hyp, None, 1, 0, None, None, None, bc.data_ptr(),
+                                                           eng._stream()))
+                a.group_bc = bc.data_ptr()
+            eng.optim_step_ex(a)
+            out.append((M.bits(), MM.bits(), VV.bits(), LP.bits()))
+        runs.append(out)
+    for step, (a_, b_) in enumerate(zip(*runs)):
+        for name, x, y in zip(("master", "exp_avg", "exp_avg_sq", "bf16"), a_, b_):
+            assert torch.equal(x, y), (step, name)
 
 
 def test_step_epilogue_follows_amp_update_scale(eng):

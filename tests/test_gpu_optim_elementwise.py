@@ -518,14 +518,14 @@ def test_checkpoint_round_trip_with_plain_torch(cls, kw):
     opt2.close()
 
 
-def test_torch_checkpoint_with_unstepped_parameter_and_differing_asgd_scalars():
-    """A torch-written ASGD state where one parameter was never stepped (no entry) and the others took different numbers of
-    steps: the fused optimizer goes per parameter and continues exactly like torch."""
+def _continue_torch_checkpoint_with_unstepped_parameter(cls, kw):
+    """A torch-written state where one parameter was never stepped (no entry) and the others took different numbers of
+    steps: the fused optimizer goes per parameter, restarts the unstepped one at step 0 like torch, and continues exactly
+    like torch, scalar state (ASGD's eta / mu, NAdam's mu_product) included."""
     torch.cuda.set_device(0)
-    kw = {"lr": 1e-2, "t0": 2.0, "lambd": 1e-2}
     net = OddNet().cuda()
     cpu_params = [torch.nn.Parameter(p.detach().cpu().clone()) for p in net.parameters()]
-    topt = torch.optim.ASGD(cpu_params, **kw, foreach=False)
+    topt = cls(cpu_params, **kw, foreach=False)
     gen = torch.Generator().manual_seed(4)
     for step in range(5):
         for i, p in enumerate(cpu_params):
@@ -535,7 +535,7 @@ def test_torch_checkpoint_with_unstepped_parameter_and_differing_asgd_scalars():
     with torch.no_grad():
         for p, q in zip(net.parameters(), cpu_params):
             p.copy_(q.detach())
-    opt = _fused(net, torch.optim.ASGD, kw, None)
+    opt = _fused(net, cls, kw, None)
     opt.load_state_dict(topt.state_dict())
     assert opt.path._range_steps is not None
     for step in range(5, 9):
@@ -550,8 +550,95 @@ def test_torch_checkpoint_with_unstepped_parameter_and_differing_asgd_scalars():
     sd = opt.state_dict()
     for i, p in enumerate(cpu_params):
         assert float(sd["state"][i]["step"]) == float(topt.state[p]["step"])
-        assert float(sd["state"][i]["eta"]) == float(topt.state[p]["eta"])
-        assert float(sd["state"][i]["mu"]) == float(topt.state[p]["mu"])
+        for k in ("eta", "mu", "mu_product"):
+            if k in topt.state[p]:
+                assert float(sd["state"][i][k]) == float(topt.state[p][k]), k
+    opt.close()
+
+
+def test_torch_checkpoint_with_unstepped_parameter_and_differing_asgd_scalars():
+    """ASGD: the stepped parameters' eta / mu differ, and the unstepped one starts from torch's lazy initialisation."""
+    _continue_torch_checkpoint_with_unstepped_parameter(torch.optim.ASGD, {"lr": 1e-2, "t0": 2.0, "lambd": 1e-2})
+
+
+@pytest.mark.parametrize("cls", [torch.optim.Adam, torch.optim.NAdam])
+def test_torch_checkpoint_with_unstepped_parameter_restarts_it_at_step_0(cls):
+    """Adam and NAdam: the unstepped parameter's first bias correction (NAdam: with mu_product 1) is torch's step 1."""
+    _continue_torch_checkpoint_with_unstepped_parameter(cls, {"lr": 1e-2})
+
+
+def test_uniform_torch_checkpoint_replaces_per_parameter_counts():
+    """Adam with per-parameter step counts already on (head b unused at the first step) loads a torch state whose counts
+    are uniform: the loaded counts replace the old ones, and the step continues exactly like torch."""
+    torch.cuda.set_device(0)
+    kw = {"lr": 1e-2}
+    model = TwoHeads().cuda()
+    opt = _fused(model, torch.optim.Adam, kw, None)
+    path = opt.path
+    g = torch.Generator().manual_seed(0)
+    x, y = torch.randn(8, 16, generator=g).cuda(), torch.randn(8, 1, generator=g).cuda()
+    for step in range(3):
+        model.use_b = step > 0
+        path.begin_backward(sync=True, unscale=False)
+        torch.nn.functional.mse_loss(model(x), y).backward()
+        path.after_backward(sync=True, unscale=False)
+        opt.step()
+    assert path.param_steps() == [3, 3, 3, 3, 2, 2]
+    cpu_params = [torch.nn.Parameter(p.detach().cpu().clone()) for p in model.parameters()]
+    topt = torch.optim.Adam(cpu_params, **kw, foreach=False)
+    for step in range(2):
+        for p in cpu_params:
+            p.grad = torch.randn(p.shape, generator=g) * 1e-2
+        topt.step()
+    with torch.no_grad():
+        for p, q in zip(model.parameters(), cpu_params):
+            p.copy_(q.detach())
+    opt.load_state_dict(topt.state_dict())
+    assert path.param_steps() == [2] * 6
+    for step in range(4):
+        grads = _inject(path, step, 0, torch.float32)
+        for p, gr in zip(cpu_params, grads):
+            p.grad = gr.reshape(p.shape).clone()
+        path.after_backward(sync=True, unscale=False)
+        opt.step()
+        topt.step()
+    for a, b in zip(path.unflatten(path.gather_master().cpu()), cpu_params):
+        assert _rel(a.reshape(-1), b.detach().reshape(-1)) < TOL
+    sd = opt.state_dict()
+    assert [float(sd["state"][i]["step"]) for i in range(6)] == [6.0] * 6
+    opt.close()
+
+
+def test_torch_sgd_momentum_checkpoint_continues_the_buffer():
+    """A torch-written SGD-momentum state (no `step`; parameter 0 never stepped, so it has no buffer): the loaded buffers
+    continue as buf = momentum * buf + (1 - dampening) * g, parameter 0 starts with buf = g, as in torch."""
+    torch.cuda.set_device(0)
+    kw = {"lr": 1e-2, "momentum": 0.9, "dampening": 0.25}
+    net = OddNet().cuda()
+    cpu_params = [torch.nn.Parameter(p.detach().cpu().clone()) for p in net.parameters()]
+    topt = torch.optim.SGD(cpu_params, **kw, foreach=False)
+    gen = torch.Generator().manual_seed(6)
+    for step in range(3):
+        for i, p in enumerate(cpu_params):
+            p.grad = None if i == 0 else torch.randn(p.shape, generator=gen) * 1e-2
+        topt.step()
+    with torch.no_grad():
+        for p, q in zip(net.parameters(), cpu_params):
+            p.copy_(q.detach())
+    opt = _fused(net, torch.optim.SGD, kw, None)
+    opt.load_state_dict(topt.state_dict())
+    for step in range(3, 7):
+        grads = _inject(opt.path, step, 0, torch.float32)
+        for p, gr in zip(cpu_params, grads):
+            p.grad = gr.reshape(p.shape).clone()
+        opt.path.after_backward(sync=True, unscale=False)
+        opt.step()
+        topt.step()
+    for a, b in zip(opt.path.unflatten(opt.path.gather_master().cpu()), cpu_params):
+        assert _rel(a.reshape(-1), b.detach().reshape(-1)) < TOL
+    sd = opt.state_dict()
+    for i, p in enumerate(cpu_params):
+        assert _rel(sd["state"][i]["momentum_buffer"].cpu().reshape(-1), topt.state[p]["momentum_buffer"].reshape(-1)) < TOL
     opt.close()
 
 
