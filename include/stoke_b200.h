@@ -39,6 +39,8 @@
  *                                    without `.item()`
  *   stk_adafactor_plan / _step       torch.optim.Adafactor's step (torch/optim/_adafactor.py _single_tensor_adafactor) plus
  *                                    the clip and the GradScaler.step gate, without its two .item() per parameter
+ *   stk_layerwise_step               the step of the LAMB / LARS classes of stoke_b200.optim (per-parameter trust ratios;
+ *                                    torch.optim has neither), plus the clip and the GradScaler.step gate
  */
 #ifndef STOKE_B200_H
 #define STOKE_B200_H
@@ -381,6 +383,67 @@ int stk_adafactor_plan(stk_adafactor_param_t* params_host, int n_params, stk_ada
  * sums of g^2, their lerp, row means, ||u||^2 partials, the per-parameter coefficient, the update).  Reads the selected
  * scaler state (found_inf skips every parameter and leaves state and counts unchanged; the raw bucket is still zeroed). */
 int stk_adafactor_step(stk_ctx* ctx, const stk_adafactor_args_t* args, void* stream);
+
+/* ---- LAMB / LARS: layer-wise adaptive steps (stoke_b200.optim.LAMB / LARS) --------------------------------------------
+ * The large-batch optimizers of BERT (LAMB) and ResNet-50 (LARS): an element-wise update scaled per parameter by a trust
+ * ratio formed from two whole-parameter norms, plus clip_grad_norm_ / clip_grad_value_'s scaling and GradScaler.step's
+ * inf gate, like stk_optim_step.  Per parameter with a gradient, g the gradient after unscale, accumulation and clip,
+ * t = its own step count after the increment, adapt = weight_decay != 0 || always_adapt:
+ *   LAMB: m = lerp(m, g, 1 - beta1);  v = v beta2 + (1 - beta2) g^2
+ *         bc1, bc2 = 1 - beta1^t, 1 - beta2^t (double; 1 without bias_correction)
+ *         r = (m / bc1) / (sqrt(v / bc2) + eps) + wd w
+ *         trust = adapt && ||w|| > 0 && ||r|| > 0 ? ||w|| / ||r|| : 1          (w before this step's update)
+ *         w -= lr (trust r)
+ *   LARS: trust = adapt && ||w|| > 0 && ||g|| > 0 ? tc ||w|| / (||g|| + wd ||w|| + eps) : 1   (g before weight decay)
+ *         adapt: g = (g + wd w) trust
+ *         momentum != 0: buf = t == 1 ? g : buf momentum + (1 - dampening) g;  g = nesterov ? g + momentum buf : buf
+ *         w -= lr g
+ * A NaN norm fails the comparisons (trust 1), as torch.where does.  Three stream-ordered launches: a tile pass (per-tile
+ * partial sums of w^2 and r^2 or g^2; LAMB also updates m, v and zeroes the raw bucket), a per-parameter fold (trust
+ * ratio, step count), the update (fp32 master, low-precision copy; LARS: momentum buffer and bucket zeroing).  LAMB's
+ * update recomputes r from the stored m, v and w with the same fp32 operations as the tile pass, so the r it applies is
+ * the r whose norm it took.  Deterministic: every sum adds in an order fixed by the shapes, no floating-point atomics.
+ * found_inf skips every parameter and a set bit 7 of its group byte skips one: master, state and count are left as they
+ * are (the raw bucket is still zeroed).  Nothing is synchronised. */
+#define STK_LW_TILE 8192   /* elements per tile of the tile passes */
+typedef enum { STK_LW_LAMB = 0, STK_LW_LARS = 1 } stk_layerwise_kind;
+
+typedef struct {          /* one per parameter */
+  uint64_t offset;        /* first element in the flat master / gradient / state / lp buffers: a multiple of 16 */
+  int32_t numel;          /* 0 .. 2^31 - 1; the elements after numel up to the next parameter are padding, left as they are */
+  int32_t tile0;          /* first tile: the sum of ceil(numel / STK_LW_TILE) over the parameters before it */
+} stk_layerwise_param_t;
+
+typedef struct {          /* one per parameter group */
+  double lr;
+  double beta1, beta2;    /* LAMB */
+  double eps, weight_decay;
+  double momentum, dampening, trust_coefficient;  /* LARS */
+  int bias_correction;    /* LAMB */
+  int nesterov;           /* LARS */
+  int always_adapt;       /* 1: the trust ratio also when weight_decay == 0 */
+  int pad_;
+} stk_layerwise_hyper_t;
+
+typedef struct {
+  int kind;                                           /* stk_layerwise_kind */
+  const stk_layerwise_hyper_t* hyper; int n_groups;   /* host array, <= STK_MAX_GROUPS */
+  int clip_kind; double clip_max_norm, clip_value;
+  const stk_layerwise_param_t* params;  /* DEVICE table, ascending offsets */
+  int n_params, n_tiles;                /* n_tiles: the sum of ceil(numel / STK_LW_TILE) */
+  const uint8_t* param_group;  /* DEVICE, one per parameter: group index, bit 7 = no gradient this step (not stepped) */
+  int32_t* steps;              /* DEVICE, one per parameter: steps taken; advanced here unless skipped or found_inf */
+  float* master;               /* fp32 masters (flat indexing) */
+  float* exp_avg;              /* LAMB: exp_avg; LARS: momentum_buffer (may be NULL when no group has momentum) */
+  float* exp_avg_sq;           /* LAMB: exp_avg_sq; LARS: not used */
+  void* workspace;             /* 16 n_params + 8 n_tiles bytes, 16-byte aligned, no initialisation */
+  const void* grad; int grad_dtype; int grad_raw;  /* raw = 1: model-dtype bucket (bf16 | f32) scaled by grad_mul and
+                                                      1/loss_scale, ZEROED after the step (also when skipped);
+                                                      raw = 0: fp32 reduced main gradients */
+  const float* acc; double grad_mul;  /* raw route: optional fp32 accumulator, multiplier */
+  void* lp; int lp_dtype;      /* low-precision parameter copy written after the update (bf16 | f32), or NULL */
+} stk_layerwise_args_t;
+int stk_layerwise_step(stk_ctx* ctx, const stk_layerwise_args_t* args, void* stream);
 
 /* ---- small collectives on the signal pads -------------------------------------------------------------------------- */
 /* mean over ranks of *loss_dev (float32/bf16/f16 scalar) -> *out_host (pinned, mapped) ; synchronises `stream` */

@@ -4,10 +4,11 @@
 from .configs import *  # noqa: F401,F403
 from .configs import __all__ as _config_names
 from .data import BucketedDistributedSampler, argsort_lengths
+from .optim import LAMB, LARS
 from .status import DistributedOptions, FP16Options
 from .stoke import Stoke
 from .utils import ParamNormalize
 
 __all__ = ["Stoke", "ParamNormalize", "FP16Options", "DistributedOptions", "BucketedDistributedSampler",
-           "argsort_lengths"] + list(_config_names)
+           "argsort_lengths", "LAMB", "LARS"] + list(_config_names)
 __version__ = "0.1.0"

@@ -92,6 +92,30 @@ class AdafactorArgs(C.Structure):
                 ("lp", C.c_void_p), ("lp_dtype", C.c_int)]
 
 
+LW_TILE = 8192
+LW_LAMB, LW_LARS = 0, 1
+
+
+class LayerwiseParam(C.Structure):
+    _fields_ = [("offset", C.c_uint64), ("numel", C.c_int32), ("tile0", C.c_int32)]
+
+
+class LayerwiseHyper(C.Structure):
+    _fields_ = [("lr", C.c_double), ("beta1", C.c_double), ("beta2", C.c_double), ("eps", C.c_double),
+                ("weight_decay", C.c_double), ("momentum", C.c_double), ("dampening", C.c_double),
+                ("trust_coefficient", C.c_double), ("bias_correction", C.c_int), ("nesterov", C.c_int),
+                ("always_adapt", C.c_int), ("pad_", C.c_int)]
+
+
+class LayerwiseArgs(C.Structure):
+    _fields_ = [("kind", C.c_int), ("hyper", C.POINTER(LayerwiseHyper)), ("n_groups", C.c_int), ("clip_kind", C.c_int),
+                ("clip_max_norm", C.c_double), ("clip_value", C.c_double), ("params", C.c_void_p),
+                ("n_params", C.c_int), ("n_tiles", C.c_int), ("param_group", C.c_void_p), ("steps", C.c_void_p),
+                ("master", C.c_void_p), ("exp_avg", C.c_void_p), ("exp_avg_sq", C.c_void_p), ("workspace", C.c_void_p),
+                ("grad", C.c_void_p), ("grad_dtype", C.c_int), ("grad_raw", C.c_int), ("acc", C.c_void_p),
+                ("grad_mul", C.c_double), ("lp", C.c_void_p), ("lp_dtype", C.c_int)]
+
+
 class SamplerPlan(C.Structure):
     _fields_ = [("n", C.c_int64), ("buckets", C.c_int64), ("batch_size", C.c_int64), ("world", C.c_int64),
                 ("rank", C.c_int64), ("drop_last", C.c_int32), ("allow_bucket_overlap", C.c_int32),
@@ -145,6 +169,7 @@ _SIGNATURES = {
     "stk_step_epilogue": (C.c_int, [_P, _P]),
     "stk_adafactor_plan": (C.c_int, [C.POINTER(AdafactorParam), C.c_int, C.POINTER(AdafactorPlan)]),
     "stk_adafactor_step": (C.c_int, [_P, C.POINTER(AdafactorArgs), _P]),
+    "stk_layerwise_step": (C.c_int, [_P, C.POINTER(LayerwiseArgs), _P]),
     "stk_loss_sync": (C.c_int, [_P, _P, C.c_int, C.POINTER(C.c_double), _P]),
     "stk_loss_sync_begin": (C.c_int, [_P, _P, C.c_int, C.POINTER(C.c_int64), _P]),
     "stk_loss_sync_wait": (C.c_int, [_P, C.c_int64, C.POINTER(C.c_double)]),

@@ -96,6 +96,26 @@ __device__ __forceinline__ void fold8(float (&x)[8], float mul, float inv_scale,
   }
 }
 
+// The optimizer's gradient from one stored element, shared by K2 (k2_optim.cu) and the LAMB / LARS steps
+// (k2_layerwise.cu): a raw-bucket element (its accumulator already added) times mul and 1/loss_scale, then
+// clip_grad_norm_'s coefficient (torch/nn/utils/clip_grad.py: max_norm / (total_norm + 1e-6), clamped to 1) or
+// clip_grad_value_'s clamp.  Both clamps keep NaN like torch.clamp: a NaN norm (a NaN gradient without a loss scaler)
+// makes every gradient NaN, as clip_grad_norm_ does, and clip by value passes a NaN element through.
+__device__ __forceinline__ float clip_coef(int clip_kind, float clip_max_norm, const stk_scaler_state_t* scaler) {
+  return clip_kind == STK_CLIP_NORM ? clamp_max_nan(clip_max_norm / (scaler->grad_norm + 1e-6f), 1.0f) : 1.f;
+}
+// g: the stored element; raw: it comes from a raw bucket (mul and inv_scale apply); coef: clip_coef's value
+__device__ __forceinline__ float form_grad(float g, bool raw, float mul, float inv_scale, int clip_kind, float coef,
+                                           float clip_value) {
+  if (raw) {
+    g *= mul;
+    g *= inv_scale;
+  }
+  if (clip_kind == STK_CLIP_NORM) g *= coef;
+  else if (clip_kind == STK_CLIP_VALUE) g = clamp_nan(g, -clip_value, clip_value);
+  return g;
+}
+
 // World 1: the block's norm partial (fixed tree: run-to-run deterministic) into blk_partial[blockIdx.x], for
 // k_grad_norm_finish launched behind the kernel on the same stream.  The sign bit carries the block's inf/nan verdict
 // (partials are +0, positive, +inf or NaN for every norm kind); setting the bit keeps the magnitude, so an inf or NaN

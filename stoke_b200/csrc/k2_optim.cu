@@ -286,10 +286,7 @@ __global__ void __launch_bounds__(256, KIND >= STK_OPT_NADAM ? 2 : 0) k_optim_st
   }
   __syncthreads();
   const bool skip_all = s_skip != 0;
-  float coef = 1.f;
-  // clamps keep NaN like torch.clamp: a NaN norm (a NaN gradient without a loss scaler) makes every gradient NaN, as
-  // clip_grad_norm_ does, and clip by value passes a NaN element through
-  if (p.clip_kind == STK_CLIP_NORM) coef = clamp_max_nan(p.clip_max_norm / (p.scaler->grad_norm + 1e-6f), 1.0f);
+  const float coef = clip_coef(p.clip_kind, p.clip_max_norm, p.scaler);
   const float cv = p.clip_value;
   const float inv_scale = s_inv_scale;
 
@@ -317,13 +314,7 @@ __global__ void __launch_bounds__(256, KIND >= STK_OPT_NADAM ? 2 : 0) k_optim_st
         }
 #pragma unroll
         for (int e = 0; e < 8; ++e) {
-          float gg = g[k][e];
-          if constexpr (RAW) {
-            gg *= p.grad_mul;
-            gg *= inv_scale;
-          }
-          if (p.clip_kind == STK_CLIP_NORM) gg *= coef;
-          else if (p.clip_kind == STK_CLIP_VALUE) gg = clamp_nan(gg, -cv, cv);
+          float gg = form_grad(g[k][e], RAW, p.grad_mul, inv_scale, p.clip_kind, coef, cv);
           if (h.maximize) gg = -gg;
           float ww = w[k][e];
           if (KIND == STK_OPT_ADAM || KIND == STK_OPT_ADAMW) {

@@ -464,7 +464,7 @@ class GradPath:
                  module: Optional[torch.nn.Module] = None, sync_init: bool = True, needs_second_moment: bool = True,
                  needs_first_moment: bool = True, bucket_mb: Optional[float] = None, state_id: Optional[int] = None,
                  route: Optional[str] = None, group_of: Optional[Sequence[int]] = None, overlap: bool = True,
-                 scalar_state: int = 0, adafactor: bool = False):
+                 scalar_state: int = 0, adafactor: bool = False, layerwise: bool = False):
         self.engine = engine
         self.params = [p for p in params if p.requires_grad]
         if not self.params:
@@ -619,6 +619,9 @@ class GradPath:
         self.adafactor = bool(adafactor)
         if self.adafactor:
             self._adafactor_setup()
+        self.layerwise = bool(layerwise)
+        if self.layerwise:
+            self._layerwise_setup()
         torch.cuda.synchronize(engine.device)
         if W > 1:
             torch.distributed.barrier(group=engine.group)
@@ -646,6 +649,23 @@ class GradPath:
         self._af_desc = torch.frombuffer(bytearray(C.string_at(descs, C.sizeof(descs))), dtype=torch.uint8).to(dev)
         self.af_state = torch.zeros(max(off, 1), dtype=torch.float32, device=dev)
         self._af_ws = torch.empty(max(int(self.af_plan.workspace_bytes), 16), dtype=torch.uint8, device=dev)
+        self._range_steps = torch.zeros(len(self.params), dtype=torch.int32, device=dev)
+
+    def _layerwise_setup(self):
+        """Descriptor table, workspace and per-parameter step counts of the fused LAMB / LARS step, built once.  The state
+        lives in M (LAMB's exp_avg, LARS's momentum_buffer) and V (LAMB's exp_avg_sq) at the parameters' flat offsets.
+        The trust ratio needs whole parameters on one rank, so there is no sharded route."""
+        if self.sharded:
+            raise ValueError("Stoke -- the fused LAMB / LARS step needs whole parameters on one rank (no sharded route)")
+        dev = self._range_end.device
+        descs = (_lib.LayerwiseParam * len(self.params))()
+        tiles = 0
+        for d, p, o in zip(descs, self.params, self.offsets):
+            d.offset, d.numel, d.tile0 = o, p.numel(), tiles
+            tiles += -(-p.numel() // _lib.LW_TILE)
+        self.lw_tiles = max(tiles, 1)
+        self._lw_desc = torch.frombuffer(bytearray(C.string_at(descs, C.sizeof(descs))), dtype=torch.uint8).to(dev)
+        self._lw_ws = torch.empty(16 * len(self.params) + 8 * self.lw_tiles, dtype=torch.uint8, device=dev)
         self._range_steps = torch.zeros(len(self.params), dtype=torch.int32, device=dev)
 
     # -- layout helpers -----------------------------------------------------------------------------------------------
@@ -927,6 +947,40 @@ class GradPath:
         self._raw_has_acc = False
         e.comm_poll()
 
+    def layerwise_step(self, kind: int, hypers: Sequence[_lib.LayerwiseHyper]):
+        """One fused LAMB / LARS step (``stk_layerwise_step``: tile pass, per-parameter fold, update), then the epilogue.
+        ``kind``: ``_lib.LW_LAMB`` or ``_lib.LW_LARS``; ``hypers``: one ``LayerwiseHyper`` per group.  Parameters without a
+        gradient in this window are skipped through the skip bits of the range table; their step counts and state do
+        not move."""
+        e = self.engine
+        e.state_select(self.state_id)
+        ng = len(hypers)
+        if ng > _lib.MAX_GROUPS:
+            raise NotImplementedError(f"Stoke -- the fused step handles up to {_lib.MAX_GROUPS} parameter groups")
+        harr = (_lib.LayerwiseHyper * ng)(*hypers)
+        a = _lib.LayerwiseArgs()
+        a.kind, a.hyper, a.n_groups = kind, harr, ng
+        a.clip_kind, a.clip_max_norm, a.clip_value = self.clip.kind, self.clip.max_norm, self.clip.clip_value
+        a.params, a.n_params, a.n_tiles = self._lw_desc.data_ptr(), len(self.params), self.lw_tiles
+        self._ranges_for_step()   # refreshes the skip bits of the per-parameter group table
+        a.param_group, a.steps = self._range_group.data_ptr(), self._range_steps.data_ptr()
+        a.master, a.workspace = self.master_ptr, self._lw_ws.data_ptr()
+        a.exp_avg = self.M.ptr if self.M else None
+        a.exp_avg_sq = self.V.ptr if self.V else None
+        if self.route == "local":
+            a.grad, a.grad_dtype, a.grad_raw, a.grad_mul = self.G.ptr, _DT[self.model_dtype], 1, 1.0
+            a.acc = self.ACC.ptr if self._raw_has_acc else None
+        else:
+            a.grad, a.grad_dtype, a.grad_raw = self.MAIN.ptr, _lib.F32, 0
+        if self.low_precision:
+            a.lp, a.lp_dtype = self.P.ptr, _DT[self.model_dtype]
+        e._check(e.lib.stk_layerwise_step(e.ctx, C.byref(a), e._stream()))
+        e.launches += 3
+        e.step_epilogue()
+        self._track_touched = False
+        self._raw_has_acc = False
+        e.comm_poll()
+
     def adafactor_state_views(self) -> List[Tuple[torch.Tensor, ...]]:
         """Per parameter, views of the state buffer in torch's shapes: (row_var [..., R, 1], col_var [..., 1, C]) or
         (variance,) shaped like the parameter."""
@@ -987,6 +1041,7 @@ class GradPath:
         self.grad_views = []
         self.p_flat = self.g_flat = self.main_flat = self.m_flat = self.v_flat = self.master_flat = None
         self.af_state = self._af_ws = self._af_desc = None
+        self._lw_ws = self._lw_desc = None
         for b in self._bufs:
             try:
                 e.free(b)

@@ -16,6 +16,9 @@ means of g^2, the parameter's RMS, the update's RMS), with per-parameter step co
 state_dict layout (``row_var`` / ``col_var`` or ``variance``).  Its state is never sharded: the reductions need whole
 parameters on one rank, so at world > 1 (``fairscale_oss=True`` included) it runs replicated on the all-reduce route,
 every rank taking the same deterministic step on the same gradients, as the stock route is replicated too.
+``LAMB`` and ``LARS`` (defined here; torch.optim has neither) take ``stk_layerwise_step``: per-parameter trust ratios from
+two whole-parameter norms, per-parameter step counts on the device, the classes' own state_dict layout, and the same
+replicated all-reduce route at world > 1.
 
 ``B200StockOptimizer`` -- every other ``torch.optim`` class (the reference instantiates whatever class the user passes,
 stoke/extensions.py:53-78) and the options the fused step does not cover (amsgrad, capturable, differentiable, more than 8
@@ -50,6 +53,145 @@ _STOCK_ONLY_TRUE = ("amsgrad", "capturable", "differentiable")
 _ADAFACTOR = "adafactor"
 if hasattr(torch.optim, "Adafactor"):
     _KINDS[torch.optim.Adafactor] = _ADAFACTOR
+
+
+def _trust_where(cond_a: torch.Tensor, cond_b: torch.Tensor, value: torch.Tensor) -> torch.Tensor:
+    """``value`` where both norms are positive, else 1 (torch.where: a NaN norm fails the comparison and gives 1)."""
+    one = torch.ones_like(value)
+    return torch.where(cond_a > 0, torch.where(cond_b > 0, value, one), one)
+
+
+class LAMB(torch.optim.Optimizer):
+    """LAMB (You et al., "Large Batch Optimization for Deep Learning: Training BERT in 76 minutes", 2019): Adam's update
+    direction plus weight decay, scaled per parameter by the trust ratio ||w|| / ||r||.  For one parameter w with
+    gradient g and its own step count t (after the increment)::
+
+        m = m.lerp(g, 1 - beta1);  v = v * beta2 + (1 - beta2) * g * g
+        bc1, bc2 = (1 - beta1 ** t, 1 - beta2 ** t) if bias_correction else (1, 1)
+        r = (m / bc1) / (sqrt(v / bc2) + eps) + weight_decay * w
+        trust = ||w|| / ||r|| if (weight_decay != 0 or always_adapt) and ||w|| > 0 and ||r|| > 0 else 1
+        w = w - lr * (trust * r)
+
+    ||w|| is taken before this step's update.  A group with ``weight_decay=0`` (biases, LayerNorm weights) therefore takes
+    a plain bias-corrected Adam step unless ``always_adapt``.  State per parameter, created at its first step: ``step``
+    (0-dim fp32 tensor), ``exp_avg``, ``exp_avg_sq``.  This ``step()`` is plain per-parameter torch: what runs outside the
+    engine and on its stock route; inside ``Stoke`` the class runs on the fused sm_90a step (``stk_layerwise_step``)."""
+
+    def __init__(self, params, lr: float = 1e-3, betas=(0.9, 0.999), eps: float = 1e-6, weight_decay: float = 0.01,
+                 bias_correction: bool = True, always_adapt: bool = False):
+        if lr < 0.0:
+            raise ValueError(f"Invalid learning rate: {lr}")
+        if eps < 0.0:
+            raise ValueError(f"Invalid epsilon value: {eps}")
+        if not 0.0 <= betas[0] < 1.0 or not 0.0 <= betas[1] < 1.0:
+            raise ValueError(f"Invalid beta parameters: {betas}")
+        if weight_decay < 0.0:
+            raise ValueError(f"Invalid weight_decay value: {weight_decay}")
+        super().__init__(params, dict(lr=lr, betas=tuple(betas), eps=eps, weight_decay=weight_decay,
+                                      bias_correction=bias_correction, always_adapt=always_adapt))
+
+    @torch.no_grad()
+    def step(self, closure=None):
+        loss = None
+        if closure is not None:
+            with torch.enable_grad():
+                loss = closure()
+        for group in self.param_groups:
+            b1, b2 = group["betas"]
+            lr, eps, wd = group["lr"], group["eps"], group["weight_decay"]
+            for p in group["params"]:
+                if p.grad is None:
+                    continue
+                g = p.grad
+                state = self.state[p]
+                if not state:
+                    state["step"] = torch.tensor(0.0, dtype=torch.float32)
+                    state["exp_avg"] = torch.zeros_like(p, memory_format=torch.preserve_format)
+                    state["exp_avg_sq"] = torch.zeros_like(p, memory_format=torch.preserve_format)
+                state["step"] += 1
+                t = float(state["step"])
+                m, v = state["exp_avg"], state["exp_avg_sq"]
+                m.lerp_(g, 1 - b1)
+                v.mul_(b2).addcmul_(g, g, value=1 - b2)
+                bc1, bc2 = (1 - b1**t, 1 - b2**t) if group["bias_correction"] else (1.0, 1.0)
+                r = (m / bc1) / ((v / bc2).sqrt() + eps)
+                if wd != 0:
+                    r = r + wd * p
+                if wd != 0 or group["always_adapt"]:
+                    wn, rn = torch.linalg.vector_norm(p), torch.linalg.vector_norm(r)
+                    r = r * _trust_where(wn, rn, wn / rn)
+                p.add_(r, alpha=-lr)
+        return loss
+
+
+class LARS(torch.optim.Optimizer):
+    """LARS (You et al., "Large Batch Training of Convolutional Networks", 2017): SGD whose gradient, weight decay included,
+    is scaled per parameter by the trust ratio trust_coefficient ||w|| / (||g|| + weight_decay ||w|| + eps).  For one
+    parameter w with gradient g and its own step count t (after the increment)::
+
+        if weight_decay != 0 or always_adapt:
+            trust = tc * ||w|| / (||g|| + wd * ||w|| + eps) if ||w|| > 0 and ||g|| > 0 else 1   # g before weight decay
+            g = (g + wd * w) * trust
+        if momentum != 0:
+            buf = g.clone() if t == 1 else buf * momentum + (1 - dampening) * g             # torch SGD's seeding
+            g = g + momentum * buf if nesterov else buf
+        w = w - lr * g
+
+    A group with ``weight_decay=0`` (biases, BatchNorm weights) therefore takes a plain SGD step unless ``always_adapt``.
+    State per parameter, created at its first step: ``step`` (0-dim fp32 tensor) and, with momentum, ``momentum_buffer``.
+    Plain per-parameter torch here; inside ``Stoke`` the class runs on the fused sm_90a step (``stk_layerwise_step``)."""
+
+    def __init__(self, params, lr: float = 1.0, momentum: float = 0.9, dampening: float = 0.0, weight_decay: float = 0.0,
+                 nesterov: bool = False, trust_coefficient: float = 0.001, eps: float = 1e-8, always_adapt: bool = False):
+        if lr < 0.0:
+            raise ValueError(f"Invalid learning rate: {lr}")
+        if momentum < 0.0:
+            raise ValueError(f"Invalid momentum value: {momentum}")
+        if weight_decay < 0.0:
+            raise ValueError(f"Invalid weight_decay value: {weight_decay}")
+        if nesterov and (momentum <= 0 or dampening != 0):
+            raise ValueError("Nesterov momentum requires a momentum and zero dampening")
+        super().__init__(params, dict(lr=lr, momentum=momentum, dampening=dampening, weight_decay=weight_decay,
+                                      nesterov=nesterov, trust_coefficient=trust_coefficient, eps=eps,
+                                      always_adapt=always_adapt))
+
+    @torch.no_grad()
+    def step(self, closure=None):
+        loss = None
+        if closure is not None:
+            with torch.enable_grad():
+                loss = closure()
+        for group in self.param_groups:
+            lr, mom, damp, wd = group["lr"], group["momentum"], group["dampening"], group["weight_decay"]
+            for p in group["params"]:
+                if p.grad is None:
+                    continue
+                g = p.grad
+                state = self.state[p]
+                if not state:
+                    state["step"] = torch.tensor(0.0, dtype=torch.float32)
+                state["step"] += 1
+                t = float(state["step"])
+                if wd != 0 or group["always_adapt"]:
+                    wn, gn = torch.linalg.vector_norm(p), torch.linalg.vector_norm(g)
+                    trust = _trust_where(wn, gn, group["trust_coefficient"] * wn / (gn + wd * wn + group["eps"]))
+                    g = g.add(p, alpha=wd).mul_(trust)
+                if mom != 0:
+                    buf = state.get("momentum_buffer")
+                    if t == 1 or buf is None:
+                        buf = state["momentum_buffer"] = torch.clone(g).detach()
+                    else:
+                        buf.mul_(mom).add_(g, alpha=1 - damp)
+                    g = g.add(buf, alpha=mom) if group["nesterov"] else buf
+                p.add_(g, alpha=-lr)
+        return loss
+
+
+# LAMB and LARS run on their own entry point, stk_layerwise_step (per-parameter trust ratios), not as kinds of K2
+_LAMB, _LARS = "lamb", "lars"
+_KINDS[LAMB] = _LAMB
+_KINDS[LARS] = _LARS
+_LAYERWISE = {_LAMB: _lib.LW_LAMB, _LARS: _lib.LW_LARS}
 
 
 def _module_params(module: torch.nn.Module):
@@ -159,7 +301,7 @@ class B200FusedOptimizer(torch.optim.Optimizer):
                  bucket_mb: Optional[float] = None):
         if optim_cls not in _KINDS:
             raise NotImplementedError(
-                f"Stoke -- the fused step covers torch.optim.Adam, AdamW, SGD, NAdam, RAdam, Adamax, Adadelta, Rprop, ASGD and Adafactor; got {getattr(optim_cls, '__name__', optim_cls)}"
+                f"Stoke -- the fused step covers torch.optim.Adam, AdamW, SGD, NAdam, RAdam, Adamax, Adadelta, Rprop, ASGD and Adafactor and stoke_b200.optim.LAMB and LARS; got {getattr(optim_cls, '__name__', optim_cls)}"
                 f" (use B200StockOptimizer / build_optimizer, which routes other classes to the stock-optimizer path)")
         params, group_of, extra, kw = _group_layout(module, optim_kwargs)
         if len(extra) > _lib.MAX_GROUPS:
@@ -179,15 +321,18 @@ class B200FusedOptimizer(torch.optim.Optimizer):
         sgd = self._kind == _lib.OPT_SGD
         any_mom = any(g.get("momentum", 0) != 0 for g in probe.param_groups)
         ada = self._kind == _ADAFACTOR
-        if ada and engine.world > 1:
-            # Adafactor's per-parameter reductions need whole parameters on one rank: its state is replicated (also under
-            # fairscale_oss) and every rank runs the same deterministic step on the same all-reduced fp32 gradients
+        lw = self._kind in _LAYERWISE
+        lars = self._kind == _LARS
+        if (ada or lw) and engine.world > 1:
+            # Adafactor's per-parameter reductions and LAMB's / LARS's trust ratios need whole parameters on one rank: their
+            # state is replicated (also under fairscale_oss) and every rank runs the same deterministic step on the same
+            # all-reduced fp32 gradients
             route = "allreduce"
         self.path = GradPath(engine, params, grad_accum=grad_accum, clip=clip, sharded=sharded, lp_dtype=lp_dtype,
-                             module=module, needs_second_moment=not (sgd or ada or self._kind == _lib.OPT_ASGD),
-                             needs_first_moment=not (sgd or ada) or any_mom, state_id=state_id, route=route,
+                             module=module, needs_second_moment=not (sgd or ada or lars or self._kind == _lib.OPT_ASGD),
+                             needs_first_moment=not (sgd or ada or lars) or any_mom, state_id=state_id, route=route,
                              group_of=group_of, bucket_mb=bucket_mb, scalar_state=len(_SCALAR_KEYS.get(self._kind, ())),
-                             adafactor=ada)
+                             adafactor=ada, layerwise=lw)
         by_group: List[List[torch.nn.Parameter]] = [[] for _ in extra]
         for p, gi in zip(params, group_of):
             by_group[gi].append(p)
@@ -206,6 +351,19 @@ class B200FusedOptimizer(torch.optim.Optimizer):
         h.weight_decay = float(g["weight_decay"])
         h.eps1_none, h.eps1 = int(eps1 is None), float(eps1 if eps1 is not None else 0.0)
         h.maximize = int(bool(g.get("maximize", False)))
+        return h
+
+    @staticmethod
+    def _layerwise_hyper_of(g) -> _lib.LayerwiseHyper:
+        h = _lib.LayerwiseHyper()
+        h.lr, h.eps, h.weight_decay = float(g["lr"]), float(g["eps"]), float(g["weight_decay"])
+        h.always_adapt = int(bool(g["always_adapt"]))
+        if "betas" in g:   # LAMB
+            h.beta1, h.beta2 = (float(b) for b in g["betas"])
+            h.bias_correction = int(bool(g["bias_correction"]))
+        else:              # LARS
+            h.momentum, h.dampening = float(g["momentum"]), float(g["dampening"])
+            h.trust_coefficient, h.nesterov = float(g["trust_coefficient"]), int(bool(g["nesterov"]))
         return h
 
     def _hyper_of(self, g) -> _lib.OptimHyper:
@@ -252,6 +410,9 @@ class B200FusedOptimizer(torch.optim.Optimizer):
             raise NotImplementedError("Stoke -- closures are not supported by the fused step")
         if self._kind == _ADAFACTOR:
             self.path.adafactor_step([self._adafactor_hyper_of(g) for g in self.param_groups])
+            return
+        if self._kind in _LAYERWISE:
+            self.path.layerwise_step(_LAYERWISE[self._kind], [self._layerwise_hyper_of(g) for g in self.param_groups])
             return
         self.path.optimizer_step(self._hypers(), self._exts())
 
@@ -304,6 +465,25 @@ class B200FusedOptimizer(torch.optim.Optimizer):
                                             **{k: v.clone() for k, v in zip(keys, views)})
         return self._export(state)
 
+    def _layerwise_state_dict(self):
+        """The classes' own format: a parameter that was never stepped has no entry; ``step``, then LAMB's ``exp_avg`` /
+        ``exp_avg_sq`` or, in a LARS group with momentum, ``momentum_buffer``."""
+        path = self.path
+        steps = path.param_steps()
+        ms = path.unflatten(path.m_flat) if path.m_flat is not None else None
+        vs = path.unflatten(path.v_flat) if path.v_flat is not None else None
+        state = {}
+        for i in range(len(path.params)):
+            if steps[i] == 0:
+                continue
+            d = {"step": torch.tensor(float(steps[i]))}
+            if self._kind == _LAMB:
+                d["exp_avg"], d["exp_avg_sq"] = ms[i].clone(), vs[i].clone()
+            elif self.param_groups[self._group_of[i]]["momentum"] != 0:
+                d["momentum_buffer"] = ms[i].clone()
+            state[self._sd_index[i]] = d
+        return self._export(state)
+
     def state_dict(self):
         """torch's per-parameter format: ``step``, the scalar state (NAdam's ``mu_product``, ASGD's ``eta`` and ``mu``) as
         0-dim fp32 tensors, then the class's state tensors.  Adadelta, Rprop and ASGD omit a parameter that was never
@@ -312,6 +492,8 @@ class B200FusedOptimizer(torch.optim.Optimizer):
         path = self.path
         if self._kind == _ADAFACTOR:
             return self._adafactor_state_dict()
+        if self._kind in _LAYERWISE:
+            return self._layerwise_state_dict()
         k_m, k_v = _STATE_KEYS[self._kind]
         ms = path.unflatten(self._full(path.m_flat)) if path.m_flat is not None else None
         vs = path.unflatten(self._full(path.v_flat)) if k_v is not None else None
@@ -356,7 +538,9 @@ class B200FusedOptimizer(torch.optim.Optimizer):
                     else:
                         v.zero_()
         else:
-            for local_dst, key in zip((path.m_flat, path.v_flat), _STATE_KEYS[self._kind]):
+            keys = _STATE_KEYS[self._kind] if self._kind not in _LAYERWISE else \
+                (("exp_avg", "exp_avg_sq") if self._kind == _LAMB else ("momentum_buffer", None))
+            for local_dst, key in zip((path.m_flat, path.v_flat), keys):
                 if local_dst is None:
                     continue
                 full = torch.zeros(path.n, dtype=torch.float32, device=dev)
