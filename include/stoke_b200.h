@@ -473,6 +473,20 @@ enum { STK_ACT_RELU = 0, STK_ACT_SILU = 1, STK_ACT_HARDSWISH = 2, STK_ACT_RELU6 
 int stk_bn_act_ex(stk_ctx* ctx, int act, const void* x, const void* residual, const float* mean, const float* var,
                   const void* weight, const void* bias, double eps, void* out, float* save_invstd, size_t numel,
                   size_t channels, void* stream);
+/* Training-mode BatchNorm forward with its statistics, in one cooperative launch: torch.batch_norm_update_stats(x,
+ * running_mean, running_var, momentum) followed by stk_bn_act_ex, bit-identical to that pair.
+ *   save_mean = the batch mean, save_invstd = rsqrtf(var + eps) (var the biased batch variance), both fp32, as
+ *   torch.batch_norm_update_stats and stk_bn_act_ex compute them; the running statistics (running_dtype STK_F32 or STK_BF16)
+ *   become fma(mean, momentum, (1 - momentum) * running_mean) and the same of var * float(R / (R - 1.0)), in float,
+ *   rounded to their dtype; out as stk_bn_act_ex.
+ * Order contract: the statistics merge in the order of torch's batch_norm_collect_statistics_channels_last_kernel as
+ * launched by flexible_launch_configs(R, channels, coop) (the grid stk_bn_act_backward_ex reproduces).
+ * Coverage as stk_bn_act_ex, with at least 2 rows (R = numel / channels); the running statistics need no alignment.
+ * workspace: 3 * 128 * channels floats; no initialisation needed.  The grid barrier lives in the context, so launches on
+ * one context must not overlap (one stream, or streams ordered against each other). */
+int stk_bn_stats_act(stk_ctx* ctx, int act, const void* x, const void* residual, const void* weight, const void* bias,
+                     void* running_mean, void* running_var, int running_dtype, double momentum, double eps, void* out,
+                     float* save_mean, float* save_invstd, float* workspace, size_t numel, size_t channels, void* stream);
 /* stk_bn_act_ex with act = STK_ACT_RELU */
 int stk_bn_act(stk_ctx* ctx, const void* x, const void* residual, const float* mean, const float* var, const void* weight,
                const void* bias, double eps, void* out, float* save_invstd, size_t numel, size_t channels, void* stream);

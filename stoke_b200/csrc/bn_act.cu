@@ -8,6 +8,7 @@
 //   invstd = rsqrtf(var + eps)                   batch_norm_update_stats_and_invert
 // Bytes per element: x read 2 + out write 2 (+ residual read 2).  The unfused chain moves 8 (15 with the residual).
 #include <algorithm>
+#include <cuda/atomic>
 
 #include "common.cuh"
 #include "ctx.cuh"
@@ -65,6 +66,26 @@ __device__ __forceinline__ uint4 pack8(const uint16_t (&o)[8]) {
                     o[6] | uint32_t(o[7]) << 16);
 }
 
+// The apply over the vectors v = t, t + active, ... of one channel group, whose parameters the caller loaded.
+template <int kAct, bool kResidual>
+__device__ __forceinline__ void bn_act_vectors(const uint4* __restrict__ xv, const uint4* __restrict__ rv, uint4* __restrict__ ov,
+                                               const float (&m)[8], const float (&is)[8], const float (&w)[8],
+                                               const float (&b)[8], uint32_t t, uint32_t nvec, uint32_t active) {
+  for (uint32_t v = t; v < nvec; v += active) {
+    float xf[8], rf[8];
+    unpack16<STK_BF16>(__ldg(xv + v), xf);
+    if (kResidual) unpack16<STK_BF16>(__ldg(rv + v), rf);
+    uint16_t o[8];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      uint16_t z = bn_apply(xf[j], m[j], is[j], w[j], b[j]);
+      if (kResidual) z = bf16_bits(bf16_val(z) + rf[j]);
+      o[j] = act_out<kAct>(z);
+    }
+    ov[v] = pack8(o);
+  }
+}
+
 // Thread t owns channel group t % G (G = C / 8) and walks rows t / G, t / G + T / G, ...: T (the active thread count) is a
 // multiple of G, so the per-channel parameters stay in registers for the whole loop.
 template <int kAct, bool kResidual>
@@ -90,22 +111,8 @@ __global__ void __launch_bounds__(kBnThreads) k_bn_act(const __nv_bfloat16* __re
     unpack16<STK_BF16>(__ldg(reinterpret_cast<const uint4*>(weight + c0)), w);
     unpack16<STK_BF16>(__ldg(reinterpret_cast<const uint4*>(bias + c0)), b);
   }
-  const uint4* xv = reinterpret_cast<const uint4*>(x);
-  const uint4* rv = reinterpret_cast<const uint4*>(r);
-  uint4* ov = reinterpret_cast<uint4*>(out);
-  for (uint32_t v = t; v < nvec; v += active) {
-    float xf[8], rf[8];
-    unpack16<STK_BF16>(__ldg(xv + v), xf);
-    if (kResidual) unpack16<STK_BF16>(__ldg(rv + v), rf);
-    uint16_t o[8];
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      uint16_t z = bn_apply(xf[j], m[j], is[j], w[j], b[j]);
-      if (kResidual) z = bf16_bits(bf16_val(z) + rf[j]);
-      o[j] = act_out<kAct>(z);
-    }
-    ov[v] = pack8(o);
-  }
+  bn_act_vectors<kAct, kResidual>(reinterpret_cast<const uint4*>(x), reinterpret_cast<const uint4*>(r),
+                                  reinterpret_cast<uint4*>(out), m, is, w, b, t, nvec, active);
 }
 
 // ---- backward ------------------------------------------------------------------------------------------------------
@@ -373,6 +380,240 @@ static BnBwdConfig bn_bwd_config(uint32_t rows, uint32_t channels) {
   return {block_y, grid_y, 1 + (rows - 1) / (block_y * grid_y * kChains)};
 }
 
+// ---- forward with the statistics -----------------------------------------------------------------------------------
+// k_bn_stats_act: torch.batch_norm_update_stats followed by k_bn_act's apply in one cooperative launch of resident blocks,
+// in three phases separated by grid barriers.  Bytes per element: x read twice (2 + 2; the second read hits L2 for the
+// smaller sites) + out write 2 (+ residual read 2).  The unfused forward also launches a semaphore fill and the
+// running-statistics update.
+//  1. Welford partials in the order of torch's batch_norm_collect_statistics_channels_last_kernel<Var, BFloat16, float, 4>,
+//     launched as flexible_launch_configs(R, C, coop) (the same (block_y, grid_y, loops) as the backward reduce).
+//     Virtual thread (ty, by) keeps kChains chains; chain j takes rows m0 + (kChains * i + j) * S, i < loops, as
+//       valid row:  n++, inv = 1 / float(n), d0 = x - mean, mean = fma(d0, inv, mean), d1 = x - mean, m2 = fma(d0 * d1, 1, m2)
+//       past R:     the same with x = inv = 0 and 0 in place of 1 (so a -0 mean becomes +0, an infinite one NaN, as in torch)
+//     then folds chains 1..3 into chain 0 and halves over ty (welford_merge).  Real threads map as in k_bn_bwd_reduce;
+//     a persistent grid walks the (channel block, by) work items.  With grid_y == 1 the block's result is final.
+//  2. torch's last-block merge: thread ty merges the partials of blocks ty, ty + block_y, ... from (0, 0, 0), then the
+//     halving tree.  The channel's owner writes save_mean, save_invstd = rsqrtf(m2 / n + eps) (k_bn_act's formula) and
+//     the running statistics as torch's batch_norm_update_stats kernel computes them in float:
+//       running = fma(stat, momentum, (1 - momentum) * running),  stat = mean, or var * float(R / (R - 1.0)) for the var
+//  3. k_bn_act's apply from save_mean / save_invstd.
+struct BnStatsArgs {
+  const uint4* x;
+  const uint4* r;
+  const __nv_bfloat16* weight;
+  const __nv_bfloat16* bias;
+  void* running_mean;
+  void* running_var;
+  uint4* out;
+  float* save_mean;
+  float* save_invstd;
+  float* ws;          // [grid_y][C] partial means, then m2s, then counts (int)
+  uint32_t* bar;      // grid barrier: arrival count, generation
+  float eps, momentum, one_minus_momentum, bessel;
+  uint32_t rows, groups, block_y, grid_y, loops, nvec, active;
+};
+
+// A barrier over the whole (co-resident) grid.  The arrival count returns to 0 at every barrier and the generation only
+// grows, so the words need no reset between launches.
+__device__ __forceinline__ void grid_barrier(uint32_t* bar) {
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    cuda::atomic_ref<uint32_t, cuda::thread_scope_device> arrived(bar[0]), gen(bar[1]);
+    const uint32_t g = gen.load(cuda::memory_order_relaxed);
+    __threadfence();
+    if (arrived.fetch_add(1, cuda::memory_order_acq_rel) == gridDim.x - 1) {
+      arrived.store(0, cuda::memory_order_relaxed);
+      gen.store(g + 1, cuda::memory_order_release);
+    } else {
+      while (gen.load(cuda::memory_order_acquire) == g) __nanosleep(32);
+    }
+    __threadfence();
+  }
+  __syncthreads();
+}
+
+// torch's welford_merge_element for 8 channels of one count: (n, mean, m2) += (n2, mean2, m22), factor = 1 / float(max(1,
+// n + n2)), m2 += m22 + d * d * n2 * n * factor (the last product contracted with m22), mean = (mean2 * n2 + mean * n) *
+// factor.  torch's SASS contracts that sum differently at its two call sites: fma(mean2, n2, mean * n) where a virtual
+// thread folds its chains (kChainFold), fma(mean, n, mean2 * n2) in the vertical tree and the cross-block merge.
+template <bool kChainFold, int K>
+__device__ __forceinline__ void welford_merge(int& n, float (&mean)[K], float (&m2)[K], int n2, const float* mean2,
+                                              const float* m22) {
+  const float factor = __fdiv_rn(1.f, __int2float_rn(max(1, n + n2)));
+  const float fn = __int2float_rn(n), fn2 = __int2float_rn(n2);
+#pragma unroll
+  for (int k = 0; k < K; ++k) {
+    const float d = __fsub_rn(mean[k], mean2[k]);
+    const float s = kChainFold ? __fmaf_rn(mean2[k], fn2, __fmul_rn(mean[k], fn)) : __fmaf_rn(mean[k], fn, __fmul_rn(mean2[k], fn2));
+    m2[k] = __fadd_rn(__fmaf_rn(__fmul_rn(__fmul_rn(__fmul_rn(d, d), fn2), fn), factor, m22[k]), m2[k]);
+    mean[k] = __fmul_rn(s, factor);
+  }
+  n += n2;
+}
+
+__device__ __forceinline__ float run_load(const float* p) { return *p; }
+__device__ __forceinline__ float run_load(const __nv_bfloat16* p) { return __bfloat162float(*p); }
+__device__ __forceinline__ void run_store(float* p, float v) { *p = v; }
+__device__ __forceinline__ void run_store(__nv_bfloat16* p, float v) { *p = __float2bfloat16_rn(v); }
+
+// the outputs of channel c from its final (mean, var = m2 / n)
+template <typename RunT>
+__device__ __forceinline__ void bn_stats_finish(const BnStatsArgs& a, uint32_t c, float mean, float var) {
+  a.save_mean[c] = mean;
+  a.save_invstd[c] = rsqrtf(var + a.eps);
+  RunT* rm = static_cast<RunT*>(a.running_mean) + c;
+  RunT* rv = static_cast<RunT*>(a.running_var) + c;
+  run_store(rm, __fmaf_rn(mean, a.momentum, __fmul_rn(a.one_minus_momentum, run_load(rm))));
+  run_store(rv, __fmaf_rn(__fmul_rn(var, a.bessel), a.momentum, __fmul_rn(a.one_minus_momentum, run_load(rv))));
+}
+
+// the halving tree over ty of torch's welford_merge_block_vertical; slot(t) is this thread's shared-memory slot, the
+// partner's is slot + off * span.  Ends with the block synchronised.
+template <int K>
+__device__ __forceinline__ void welford_tree(bool owner, uint32_t ty, uint32_t block_y, uint32_t span, uint32_t slot, int& n,
+                                             float (&mean)[K], float (&m2)[K], float (*shm)[2 * K], int* shn) {
+  for (uint32_t off = block_y / 2; off > 0; off >>= 1) {
+    if (owner && ty < 2 * off) {
+#pragma unroll
+      for (int k = 0; k < K; ++k) {
+        shm[slot][k] = mean[k];
+        shm[slot][K + k] = m2[k];
+      }
+      shn[slot] = n;
+    }
+    __syncthreads();
+    if (owner && ty < off) {
+      const uint32_t p = slot + off * span;
+      welford_merge<false>(n, mean, m2, shn[p], shm[p], shm[p] + K);
+    }
+    __syncthreads();
+  }
+}
+
+template <int kAct, bool kResidual, typename RunT>
+__global__ void __launch_bounds__(kBwdThreads, 3) k_bn_stats_act(const BnStatsArgs a) {
+  __shared__ float shm[kBwdThreads][16];
+  __shared__ int shn[kBwdThreads];
+  const uint32_t t = threadIdx.x, channels = a.groups * 8;
+  // phase 1
+  {
+    const uint32_t gb = kBwdThreads / (kChains * a.block_y);
+    const uint32_t cgl = t % gb, j = t / gb % kChains, ty = t / (gb * kChains);
+    const uint32_t nxb = (a.groups + gb - 1) / gb, stride = a.block_y * a.grid_y;
+    for (uint32_t item = blockIdx.x; item < nxb * a.grid_y; item += gridDim.x) {
+      const uint32_t by = item / nxb, cg = (item % nxb) * gb + cgl;
+      const bool live = cg < a.groups;
+      const uint32_t m0 = by * a.block_y + ty;
+      int n = 0;
+      float mean[8], m2[8];
+#pragma unroll
+      for (int k = 0; k < 8; ++k) mean[k] = m2[k] = 0.f;
+      // four rows' loads in flight before their (sequential) Welford updates
+      for (uint32_t i0 = 0; i0 < a.loops; i0 += 4) {
+        uint4 xv[4];
+#pragma unroll
+        for (int u = 0; u < 4; ++u) {
+          const uint32_t row = m0 + (kChains * (i0 + u) + j) * stride;
+          xv[u] = live && i0 + u < a.loops && row < a.rows ? __ldg(a.x + size_t(row) * a.groups + cg) : make_uint4(0, 0, 0, 0);
+        }
+#pragma unroll
+        for (int u = 0; u < 4; ++u) {
+          if (i0 + u >= a.loops) break;
+          const bool in = live && m0 + (kChains * (i0 + u) + j) * stride < a.rows;
+          float inv = 0.f, valid = 0.f;
+          if (in) {
+            ++n;
+            inv = __fdiv_rn(1.f, __int2float_rn(n));
+            valid = 1.f;
+          }
+          float xf[8];
+          unpack16<STK_BF16>(xv[u], xf);
+#pragma unroll
+          for (int k = 0; k < 8; ++k) {
+            const float d0 = __fsub_rn(xf[k], mean[k]);
+            mean[k] = __fmaf_rn(d0, inv, mean[k]);
+            const float d1 = __fsub_rn(xf[k], mean[k]);
+            m2[k] = __fmaf_rn(__fmul_rn(d0, d1), valid, m2[k]);
+          }
+        }
+      }
+#pragma unroll
+      for (int k = 0; k < 8; ++k) {
+        shm[t][k] = mean[k];
+        shm[t][8 + k] = m2[k];
+      }
+      shn[t] = n;
+      __syncthreads();
+      const bool owner = j == 0;
+      if (owner)
+        for (uint32_t q = 1; q < kChains; ++q) welford_merge<true>(n, mean, m2, shn[t + q * gb], shm[t + q * gb], shm[t + q * gb] + 8);
+      __syncthreads();
+      welford_tree(owner, ty, a.block_y, gb * kChains, t, n, mean, m2, shm, shn);
+      if (owner && ty == 0 && live) {
+        const uint32_t c0 = cg * 8;
+        if (a.grid_y == 1) {
+          for (int k = 0; k < 8; ++k) bn_stats_finish<RunT>(a, c0 + k, mean[k], __fdiv_rn(m2[k], __int2float_rn(n)));
+        } else {
+          float* pm = a.ws + size_t(by) * channels + c0;
+          float* p2 = pm + size_t(a.grid_y) * channels;
+          int* pn = reinterpret_cast<int*>(p2 + size_t(a.grid_y) * channels);
+#pragma unroll
+          for (int k = 0; k < 8; ++k) {
+            pm[k] = mean[k];
+            p2[k] = m2[k];
+            pn[k] = n;
+          }
+        }
+      }
+      __syncthreads();
+    }
+  }
+  // phase 2
+  if (a.grid_y > 1) {
+    grid_barrier(a.bar);
+    const uint32_t cb = kBwdThreads / a.block_y, ty = t / cb;
+    const float* pm = a.ws;
+    const float* p2 = pm + size_t(a.grid_y) * channels;
+    const int* pn = reinterpret_cast<const int*>(p2 + size_t(a.grid_y) * channels);
+    float (*shm1)[2] = reinterpret_cast<float (*)[2]>(&shm[0][0]);
+    for (uint32_t item = blockIdx.x; item * cb < channels; item += gridDim.x) {
+      const uint32_t c = item * cb + t % cb;
+      const bool live = c < channels;
+      int n = 0;
+      float mean[1] = {0.f}, m2[1] = {0.f};
+      if (live)
+        for (uint32_t y = ty; y < a.grid_y; y += a.block_y) {
+          const size_t o = size_t(y) * channels + c;
+          const float mn = __ldcg(pm + o), m2n = __ldcg(p2 + o);
+          welford_merge<false>(n, mean, m2, __ldcg(pn + o), &mn, &m2n);
+        }
+      welford_tree(true, ty, a.block_y, cb, t, n, mean, m2, shm1, shn);
+      if (ty == 0 && live) bn_stats_finish<RunT>(a, c, mean[0], __fdiv_rn(m2[0], __int2float_rn(n)));
+    }
+  }
+  // phase 3
+  grid_barrier(a.bar);
+  const uint32_t tg = blockIdx.x * kBwdThreads + t;
+  if (tg >= a.active) return;
+  const uint32_t c0 = (tg % a.groups) * 8;
+  float m[8], is[8], w[8], b[8];
+#pragma unroll
+  for (int k = 0; k < 8; ++k) {
+    m[k] = __ldcg(a.save_mean + c0 + k);
+    is[k] = __ldcg(a.save_invstd + c0 + k);
+  }
+  unpack16<STK_BF16>(__ldg(reinterpret_cast<const uint4*>(a.weight + c0)), w);
+  unpack16<STK_BF16>(__ldg(reinterpret_cast<const uint4*>(a.bias + c0)), b);
+  bn_act_vectors<kAct, kResidual>(a.x, a.r, a.out, m, is, w, b, tg, a.nvec, a.active);
+}
+
+// k_bn_stats_act for one running-statistics dtype, in the form STK_BN_KERNEL takes
+template <typename RunT>
+struct BnStatsKernel {
+  template <int kAct, bool kResidual>
+  static constexpr auto k = k_bn_stats_act<kAct, kResidual, RunT>;
+};
+
 // The instantiation of `kernel` for (act, residual): every activation without a residual, and ReLU with one.
 #define STK_BN_KERNEL(kernel, act, res)                                                                              \
   ((act) == STK_ACT_SILU        ? kernel<STK_ACT_SILU, false>                                                        \
@@ -417,6 +658,68 @@ int stk_bn_act_ex(stk_ctx* c, int act, const void* x, const void* residual, cons
                                                static_cast<__nv_bfloat16*>(out), save_invstd, nvec, groups, active,
                                                uint32_t(channels));
   STK_CUDA(c, cudaGetLastError());
+  return STK_OK;
+}
+
+int stk_bn_stats_act(stk_ctx* c, int act, const void* x, const void* residual, const void* weight, const void* bias,
+                     void* running_mean, void* running_var, int running_dtype, double momentum, double eps, void* out,
+                     float* save_mean, float* save_invstd, float* workspace, size_t numel, size_t channels, void* stream) {
+  STK_REQUIRE(c, c && x && weight && bias && running_mean && running_var && out && save_mean && save_invstd && workspace,
+              "stk_bn_stats_act: NULL argument");
+  STK_REQUIRE(c, act_valid(act, residual != nullptr),
+              "stk_bn_stats_act: act must be an STK_ACT_* kind, and only STK_ACT_RELU takes a residual");
+  STK_REQUIRE(c, running_dtype == STK_F32 || running_dtype == STK_BF16, "stk_bn_stats_act: running statistics must be STK_F32 or STK_BF16");
+  STK_REQUIRE(c, channels > 0 && channels % 8 == 0 && numel % channels == 0 && numel >= 2 * channels,
+              "stk_bn_stats_act: channels must be a positive multiple of 8 dividing numel, with at least 2 rows");
+  STK_REQUIRE(c, numel < (size_t(1) << 31), "stk_bn_stats_act: numel must be below 2^31");
+  const uintptr_t align = uintptr_t(x) | uintptr_t(residual) | uintptr_t(weight) | uintptr_t(bias) | uintptr_t(out);
+  STK_REQUIRE(c, align % 16 == 0, "stk_bn_stats_act: x, residual, weight, bias and out must be 16-byte aligned");
+  DeviceGuard g(c->device);
+  const uint32_t rows = uint32_t(numel / channels), groups = uint32_t(channels / 8);
+  const BnBwdConfig cfg = bn_bwd_config(rows, uint32_t(channels));
+  const bool bf16_run = running_dtype == STK_BF16;
+  auto kern = bf16_run ? STK_BN_KERNEL(BnStatsKernel<__nv_bfloat16>::k, act, residual != nullptr)
+                       : STK_BN_KERNEL(BnStatsKernel<float>::k, act, residual != nullptr);
+  // as many blocks as the busiest phase uses, at most every resident one (the grid barriers need them all resident)
+  const uint32_t gb = kBwdThreads / (kChains * cfg.block_y), cb = kBwdThreads / cfg.block_y;
+  const size_t items = std::max(size_t((groups + gb - 1) / gb) * cfg.grid_y, size_t((channels + cb - 1) / cb));
+  const uint32_t nvec = uint32_t(numel / 8);
+  const size_t resident = size_t(blocks_per_sm(c, kern, kBwdThreads)) * c->sm_count;
+  size_t blocks = std::min(resident, std::max(items, (size_t(nvec) + kBwdThreads - 1) / kBwdThreads));
+  STK_REQUIRE(c, blocks * kBwdThreads >= groups, "stk_bn_stats_act: too many channels for one resident grid");
+  BnStatsArgs a;
+  a.x = static_cast<const uint4*>(x);
+  a.r = static_cast<const uint4*>(residual);
+  a.weight = static_cast<const __nv_bfloat16*>(weight);
+  a.bias = static_cast<const __nv_bfloat16*>(bias);
+  a.running_mean = running_mean;
+  a.running_var = running_var;
+  a.out = static_cast<uint4*>(out);
+  a.save_mean = save_mean;
+  a.save_invstd = save_invstd;
+  a.ws = workspace;
+  a.bar = c->grid_bar_dev;
+  a.eps = float(eps);
+  a.momentum = float(momentum);
+  a.one_minus_momentum = 1.f - a.momentum;
+  a.bessel = float(double(rows) / double(rows - 1));
+  a.rows = rows;
+  a.groups = groups;
+  a.block_y = cfg.block_y;
+  a.grid_y = cfg.grid_y;
+  a.loops = cfg.loops;
+  a.nvec = nvec;
+  a.active = uint32_t(blocks * kBwdThreads / groups * groups);
+  cudaLaunchConfig_t lc{};
+  lc.gridDim = dim3(unsigned(blocks));
+  lc.blockDim = dim3(kBwdThreads);
+  lc.stream = reinterpret_cast<cudaStream_t>(stream);
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeCooperative;
+  attr[0].val.cooperative = 1;
+  lc.attrs = attr;
+  lc.numAttrs = 1;
+  STK_CUDA(c, cudaLaunchKernelEx(&lc, kern, a));
   return STK_OK;
 }
 

@@ -75,6 +75,8 @@ int stk_ctx_create(int rank, int world, int device, unsigned flags, stk_ctx** ou
   cudaError_t e;
   if ((e = cudaMalloc(&c->prof_ns_dev, 8 * sizeof(unsigned long long))) != cudaSuccess ||
       (e = cudaMemset(c->prof_ns_dev, 0, 8 * sizeof(unsigned long long))) != cudaSuccess ||
+      (e = cudaMalloc(&c->grid_bar_dev, 2 * sizeof(uint32_t))) != cudaSuccess ||
+      (e = cudaMemset(c->grid_bar_dev, 0, 2 * sizeof(uint32_t))) != cudaSuccess ||
       (e = cudaHostAlloc(&c->host_scratch, sizeof(double) * 16, cudaHostAllocMapped)) != cudaSuccess ||
       (e = cudaHostGetDevicePointer(&c->host_scratch_dev, c->host_scratch, 0)) != cudaSuccess ||
       (e = cudaHostAlloc(&c->loss_ring, sizeof(double) * STK_LOSS_RING, cudaHostAllocMapped)) != cudaSuccess ||
@@ -130,6 +132,7 @@ int stk_ctx_destroy(stk_ctx* c) {
   if (c->loss_ring) cudaFreeHost(c->loss_ring);
   cudaFree(c->blk_partial_dev);
   cudaFree(c->prof_ns_dev);
+  cudaFree(c->grid_bar_dev);
   cudaFreeHost(c->host_scratch);
   delete c;
   return STK_OK;

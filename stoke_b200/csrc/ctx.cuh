@@ -71,6 +71,7 @@ struct stk_ctx {
   bool profiling = false;
   std::vector<std::pair<cudaEvent_t, cudaEvent_t>> prof[4];  // 0: K1 reduce, 1: K2 optimizer step, 2: accumulate, 3: norm pass
   unsigned long long* prof_ns_dev = nullptr;                   // {ns, launches} written by K1's block 0 (device timer)
+  uint32_t* grid_bar_dev = nullptr;   // [2] grid barrier of k_bn_stats_act (arrival count, generation), zeroed once
   std::map<const void*, int> occupancy;                       // kernel -> resident blocks per SM (cached query)
   // pinned, mapped host scratch: [0..3] doubles (loss sync), [4..11] scaler staging, word at [12] = error mirror
   double* host_scratch = nullptr;     // [16]

@@ -336,6 +336,21 @@ class Engine:
                                            out.data_ptr(), save_invstd.data_ptr(), x.numel(), x.shape[1], self._stream()))
         self.launches += 1
 
+    def bn_stats_act(self, x: torch.Tensor, residual: Optional[torch.Tensor], weight: torch.Tensor, bias: torch.Tensor,
+                     running_mean: torch.Tensor, running_var: torch.Tensor, momentum: float, eps: float, out: torch.Tensor,
+                     save_mean: torch.Tensor, save_invstd: torch.Tensor, act: int = _lib.ACT_RELU):
+        """``torch.batch_norm_update_stats`` followed by ``bn_act`` in one launch (``stk_bn_stats_act``): writes ``out``,
+        ``save_mean``, ``save_invstd`` and updates the running statistics (fp32 or bf16) in place.  ``fuse.py`` checks
+        dtypes, layout and alignment before calling."""
+        c = x.shape[1]
+        ws = torch.empty(3 * 128 * c, dtype=torch.float32, device=x.device)
+        self._check(self.lib.stk_bn_stats_act(self.ctx, act, x.data_ptr(), residual.data_ptr() if residual is not None else None,
+                                              weight.data_ptr(), bias.data_ptr(), running_mean.data_ptr(),
+                                              running_var.data_ptr(), _DT[running_mean.dtype], float(momentum), float(eps),
+                                              out.data_ptr(), save_mean.data_ptr(), save_invstd.data_ptr(), ws.data_ptr(),
+                                              x.numel(), c, self._stream()))
+        self.launches += 1
+
     def bn_act_backward(self, grad: torch.Tensor, x: torch.Tensor, out: Optional[torch.Tensor], mean: torch.Tensor,
                         invstd: torch.Tensor, weight: torch.Tensor, bias: Optional[torch.Tensor],
                         grad_x: Optional[torch.Tensor], grad_weight: torch.Tensor, grad_bias: torch.Tensor,

@@ -10,16 +10,16 @@ parameter and buffer with ``module``, in which each ``BatchNorm2d -> act`` and `
 only, no hooks) and ``module`` itself for every other call, or None when tracing or rewriting fails or nothing matches;
 the caller then keeps running ``module``.
 
-What stays torch's: the forward statistics and the running-statistics update (``torch.batch_norm_update_stats``, the
-reduction the native training forward runs).  The forward's elementwise apply / add / activation is one kernel, which
-rounds every intermediate as the unfused ops do.  The backward (``stk_bn_act_backward_ex``) folds the activation's
+The forward is one kernel (``stk_bn_stats_act``): the batch statistics and the running-statistics update, merged in the
+order of torch's ``batch_norm_update_stats`` (the reduction the native training forward runs), then the apply / add /
+activation, which rounds every intermediate as the unfused ops do.  The backward (``stk_bn_act_backward_ex``) folds the activation's
 backward op (``threshold_backward``, ``silu_backward``, ``hardswish_backward``, ``hardtanh_backward``) into the two
 passes of torch's channels-last ``native_batch_norm_backward`` and adds its per-channel sums in torch's order, so every
 result is bit-identical to the calls autograd makes for the unfused chain.  It takes the gradient when torch's BatchNorm
 backward would run its channels-last kernels on it (the activation backward's output is channels-last; another layout
 is made channels-last first) and it is bf16 and aligned; otherwise it runs those calls.
 Each call falls back to the unfused torch ops when the kernel does not cover its inputs (eval mode, no running statistics,
-not bf16, not channels-last, misaligned, C % 8 != 0, 2^31 elements or more, a CPU tensor), so the same inputs give the
+running statistics neither fp32 nor bf16, not bf16, not channels-last, misaligned, C % 8 != 0, 2^31 elements or more, a CPU tensor), so the same inputs give the
 same results whether or not the model was rewritten.
 """
 import functools
@@ -68,6 +68,10 @@ def _covered(bn: torch.nn.BatchNorm2d, x: torch.Tensor, r: Optional[torch.Tensor
     w, b = bn.weight, bn.bias
     if w is None or b is None or w.dtype != torch.bfloat16 or b.dtype != torch.bfloat16:
         return False
+    rm, rv = bn.running_mean, bn.running_var
+    if not (rm.dtype in (torch.float32, torch.bfloat16) and rv.dtype == rm.dtype and rm.device == x.device
+            and rv.device == x.device and rm.is_contiguous() and rv.is_contiguous()):
+        return False
     if not (x.is_cuda and x.dtype == torch.bfloat16 and x.dim() == 4 and x.is_contiguous(memory_format=torch.channels_last)):
         return False
     n, c = x.numel(), x.shape[1]
@@ -105,10 +109,11 @@ class _BnActFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x, weight, bias, residual, bn, engine, act):
         momentum = _momentum(bn)
-        mean, var = torch.batch_norm_update_stats(x, bn.running_mean, bn.running_var, momentum)
         out = torch.empty_like(x)
+        mean = torch.empty(x.shape[1], dtype=torch.float32, device=x.device)
         invstd = torch.empty_like(mean)
-        engine.bn_act(x, residual, mean, var, weight, bias, bn.eps, out, invstd, act)
+        engine.bn_stats_act(x, residual, weight, bias, bn.running_mean, bn.running_var, momentum, bn.eps, out, mean,
+                            invstd, act)
         # the ReLU mask: out at a site with a residual; otherwise the activation's input is recomputed from x and the
         # parameters (bias saved instead)
         ctx.save_for_backward(x, weight, out if residual is not None else bias, mean, invstd)
@@ -144,7 +149,7 @@ class _BnActFn(torch.autograd.Function):
 
 
 class BnAct(torch.nn.Module):
-    """``act(bn(x) [+ residual])``: one ``stk_bn_act_ex`` launch when the kernel covers the inputs, the unfused torch
+    """``act(bn(x) [+ residual])``: one ``stk_bn_stats_act`` launch when the kernel covers the inputs, the unfused torch
     ops otherwise (``inplace``: the add was ``out += residual``, which keeps ``out``'s dtype).  ``act`` is one of
     ``_lib.ACT_*``; only ReLU takes a residual.  ``act_fn`` is the unfused activation (the user's module or function),
     by default ``torch.relu``, ``F.silu``, ``F.hardswish`` or ``F.relu6``.  Holds a reference to the user's BatchNorm2d
