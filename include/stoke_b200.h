@@ -482,11 +482,19 @@ int stk_bn_act_ex(stk_ctx* ctx, int act, const void* x, const void* residual, co
  * Order contract: the statistics merge in the order of torch's batch_norm_collect_statistics_channels_last_kernel as
  * launched by flexible_launch_configs(R, channels, coop) (the grid stk_bn_act_backward_ex reproduces).
  * Coverage as stk_bn_act_ex, with at least 2 rows (R = numel / channels); the running statistics need no alignment.
- * workspace: 3 * 128 * channels floats; no initialisation needed.  The grid barrier lives in the context, so launches on
- * one context must not overlap (one stream, or streams ordered against each other). */
+ * workspace: 3 * 128 * channels floats (twice that with a second BatchNorm); no initialisation needed.  The grid barrier
+ * lives in the context, so launches on one context must not overlap (one stream, or streams ordered against each other).
+ * weight2, when not NULL (STK_ACT_RELU with a residual only), makes the residual the input of a second training-mode
+ * BatchNorm (bias2, running_mean2 / running_var2 of running_dtype, momentum2, eps2; 16-byte aligned weight2 / bias2):
+ * its statistics, save_mean2 / save_invstd2 and running statistics are computed as the first one's, and
+ *   out = relu(bf16(bf16(bn(x)) + bf16(bn2(residual)))),
+ * bit-identical to the two BatchNorms, `out += identity` and the ReLU; bn2's output is never written.  weight2 NULL:
+ * the other trailing arguments are ignored. */
 int stk_bn_stats_act(stk_ctx* ctx, int act, const void* x, const void* residual, const void* weight, const void* bias,
                      void* running_mean, void* running_var, int running_dtype, double momentum, double eps, void* out,
-                     float* save_mean, float* save_invstd, float* workspace, size_t numel, size_t channels, void* stream);
+                     float* save_mean, float* save_invstd, float* workspace, size_t numel, size_t channels, void* stream,
+                     const void* weight2, const void* bias2, void* running_mean2, void* running_var2, double momentum2,
+                     double eps2, float* save_mean2, float* save_invstd2);
 /* stk_bn_act_ex with act = STK_ACT_RELU */
 int stk_bn_act(stk_ctx* ctx, const void* x, const void* residual, const float* mean, const float* var, const void* weight,
                const void* bias, double eps, void* out, float* save_invstd, size_t numel, size_t channels, void* stream);
@@ -507,6 +515,14 @@ int stk_bn_act(stk_ctx* ctx, const void* x, const void* residual, const float* m
  * <= 0 iff y <= 0); grad_residual is unused.  grad_pre, when not NULL, receives g (2 B/element more; it exists so the
  * derivative can be tested apart from the sums, and must be NULL for STK_ACT_RELU, whose g keeps grad's bits or is +0).
  * grad_x may be NULL (no elementwise pass).
+ * grad2, when not NULL (a residual site only), is a second part of the output's gradient, laid out and aligned as grad:
+ * the kernel takes bf16(float(grad) + float(grad2)) in place of grad, which is the sum autograd's bf16 add forms when
+ * the output has two users (2 B/element more, the add's 6 B/element and its launch saved).
+ * x2, when not NULL (a residual site only), is the input of the residual's BatchNorm (stk_bn_stats_act's weight2): with
+ * its mean2, invstd2 and weight2 it gets torch's BatchNorm backward for the same g, in the same order: grad_bias2 =
+ * bf16(sum_dy) (the same sum), grad_weight2 = bf16(sum_dy_xmu2 * invstd2), grad_x2 by the grad_x formula with its own
+ * mean, invstd, weight and sum_dy_xmu2; grad_residual then holds g, and grad_x2 is given exactly when grad_x is.  The
+ * workspace is then 3 * (1 + 128) * channels floats.  x2 NULL: the other trailing arguments are ignored.
  * Order contract: the two sums add in the order of torch's batch_norm_backward_reduce_channels_last_kernel as launched by
  * flexible_launch_configs(R, channels, coop) with MAX_BLOCK_SIZE 512 (a function of R and channels only), so all four
  * outputs are bit-identical to act_backward + native_batch_norm_backward on channels-last bf16 inputs.
@@ -514,7 +530,9 @@ int stk_bn_act(stk_ctx* ctx, const void* x, const void* residual, const float* m
 int stk_bn_act_backward_ex(stk_ctx* ctx, int act, const void* grad, const void* x, const void* out, const float* mean,
                            const float* invstd, const void* weight, const void* bias, void* grad_x, void* grad_weight,
                            void* grad_bias, void* grad_residual, void* grad_pre, float* workspace, size_t numel,
-                           size_t channels, void* stream);
+                           size_t channels, void* stream, const void* grad2, const void* x2, const float* mean2,
+                           const float* invstd2, const void* weight2, void* grad_x2, void* grad_weight2,
+                           void* grad_bias2);
 /* stk_bn_act_backward_ex with act = STK_ACT_RELU and no grad_pre */
 int stk_bn_act_backward(stk_ctx* ctx, const void* grad, const void* x, const void* out, const float* mean,
                         const float* invstd, const void* weight, const void* bias, void* grad_x, void* grad_weight,

@@ -179,9 +179,9 @@ _SIGNATURES = {
     "stk_bn_act_backward": (C.c_int, [_P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, C.c_size_t, C.c_size_t, _P]),
     "stk_bn_act_ex": (C.c_int, [_P, C.c_int, _P, _P, _P, _P, _P, _P, C.c_double, _P, _P, C.c_size_t, C.c_size_t, _P]),
     "stk_bn_act_backward_ex": (C.c_int, [_P, C.c_int, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, C.c_size_t,
-                                         C.c_size_t, _P]),
+                                         C.c_size_t, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     "stk_bn_stats_act": (C.c_int, [_P, C.c_int, _P, _P, _P, _P, _P, _P, C.c_int, C.c_double, C.c_double, _P, _P, _P, _P,
-                                   C.c_size_t, C.c_size_t, _P]),
+                                   C.c_size_t, C.c_size_t, _P, _P, _P, _P, _P, C.c_double, C.c_double, _P, _P]),
     "stk_randperm": (C.c_int, [C.c_uint64, C.POINTER(C.c_int64), C.c_int, _P]),
     "stk_sampler_plan": (C.c_int, [C.POINTER(SamplerPlan)]),
     "stk_sampler_last_slice": (C.c_int, [C.POINTER(SamplerPlan), C.c_int64, _P]),

@@ -163,32 +163,51 @@ __device__ __forceinline__ void load8(const float* __restrict__ p, float (&f)[8]
 // of its by for kBwdThreads / (kChains * block_y) channel groups.  With grid_y == 1 the block's sums are final;
 // otherwise they go to the workspace partials and k_bn_bwd_finish adds them.  g_out receives g: the residual's gradient
 // (ReLU), or the optional grad_pre of another activation.  ReLU without a residual has no g_out: a run-time checked
-// store there would take its instantiation from 80 to 99 registers.
-template <int kAct, bool kResidual>
-__global__ void __launch_bounds__(kBwdThreads) k_bn_bwd_reduce(const uint4* __restrict__ grad, const uint4* __restrict__ x,
+// store there would take its instantiation from 80 to 99 registers.  kSum (residual sites): the output's gradient
+// arrives in two parts, grad and grad2, summed first as autograd's bf16 add sums them: bf16(float(grad) + float(grad2)).
+// kTwo (residual sites whose residual is a second BatchNorm's output, relu(bn(x) + bn2(x2))): torch's backward of bn2
+// sees the same g on the same grid, so sum_dy serves both; a third row sums g * (x2 - mean2) in the same order.
+struct BnBwdSecond {   // the second BatchNorm of a kTwo site
+  const uint4* x;
+  const float* mean;
+  const float* invstd;
+  const __nv_bfloat16* weight;
+  float* ws;           // its sum_dy_xmu [C], then per-block partials [grid_y][C]
+  __nv_bfloat16* dweight;
+  __nv_bfloat16* dbias;
+  uint4* dx;
+};
+
+template <int kAct, bool kResidual, bool kSum = false, bool kTwo = false>
+__global__ void __launch_bounds__(kBwdThreads) k_bn_bwd_reduce(const uint4* __restrict__ grad, const uint4* __restrict__ grad2,
+                                                               const uint4* __restrict__ x,
                                                                const uint4* __restrict__ out, const float* __restrict__ mean,
                                                                const float* __restrict__ invstd,
                                                                const __nv_bfloat16* __restrict__ weight,
                                                                const __nv_bfloat16* __restrict__ bias, uint4* __restrict__ g_out,
                                                                float* __restrict__ ws, __nv_bfloat16* __restrict__ dweight,
                                                                __nv_bfloat16* __restrict__ dbias, uint32_t rows,
-                                                               uint32_t groups, uint32_t block_y, uint32_t loops) {
-  __shared__ float4 sh[kBwdThreads][4];   // per thread: 8 sums of g, then 8 sums of g * (x - mean)
+                                                               uint32_t groups, uint32_t block_y, uint32_t loops,
+                                                               const BnBwdSecond s2) {
+  constexpr int kS = kTwo ? 24 : 16;   // sums per thread
+  // per thread: 8 sums of g, then 8 sums of g * (x - mean) (then 8 of g * (x2 - mean2))
+  __shared__ float4 sh[kBwdThreads][kS / 4];
   const uint32_t t = threadIdx.x, gb = kBwdThreads / (kChains * block_y);
   const uint32_t cgl = t % gb, j = t / gb % kChains, ty = t / (gb * kChains);
   const uint32_t cg = blockIdx.x * gb + cgl, c0 = cg * 8, channels = groups * 8;
   const bool live = cg < groups;
-  float sdy[8], sxm[8];
+  float sdy[8], sxm[8], sxm2[8];
 #pragma unroll
-  for (int k = 0; k < 8; ++k) sdy[k] = sxm[k] = 0.f;
+  for (int k = 0; k < 8; ++k) sdy[k] = sxm[k] = sxm2[k] = 0.f;
   if (live) {
-    float m[8], is[8], w[8], b[8];
+    float m[8], is[8], w[8], b[8], m2[8];
     if (!kResidual) {
       load8(invstd + c0, is);
       unpack16<STK_BF16>(__ldg(reinterpret_cast<const uint4*>(weight + c0)), w);
       unpack16<STK_BF16>(__ldg(reinterpret_cast<const uint4*>(bias + c0)), b);
     }
     load8(mean + c0, m);
+    if (kTwo) load8(s2.mean + c0, m2);
     const uint32_t stride = block_y * gridDim.y, m0 = blockIdx.y * block_y + ty;
 #pragma unroll 2
     for (uint32_t i = 0; i < loops; ++i) {
@@ -196,8 +215,18 @@ __global__ void __launch_bounds__(kBwdThreads) k_bn_bwd_reduce(const uint4* __re
       const bool in = row < rows;
       const size_t v = size_t(row) * groups + cg;
       const uint4 zero = make_uint4(0, 0, 0, 0);
-      const uint4 gv = in ? __ldg(grad + v) : zero, xv = in ? __ldg(x + v) : zero;
+      uint4 gv = in ? __ldg(grad + v) : zero;
+      const uint4 xv = in ? __ldg(x + v) : zero;
       float xf[8], gf[8], mf[8];
+      if (kSum) {
+        float g2[8];
+        unpack16<STK_BF16>(gv, gf);
+        unpack16<STK_BF16>(in ? __ldg(grad2 + v) : zero, g2);
+        uint16_t o[8];
+#pragma unroll
+        for (int k = 0; k < 8; ++k) o[k] = bf16_bits(__fadd_rn(gf[k], g2[k]));
+        gv = pack8(o);
+      }
       unpack16<STK_BF16>(xv, xf);
       uint4 g;
       if (kResidual) {
@@ -220,25 +249,34 @@ __global__ void __launch_bounds__(kBwdThreads) k_bn_bwd_reduce(const uint4* __re
         sdy[k] = __fadd_rn(sdy[k], gf[k]);
         sxm[k] = __fmaf_rn(gf[k], __fsub_rn(xf[k], m[k]), sxm[k]);
       }
+      if (kTwo) {
+        unpack16<STK_BF16>(in ? __ldg(s2.x + v) : zero, xf);
+#pragma unroll
+        for (int k = 0; k < 8; ++k) sxm2[k] = __fmaf_rn(gf[k], __fsub_rn(xf[k], m2[k]), sxm2[k]);
+      }
     }
   }
   sh[t][0] = make_float4(sdy[0], sdy[1], sdy[2], sdy[3]);
   sh[t][1] = make_float4(sdy[4], sdy[5], sdy[6], sdy[7]);
   sh[t][2] = make_float4(sxm[0], sxm[1], sxm[2], sxm[3]);
   sh[t][3] = make_float4(sxm[4], sxm[5], sxm[6], sxm[7]);
+  if (kTwo) {
+    sh[t][kS / 4 - 2] = make_float4(sxm2[0], sxm2[1], sxm2[2], sxm2[3]);
+    sh[t][kS / 4 - 1] = make_float4(sxm2[4], sxm2[5], sxm2[6], sxm2[7]);
+  }
   __syncthreads();
   // fold the chains, then halve over ty; thread (cgl, ty) of chain 0 owns the slot of that virtual thread
   const bool owner = j == 0;
-  float s[16];
+  float s[kS];
   if (owner) {
     const float* p = reinterpret_cast<const float*>(sh[t]);
 #pragma unroll
-    for (int k = 0; k < 16; ++k) s[k] = p[k];
+    for (int k = 0; k < kS; ++k) s[k] = p[k];
 #pragma unroll
     for (int q = 1; q < kChains; ++q) {
       const float* r = reinterpret_cast<const float*>(sh[t + q * gb]);
 #pragma unroll
-      for (int k = 0; k < 16; ++k) s[k] = __fadd_rn(s[k], r[k]);
+      for (int k = 0; k < kS; ++k) s[k] = __fadd_rn(s[k], r[k]);
     }
   }
   __syncthreads();
@@ -246,17 +284,36 @@ __global__ void __launch_bounds__(kBwdThreads) k_bn_bwd_reduce(const uint4* __re
     if (owner && ty < 2 * off) {
       float* p = reinterpret_cast<float*>(sh[t]);
 #pragma unroll
-      for (int k = 0; k < 16; ++k) p[k] = s[k];
+      for (int k = 0; k < kS; ++k) p[k] = s[k];
     }
     __syncthreads();
     if (owner && ty < off) {
       const float* r = reinterpret_cast<const float*>(sh[t + off * gb * kChains]);
 #pragma unroll
-      for (int k = 0; k < 16; ++k) s[k] = __fadd_rn(s[k], r[k]);
+      for (int k = 0; k < kS; ++k) s[k] = __fadd_rn(s[k], r[k]);
     }
     __syncthreads();
   }
   if (!(owner && ty == 0 && live)) return;
+  if (kTwo) {
+    if (gridDim.y == 1) {
+      float is2[8];
+      load8(s2.invstd + c0, is2);
+      uint16_t dw[8], db[8];
+#pragma unroll
+      for (int k = 0; k < 8; ++k) {
+        s2.ws[c0 + k] = s[16 + k];
+        db[k] = bf16_bits(s[k]);
+        dw[k] = bf16_bits(__fmul_rn(s[16 + k], is2[k]));
+      }
+      *reinterpret_cast<uint4*>(s2.dbias + c0) = pack8(db);
+      *reinterpret_cast<uint4*>(s2.dweight + c0) = pack8(dw);
+    } else {
+      float* p = s2.ws + channels + size_t(blockIdx.y) * channels + c0;
+#pragma unroll
+      for (int k = 0; k < 8; ++k) p[k] = s[16 + k];
+    }
+  }
   if (gridDim.y == 1) {
     float is[8];
     load8(invstd + c0, is);
@@ -284,29 +341,34 @@ __global__ void __launch_bounds__(kBwdThreads) k_bn_bwd_reduce(const uint4* __re
 }
 
 // torch's cross-block finish: thread ty adds the partials of blocks ty, ty + block_y, ... from +0, then the halving
-// tree over ty.  One thread per (channel, ty).
+// tree over ty.  One thread per (channel, ty).  kTwo: the third row too (the second BatchNorm's sum_dy_xmu).
+template <bool kTwo>
 __global__ void __launch_bounds__(kBwdThreads) k_bn_bwd_finish(float* __restrict__ ws, const float* __restrict__ invstd,
                                                                __nv_bfloat16* __restrict__ dweight,
                                                                __nv_bfloat16* __restrict__ dbias, uint32_t channels,
-                                                               uint32_t block_y, uint32_t grid_y) {
-  __shared__ float sh[2][kBwdThreads];
+                                                               uint32_t block_y, uint32_t grid_y, const BnBwdSecond s2) {
+  __shared__ float sh[kTwo ? 3 : 2][kBwdThreads];
   const uint32_t t = threadIdx.x, cb = kBwdThreads / block_y, ty = t / cb, c = blockIdx.x * cb + t % cb;
   const bool live = c < channels;
   const float* pdy = ws + 2 * channels;
   const float* pxm = pdy + size_t(grid_y) * channels;
-  float dy = 0.f, xm = 0.f;
+  const float* pxm2 = s2.ws + channels;
+  float dy = 0.f, xm = 0.f, xm2 = 0.f;
   if (live)
     for (uint32_t y = ty; y < grid_y; y += block_y) {
       dy = __fadd_rn(dy, pdy[size_t(y) * channels + c]);
       xm = __fadd_rn(xm, pxm[size_t(y) * channels + c]);
+      if (kTwo) xm2 = __fadd_rn(xm2, pxm2[size_t(y) * channels + c]);
     }
   for (uint32_t off = block_y / 2; off > 0; off >>= 1) {
     sh[0][t] = dy;
     sh[1][t] = xm;
+    if (kTwo) sh[kTwo ? 2 : 0][t] = xm2;
     __syncthreads();
     if (ty < off) {
       dy = __fadd_rn(dy, sh[0][t + off * cb]);
       xm = __fadd_rn(xm, sh[1][t + off * cb]);
+      if (kTwo) xm2 = __fadd_rn(xm2, sh[kTwo ? 2 : 0][t + off * cb]);
     }
     __syncthreads();
   }
@@ -315,21 +377,69 @@ __global__ void __launch_bounds__(kBwdThreads) k_bn_bwd_finish(float* __restrict
   ws[channels + c] = xm;
   dbias[c] = __float2bfloat16_rn(dy);
   dweight[c] = __float2bfloat16_rn(__fmul_rn(xm, invstd[c]));
+  if (kTwo) {
+    s2.ws[c] = xm2;
+    s2.dbias[c] = __float2bfloat16_rn(dy);
+    s2.dweight[c] = __float2bfloat16_rn(__fmul_rn(xm2, s2.invstd[c]));
+  }
 }
 
 // dx = bf16(((g - sum_dy * n) - (x - mean) * k1) * k2), k1 = invstd * invstd * sum_dy_xmu * n, k2 = w * invstd,
 // n = float(1.0 / rows): torch's channels-last elementwise backward, whose SASS contracts both subtractions with their
 // products (FFMA -sum_dy * n + g; FADD x - mean; FFMA -k1 * (x - mean) + t; FMUL k2).  Thread layout as in k_bn_act.
-template <int kAct, bool kResidual>
+// kTwo: the second BatchNorm's dx2 from the same g and sum_dy, with its own mean, k1 and k2.
+template <int kAct, bool kResidual, bool kTwo = false>
 __global__ void __launch_bounds__(kBnThreads) k_bn_bwd_elemt(const uint4* __restrict__ grad, const uint4* __restrict__ x,
                                                             const float* __restrict__ mean, const float* __restrict__ invstd,
                                                             const __nv_bfloat16* __restrict__ weight,
                                                             const __nv_bfloat16* __restrict__ bias,
                                                             const float* __restrict__ ws, uint4* __restrict__ dx, float n,
-                                                            uint32_t nvec, uint32_t groups, uint32_t active) {
+                                                            uint32_t nvec, uint32_t groups, uint32_t active,
+                                                            const BnBwdSecond s2) {
   const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
   if (t >= active) return;
   const uint32_t c0 = (t % groups) * 8, channels = groups * 8;
+  if (kTwo) {
+    float m[8], m2[8], sdy[8], k1[8], k2[8], k1b[8], k2b[8];
+    {
+      float is[8], w[8], sxm[8];
+      load8(mean + c0, m);
+      load8(invstd + c0, is);
+      load8(ws + c0, sdy);
+      load8(ws + channels + c0, sxm);
+      unpack16<STK_BF16>(__ldg(reinterpret_cast<const uint4*>(weight + c0)), w);
+#pragma unroll
+      for (int k = 0; k < 8; ++k) {
+        k1[k] = __fmul_rn(__fmul_rn(__fmul_rn(is[k], is[k]), sxm[k]), n);
+        k2[k] = __fmul_rn(w[k], is[k]);
+      }
+      load8(s2.mean + c0, m2);
+      load8(s2.invstd + c0, is);
+      load8(s2.ws + c0, sxm);
+      unpack16<STK_BF16>(__ldg(reinterpret_cast<const uint4*>(s2.weight + c0)), w);
+#pragma unroll
+      for (int k = 0; k < 8; ++k) {
+        k1b[k] = __fmul_rn(__fmul_rn(__fmul_rn(is[k], is[k]), sxm[k]), n);
+        k2b[k] = __fmul_rn(w[k], is[k]);
+      }
+    }
+    for (uint32_t v = t; v < nvec; v += active) {
+      float xf[8], x2f[8], gf[8];
+      unpack16<STK_BF16>(__ldg(x + v), xf);
+      unpack16<STK_BF16>(__ldg(s2.x + v), x2f);
+      unpack16<STK_BF16>(__ldg(grad + v), gf);
+      uint16_t o[8], o2[8];
+#pragma unroll
+      for (int k = 0; k < 8; ++k) {
+        const float gc = __fmaf_rn(-sdy[k], n, gf[k]);
+        o[k] = bf16_bits(__fmul_rn(__fmaf_rn(-__fsub_rn(xf[k], m[k]), k1[k], gc), k2[k]));
+        o2[k] = bf16_bits(__fmul_rn(__fmaf_rn(-__fsub_rn(x2f[k], m2[k]), k1b[k], gc), k2b[k]));
+      }
+      dx[v] = pack8(o);
+      s2.dx[v] = pack8(o2);
+    }
+    return;
+  }
   float m[8], is[8], w[8], b[8], sdy[8], k1[8], k2[8];
   {
     float sxm[8];
@@ -407,10 +517,18 @@ struct BnStatsArgs {
   uint4* out;
   float* save_mean;
   float* save_invstd;
-  float* ws;          // [grid_y][C] partial means, then m2s, then counts (int)
+  float* ws;          // [grid_y][C] partial means, then m2s, then counts (int); the second BatchNorm's after them
   uint32_t* bar;      // grid barrier: arrival count, generation
   float eps, momentum, one_minus_momentum, bessel;
   uint32_t rows, groups, block_y, grid_y, loops, nvec, active;
+  // the residual's BatchNorm at a kTwo site (its input is r)
+  const __nv_bfloat16* weight2;
+  const __nv_bfloat16* bias2;
+  void* running_mean2;
+  void* running_var2;
+  float* save_mean2;
+  float* save_invstd2;
+  float eps2, momentum2, one_minus_momentum2;
 };
 
 // A barrier over the whole (co-resident) grid.  The arrival count returns to 0 at every barrier and the generation only
@@ -456,15 +574,17 @@ __device__ __forceinline__ float run_load(const __nv_bfloat16* p) { return __bfl
 __device__ __forceinline__ void run_store(float* p, float v) { *p = v; }
 __device__ __forceinline__ void run_store(__nv_bfloat16* p, float v) { *p = __float2bfloat16_rn(v); }
 
-// the outputs of channel c from its final (mean, var = m2 / n)
+// the outputs of channel c from its final (mean, var = m2 / n), for BatchNorm `side` (1: the residual's at a kTwo site)
 template <typename RunT>
-__device__ __forceinline__ void bn_stats_finish(const BnStatsArgs& a, uint32_t c, float mean, float var) {
-  a.save_mean[c] = mean;
-  a.save_invstd[c] = rsqrtf(var + a.eps);
-  RunT* rm = static_cast<RunT*>(a.running_mean) + c;
-  RunT* rv = static_cast<RunT*>(a.running_var) + c;
-  run_store(rm, __fmaf_rn(mean, a.momentum, __fmul_rn(a.one_minus_momentum, run_load(rm))));
-  run_store(rv, __fmaf_rn(__fmul_rn(var, a.bessel), a.momentum, __fmul_rn(a.one_minus_momentum, run_load(rv))));
+__device__ __forceinline__ void bn_stats_finish(const BnStatsArgs& a, int side, uint32_t c, float mean, float var) {
+  const float eps = side ? a.eps2 : a.eps, mom = side ? a.momentum2 : a.momentum;
+  const float omm = side ? a.one_minus_momentum2 : a.one_minus_momentum;
+  (side ? a.save_mean2 : a.save_mean)[c] = mean;
+  (side ? a.save_invstd2 : a.save_invstd)[c] = rsqrtf(var + eps);
+  RunT* rm = static_cast<RunT*>(side ? a.running_mean2 : a.running_mean) + c;
+  RunT* rv = static_cast<RunT*>(side ? a.running_var2 : a.running_var) + c;
+  run_store(rm, __fmaf_rn(mean, mom, __fmul_rn(omm, run_load(rm))));
+  run_store(rv, __fmaf_rn(__fmul_rn(var, a.bessel), mom, __fmul_rn(omm, run_load(rv))));
 }
 
 // the halving tree over ty of torch's welford_merge_block_vertical; slot(t) is this thread's shared-memory slot, the
@@ -490,7 +610,9 @@ __device__ __forceinline__ void welford_tree(bool owner, uint32_t ty, uint32_t b
   }
 }
 
-template <int kAct, bool kResidual, typename RunT>
+// kTwo (ReLU with a residual): the residual r is the input of a second BatchNorm (weight2, ...), whose statistics are
+// gathered after x's in the same phases and applied before the add.
+template <int kAct, bool kResidual, typename RunT, bool kTwo = false>
 __global__ void __launch_bounds__(kBwdThreads, 3) k_bn_stats_act(const BnStatsArgs a) {
   __shared__ float shm[kBwdThreads][16];
   __shared__ int shn[kBwdThreads];
@@ -500,7 +622,12 @@ __global__ void __launch_bounds__(kBwdThreads, 3) k_bn_stats_act(const BnStatsAr
     const uint32_t gb = kBwdThreads / (kChains * a.block_y);
     const uint32_t cgl = t % gb, j = t / gb % kChains, ty = t / (gb * kChains);
     const uint32_t nxb = (a.groups + gb - 1) / gb, stride = a.block_y * a.grid_y;
+    // kTwo: x, then the residual through its own BatchNorm, one after the other (one Welford state at a time)
+#pragma unroll 1
+    for (int side = 0; side < (kTwo ? 2 : 1); ++side)
     for (uint32_t item = blockIdx.x; item < nxb * a.grid_y; item += gridDim.x) {
+      const uint4* xs = side ? a.r : a.x;
+      float* ws = a.ws + size_t(side) * 3 * a.grid_y * channels;
       const uint32_t by = item / nxb, cg = (item % nxb) * gb + cgl;
       const bool live = cg < a.groups;
       const uint32_t m0 = by * a.block_y + ty;
@@ -514,7 +641,7 @@ __global__ void __launch_bounds__(kBwdThreads, 3) k_bn_stats_act(const BnStatsAr
 #pragma unroll
         for (int u = 0; u < 4; ++u) {
           const uint32_t row = m0 + (kChains * (i0 + u) + j) * stride;
-          xv[u] = live && i0 + u < a.loops && row < a.rows ? __ldg(a.x + size_t(row) * a.groups + cg) : make_uint4(0, 0, 0, 0);
+          xv[u] = live && i0 + u < a.loops && row < a.rows ? __ldg(xs + size_t(row) * a.groups + cg) : make_uint4(0, 0, 0, 0);
         }
 #pragma unroll
         for (int u = 0; u < 4; ++u) {
@@ -552,9 +679,9 @@ __global__ void __launch_bounds__(kBwdThreads, 3) k_bn_stats_act(const BnStatsAr
       if (owner && ty == 0 && live) {
         const uint32_t c0 = cg * 8;
         if (a.grid_y == 1) {
-          for (int k = 0; k < 8; ++k) bn_stats_finish<RunT>(a, c0 + k, mean[k], __fdiv_rn(m2[k], __int2float_rn(n)));
+          for (int k = 0; k < 8; ++k) bn_stats_finish<RunT>(a, side, c0 + k, mean[k], __fdiv_rn(m2[k], __int2float_rn(n)));
         } else {
-          float* pm = a.ws + size_t(by) * channels + c0;
+          float* pm = ws + size_t(by) * channels + c0;
           float* p2 = pm + size_t(a.grid_y) * channels;
           int* pn = reinterpret_cast<int*>(p2 + size_t(a.grid_y) * channels);
 #pragma unroll
@@ -572,11 +699,13 @@ __global__ void __launch_bounds__(kBwdThreads, 3) k_bn_stats_act(const BnStatsAr
   if (a.grid_y > 1) {
     grid_barrier(a.bar);
     const uint32_t cb = kBwdThreads / a.block_y, ty = t / cb;
-    const float* pm = a.ws;
-    const float* p2 = pm + size_t(a.grid_y) * channels;
-    const int* pn = reinterpret_cast<const int*>(p2 + size_t(a.grid_y) * channels);
     float (*shm1)[2] = reinterpret_cast<float (*)[2]>(&shm[0][0]);
+#pragma unroll 1
+    for (int side = 0; side < (kTwo ? 2 : 1); ++side)
     for (uint32_t item = blockIdx.x; item * cb < channels; item += gridDim.x) {
+      const float* pm = a.ws + size_t(side) * 3 * a.grid_y * channels;
+      const float* p2 = pm + size_t(a.grid_y) * channels;
+      const int* pn = reinterpret_cast<const int*>(p2 + size_t(a.grid_y) * channels);
       const uint32_t c = item * cb + t % cb;
       const bool live = c < channels;
       int n = 0;
@@ -588,7 +717,7 @@ __global__ void __launch_bounds__(kBwdThreads, 3) k_bn_stats_act(const BnStatsAr
           welford_merge<false>(n, mean, m2, __ldcg(pn + o), &mn, &m2n);
         }
       welford_tree(true, ty, a.block_y, cb, t, n, mean, m2, shm1, shn);
-      if (ty == 0 && live) bn_stats_finish<RunT>(a, c, mean[0], __fdiv_rn(m2[0], __int2float_rn(n)));
+      if (ty == 0 && live) bn_stats_finish<RunT>(a, side, c, mean[0], __fdiv_rn(m2[0], __int2float_rn(n)));
     }
   }
   // phase 3
@@ -604,7 +733,31 @@ __global__ void __launch_bounds__(kBwdThreads, 3) k_bn_stats_act(const BnStatsAr
   }
   unpack16<STK_BF16>(__ldg(reinterpret_cast<const uint4*>(a.weight + c0)), w);
   unpack16<STK_BF16>(__ldg(reinterpret_cast<const uint4*>(a.bias + c0)), b);
-  bn_act_vectors<kAct, kResidual>(a.x, a.r, a.out, m, is, w, b, tg, a.nvec, a.active);
+  if (!kTwo) {
+    bn_act_vectors<kAct, kResidual>(a.x, a.r, a.out, m, is, w, b, tg, a.nvec, a.active);
+    return;
+  }
+  // z = bf16(float(bn_apply(x)) + float(bn_apply2(r))): `out += identity` with identity the residual BatchNorm's output
+  float m2[8], is2[8], w2[8], b2[8];
+#pragma unroll
+  for (int k = 0; k < 8; ++k) {
+    m2[k] = __ldcg(a.save_mean2 + c0 + k);
+    is2[k] = __ldcg(a.save_invstd2 + c0 + k);
+  }
+  unpack16<STK_BF16>(__ldg(reinterpret_cast<const uint4*>(a.weight2 + c0)), w2);
+  unpack16<STK_BF16>(__ldg(reinterpret_cast<const uint4*>(a.bias2 + c0)), b2);
+  for (uint32_t v = tg; v < a.nvec; v += a.active) {
+    float xf[8], rf[8];
+    unpack16<STK_BF16>(__ldg(a.x + v), xf);
+    unpack16<STK_BF16>(__ldg(a.r + v), rf);
+    uint16_t o[8];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      const uint16_t y = bn_apply(xf[j], m[j], is[j], w[j], b[j]), y2 = bn_apply(rf[j], m2[j], is2[j], w2[j], b2[j]);
+      o[j] = act_out<STK_ACT_RELU>(bf16_bits(bf16_val(y) + bf16_val(y2)));
+    }
+    a.out[v] = pack8(o);
+  }
 }
 
 // k_bn_stats_act for one running-statistics dtype, in the form STK_BN_KERNEL takes
@@ -663,11 +816,17 @@ int stk_bn_act_ex(stk_ctx* c, int act, const void* x, const void* residual, cons
 
 int stk_bn_stats_act(stk_ctx* c, int act, const void* x, const void* residual, const void* weight, const void* bias,
                      void* running_mean, void* running_var, int running_dtype, double momentum, double eps, void* out,
-                     float* save_mean, float* save_invstd, float* workspace, size_t numel, size_t channels, void* stream) {
+                     float* save_mean, float* save_invstd, float* workspace, size_t numel, size_t channels, void* stream,
+                     const void* weight2, const void* bias2, void* running_mean2, void* running_var2, double momentum2,
+                     double eps2, float* save_mean2, float* save_invstd2) {
   STK_REQUIRE(c, c && x && weight && bias && running_mean && running_var && out && save_mean && save_invstd && workspace,
               "stk_bn_stats_act: NULL argument");
   STK_REQUIRE(c, act_valid(act, residual != nullptr),
               "stk_bn_stats_act: act must be an STK_ACT_* kind, and only STK_ACT_RELU takes a residual");
+  const bool two = weight2 != nullptr;
+  STK_REQUIRE(c, !two || (residual && bias2 && running_mean2 && running_var2 && save_mean2 && save_invstd2),
+              "stk_bn_stats_act: a second BatchNorm needs a residual, bias2, running statistics and save_mean2 / save_invstd2");
+  STK_REQUIRE(c, ((uintptr_t(weight2) | uintptr_t(bias2)) % 16) == 0, "stk_bn_stats_act: weight2 and bias2 must be 16-byte aligned");
   STK_REQUIRE(c, running_dtype == STK_F32 || running_dtype == STK_BF16, "stk_bn_stats_act: running statistics must be STK_F32 or STK_BF16");
   STK_REQUIRE(c, channels > 0 && channels % 8 == 0 && numel % channels == 0 && numel >= 2 * channels,
               "stk_bn_stats_act: channels must be a positive multiple of 8 dividing numel, with at least 2 rows");
@@ -678,8 +837,9 @@ int stk_bn_stats_act(stk_ctx* c, int act, const void* x, const void* residual, c
   const uint32_t rows = uint32_t(numel / channels), groups = uint32_t(channels / 8);
   const BnBwdConfig cfg = bn_bwd_config(rows, uint32_t(channels));
   const bool bf16_run = running_dtype == STK_BF16;
-  auto kern = bf16_run ? STK_BN_KERNEL(BnStatsKernel<__nv_bfloat16>::k, act, residual != nullptr)
-                       : STK_BN_KERNEL(BnStatsKernel<float>::k, act, residual != nullptr);
+  auto kern = two ? (bf16_run ? k_bn_stats_act<STK_ACT_RELU, true, __nv_bfloat16, true> : k_bn_stats_act<STK_ACT_RELU, true, float, true>)
+              : bf16_run ? STK_BN_KERNEL(BnStatsKernel<__nv_bfloat16>::k, act, residual != nullptr)
+                         : STK_BN_KERNEL(BnStatsKernel<float>::k, act, residual != nullptr);
   // as many blocks as the busiest phase uses, at most every resident one (the grid barriers need them all resident)
   const uint32_t gb = kBwdThreads / (kChains * cfg.block_y), cb = kBwdThreads / cfg.block_y;
   const size_t items = std::max(size_t((groups + gb - 1) / gb) * cfg.grid_y, size_t((channels + cb - 1) / cb));
@@ -710,6 +870,15 @@ int stk_bn_stats_act(stk_ctx* c, int act, const void* x, const void* residual, c
   a.loops = cfg.loops;
   a.nvec = nvec;
   a.active = uint32_t(blocks * kBwdThreads / groups * groups);
+  a.weight2 = static_cast<const __nv_bfloat16*>(weight2);
+  a.bias2 = static_cast<const __nv_bfloat16*>(bias2);
+  a.running_mean2 = running_mean2;
+  a.running_var2 = running_var2;
+  a.save_mean2 = save_mean2;
+  a.save_invstd2 = save_invstd2;
+  a.eps2 = float(eps2);
+  a.momentum2 = float(momentum2);
+  a.one_minus_momentum2 = 1.f - a.momentum2;
   cudaLaunchConfig_t lc{};
   lc.gridDim = dim3(unsigned(blocks));
   lc.blockDim = dim3(kBwdThreads);
@@ -732,20 +901,31 @@ int stk_bn_act(stk_ctx* c, const void* x, const void* residual, const float* mea
 int stk_bn_act_backward_ex(stk_ctx* c, int act, const void* grad, const void* x, const void* out, const float* mean,
                            const float* invstd, const void* weight, const void* bias, void* grad_x, void* grad_weight,
                            void* grad_bias, void* grad_residual, void* grad_pre, float* workspace, size_t numel,
-                           size_t channels, void* stream) {
+                           size_t channels, void* stream, const void* grad2, const void* x2, const float* mean2,
+                           const float* invstd2, const void* weight2, void* grad_x2, void* grad_weight2,
+                           void* grad_bias2) {
   STK_REQUIRE(c, c && grad && x && mean && invstd && weight && grad_weight && grad_bias && workspace,
               "stk_bn_act_backward: NULL argument");
   STK_REQUIRE(c, act_valid(act, out != nullptr),
               "stk_bn_act_backward: act must be an STK_ACT_* kind, and only STK_ACT_RELU takes a residual");
   STK_REQUIRE(c, out ? grad_residual != nullptr : bias != nullptr,
               "stk_bn_act_backward: a residual site needs grad_residual, a site without one needs bias");
+  STK_REQUIRE(c, grad2 == nullptr || out != nullptr, "stk_bn_act_backward: only a residual site takes grad2");
+  STK_REQUIRE(c, x2 == nullptr || (out && mean2 && invstd2 && weight2 && grad_weight2 && grad_bias2 &&
+                                   (grad_x == nullptr) == (grad_x2 == nullptr)),
+              "stk_bn_act_backward: x2 needs a residual site, mean2, invstd2, weight2, grad_weight2, grad_bias2, and "
+              "grad_x2 exactly when grad_x");
+  const uintptr_t align2 = uintptr_t(x2) | uintptr_t(mean2) | uintptr_t(invstd2) | uintptr_t(weight2) |
+                           uintptr_t(grad_x2) | uintptr_t(grad_weight2) | uintptr_t(grad_bias2);
+  STK_REQUIRE(c, align2 % 16 == 0, "stk_bn_act_backward: every tensor must be 16-byte aligned");
   STK_REQUIRE(c, grad_pre == nullptr || act != STK_ACT_RELU, "stk_bn_act_backward: grad_pre is not written for STK_ACT_RELU");
   STK_REQUIRE(c, channels > 0 && channels % 8 == 0 && numel % channels == 0 && numel >= channels,
               "stk_bn_act_backward: channels must be a positive multiple of 8 dividing numel");
   STK_REQUIRE(c, numel < (size_t(1) << 31), "stk_bn_act_backward: numel must be below 2^31");
   const uintptr_t align = uintptr_t(grad) | uintptr_t(x) | uintptr_t(out) | uintptr_t(mean) | uintptr_t(invstd) |
                           uintptr_t(weight) | uintptr_t(bias) | uintptr_t(grad_x) | uintptr_t(grad_weight) |
-                          uintptr_t(grad_bias) | uintptr_t(grad_residual) | uintptr_t(grad_pre) | uintptr_t(workspace);
+                          uintptr_t(grad_bias) | uintptr_t(grad_residual) | uintptr_t(grad_pre) | uintptr_t(workspace) |
+                          uintptr_t(grad2);
   STK_REQUIRE(c, align % 16 == 0, "stk_bn_act_backward: every tensor must be 16-byte aligned");
   DeviceGuard g(c->device);
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
@@ -754,24 +934,31 @@ int stk_bn_act_backward_ex(stk_ctx* c, int act, const void* grad, const void* x,
   const bool res = out != nullptr;
   const uint32_t gb = kBwdThreads / (kChains * cfg.block_y);   // block_y <= 512 / 8 since channels >= 8
   const dim3 grid((groups + gb - 1) / gb, cfg.grid_y);
-  auto reduce = STK_BN_KERNEL(k_bn_bwd_reduce, act, res);
+  const bool two = x2 != nullptr;
+  BnBwdSecond s2{static_cast<const uint4*>(x2), mean2, invstd2, static_cast<const __nv_bfloat16*>(weight2),
+                 workspace + 2 * channels * (1 + size_t(cfg.grid_y)), static_cast<__nv_bfloat16*>(grad_weight2),
+                 static_cast<__nv_bfloat16*>(grad_bias2), static_cast<uint4*>(grad_x2)};
+  auto reduce = two ? (grad2 ? k_bn_bwd_reduce<STK_ACT_RELU, true, true, true> : k_bn_bwd_reduce<STK_ACT_RELU, true, false, true>)
+                : grad2 ? k_bn_bwd_reduce<STK_ACT_RELU, true, true>
+                        : STK_BN_KERNEL(k_bn_bwd_reduce, act, res);
   auto bf = [](const void* p) { return static_cast<const __nv_bfloat16*>(p); };
-  reduce<<<grid, kBwdThreads, 0, s>>>(static_cast<const uint4*>(grad), static_cast<const uint4*>(x),
+  reduce<<<grid, kBwdThreads, 0, s>>>(static_cast<const uint4*>(grad), static_cast<const uint4*>(grad2),
+                                      static_cast<const uint4*>(x),
                                       static_cast<const uint4*>(out), mean, invstd, bf(weight), bf(bias),
                                       static_cast<uint4*>(res ? grad_residual : grad_pre), workspace,
                                       static_cast<__nv_bfloat16*>(grad_weight), static_cast<__nv_bfloat16*>(grad_bias),
-                                      rows, groups, cfg.block_y, cfg.loops);
+                                      rows, groups, cfg.block_y, cfg.loops, s2);
   STK_CUDA(c, cudaGetLastError());
   if (cfg.grid_y > 1) {
     const uint32_t cb = kBwdThreads / cfg.block_y;
-    k_bn_bwd_finish<<<unsigned((channels + cb - 1) / cb), kBwdThreads, 0, s>>>(
+    (two ? k_bn_bwd_finish<true> : k_bn_bwd_finish<false>)<<<unsigned((channels + cb - 1) / cb), kBwdThreads, 0, s>>>(
         workspace, invstd, static_cast<__nv_bfloat16*>(grad_weight), static_cast<__nv_bfloat16*>(grad_bias),
-        uint32_t(channels), cfg.block_y, cfg.grid_y);
+        uint32_t(channels), cfg.block_y, cfg.grid_y, s2);
     STK_CUDA(c, cudaGetLastError());
   }
   if (grad_x) {
     const uint32_t nvec = uint32_t(numel / 8);
-    auto elemt = STK_BN_KERNEL(k_bn_bwd_elemt, act, res);
+    auto elemt = two ? k_bn_bwd_elemt<STK_ACT_RELU, true, true> : STK_BN_KERNEL(k_bn_bwd_elemt, act, res);
     const size_t resident = size_t(blocks_per_sm(c, elemt, kBnThreads)) * c->sm_count;
     size_t blocks = std::min(resident, (size_t(nvec) + kBnThreads - 1) / kBnThreads);
     blocks = std::max(blocks, (size_t(groups) + kBnThreads - 1) / kBnThreads);
@@ -779,7 +966,7 @@ int stk_bn_act_backward_ex(stk_ctx* c, int act, const void* grad, const void* x,
     elemt<<<unsigned(blocks), kBnThreads, 0, s>>>(static_cast<const uint4*>(res ? grad_residual : grad),
                                                   static_cast<const uint4*>(x), mean, invstd, bf(weight), bf(bias),
                                                   workspace, static_cast<uint4*>(grad_x), float(1.0 / double(rows)),
-                                                  nvec, groups, active);
+                                                  nvec, groups, active, s2);
     STK_CUDA(c, cudaGetLastError());
   }
   return STK_OK;
@@ -789,7 +976,8 @@ int stk_bn_act_backward(stk_ctx* c, const void* grad, const void* x, const void*
                         const void* weight, const void* bias, void* grad_x, void* grad_weight, void* grad_bias,
                         void* grad_residual, float* workspace, size_t numel, size_t channels, void* stream) {
   return stk_bn_act_backward_ex(c, STK_ACT_RELU, grad, x, out, mean, invstd, weight, bias, grad_x, grad_weight, grad_bias,
-                                grad_residual, nullptr, workspace, numel, channels, stream);
+                                grad_residual, nullptr, workspace, numel, channels, stream, nullptr, nullptr, nullptr,
+                                nullptr, nullptr, nullptr, nullptr, nullptr);
 }
 
 }  // extern "C"

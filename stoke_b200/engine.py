@@ -338,37 +338,49 @@ class Engine:
 
     def bn_stats_act(self, x: torch.Tensor, residual: Optional[torch.Tensor], weight: torch.Tensor, bias: torch.Tensor,
                      running_mean: torch.Tensor, running_var: torch.Tensor, momentum: float, eps: float, out: torch.Tensor,
-                     save_mean: torch.Tensor, save_invstd: torch.Tensor, act: int = _lib.ACT_RELU):
+                     save_mean: torch.Tensor, save_invstd: torch.Tensor, act: int = _lib.ACT_RELU,
+                     residual_bn: Optional[tuple] = None):
         """``torch.batch_norm_update_stats`` followed by ``bn_act`` in one launch (``stk_bn_stats_act``): writes ``out``,
-        ``save_mean``, ``save_invstd`` and updates the running statistics (fp32 or bf16) in place.  ``fuse.py`` checks
-        dtypes, layout and alignment before calling."""
+        ``save_mean``, ``save_invstd`` and updates the running statistics (fp32 or bf16) in place.  ``residual_bn``
+        (ReLU with a residual): ``(weight, bias, running_mean, running_var, momentum, eps, save_mean, save_invstd)`` of a
+        second BatchNorm the residual passes through first, whose statistics are computed and written as the first's
+        (running statistics of the same dtype).  ``fuse.py`` checks dtypes, layout and alignment before calling."""
         c = x.shape[1]
-        ws = torch.empty(3 * 128 * c, dtype=torch.float32, device=x.device)
-        self._check(self.lib.stk_bn_stats_act(self.ctx, act, x.data_ptr(), residual.data_ptr() if residual is not None else None,
+        ws = torch.empty((2 if residual_bn else 1) * 3 * 128 * c, dtype=torch.float32, device=x.device)
+        w2, b2, rm2, rv2, mom2, eps2, sm2, si2 = residual_bn if residual_bn else (None,) * 8
+        ptr = lambda t: t.data_ptr() if t is not None else None  # noqa: E731
+        self._check(self.lib.stk_bn_stats_act(self.ctx, act, x.data_ptr(), ptr(residual),
                                               weight.data_ptr(), bias.data_ptr(), running_mean.data_ptr(),
                                               running_var.data_ptr(), _DT[running_mean.dtype], float(momentum), float(eps),
                                               out.data_ptr(), save_mean.data_ptr(), save_invstd.data_ptr(), ws.data_ptr(),
-                                              x.numel(), c, self._stream()))
+                                              x.numel(), c, self._stream(), ptr(w2), ptr(b2), ptr(rm2), ptr(rv2),
+                                              float(mom2 or 0.0), float(eps2 or 0.0), ptr(sm2), ptr(si2)))
         self.launches += 1
 
     def bn_act_backward(self, grad: torch.Tensor, x: torch.Tensor, out: Optional[torch.Tensor], mean: torch.Tensor,
                         invstd: torch.Tensor, weight: torch.Tensor, bias: Optional[torch.Tensor],
                         grad_x: Optional[torch.Tensor], grad_weight: torch.Tensor, grad_bias: torch.Tensor,
                         grad_residual: Optional[torch.Tensor], act: int = _lib.ACT_RELU,
-                        grad_pre: Optional[torch.Tensor] = None):
+                        grad_pre: Optional[torch.Tensor] = None, grad2: Optional[torch.Tensor] = None,
+                        residual_bn: Optional[tuple] = None):
         """Backward of ``bn_act`` (``stk_bn_act_backward_ex``): the ReLU mask comes from ``out`` at a site with a
         residual (``grad_residual`` receives the masked gradient); otherwise (``out`` None) the activation's input is
         recomputed from ``x``, ``weight``, ``bias``, and ``grad_pre``, when given, receives the gradient at it (not for
-        ReLU).  ``grad_x`` None skips the elementwise pass.  ``fuse.py`` checks dtypes, layout and alignment before
-        calling."""
+        ReLU).  ``grad2``, at a site with a residual, is a second part of the output's gradient, added to ``grad`` in
+        bf16 as autograd adds them.  ``residual_bn``, at a site with a residual: ``(x2, mean2, invstd2, weight2,
+        grad_x2, grad_weight2, grad_bias2)`` of the residual's BatchNorm (``bn_stats_act``'s ``residual_bn``), whose
+        backward runs in the same kernels; ``grad_residual`` then receives g, and ``grad_x2`` is given exactly when
+        ``grad_x`` is.  ``grad_x`` None skips the elementwise pass.  ``fuse.py`` checks dtypes, layout and alignment
+        before calling."""
         c = x.shape[1]
-        ws = torch.empty(2 * (1 + 128) * c, dtype=torch.float32, device=x.device)
+        ws = torch.empty((3 if residual_bn else 2) * (1 + 128) * c, dtype=torch.float32, device=x.device)
         ptr = lambda t: t.data_ptr() if t is not None else None  # noqa: E731
+        second = [ptr(t) for t in residual_bn] if residual_bn else [None] * 7
         self._check(self.lib.stk_bn_act_backward_ex(self.ctx, act, grad.data_ptr(), x.data_ptr(), ptr(out),
                                                     mean.data_ptr(), invstd.data_ptr(), weight.data_ptr(), ptr(bias),
                                                     ptr(grad_x), grad_weight.data_ptr(), grad_bias.data_ptr(),
                                                     ptr(grad_residual), ptr(grad_pre), ws.data_ptr(), x.numel(), c,
-                                                    self._stream()))
+                                                    self._stream(), ptr(grad2), *second))
         self.launches += _bn_bwd_launches(x.numel() // c, c, grad_x is not None)
 
     def barrier(self):

@@ -17,7 +17,11 @@ backward op (``threshold_backward``, ``silu_backward``, ``hardswish_backward``, 
 passes of torch's channels-last ``native_batch_norm_backward`` and adds its per-channel sums in torch's order, so every
 result is bit-identical to the calls autograd makes for the unfused chain.  It takes the gradient when torch's BatchNorm
 backward would run its channels-last kernels on it (the activation backward's output is channels-last; another layout
-is made channels-last first) and it is bf16 and aligned; otherwise it runs those calls.
+is made channels-last first) and it is bf16 and aligned; otherwise it runs those calls.  A residual that is itself a
+single-use BatchNorm2d output (a ResNet downsample) joins the site (``BnAct.residual_bn``): both BatchNorms' statistics,
+applies, add and ReLU in the one forward launch, both backwards in its kernels.  A residual site whose output
+has two users that only read it (a ResNet block output) returns it once per user (``BnAct.fork``), so that its backward
+adds the two gradients in its reduce kernel, with the rounding of the bf16 add autograd would otherwise run.
 Each call falls back to the unfused torch ops when the kernel does not cover its inputs (eval mode, no running statistics,
 running statistics neither fp32 nor bf16, not bf16, not channels-last, misaligned, C % 8 != 0, 2^31 elements or more, a CPU tensor), so the same inputs give the
 same results whether or not the model was rewritten.
@@ -107,36 +111,63 @@ def _mask_output_channels_last(grad: torch.Tensor, x: torch.Tensor, act: int = A
 
 class _BnActFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, x, weight, bias, residual, bn, engine, act):
+    def forward(ctx, x, weight, bias, residual, bn, engine, act, fork, weight2, bias2, rbn):
         momentum = _momentum(bn)
         out = torch.empty_like(x)
         mean = torch.empty(x.shape[1], dtype=torch.float32, device=x.device)
         invstd = torch.empty_like(mean)
+        second, saved2 = None, ()
+        if rbn is not None:   # the residual is rbn's input: relu(bn(x) + rbn(residual))
+            mean2, invstd2 = torch.empty_like(mean), torch.empty_like(mean)
+            second = (weight2, bias2, rbn.running_mean, rbn.running_var, _momentum(rbn), rbn.eps, mean2, invstd2)
+            saved2 = (residual, weight2, mean2, invstd2)
         engine.bn_stats_act(x, residual, weight, bias, bn.running_mean, bn.running_var, momentum, bn.eps, out, mean,
-                            invstd, act)
+                            invstd, act, residual_bn=second)
         # the ReLU mask: out at a site with a residual; otherwise the activation's input is recomputed from x and the
         # parameters (bias saved instead)
-        ctx.save_for_backward(x, weight, out if residual is not None else bias, mean, invstd)
-        ctx.bn, ctx.engine, ctx.act = bn, engine, act
+        ctx.save_for_backward(x, weight, out if residual is not None else bias, mean, invstd, *saved2)
+        ctx.bn, ctx.engine, ctx.act, ctx.rbn = bn, engine, act, rbn
         ctx.has_residual = residual is not None
-        return out
+        if not fork:
+            return out
+        # two outputs over one storage, one per user: autograd hands their gradients to backward separately, which adds
+        # them inside the reduce kernel instead of in a bf16 add of its own
+        ctx.set_materialize_grads(False)
+        return out, out.detach()
 
     @staticmethod
-    def backward(ctx, grad_out):
-        x, weight, out_or_bias, mean, invstd = ctx.saved_tensors
-        bn, res, act = ctx.bn, ctx.has_residual, ctx.act
+    def backward(ctx, grad_out, grad2=None):
+        x, weight, out_or_bias, mean, invstd, *saved2 = ctx.saved_tensors
+        bn, res, act, rbn = ctx.bn, ctx.has_residual, ctx.act, ctx.rbn
         need_x, need_w, need_b, need_r = ctx.needs_input_grad[:4]
+        need_w2, need_b2 = ctx.needs_input_grad[8:10]
+        if grad_out is None:
+            grad_out, grad2 = grad2, None
+        if grad_out is None:
+            return (None,) * 11
+        if grad2 is not None and not (_grad_covered(grad_out, x) and _grad_covered(grad2, x)):
+            grad_out, grad2 = grad_out + grad2, None   # the add autograd runs for an output with two users
         if (grad_out.dtype == torch.bfloat16 and grad_out.shape == x.shape
                 and not grad_out.is_contiguous(memory_format=torch.channels_last)
                 and _mask_output_channels_last(grad_out, x, act)):
             grad_out = grad_out.contiguous(memory_format=torch.channels_last)   # same values, so the same g
         if _grad_covered(grad_out, x):
-            dx = torch.empty_like(x) if need_x else None
             dw, db = torch.empty_like(weight), torch.empty_like(weight)
-            dr = torch.empty_like(x) if res else None
+            dr = torch.empty_like(x) if res else None   # g at a site whose residual has its own BatchNorm
+            if rbn is not None:
+                x2, w2, mean2, invstd2 = saved2
+                dx = torch.empty_like(x) if need_x or need_r else None
+                dx2 = torch.empty_like(x2) if dx is not None else None
+                dw2, db2 = torch.empty_like(w2), torch.empty_like(w2)
+                ctx.engine.bn_act_backward(grad_out, x, out_or_bias, mean, invstd, weight, None, dx, dw, db, dr, act,
+                                           grad2=grad2, residual_bn=(x2, mean2, invstd2, w2, dx2, dw2, db2))
+                return (dx if need_x else None, dw if need_w else None, db if need_b else None,
+                        dx2 if need_r else None, None, None, None, None,
+                        dw2 if need_w2 else None, db2 if need_b2 else None, None)
+            dx = torch.empty_like(x) if need_x else None
             ctx.engine.bn_act_backward(grad_out, x, out_or_bias if res else None, mean, invstd, weight,
-                                       None if res else out_or_bias, dx, dw, db, dr, act)
-            return dx, dw if need_w else None, db if need_b else None, dr if need_r else None, None, None, None
+                                       None if res else out_or_bias, dx, dw, db, dr, act, grad2=grad2)
+            return (dx, dw if need_w else None, db if need_b else None, dr if need_r else None) + (None,) * 7
         # without a residual y = batch_norm_elemt(x) (the transform the forward kernel reproduces) is the activation's
         # input, which its backward op takes (threshold_backward takes relu's output, but relu(y) <= 0 exactly when y <= 0)
         out = out_or_bias if res else torch.batch_norm_elemt(x, weight, out_or_bias, mean, invstd, bn.eps)
@@ -144,8 +175,13 @@ class _BnActFn(torch.autograd.Function):
         mask = [need_x, need_w, need_b]
         dx, dw, db = torch.ops.aten.native_batch_norm_backward(g, x, weight, bn.running_mean, bn.running_var, mean, invstd,
                                                               True, bn.eps, mask)
+        if rbn is not None:   # the residual BatchNorm's backward of the same g
+            x2, w2, mean2, invstd2 = saved2
+            dx2, dw2, db2 = torch.ops.aten.native_batch_norm_backward(g, x2, w2, rbn.running_mean, rbn.running_var, mean2,
+                                                                     invstd2, True, rbn.eps, [need_r, need_w2, need_b2])
+            return dx, dw, db, dx2, None, None, None, None, dw2, db2, None
         dr = g if res and need_r else None
-        return dx, dw, db, dr, None, None, None
+        return (dx, dw, db, dr) + (None,) * 7
 
 
 class BnAct(torch.nn.Module):
@@ -153,14 +189,24 @@ class BnAct(torch.nn.Module):
     ops otherwise (``inplace``: the add was ``out += residual``, which keeps ``out``'s dtype).  ``act`` is one of
     ``_lib.ACT_*``; only ReLU takes a residual.  ``act_fn`` is the unfused activation (the user's module or function),
     by default ``torch.relu``, ``F.silu``, ``F.hardswish`` or ``F.relu6``.  Holds a reference to the user's BatchNorm2d
-    (shared, not copied)."""
+    (shared, not copied).  ``fork`` (a site with a residual whose output has two users that do not mutate it): returns
+    the output twice, as two tensors over one storage, so that the backward receives the two users' gradients apart
+    and adds them in its reduce kernel; the unfused fallback returns the same tensor twice, which autograd sums.
+    ``residual_bn`` (a ReLU site; shared with the user's model, not copied): the residual passes through this second
+    BatchNorm2d first, ``relu(bn(x) + residual_bn(residual))``, in the same launch when the kernel covers both; when it
+    covers only the first, ``residual_bn`` runs in torch and its output is the residual."""
 
-    def __init__(self, bn: torch.nn.BatchNorm2d, engine, inplace: bool = False, act: int = ACT_RELU, act_fn=None):
+    def __init__(self, bn: torch.nn.BatchNorm2d, engine, inplace: bool = False, act: int = ACT_RELU, act_fn=None,
+                 fork: bool = False, residual_bn: Optional[torch.nn.BatchNorm2d] = None):
         super().__init__()
         if act not in _DEFAULT_ACT_FN:
             raise ValueError(f"unknown activation kind {act}")
+        if residual_bn is not None and (act != ACT_RELU or residual_bn is bn):
+            raise ValueError("BnAct: residual_bn needs a ReLU site and a BatchNorm2d of its own")
         self.bn = bn
+        self.residual_bn = residual_bn
         self.act = act
+        self.fork = fork
         self._engine = engine
         self._inplace = inplace
         self._act_fn = act_fn if act_fn is not None else _DEFAULT_ACT_FN[act]
@@ -168,15 +214,28 @@ class BnAct(torch.nn.Module):
     def forward(self, x, residual=None):
         if residual is not None and self.act != ACT_RELU:
             raise ValueError("BnAct: only a ReLU site takes a residual")
+        if self.fork and residual is None:
+            raise ValueError("BnAct: only a site with a residual forks")
+        rbn = self.residual_bn
+        if rbn is not None:
+            if residual is None:
+                raise ValueError("BnAct: a site with residual_bn takes a residual")
+            if (_covered(self.bn, x, residual) and _covered(rbn, residual, None)
+                    and rbn.running_mean.dtype == self.bn.running_mean.dtype):
+                return _BnActFn.apply(x, self.bn.weight, self.bn.bias, residual, self.bn, self._engine, self.act,
+                                      self.fork, rbn.weight, rbn.bias, rbn)
+            residual = rbn(residual)
         if _covered(self.bn, x, residual):
-            return _BnActFn.apply(x, self.bn.weight, self.bn.bias, residual, self.bn, self._engine, self.act)
+            return _BnActFn.apply(x, self.bn.weight, self.bn.bias, residual, self.bn, self._engine, self.act, self.fork,
+                                  None, None, None)
         y = self.bn(x)
         if residual is not None:
             if self._inplace:
                 y += residual
             else:
                 y = y + residual
-        return self._act_fn(y)
+        y = self._act_fn(y)
+        return (y, y) if self.fork else y
 
 
 class _InplaceProxy(torch.fx.Proxy):
@@ -297,15 +356,48 @@ def _rewrite(gm: torch.fx.GraphModule, engine) -> int:
             continue
         name = bn_node.target.replace(".", "_") + "_act"
         bn = gm.get_submodule(bn_node.target)
-        gm.add_submodule(name, BnAct(bn, engine, inplace) if other is None else BnAct(bn, engine, act=other[0],
-                                                                                         act_fn=other[1]))
+        # a residual that is itself a BatchNorm's single-use output (a ResNet downsample) joins the site
+        rbn_node = None
+        if (residual is not None and _single_bn_input(gm, residual)
+                and gm.get_submodule(residual.target) is not bn):
+            rbn_node, residual = residual, residual.args[0]
+        gm.add_submodule(name, BnAct(bn, engine, inplace, residual_bn=rbn_node and gm.get_submodule(rbn_node.target))
+                         if other is None else BnAct(bn, engine, act=other[0], act_fn=other[1]))
         with gm.graph.inserting_before(relu):
             fused = gm.graph.call_module(name, (bn_node.args[0],) + ((residual,) if residual is not None else ()))
         relu.replace_all_uses_with(fused)
-        for n in chain + [bn_node]:
+        for n in chain + [bn_node] + ([rbn_node] if rbn_node is not None else []):
             gm.graph.erase_node(n)
         sites += 1
     return sites
+
+
+def _reads_only(gm: torch.fx.GraphModule, user: torch.fx.Node, node: torch.fx.Node) -> bool:
+    """``user`` takes ``node`` once and does not mutate it: a Conv2d, or a BnAct (which never writes its inputs)."""
+    if user.op != "call_module" or user.kwargs or list(user.args).count(node) != 1:
+        return False
+    m = gm.get_submodule(user.target)
+    return type(m) is torch.nn.Conv2d or isinstance(m, BnAct)
+
+
+def _fork(gm: torch.fx.GraphModule) -> int:
+    """Sets ``fork`` on each residual-site BnAct whose output has exactly two users that only read it (a ResNet block
+    output: the next block's conv1, and its identity or downsample conv), and gives each user its own output."""
+    forks = 0
+    for node in list(gm.graph.nodes):
+        if not (node.op == "call_module" and len(node.args) == 2 and isinstance(gm.get_submodule(node.target), BnAct)):
+            continue
+        users = list(node.users)
+        if len(users) != 2 or not all(_reads_only(gm, u, node) for u in users):
+            continue
+        gm.get_submodule(node.target).fork = True
+        prev = node
+        for i, user in enumerate(users):
+            with gm.graph.inserting_after(prev):
+                prev = gm.graph.call_function(operator.getitem, (node, i))
+            user.replace_input_with(node, prev)
+        forks += 1
+    return forks
 
 
 def site_shapes(fwd: FusedForward, *example) -> Dict[tuple, int]:
@@ -334,6 +426,7 @@ def fuse_bn_act(module: torch.nn.Module, engine) -> Optional[FusedForward]:
         sites = _rewrite(gm, engine)
         if sites == 0:
             return None
+        _fork(gm)
         gm.graph.lint()
         gm.recompile()
     except Exception:  # noqa: BLE001 -- a model fx cannot trace or rewrite runs unchanged
