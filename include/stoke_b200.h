@@ -41,6 +41,8 @@
  *                                    the clip and the GradScaler.step gate, without its two .item() per parameter
  *   stk_layerwise_step               the step of the LAMB / LARS classes of stoke_b200.optim (per-parameter trust ratios;
  *                                    torch.optim has neither), plus the clip and the GradScaler.step gate
+ *   stk_weight_avg                   torch.optim.swa_utils.AveragedModel.update_parameters (EMA / SWA) over the fp32
+ *                                    master weights; the reference has no weight averaging
  */
 #ifndef STOKE_B200_H
 #define STOKE_B200_H
@@ -288,6 +290,14 @@ typedef struct {
                              prologue, not in every block.  ASGD takes no exp_avg_sq */
 } stk_optim_args_t;
 int stk_optim_step_ex(stk_ctx* ctx, const stk_optim_args_t* args, void* stream);
+
+/* Weight-average update over n fp32 elements (n a multiple of 4, both pointers 16-byte aligned), one launch on `stream`:
+ * mode 1: avg = master;  mode 2: avg = torch.lerp(avg, master, weight) on fp32 -- for |weight| < 0.5
+ * fma(weight, master - avg, avg), otherwise fma(-(master - avg), 1 - weight, master), the contraction of torch's CUDA
+ * foreach-lerp kernel.  That is one update of torch.optim.swa_utils.AveragedModel over fp32 parameters: EMA with
+ * weight = fp32(1 - decay), SWA with weight = fp32(1 / (n_averaged + 1)).  12 B/element (lerp), 8 (copy).  Every
+ * optimizer route calls it after its step, skipped (found_inf) or not. */
+int stk_weight_avg(stk_ctx* ctx, float* avg, const float* master, size_t n, int mode, float weight, void* stream);
 /* Step bookkeeping for every kind, including the per-entry scalar state of NAdam and ASGD (call it right before
  * stk_optim_step_ex, same stream).
  * n_ranges > 0: per range j: the scalars of step t = range_steps[j] + 1 with the group hyper[range_group[j] & 0x7f] go to

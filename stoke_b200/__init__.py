@@ -8,7 +8,8 @@ from .optim import LAMB, LARS
 from .status import DistributedOptions, FP16Options
 from .stoke import Stoke
 from .utils import ParamNormalize
+from .weight_average import WeightAverage
 
 __all__ = ["Stoke", "ParamNormalize", "FP16Options", "DistributedOptions", "BucketedDistributedSampler",
-           "argsort_lengths", "LAMB", "LARS"] + list(_config_names)
+           "argsort_lengths", "LAMB", "LARS", "WeightAverage"] + list(_config_names)
 __version__ = "0.1.0"

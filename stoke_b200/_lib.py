@@ -170,6 +170,7 @@ _SIGNATURES = {
     "stk_adafactor_plan": (C.c_int, [C.POINTER(AdafactorParam), C.c_int, C.POINTER(AdafactorPlan)]),
     "stk_adafactor_step": (C.c_int, [_P, C.POINTER(AdafactorArgs), _P]),
     "stk_layerwise_step": (C.c_int, [_P, C.POINTER(LayerwiseArgs), _P]),
+    "stk_weight_avg": (C.c_int, [_P, _P, _P, C.c_size_t, C.c_int, C.c_float, _P]),
     "stk_loss_sync": (C.c_int, [_P, _P, C.c_int, C.POINTER(C.c_double), _P]),
     "stk_loss_sync_begin": (C.c_int, [_P, _P, C.c_int, C.POINTER(C.c_int64), _P]),
     "stk_loss_sync_wait": (C.c_int, [_P, C.c_int64, C.POINTER(C.c_double)]),

@@ -97,6 +97,31 @@ class FairscaleSDDPConfig:
     warn_on_trainable_params_changed: bool = True
 
 
+@_cfg
+class WeightAverageConfig:
+    """An fp32 moving average of the trainable weights kept by the engine (``Stoke.weight_average``), with the semantics of
+    ``torch.optim.swa_utils.AveragedModel`` applied to fp32 copies of the master weights.  ``kind="ema"`` is
+    ``multi_avg_fn=get_ema_multi_avg_fn(decay)``; ``kind="swa"`` is the default equal average.  After optimizer step s
+    (1-based; accumulation micro-steps do not count) an update is due when ``s > start_step`` and
+    ``(s - start_step) % every == 0``.  ``use_buffers`` averages the floating buffers too (AveragedModel's option);
+    otherwise the average takes the model's current buffers.  Not in the reference: an extension of this engine."""
+    kind: str = "ema"
+    decay: float = 0.999
+    every: int = 1
+    start_step: int = 0
+    use_buffers: bool = False
+
+    def __attrs_post_init__(self):
+        if self.kind not in ("ema", "swa"):
+            raise ValueError(f"Stoke -- WeightAverageConfig kind must be 'ema' or 'swa', got {self.kind!r}")
+        if not 0.0 <= float(self.decay) <= 1.0:
+            raise ValueError(f"Stoke -- WeightAverageConfig decay must be in [0, 1], got {self.decay}")
+        if int(self.every) != self.every or self.every < 1:
+            raise ValueError(f"Stoke -- WeightAverageConfig every must be an integer >= 1, got {self.every}")
+        if int(self.start_step) != self.start_step or self.start_step < 0:
+            raise ValueError(f"Stoke -- WeightAverageConfig start_step must be an integer >= 0, got {self.start_step}")
+
+
 # ---- accepted for import compatibility only (engines out of scope) -----------------------------------------------------
 @_cfg
 class ApexConfig:

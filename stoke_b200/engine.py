@@ -479,6 +479,8 @@ class GradPath:
                                                                               | absent (local route)
       MASTER fp32 master weights                               local          aliases P when the model is fp32 and unsharded
       M, V   fp32 optimizer state                              local          owned shards (sharded) | all n
+      AVG    fp32 weight average (EMA / SWA)                   local          indexed like MASTER; only when averaging is
+                                                                              configured (``enable_weight_average``)
 
     Gradient buckets: contiguous element ranges cut at parameter boundaries, ``bucket_mb`` of gradient bytes each, in
     reverse registration order (what DDP does, torch/nn/parallel/distributed.py) -- bucket 0 holds the LAST parameters,
@@ -649,6 +651,8 @@ class GradPath:
         self.layerwise = bool(layerwise)
         if self.layerwise:
             self._layerwise_setup()
+        self.avg_flat = None   # AVG, allocated by enable_weight_average
+        self.avg_due = None    # (mode, weight) of the weight-average update the next step carries, set by Stoke.step
         torch.cuda.synchronize(engine.device)
         if W > 1:
             torch.distributed.barrier(group=engine.group)
@@ -938,6 +942,7 @@ class GradPath:
             else:
                 a.group_bc = bc.data_ptr()
         e.optim_step_ex(a)
+        self.weight_avg_after_step()
         e.step_epilogue()
         self._track_touched = False
         self._raw_has_acc = False
@@ -969,6 +974,7 @@ class GradPath:
             a.lp, a.lp_dtype = self.P.ptr, _DT[self.model_dtype]
         e._check(e.lib.stk_adafactor_step(e.ctx, C.byref(a), e._stream()))
         e.launches += 8 if self.af_plan.n_line else 5
+        self.weight_avg_after_step()
         e.step_epilogue()
         self._track_touched = False
         self._raw_has_acc = False
@@ -1003,6 +1009,7 @@ class GradPath:
             a.lp, a.lp_dtype = self.P.ptr, _DT[self.model_dtype]
         e._check(e.lib.stk_layerwise_step(e.ctx, C.byref(a), e._stream()))
         e.launches += 3
+        self.weight_avg_after_step()
         e.step_epilogue()
         self._track_touched = False
         self._raw_has_acc = False
@@ -1022,6 +1029,47 @@ class GradPath:
             else:
                 out.append((self.af_state[o: o + lay["numel"]].view(p.shape),))
         return out
+
+    # -- weight average (EMA / SWA over the fp32 master) ------------------------------------------------------------------
+    def enable_weight_average(self):
+        """Allocates AVG (+4 B per local element) holding a copy of the master, as AveragedModel starts from a copy of
+        the model.  The updates are scheduled by the caller through ``avg_due``."""
+        if self.avg_flat is None:
+            buf = torch.empty(max(self.n_local, ALIGN_ELEMS), dtype=torch.float32, device=self._range_end.device)
+            self.avg_flat = buf[: self.n_local]
+            self.avg_flat.copy_(self.master_flat)
+
+    def weight_avg_after_step(self):
+        """The due weight-average update: one ``stk_weight_avg`` over the local master, on the step's stream, after
+        every optimizer route's step, skipped (found_inf) or not.  It is not fused into K2: on the H100 the fused form
+        was slower than the separate pass (DESIGN.md)."""
+        due, self.avg_due = self.avg_due, None
+        if due is None:
+            return
+        e = self.engine
+        e._check(e.lib.stk_weight_avg(e.ctx, self.avg_flat.data_ptr(), self.master_ptr, self.n_local, due[0], due[1],
+                                      e._stream()))
+        e.launches += 1 if self.n_local else 0   # an empty shard launches nothing
+
+    def gather_avg(self) -> torch.Tensor:
+        """Full fp32 weight average (all-gathered across shards when sharded: collective)."""
+        return self._gather_shards(self.avg_flat) if self.sharded else self.avg_flat.clone()
+
+    def params_from_average(self) -> Optional[torch.Tensor]:
+        """P <- the weight average cast to the model dtype (round to nearest even).  Returns what ``params_restore``
+        needs: a copy of P where P is itself the master (fp32 model, unsharded), else None (P is the master's cast).
+        Sharded: gathers (collective) and writes this rank's own P only.  Peers write into it only from the sharded K2,
+        whose start barrier waits for this rank's K2, which its stream runs after ``params_restore``."""
+        saved = self.p_flat.clone() if self.master_flat is self.p_flat else None
+        self.p_flat.copy_(self.gather_avg())
+        return saved
+
+    def params_restore(self, saved: Optional[torch.Tensor]):
+        """Undoes ``params_from_average`` bit for bit: P is the model-dtype cast of the master after every step."""
+        if saved is not None:
+            self.p_flat.copy_(saved)
+        else:
+            self.p_flat.copy_(self.gather_master() if self.sharded else self.master_flat)
 
     # -- inspection (tests, checkpoints) ----------------------------------------------------------------------------------
     def gather_master(self) -> torch.Tensor:
@@ -1066,7 +1114,7 @@ class GradPath:
                 p.data = p.data.clone()
                 p.grad = None
         self.grad_views = []
-        self.p_flat = self.g_flat = self.main_flat = self.m_flat = self.v_flat = self.master_flat = None
+        self.p_flat = self.g_flat = self.main_flat = self.m_flat = self.v_flat = self.master_flat = self.avg_flat = None
         self.af_state = self._af_ws = self._af_desc = None
         self._lw_ws = self._lw_desc = None
         for b in self._bufs:

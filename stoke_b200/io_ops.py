@@ -25,7 +25,7 @@ class BaseStokeIO:
 
     def save(self, model, optimizer, path: str, backward_step: int, grad_accum_step: int, optimizer_step: int, name: str,
              status: dict, scaler_dict: Optional[dict] = None, extension: str = "pt", create_directory: bool = True,
-             extras: Optional[dict] = None):
+             extras: Optional[dict] = None, weight_average: Optional[dict] = None):
         tag = f"{self._make_tag(name, backward_step)}.{extension}"
         full = f"{path}/{tag}"
         if self._verbose:
@@ -38,10 +38,12 @@ class BaseStokeIO:
             try:
                 if create_directory:
                     make_folder(path)
-                torch.save({"backward_step": backward_step, "grad_accum_step": grad_accum_step,
-                            "optimizer_step": optimizer_step, "stoke_status": status, "model_state_dict": model_dict,
-                            "optimizer_state_dict": optimizer_dict, "scaler_state_dict": scaler_dict, "extras": extras},
-                           full)
+                ckpt = {"backward_step": backward_step, "grad_accum_step": grad_accum_step,
+                        "optimizer_step": optimizer_step, "stoke_status": status, "model_state_dict": model_dict,
+                        "optimizer_state_dict": optimizer_dict, "scaler_state_dict": scaler_dict, "extras": extras}
+                if weight_average is not None:   # the one key averaging adds (WeightAverageConfig)
+                    ckpt["weight_average_state_dict"] = weight_average
+                torch.save(ckpt, full)
             except OSError as e:
                 self._print_device(f"Unable to save model to given path: {full}")
                 raise e
@@ -49,7 +51,7 @@ class BaseStokeIO:
         return path, tag
 
     def load(self, model, optimizer, gpu: bool, path: str, tag: str, scaler_dict_fn: Optional[Callable] = None,
-             strict: bool = True):
+             strict: bool = True, weight_average_fn: Optional[Callable] = None):
         self.barrier()
         try:
             load_dict = torch.load(f"{path}/{tag}", map_location=f"cuda:{self.device_id}", weights_only=False)
@@ -61,6 +63,8 @@ class BaseStokeIO:
         optimizer.load_state_dict(load_dict["optimizer_state_dict"])
         if scaler_dict_fn is not None and load_dict["scaler_state_dict"] is not None:
             scaler_dict_fn(load_dict["scaler_state_dict"])
+        if weight_average_fn is not None:   # None: a checkpoint without an average starts one afresh
+            weight_average_fn(load_dict.get("weight_average_state_dict"))
         self.barrier()
         return load_dict["backward_step"], load_dict["grad_accum_step"], load_dict["optimizer_step"], load_dict["extras"]
 

@@ -613,6 +613,7 @@ class B200StockOptimizer(torch.optim.Optimizer):
             self.inner.step(closure) if closure is not None else self.inner.step()
             if path.master_flat is not path.p_flat:
                 path.p_flat.copy_(path.master_flat)   # fp32 -> model dtype, round-to-nearest-even
+        path.weight_avg_after_step()
         e.step_epilogue()
         e.comm_poll()
 

@@ -17,7 +17,7 @@ import attr
 import torch
 
 from .configs import (AMPConfig, ClipGradConfig, ClipGradNormConfig, DDPConfig, FairscaleOSSConfig,
-                      FairscaleSDDPConfig)
+                      FairscaleSDDPConfig, WeightAverageConfig)
 
 
 class DistributedOptions(Enum):
@@ -44,7 +44,7 @@ def _value(opt):
 
 class StokeStatus:
     _CONFIG_NAMES = ("AMPConfig", "ApexConfig", "DDPConfig", "DeepspeedConfig", "FairscaleOSSConfig",
-                     "FairscaleSDDPConfig", "FairscaleFSDPConfig", "HorovodConfig")
+                     "FairscaleSDDPConfig", "FairscaleFSDPConfig", "HorovodConfig", "WeightAverageConfig")
 
     def __init__(self, batch_size_per_device: int, grad_accum: Optional[int],
                  grad_clip: Optional[Union[ClipGradConfig, ClipGradNormConfig]], gpu: bool, fp16, distributed,
@@ -153,6 +153,10 @@ class StokeStatus:
     @property
     def sddp_config(self):
         return self._configs.get("FairscaleSDDPConfig") or FairscaleSDDPConfig()
+
+    @property
+    def weight_average_config(self) -> Optional[WeightAverageConfig]:
+        return self._configs.get("WeightAverageConfig")
 
     def __repr__(self):
         clip = self.grad_clip

@@ -27,6 +27,7 @@ from .fuse import fuse_bn_act
 from .io_ops import RunnerIOEnum
 from .status import StokeStatus
 from .utils import ParamNormalize, zero_optimizer_grads
+from .weight_average import WeightAverage
 
 
 def build_runner(status: StokeStatus, verbose: bool, info_rank, loss, configs: dict):
@@ -100,6 +101,8 @@ class Stoke:
                 self._model.set_forward(fused)
             elif fused is not None:
                 self._forward = fused
+        wa = self._status.weight_average_config
+        self._weight_average = WeightAverage(wa, self._optimizer.path, self.model_access) if wa is not None else None
         self.reset_tracking()
         self._status.set_post_init_values(world_size=self.world_size)
         if self._verbose:
@@ -213,6 +216,8 @@ class Stoke:
         return (self._ema_weight * value) + ((1.0 - self._ema_weight) * current_mean)
 
     def backward(self, loss):
+        if self._weight_average is not None:
+            self._weight_average._check_idle("backward")
         self._grad_accum_counter += 1
         ctx = nullcontext() if self._check_accum() else self._runner.grad_accum_context(self._model)
         with ctx:
@@ -220,6 +225,8 @@ class Stoke:
         self._backward_steps += 1
 
     def step(self):
+        if self._weight_average is not None:
+            self._weight_average._check_idle("step")
         if not self._check_accum():
             return
         if self._verbose and self.grad_accum > 0:
@@ -228,6 +235,8 @@ class Stoke:
             self._runner.clip_grad(self.grad_clip, self.model_access, self._optimizer, oss=self.oss, horovod=False,
                                    deepspeed=False, fsdp=False)
         step_cm = self._runner.step_context(self._optimizer) if self.grad_clip is not None else nullcontext()
+        if self._weight_average is not None:
+            self._weight_average._schedule(self._optimizer_steps + 1)   # a due update rides in this step
         with step_cm:
             self._runner.step_call(model=self.model_access, optimizer=self._optimizer)
         self._reset()
@@ -302,19 +311,22 @@ class Stoke:
     def save(self, path: str, name: str = None, extension: str = "pt", create_directory: bool = True,
              extras: Optional[dict] = None):
         name = uuid4() if name is None else name
+        wa = self._weight_average._checkpoint() if self._weight_average is not None else None  # collective when sharded
         out_path, tag = self._runner.save(model=self.model_access, optimizer=self.optimizer, path=path,
                                           backward_step=self._backward_steps, grad_accum_step=self._grad_accum_counter,
                                           optimizer_step=self._optimizer_steps, name=name,
                                           scaler_dict=self.fp16_state_dict, extension=extension,
-                                          create_directory=create_directory, extras=extras, status=self.status.status)
+                                          create_directory=create_directory, extras=extras, status=self.status.status,
+                                          weight_average=wa)
         self.print(f"Successfully saved model checkpoint to {out_path}/{tag}")
         return out_path, tag
 
     def load(self, path: str, tag: str, strict: bool = True):
         fn = self.scaler.load_state_dict if self.scaler is not None else None
+        wa_fn = self._weight_average._load_checkpoint if self._weight_average is not None else None
         backward_step, grad_accum_step, optimizer_step, extras = self._runner.load(
             model=self.model_access, optimizer=self.optimizer, gpu=self.gpu, path=path, tag=tag, scaler_dict_fn=fn,
-            strict=strict)
+            strict=strict, weight_average_fn=wa_fn)
         self._backward_steps, self._grad_accum_counter, self._optimizer_steps = backward_step, grad_accum_step, optimizer_step
         self.print(f"Successfully loaded model checkpoint from {path}/{tag}")
         return extras
@@ -383,6 +395,8 @@ class Stoke:
     rank = property(lambda self: self._runner.rank)
     ema_loss = property(lambda self: self._rolling_mean_loss)
     engine = property(lambda self: self._runner.engine)
+    # the fp32 EMA / SWA of the weights (WeightAverageConfig), None when not configured
+    weight_average = property(lambda self: self._weight_average)
 
     @property
     def fp16_state_dict(self):
