@@ -1,15 +1,16 @@
 # -*- coding: utf-8 -*-
 """torch.optim classes on the fused step, on one GPU, at ResNet-50 size (25.6 M elements) and BERT-base size
 (109.5 M elements), with Adam as the yardstick.  By default Adam, NAdam, RAdam and Adamax; ``--kinds`` picks others, e.g.
-``--kinds adadelta,rprop,asgd``:
+``--kinds adadelta,rprop,asgd`` or ``--kinds adam,lion`` (stoke_b200.Lion):
 
   k_optim_step[raw]    the world-1 route: the step reads and zeroes the raw bf16 bucket and writes the bf16 model copy
                        (30 B/element algorithmic: read g 2, p m v 12; write p m v 12, bf16 copy 2, zeroing 2), with the
                        step prologue in front of it.  ASGD keeps one state tensor and, while mu == 1 (torch's default
-                       t0 = 1e6), writes it without reading it: 18 B/element
-  k_optim_step[main]   fp32 model, fp32 main gradients (28 B/element: read g p m v 16, write p m v 12; ASGD 16)
+                       t0 = 1e6), writes it without reading it: 18 B/element.  Lion keeps one state tensor, reads it
+                       and runs without the prologue: 22 B/element
+  k_optim_step[main]   fp32 model, fp32 main gradients (28 B/element: read g p m v 16, write p m v 12; ASGD 16, Lion 20)
   optimizer step       gradient pass + step, the fused route (k_grad_norm + prologue + k_optim_step) against
-                       B200StockOptimizer (K1 main-gradient reduce + the class's own torch update on fp32 views + the cast
+                       B200StockOptimizer (K1 main-gradient reduce + the class's own update on fp32 views + the cast
                        into the bf16 model), same class, same gradients, timed in alternating rounds in the same run
 
     python bench_optim.py [--out optim.json] [--iters 30] [--kinds adam,nadam,radam,adamax]
@@ -28,6 +29,8 @@ import torch
 ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 
+import stoke_b200  # noqa: E402
+
 
 def card():
     info = {"name": torch.cuda.get_device_name(0), "power_limit_w": None}
@@ -43,7 +46,10 @@ def card():
 CLASSES = {"adam": (torch.optim.Adam, {"lr": 1e-3}), "nadam": (torch.optim.NAdam, {"lr": 2e-3}),
            "radam": (torch.optim.RAdam, {"lr": 1e-3}), "adamax": (torch.optim.Adamax, {"lr": 2e-3}),
            "adadelta": (torch.optim.Adadelta, {"lr": 1.0}), "rprop": (torch.optim.Rprop, {"lr": 1e-2}),
-           "asgd": (torch.optim.ASGD, {"lr": 1e-2})}
+           "asgd": (torch.optim.ASGD, {"lr": 1e-2}), "lion": (stoke_b200.Lion, {"lr": 1e-4, "weight_decay": 0.1})}
+# algorithmic bytes per element (raw bf16 route, main fp32 route) of the kinds with one state tensor; the others: 30, 28
+ONE_STATE_BYTES = {"asgd": (18, 16),   # ax written without being read while mu == 1
+                   "lion": (22, 20)}
 
 
 def main():
@@ -100,8 +106,8 @@ def main():
         flush_l2 = n < 60_000_000
         for tag, cls, kw in classes:
             # ---- the kernel alone, both gradient sources ----
-            one_state = tag == "asgd"   # one state tensor, written without being read while mu == 1
-            for route, lp, per in (("local", torch.bfloat16, 18 if one_state else 30), ("main", None, 16 if one_state else 28)):
+            raw_b, main_b = ONE_STATE_BYTES.get(tag, (30, 28))
+            for route, lp, per in (("local", torch.bfloat16, raw_b), ("main", None, main_b)):
                 net = Flat(n).cuda()
                 opt = B200FusedOptimizer(net, cls, kw, engine=eng, route=route, clip=clip, lp_dtype=lp)
                 path = opt.path

@@ -84,7 +84,9 @@ typedef enum {
   STK_OPT_ADAMAX = 5,  /* torch.optim.Adamax (torch/optim/adamax.py, _single_tensor_adamax); exp_avg_sq holds exp_inf */
   STK_OPT_ADADELTA = 6,  /* torch.optim.Adadelta (_single_tensor_adadelta); exp_avg = square_avg, exp_avg_sq = acc_delta */
   STK_OPT_RPROP = 7,   /* torch.optim.Rprop (_single_tensor_rprop); exp_avg = prev, exp_avg_sq = step_size */
-  STK_OPT_ASGD = 8     /* torch.optim.ASGD (_single_tensor_asgd); exp_avg = ax, no exp_avg_sq */
+  STK_OPT_ASGD = 8,    /* torch.optim.ASGD (_single_tensor_asgd); exp_avg = ax, no exp_avg_sq */
+  STK_OPT_LION = 9     /* stoke_b200.optim.Lion (Chen et al. 2023; torch.optim has none); exp_avg = exp_avg, no exp_avg_sq.
+                          Reads lr, beta1, beta2, weight_decay (decoupled) and maximize of stk_optim_hyper_t */
 } stk_optim_kind;
 
 /* flags of stk_grad_reduce */
@@ -128,7 +130,8 @@ typedef struct {
 
 /* Per-group hyper-parameters of the kinds after SGD that stk_optim_hyper_t has no field for (one entry per group, same
  * order as the stk_optim_hyper_t array).  A NULL array means every field is 0.  stk_optim_hyper_t's lr, eps, weight_decay
- * and maximize apply to every kind that has them (Adadelta: lr, eps, weight_decay; Rprop: lr; ASGD: lr, weight_decay). */
+ * and maximize apply to every kind that has them (Adadelta: lr, eps, weight_decay; Rprop: lr; ASGD: lr, weight_decay).
+ * Lion needs none of these fields. */
 typedef struct {
   double momentum_decay;        /* NAdam: momentum_decay (psi): mu_t = beta1 (1 - 0.5 * 0.96^(t psi)), torch/optim/nadam.py */
   int decoupled_weight_decay;   /* NAdam / RAdam: 1 = param *= 1 - lr wd before the update (AdamW-style); 0 = L2, grad += wd param */
@@ -287,7 +290,8 @@ typedef struct {
                              range_bc is NULL.  NULL: ADAM / ADAMW / SGD form the scalars of the optimizer-wide step
                              themselves.  Every kind after SGD needs group_bc or range_bc: their per-step scalars (NAdam's
                              and ASGD's come from scalar state that only the prologue advances) are formed once by the
-                             prologue, not in every block.  ASGD takes no exp_avg_sq */
+                             prologue, not in every block.  Lion has no per-step scalars and needs neither (the prologue
+                             runs for it only to keep per-parameter step counts).  ASGD and Lion take no exp_avg_sq */
 } stk_optim_args_t;
 int stk_optim_step_ex(stk_ctx* ctx, const stk_optim_args_t* args, void* stream);
 
@@ -320,6 +324,9 @@ int stk_weight_avg(stk_ctx* ctx, float* avg, const float* master, size_t n, int 
  *   ASGD:   {-eta, 1 - lambd eta, mu, 0} with the STORED fp32 eta and mu (the lr and 1 at t == 1, torch's lazy
  *           initialisation): param = param (1 - lambd eta) - eta grad; ax = param if mu == 1 (ax not read), else
  *           ax + (param - ax) mu.  Then eta = lr / (1 + lambd lr t)^alpha and mu = 1 / max(1, t - t0), as fp32
+ *   LION:   {0, 0, 0, 0}: no per-step scalars; exp_avg only.  c = fma(g, 1 - beta1, exp_avg beta1),
+ *           param = fma(-lr, sign(c), param (1 - lr wd)) (the decay only when wd != 0), exp_avg = fma(g, 1 - beta2,
+ *           exp_avg beta2)
  * with bc1 = 1 - beta1^t, bc2 = 1 - beta2^t.  The scalar state `scalar_state` (fp32, torch keeps it per parameter) holds per
  * range or per group: NADAM one float, mu_product (torch initialises it to 1); ASGD two floats, {eta, mu}.  It is read and
  * written only for those two kinds and may be NULL for the others; hyper_ext may be NULL (all zero).

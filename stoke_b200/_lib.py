@@ -15,7 +15,7 @@ REDUCE_ALL, REDUCE_SCATTER = 0, 1
 NORM_NONE, NORM_L2, NORM_INF, NORM_P = 0, 1, 2, 3
 CLIP_NONE, CLIP_NORM, CLIP_VALUE = 0, 1, 2
 OPT_ADAM, OPT_ADAMW, OPT_SGD, OPT_NADAM, OPT_RADAM, OPT_ADAMAX = 0, 1, 2, 3, 4, 5
-OPT_ADADELTA, OPT_RPROP, OPT_ASGD = 6, 7, 8
+OPT_ADADELTA, OPT_RPROP, OPT_ASGD, OPT_LION = 6, 7, 8, 9
 ACT_RELU, ACT_SILU, ACT_HARDSWISH, ACT_RELU6 = 0, 1, 2, 3
 RF_FINAL, RF_ZERO_INPUT, RF_UNSCALE = 1, 2, 4
 OPT_K1_ALGO, OPT_MEM_MODE, OPT_K1_MAX_BLOCKS, OPT_COOP_LAUNCH, OPT_NVLS_MAX_BLOCKS, OPT_K2_AG_MC = 1, 2, 3, 4, 5, 6

@@ -1,5 +1,6 @@
 // k2_optim.cu -- K2: single-pass fused optimizer step (Adam / AdamW / SGD-momentum / NAdam / RAdam / Adamax / Adadelta /
-// Rprop / ASGD), plus the step prologue (per-parameter step counts, NAdam's mu_product, ASGD's eta and mu) and epilogue.
+// Rprop / ASGD / Lion), plus the step prologue (per-parameter step counts, NAdam's mu_product, ASGD's eta and mu) and
+// epilogue.
 //
 // One sweep over (grad, master, exp_avg, exp_avg_sq) does what the reference spreads over clip_grad_norm_'s scaling pass /
 // clip_grad_value_, GradScaler.step's inf gate, the ~7 foreach kernels of torch.optim.Adam and (mixed precision) the
@@ -8,8 +9,9 @@
 // write p,m,v (12) [+ 2 for the bf16 copy] = 28 / 30, for every kind but SGD and ASGD (NAdam, RAdam, Adamax, Adadelta and
 // Rprop keep two fp32 state tensors like Adam; Adamax's exp_inf, Adadelta's acc_delta and Rprop's step_size live in the
 // exp_avg_sq buffer).  ASGD keeps one (ax, in exp_avg): read g,p,ax + write p,ax = 20 / 22, and 16 / 18 while mu == 1,
-// when ax is written without being read.  The clip coefficient, the skip decision and the bias corrections
-// come from device memory, so there is no host synchronisation anywhere on the step.
+// when ax is written without being read.  Lion keeps one (exp_avg) and reads it: 20 / 22.  The clip coefficient, the
+// skip decision and the bias corrections come from device memory, so there is no host synchronisation anywhere on the
+// step.
 //
 // Gradient sources:  MAIN  -- fp32 reduced / unscaled gradients written by K1 (cross-rank routes), indexed like the state;
 //                    RAW   -- the local model-dtype bucket itself (+ optional fp32 accumulator), scaled by mul and 1/scale
@@ -22,8 +24,8 @@
 // Arithmetic follows torch/optim/adam.py (_single_tensor_adam, the path torch takes on CPU -- the oracle),
 // torch/optim/sgd.py (_single_tensor_sgd), nadam.py (_single_tensor_nadam), radam.py (_single_tensor_radam), adamax.py
 // (_single_tensor_adamax), adadelta.py (_single_tensor_adadelta), rprop.py (_single_tensor_rprop) and asgd.py
-// (_single_tensor_asgd); the clip follows torch/nn/utils/clip_grad.py:165-174 (coef = max_norm /
-// (total_norm + 1e-6), clamped to 1) and :291-292 (clamp).
+// (_single_tensor_asgd), and Lion follows stoke_b200.optim.Lion.step (torch has no Lion); the clip follows
+// torch/nn/utils/clip_grad.py:165-174 (coef = max_norm / (total_norm + 1e-6), clamped to 1) and :291-292 (clamp).
 #include <cstdlib>
 
 #include "k1_common.cuh"
@@ -44,7 +46,12 @@ struct GroupHyperS {   // what the inner loop reads (shared memory, one entry pe
   int nesterov, maximize;
   float c0, c1, c2;  // the per-step scalars of step_scalars (the layout documented at stk_optim_step_prologue)
   int decoupled;
-  float rho, one_m_rho;                         // Adadelta
+  // Adadelta's rho and Lion's beta1 share a slot: a wider struct changes every kind's shared-memory loads (and registers)
+  union {
+    float rho;                                  // Adadelta
+    float b1;                                   // Lion
+  };
+  float one_m_rho;                              // Adadelta
   float etaminus, etaplus, ss_min, ss_max;      // Rprop
 };
 
@@ -127,6 +134,7 @@ __device__ __forceinline__ float4 step_scalars(int kind, const GroupHyperD& h, d
     }
     return make_float4((float)(h.lr / bc1), 0.f, 0.f, 0.f);
   }
+  if (kind == STK_OPT_LION) return make_float4(0.f, 0.f, 0.f, 0.f);  // none: only the step count advances
   return make_float4((float)(h.lr / bc1), 0.f, 0.f, 0.f);  // Adamax: clr = lr / bias_correction
 }
 
@@ -208,7 +216,8 @@ __global__ void __launch_bounds__(256, KIND >= STK_OPT_NADAM ? 2 : 0) k_optim_st
   if (PERSIST && p.prof_ns && blockIdx.x == 0 && threadIdx.x == 0) t_begin = globaltimer_ns();
 
   const bool use_m = (KIND != STK_OPT_SGD) || p.m != nullptr;
-  constexpr bool kHasV = KIND != STK_OPT_SGD && KIND != STK_OPT_ASGD;  // ASGD: one state tensor (ax, in p.m)
+  // ASGD and Lion: one state tensor (ax / exp_avg, in p.m)
+  constexpr bool kHasV = KIND != STK_OPT_SGD && KIND != STK_OPT_ASGD && KIND != STK_OPT_LION;
   const size_t stride = PERSIST ? size_t(gridDim.x) * blockDim.x * VPT : 0;
   size_t i = (size_t(blockIdx.x) * blockDim.x + threadIdx.x) * VPT;
 
@@ -282,6 +291,7 @@ __global__ void __launch_bounds__(256, KIND >= STK_OPT_NADAM ? 2 : 0) k_optim_st
       o.ss_min = (float)h.step_size_min;
       o.ss_max = (float)h.step_size_max;
     }
+    if constexpr (KIND == STK_OPT_LION) o.b1 = (float)h.beta1;
     s_g[threadIdx.x] = o;
   }
   __syncthreads();
@@ -388,6 +398,14 @@ __global__ void __launch_bounds__(256, KIND >= STK_OPT_NADAM ? 2 : 0) k_optim_st
             ww = fmaf(h.c0, gg, __fmul_rn(ww, h.c1));                // param.mul_(1 - lambd eta).add_(grad, alpha=-eta)
             // ax.add_(param.sub(ax).mul_(mu)), or ax.copy_(param) while mu == 1
             m[k][e] = h.c2 == 1.f ? ww : __fadd_rn(m[k][e], __fmul_rn(ww - m[k][e], h.c2));
+          } else if (KIND == STK_OPT_LION) {
+            if (h.wd != 0.f) ww *= h.decay_mul;                     // param.mul_(1 - lr * wd), before the update
+            const float mm = m[k][e];
+            // exp_avg.mul(beta1).add_(g, alpha=1 - beta1): torch's CUDA add(alpha) contracts to one FFMA
+            const float c = fmaf(gg, h.one_m_b1, __fmul_rn(mm, h.b1));
+            const float sg = (float)((c > 0.f) - (c < 0.f));       // .sign_(): NaN and +-0 give 0
+            ww = fmaf(-h.lr, sg, ww);                                // param.add_(u, alpha=-lr)
+            m[k][e] = fmaf(gg, h.one_m_b2, __fmul_rn(mm, h.b2));    // exp_avg.mul_(beta2).add_(g, alpha=1 - beta2)
           } else {  // SGD
             if (h.wd != 0.f) gg = fmaf(ww, h.wd, gg);
             if (h.mom != 0.f) {
@@ -556,12 +574,13 @@ int stk_optim_step_ex(stk_ctx* c, const stk_optim_args_t* a, void* stream) {
   STK_REQUIRE(c, a->n_groups >= 1 && a->n_groups <= STK_MAX_GROUPS, "stk_optim_step_ex: n_groups must be in [1, 8]");
   STK_REQUIRE(c, a->n_local % 8 == 0, "stk_optim_step_ex: n_local must be a multiple of 8");
   const stk_optim_hyper_t* h = a->hyper;
-  STK_REQUIRE(c, h->kind >= STK_OPT_ADAM && h->kind <= STK_OPT_ASGD, "stk_optim_step_ex: bad optimizer kind");
-  STK_REQUIRE(c, h->kind <= STK_OPT_SGD || a->group_bc || (a->n_ranges > 0 && a->range_bc),
+  STK_REQUIRE(c, h->kind >= STK_OPT_ADAM && h->kind <= STK_OPT_LION, "stk_optim_step_ex: bad optimizer kind");
+  STK_REQUIRE(c, h->kind <= STK_OPT_SGD || h->kind == STK_OPT_LION || a->group_bc || (a->n_ranges > 0 && a->range_bc),
               "stk_optim_step_ex: the kinds after SGD need the scalars of stk_optim_step_prologue (group_bc or range_bc)");
   STK_REQUIRE(c, (reinterpret_cast<uintptr_t>(a->group_bc) & 15) == 0, "stk_optim_step_ex: group_bc must be 16-byte aligned");
-  STK_REQUIRE(c, h->kind == STK_OPT_SGD || (a->exp_avg && (a->exp_avg_sq || h->kind == STK_OPT_ASGD)),
-              "stk_optim_step_ex: this kind needs exp_avg and exp_avg_sq (ASGD: exp_avg)");
+  STK_REQUIRE(c, h->kind == STK_OPT_SGD ||
+                     (a->exp_avg && (a->exp_avg_sq || h->kind == STK_OPT_ASGD || h->kind == STK_OPT_LION)),
+              "stk_optim_step_ex: this kind needs exp_avg and exp_avg_sq (ASGD, Lion: exp_avg)");
   bool any_mom = false;
   for (int gi = 0; gi < a->n_groups; ++gi) {
     STK_REQUIRE(c, h[gi].kind == h->kind, "stk_optim_step_ex: all groups must use the same optimizer kind");
@@ -671,6 +690,7 @@ int stk_optim_step_ex(stk_ctx* c, const stk_optim_args_t* a, void* stream) {
     case STK_OPT_ADADELTA: err = launch_optim<STK_OPT_ADADELTA>(c, p, a->lp_dtype, a->grad_dtype, raw, pair_ok, s); break;
     case STK_OPT_RPROP: err = launch_optim<STK_OPT_RPROP>(c, p, a->lp_dtype, a->grad_dtype, raw, pair_ok, s); break;
     case STK_OPT_ASGD: err = launch_optim<STK_OPT_ASGD>(c, p, a->lp_dtype, a->grad_dtype, raw, pair_ok, s); break;
+    case STK_OPT_LION: err = launch_optim<STK_OPT_LION>(c, p, a->lp_dtype, a->grad_dtype, raw, pair_ok, s); break;
     default: err = launch_optim<STK_OPT_SGD>(c, p, a->lp_dtype, a->grad_dtype, raw, pair_ok, s); break;
   }
   if (err == cudaErrorNotSupported)
@@ -706,7 +726,7 @@ int stk_optim_step_prologue(stk_ctx* c, const stk_optim_hyper_t* h, const stk_op
   STK_REQUIRE(c, n_groups >= 1 && n_groups <= STK_MAX_GROUPS, "stk_optim_step_prologue: n_groups must be in [1, 8]");
   STK_REQUIRE(c, n_ranges >= 0, "stk_optim_step_prologue: negative n_ranges");
   STK_REQUIRE(c, n_ranges == 0 || (range_group && range_steps), "stk_optim_step_prologue: range arrays are NULL");
-  STK_REQUIRE(c, h->kind >= STK_OPT_ADAM && h->kind <= STK_OPT_ASGD, "stk_optim_step_prologue: bad optimizer kind");
+  STK_REQUIRE(c, h->kind >= STK_OPT_ADAM && h->kind <= STK_OPT_LION, "stk_optim_step_prologue: bad optimizer kind");
   STK_REQUIRE(c, scalar_state_width(h->kind) == 0 || scalar_state,
               "stk_optim_step_prologue: NAdam and ASGD need their scalar state");
   STK_REQUIRE(c, (reinterpret_cast<uintptr_t>(bc) & 15) == 0, "stk_optim_step_prologue: bc must be 16-byte aligned");

@@ -4,13 +4,17 @@
 ``B200FusedOptimizer`` -- a ``torch.optim.Optimizer`` (so LR schedulers and ``param_groups`` edits work, README.md:241-250
 of the reference) whose ``step()`` is the single fused K2 launch over the flat fp32 master / moment buffers; its sharded
 flavour is the ZeRO-1 analogue of fairscale ``OSS`` (/root/reference/stoke/extensions.py:109-141): same ``clip_grad_norm`` /
-``consolidate_state_dict`` surface.  Adam, AdamW, SGD(-momentum), NAdam, RAdam, Adamax, Adadelta, Rprop and ASGD, up to 8
-parameter groups (per-group lr / betas / eps / weight decay / momentum ... selected inside the kernel by element range).
+``consolidate_state_dict`` surface.  Adam, AdamW, SGD(-momentum), NAdam, RAdam, Adamax, Adadelta, Rprop, ASGD and the
+package's own ``Lion``, up to 8 parameter groups (per-group lr / betas / eps / weight decay / momentum ... selected inside
+the kernel by element range).
 NAdam, RAdam, Adamax, Adadelta and Rprop keep two fp32 state tensors per parameter like Adam (Adamax's ``exp_inf``,
-Adadelta's ``acc_delta`` and Rprop's ``step_size`` in the second-moment buffer); ASGD keeps one (``ax``).  Their per-step
+Adadelta's ``acc_delta`` and Rprop's ``step_size`` in the second-moment buffer); ASGD keeps one (``ax``), as does Lion
+(``exp_avg``, with no per-step scalars).  Their per-step
 scalars, NAdam's ``mu_product`` and ASGD's ``eta`` / ``mu`` are formed on the device by ``stk_optim_step_prologue``, so
 none of them reads a scalar back to the host (torch's single-tensor ASGD calls ``.item()`` three times per parameter).
-Adadelta, Rprop and ASGD create their state lazily like torch: a parameter never stepped has no ``state_dict`` entry.
+Adadelta, Rprop, ASGD and Lion create their state lazily like torch: a parameter never stepped has no ``state_dict``
+entry.  Lion is element-wise and independent of the partition, so under DDP / ``fairscale_oss`` it is sharded like the
+other kinds.
 ``torch.optim.Adafactor`` takes its own fused entry point, ``stk_adafactor_step`` (per-parameter reductions: row / column
 means of g^2, the parameter's RMS, the update's RMS), with per-parameter step counts on the device and torch's
 state_dict layout (``row_var`` / ``col_var`` or ``variance``).  Its state is never sharded: the reductions need whole
@@ -39,13 +43,13 @@ _KINDS = {torch.optim.Adam: _lib.OPT_ADAM, torch.optim.AdamW: _lib.OPT_ADAMW, to
 # per-step scalars from stk_optim_step_prologue
 _EXT_KINDS = (_lib.OPT_NADAM, _lib.OPT_RADAM, _lib.OPT_ADAMAX, _lib.OPT_ADADELTA, _lib.OPT_RPROP, _lib.OPT_ASGD)
 # element-wise classes whose state torch creates at a parameter's first step (no state_dict entry before it)
-_LAZY_KINDS = (_lib.OPT_ADADELTA, _lib.OPT_RPROP, _lib.OPT_ASGD)
+_LAZY_KINDS = (_lib.OPT_ADADELTA, _lib.OPT_RPROP, _lib.OPT_ASGD, _lib.OPT_LION)
 # torch's per-parameter state keys of the two fp32 buffers M and V (None: no V buffer)
 _STATE_KEYS = {_lib.OPT_SGD: ("momentum_buffer", None),
                _lib.OPT_ADAM: ("exp_avg", "exp_avg_sq"), _lib.OPT_ADAMW: ("exp_avg", "exp_avg_sq"),
                _lib.OPT_NADAM: ("exp_avg", "exp_avg_sq"), _lib.OPT_RADAM: ("exp_avg", "exp_avg_sq"),
                _lib.OPT_ADAMAX: ("exp_avg", "exp_inf"), _lib.OPT_ADADELTA: ("square_avg", "acc_delta"),
-               _lib.OPT_RPROP: ("prev", "step_size"), _lib.OPT_ASGD: ("ax", None)}
+               _lib.OPT_RPROP: ("prev", "step_size"), _lib.OPT_ASGD: ("ax", None), _lib.OPT_LION: ("exp_avg", None)}
 # per-entry scalar state carried by the step prologue: NAdam's mu_product, ASGD's (eta, mu), torch's 0-dim fp32 tensors
 _SCALAR_KEYS = {_lib.OPT_NADAM: ("mu_product",), _lib.OPT_ASGD: ("eta", "mu")}
 _STOCK_ONLY_TRUE = ("amsgrad", "capturable", "differentiable")
@@ -187,6 +191,59 @@ class LARS(torch.optim.Optimizer):
         return loss
 
 
+class Lion(torch.optim.Optimizer):
+    """Lion (Chen et al., "Symbolic Discovery of Optimization Algorithms", 2023): the sign of an interpolation between
+    the momentum and the gradient, with decoupled weight decay applied before the update (as timm and lion-pytorch do).
+    For one parameter w with gradient g::
+
+        g = -g if maximize else g
+        if weight_decay != 0: w = w * (1 - lr * weight_decay)
+        w = w - lr * sign(beta1 * m + (1 - beta1) * g)
+        m = beta2 * m + (1 - beta2) * g
+
+    sign is ``torch.sign``: a NaN or a zero interpolation leaves w unchanged.  State per parameter, created at its first
+    step: ``step`` (0-dim fp32 tensor; the update does not use it) and ``exp_avg``.  This ``step()`` is plain
+    per-parameter torch: what runs outside the engine and on its stock route; inside ``Stoke`` the class runs on the fused
+    sm_90a step (``k_optim_step``, kind ``STK_OPT_LION``)."""
+
+    def __init__(self, params, lr: float = 1e-4, betas=(0.9, 0.99), weight_decay: float = 0.0, maximize: bool = False):
+        if lr < 0.0:
+            raise ValueError(f"Invalid learning rate: {lr}")
+        if not 0.0 <= betas[0] < 1.0 or not 0.0 <= betas[1] < 1.0:
+            raise ValueError(f"Invalid beta parameters: {betas}")
+        if weight_decay < 0.0:
+            raise ValueError(f"Invalid weight_decay value: {weight_decay}")
+        super().__init__(params, dict(lr=lr, betas=tuple(betas), weight_decay=weight_decay, maximize=maximize))
+
+    @torch.no_grad()
+    def step(self, closure=None):
+        loss = None
+        if closure is not None:
+            with torch.enable_grad():
+                loss = closure()
+        for group in self.param_groups:
+            b1, b2 = group["betas"]
+            lr, wd = group["lr"], group["weight_decay"]
+            for p in group["params"]:
+                if p.grad is None:
+                    continue
+                g = -p.grad if group["maximize"] else p.grad
+                state = self.state[p]
+                if not state:
+                    state["step"] = torch.tensor(0.0, dtype=torch.float32)
+                    state["exp_avg"] = torch.zeros_like(p, memory_format=torch.preserve_format)
+                state["step"] += 1
+                m = state["exp_avg"]
+                if wd != 0:
+                    p.mul_(1 - lr * wd)
+                u = m.mul(b1).add_(g, alpha=1 - b1).sign_()
+                p.add_(u, alpha=-lr)
+                m.mul_(b2).add_(g, alpha=1 - b2)
+        return loss
+
+
+_KINDS[Lion] = _lib.OPT_LION
+
 # LAMB and LARS run on their own entry point, stk_layerwise_step (per-parameter trust ratios), not as kinds of K2
 _LAMB, _LARS = "lamb", "lars"
 _KINDS[LAMB] = _LAMB
@@ -301,7 +358,7 @@ class B200FusedOptimizer(torch.optim.Optimizer):
                  bucket_mb: Optional[float] = None):
         if optim_cls not in _KINDS:
             raise NotImplementedError(
-                f"Stoke -- the fused step covers torch.optim.Adam, AdamW, SGD, NAdam, RAdam, Adamax, Adadelta, Rprop, ASGD and Adafactor and stoke_b200.optim.LAMB and LARS; got {getattr(optim_cls, '__name__', optim_cls)}"
+                f"Stoke -- the fused step covers torch.optim.Adam, AdamW, SGD, NAdam, RAdam, Adamax, Adadelta, Rprop, ASGD and Adafactor and stoke_b200.optim.LAMB, LARS and Lion; got {getattr(optim_cls, '__name__', optim_cls)}"
                 f" (use B200StockOptimizer / build_optimizer, which routes other classes to the stock-optimizer path)")
         params, group_of, extra, kw = _group_layout(module, optim_kwargs)
         if len(extra) > _lib.MAX_GROUPS:
@@ -323,13 +380,14 @@ class B200FusedOptimizer(torch.optim.Optimizer):
         ada = self._kind == _ADAFACTOR
         lw = self._kind in _LAYERWISE
         lars = self._kind == _LARS
+        one_state = self._kind in (_lib.OPT_ASGD, _lib.OPT_LION)   # a single fp32 state tensor, in M
         if (ada or lw) and engine.world > 1:
             # Adafactor's per-parameter reductions and LAMB's / LARS's trust ratios need whole parameters on one rank: their
             # state is replicated (also under fairscale_oss) and every rank runs the same deterministic step on the same
             # all-reduced fp32 gradients
             route = "allreduce"
         self.path = GradPath(engine, params, grad_accum=grad_accum, clip=clip, sharded=sharded, lp_dtype=lp_dtype,
-                             module=module, needs_second_moment=not (sgd or ada or lars or self._kind == _lib.OPT_ASGD),
+                             module=module, needs_second_moment=not (sgd or ada or lars or one_state),
                              needs_first_moment=not (sgd or ada or lars) or any_mom, state_id=state_id, route=route,
                              group_of=group_of, bucket_mb=bucket_mb, scalar_state=len(_SCALAR_KEYS.get(self._kind, ())),
                              adafactor=ada, layerwise=lw)
@@ -378,7 +436,7 @@ class B200FusedOptimizer(torch.optim.Optimizer):
             h.nesterov = int(bool(g.get("nesterov", False)))
         elif "betas" in g:
             h.beta1, h.beta2 = (float(b) for b in g["betas"])
-            h.eps = float(g["eps"])
+            h.eps = float(g.get("eps", 0.0))   # Lion has no eps
         elif "eps" in g:   # Adadelta
             h.eps = float(g["eps"])
         return h
@@ -486,7 +544,7 @@ class B200FusedOptimizer(torch.optim.Optimizer):
 
     def state_dict(self):
         """torch's per-parameter format: ``step``, the scalar state (NAdam's ``mu_product``, ASGD's ``eta`` and ``mu``) as
-        0-dim fp32 tensors, then the class's state tensors.  Adadelta, Rprop and ASGD omit a parameter that was never
+        0-dim fp32 tensors, then the class's state tensors.  Adadelta, Rprop, ASGD and Lion omit a parameter that was never
         stepped (torch creates their state at its first gradient); the other kinds emit it.  SGD emits only
         ``momentum_buffer``, None before a parameter's first step or without momentum."""
         path = self.path
