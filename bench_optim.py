@@ -1,17 +1,23 @@
 # -*- coding: utf-8 -*-
 """torch.optim classes on the fused step, on one GPU, at ResNet-50 size (25.6 M elements) and BERT-base size
 (109.5 M elements), with Adam as the yardstick.  By default Adam, NAdam, RAdam and Adamax; ``--kinds`` picks others, e.g.
-``--kinds adadelta,rprop,asgd`` or ``--kinds adam,lion`` (stoke_b200.Lion):
+``--kinds adadelta,rprop,asgd``, ``--kinds adam,lion`` (stoke_b200.Lion) or ``--kinds adam,sf_adamw,sgd,sf_sgd``
+(stoke_b200.AdamWScheduleFree and SGDScheduleFree against the kinds whose bytes they move):
 
   k_optim_step[raw]    the world-1 route: the step reads and zeroes the raw bf16 bucket and writes the bf16 model copy
                        (30 B/element algorithmic: read g 2, p m v 12; write p m v 12, bf16 copy 2, zeroing 2), with the
                        step prologue in front of it.  ASGD keeps one state tensor and, while mu == 1 (torch's default
                        t0 = 1e6), writes it without reading it: 18 B/element.  Lion keeps one state tensor, reads it
-                       and runs without the prologue: 22 B/element
-  k_optim_step[main]   fp32 model, fp32 main gradients (28 B/element: read g p m v 16, write p m v 12; ASGD 16, Lion 20)
+                       and runs without the prologue: 22 B/element.  SGD with momentum and schedule-free SGD keep one
+                       (momentum_buffer / z): 22 B/element; schedule-free AdamW keeps two like Adam: 30
+  k_optim_step[main]   fp32 model, fp32 main gradients (28 B/element: read g p m v 16, write p m v 12; ASGD 16, Lion, SGD
+                       and schedule-free SGD 20)
   optimizer step       gradient pass + step, the fused route (k_grad_norm + prologue + k_optim_step) against
                        B200StockOptimizer (K1 main-gradient reduce + the class's own update on fp32 views + the cast
                        into the bf16 model), same class, same gradients, timed in alternating rounds in the same run
+  schedule-free swap   eval() + train() of the fused schedule-free optimizers on a bf16 model: per call one stk_weight_avg
+                       lerp of the master toward z (read master, z; write master: 12 B/element) and the cast of the
+                       master into the bf16 model (6 B/element), 36 B/element per pair
 
     python bench_optim.py [--out optim.json] [--iters 30] [--kinds adam,nadam,radam,adamax]
 
@@ -46,10 +52,14 @@ def card():
 CLASSES = {"adam": (torch.optim.Adam, {"lr": 1e-3}), "nadam": (torch.optim.NAdam, {"lr": 2e-3}),
            "radam": (torch.optim.RAdam, {"lr": 1e-3}), "adamax": (torch.optim.Adamax, {"lr": 2e-3}),
            "adadelta": (torch.optim.Adadelta, {"lr": 1.0}), "rprop": (torch.optim.Rprop, {"lr": 1e-2}),
-           "asgd": (torch.optim.ASGD, {"lr": 1e-2}), "lion": (stoke_b200.Lion, {"lr": 1e-4, "weight_decay": 0.1})}
+           "asgd": (torch.optim.ASGD, {"lr": 1e-2}), "lion": (stoke_b200.Lion, {"lr": 1e-4, "weight_decay": 0.1}),
+           "sgd": (torch.optim.SGD, {"lr": 0.1, "momentum": 0.9}),
+           "sf_adamw": (stoke_b200.AdamWScheduleFree, {"lr": 2.5e-3, "weight_decay": 0.01}),
+           "sf_sgd": (stoke_b200.SGDScheduleFree, {"lr": 1.0, "weight_decay": 1e-4})}
 # algorithmic bytes per element (raw bf16 route, main fp32 route) of the kinds with one state tensor; the others: 30, 28
 ONE_STATE_BYTES = {"asgd": (18, 16),   # ax written without being read while mu == 1
-                   "lion": (22, 20)}
+                   "lion": (22, 20), "sgd": (22, 20), "sf_sgd": (22, 20)}
+SCHEDULE_FREE = ("sf_adamw", "sf_sgd")   # a new optimizer is in eval mode: train() before stepping
 
 
 def main():
@@ -110,6 +120,8 @@ def main():
             for route, lp, per in (("local", torch.bfloat16, raw_b), ("main", None, main_b)):
                 net = Flat(n).cuda()
                 opt = B200FusedOptimizer(net, cls, kw, engine=eng, route=route, clip=clip, lp_dtype=lp)
+                if tag in SCHEDULE_FREE:
+                    opt.train()
                 path = opt.path
                 path.g_flat.copy_((torch.randn(path.n, device="cuda") * 1e-3).to(path.g_flat.dtype))
                 if route == "main":
@@ -130,6 +142,9 @@ def main():
             nets = {"fused": Flat(n).cuda(), "stock": Flat(n).cuda()}
             opts = {"fused": B200FusedOptimizer(nets["fused"], cls, kw, engine=eng, clip=clip, lp_dtype=torch.bfloat16),
                     "stock": B200StockOptimizer(nets["stock"], cls, kw, engine=eng, clip=clip, lp_dtype=torch.bfloat16)}
+            if tag in SCHEDULE_FREE:
+                for o in opts.values():
+                    o.train()
             grads = (torch.randn(opts["fused"].path.n, device="cuda") * 1e-3).to(torch.bfloat16)
 
             def whole(o):
@@ -155,6 +170,15 @@ def main():
                     "fused_us_median": med["fused"] * 1e3, "stock_us_median": med["stock"] * 1e3,
                     "stock_over_fused": med["stock"] / med["fused"], "rounds": args.rounds,
                     "l2_flush_between_launches": flush_l2})
+            if tag in SCHEDULE_FREE:
+                o = opts["fused"]
+                swap = lambda: (o.eval(), o.train())   # noqa: E731
+                measure(swap, 3, False)
+                ms = sorted(measure(swap, args.iters, flush_l2))
+                nbytes = o.path.n * 36
+                report({"row": f"schedule_free_swap[{tag}] eval() + train(), bf16 model", "size": size_name,
+                        "us_median": ms[len(ms) // 2] * 1e3, "us_min": ms[0] * 1e3, "bytes_per_elem": 36,
+                        "achieved_gbs": nbytes / (ms[len(ms) // 2] * 1e-3) / 1e9, "l2_flush_between_launches": flush_l2})
             for o in opts.values():
                 o.close()
             del opts, nets, runs

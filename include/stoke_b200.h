@@ -85,8 +85,13 @@ typedef enum {
   STK_OPT_ADADELTA = 6,  /* torch.optim.Adadelta (_single_tensor_adadelta); exp_avg = square_avg, exp_avg_sq = acc_delta */
   STK_OPT_RPROP = 7,   /* torch.optim.Rprop (_single_tensor_rprop); exp_avg = prev, exp_avg_sq = step_size */
   STK_OPT_ASGD = 8,    /* torch.optim.ASGD (_single_tensor_asgd); exp_avg = ax, no exp_avg_sq */
-  STK_OPT_LION = 9     /* stoke_b200.optim.Lion (Chen et al. 2023; torch.optim has none); exp_avg = exp_avg, no exp_avg_sq.
+  STK_OPT_LION = 9,    /* stoke_b200.optim.Lion (Chen et al. 2023; torch.optim has none); exp_avg = exp_avg, no exp_avg_sq.
                           Reads lr, beta1, beta2, weight_decay (decoupled) and maximize of stk_optim_hyper_t */
+  STK_OPT_SF_ADAMW = 10,  /* stoke_b200.optim.AdamWScheduleFree (Defazio et al. 2024); exp_avg = z, exp_avg_sq = exp_avg_sq.
+                             Reads beta2, eps and weight_decay of stk_optim_hyper_t; the rest from group_bc
+                             (stk_sf_step_prologue) */
+  STK_OPT_SF_SGD = 11     /* stoke_b200.optim.SGDScheduleFree; exp_avg = z, no exp_avg_sq.  Reads weight_decay of
+                             stk_optim_hyper_t; the rest from group_bc (stk_sf_step_prologue) */
 } stk_optim_kind;
 
 /* flags of stk_grad_reduce */
@@ -291,7 +296,10 @@ typedef struct {
                              themselves.  Every kind after SGD needs group_bc or range_bc: their per-step scalars (NAdam's
                              and ASGD's come from scalar state that only the prologue advances) are formed once by the
                              prologue, not in every block.  Lion has no per-step scalars and needs neither (the prologue
-                             runs for it only to keep per-parameter step counts).  ASGD and Lion take no exp_avg_sq */
+                             runs for it only to keep per-parameter step counts).  ASGD and Lion take no exp_avg_sq.
+                             The schedule-free kinds need group_bc from stk_sf_step_prologue and ignore range_bc: their
+                             step count and scalars belong to the group, not to the parameter.  SF_SGD takes no
+                             exp_avg_sq */
 } stk_optim_args_t;
 int stk_optim_step_ex(stk_ctx* ctx, const stk_optim_args_t* args, void* stream);
 
@@ -327,6 +335,8 @@ int stk_weight_avg(stk_ctx* ctx, float* avg, const float* master, size_t n, int 
  *   LION:   {0, 0, 0, 0}: no per-step scalars; exp_avg only.  c = fma(g, 1 - beta1, exp_avg beta1),
  *           param = fma(-lr, sign(c), param (1 - lr wd)) (the decay only when wd != 0), exp_avg = fma(g, 1 - beta2,
  *           exp_avg beta2)
+ *   SF_ADAMW, SF_SGD: {0, 0, 0, 0}: the prologue runs for them only to keep per-parameter step counts (which decide the
+ *           state_dict entries); their scalars come from stk_sf_step_prologue
  * with bc1 = 1 - beta1^t, bc2 = 1 - beta2^t.  The scalar state `scalar_state` (fp32, torch keeps it per parameter) holds per
  * range or per group: NADAM one float, mu_product (torch initialises it to 1); ASGD two floats, {eta, mu}.  It is read and
  * written only for those two kinds and may be NULL for the others; hyper_ext may be NULL (all zero).
@@ -334,6 +344,27 @@ int stk_weight_avg(stk_ctx* ctx, float* avg, const float* master, size_t n, int 
 int stk_optim_step_prologue(stk_ctx* ctx, const stk_optim_hyper_t* hyper, const stk_optim_hyper_ext_t* hyper_ext,
                             int n_groups, int n_ranges, const uint8_t* range_group, int32_t* range_steps,
                             float* scalar_state, float* bc, void* stream);
+
+/* Per-group hyper-parameters of the schedule-free kinds (facebookresearch/schedule_free's AdamWScheduleFree and
+ * SGDScheduleFree).  beta1 is betas[0] (AdamW) or momentum (SGD); beta2 is only read for SF_ADAMW. */
+typedef struct {
+  double lr, beta1, beta2, r, weight_lr_power;
+  int64_t warmup_steps;
+} stk_sf_hyper_t;
+/* The per-step group scalars of the schedule-free kinds (call it right before stk_optim_step_ex, same stream; pass bc as
+ * the step's group_bc).  One thread per group, in double, with k = the selected state's optimizer-wide step count:
+ *   sched = (k + 1) / warmup_steps if k < warmup_steps else 1;  lr = hyper.lr sched
+ *   lr_max = max(lr, group_state[2g]);  weight = (k + 1)^r lr_max^weight_lr_power
+ *   weight_sum = group_state[2g + 1] + weight;  ckp1 = weight / weight_sum (0 when weight_sum == 0)
+ *   bc[4g..4g+3] = fp32 {ckp1, lr (beta1 (1 - ckp1) - 1), lr, 1 / fp32(1 - beta2^(k + 1))}
+ * and, unless the selected state says found_inf, group_state[2g] = lr_max and group_state[2g + 1] = weight_sum.
+ * group_state: DEVICE double[2 n_groups], {lr_max, weight_sum} per group, starting at {-1, 0}.  The update of one element
+ * with y = master, z = exp_avg, v = exp_avg_sq and the formed gradient g:
+ *   SF_ADAMW: v = fma((1 - beta2) g, g, v beta2);  d = g / (sqrt(v bc.w) + eps);  SF_SGD: d = g
+ *   d = fma(y, wd, d) if wd != 0;  y = lerp(y, z, ckp1) (torch's fp32 lerp, see stk_weight_avg);  y = fma(bc.y, d, y);
+ *   z = fma(-lr, d, z) */
+int stk_sf_step_prologue(stk_ctx* ctx, const stk_sf_hyper_t* hyper, int n_groups, double* group_state, float* bc,
+                         void* stream);
 
 /* scaler.update(), opt_steps/skipped_steps bookkeeping, reset of the per-step accumulators */
 int stk_step_epilogue(stk_ctx* ctx, void* stream);

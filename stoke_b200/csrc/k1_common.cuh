@@ -116,6 +116,14 @@ __device__ __forceinline__ float form_grad(float g, bool raw, float mul, float i
   return g;
 }
 
+// torch.lerp(a, b, w) on fp32 (ATen/native/Lerp.h) with the FMA contraction nvcc gives torch's CUDA lerp kernels (the
+// Tensor.lerp_ and foreach forms round alike): |w| < 0.5: a + w (b - a) -> FFMA(w, b - a, a);
+// else b - (b - a)(1 - w) -> FFMA(-(b - a), 1 - w, b).  Shared by stk_weight_avg and the schedule-free step of K2.
+__device__ __forceinline__ float lerp_torch(float a, float b, float w) {
+  const float d = b - a;
+  return fabsf(w) < 0.5f ? fmaf(w, d, a) : fmaf(-d, 1.f - w, b);
+}
+
 // World 1: the block's norm partial (fixed tree: run-to-run deterministic) into blk_partial[blockIdx.x], for
 // k_grad_norm_finish launched behind the kernel on the same stream.  The sign bit carries the block's inf/nan verdict
 // (partials are +0, positive, +inf or NaN for every norm kind); setting the bit keeps the magnitude, so an inf or NaN

@@ -1,6 +1,6 @@
 // k2_optim.cu -- K2: single-pass fused optimizer step (Adam / AdamW / SGD-momentum / NAdam / RAdam / Adamax / Adadelta /
-// Rprop / ASGD / Lion), plus the step prologue (per-parameter step counts, NAdam's mu_product, ASGD's eta and mu) and
-// epilogue.
+// Rprop / ASGD / Lion / schedule-free AdamW and SGD), plus the step prologues (per-parameter step counts, NAdam's
+// mu_product, ASGD's eta and mu; the schedule-free group scalars) and epilogue.
 //
 // One sweep over (grad, master, exp_avg, exp_avg_sq) does what the reference spreads over clip_grad_norm_'s scaling pass /
 // clip_grad_value_, GradScaler.step's inf gate, the ~7 foreach kernels of torch.optim.Adam and (mixed precision) the
@@ -9,7 +9,8 @@
 // write p,m,v (12) [+ 2 for the bf16 copy] = 28 / 30, for every kind but SGD and ASGD (NAdam, RAdam, Adamax, Adadelta and
 // Rprop keep two fp32 state tensors like Adam; Adamax's exp_inf, Adadelta's acc_delta and Rprop's step_size live in the
 // exp_avg_sq buffer).  ASGD keeps one (ax, in exp_avg): read g,p,ax + write p,ax = 20 / 22, and 16 / 18 while mu == 1,
-// when ax is written without being read.  Lion keeps one (exp_avg) and reads it: 20 / 22.  The clip coefficient, the
+// when ax is written without being read.  Lion keeps one (exp_avg) and reads it: 20 / 22.  Schedule-free AdamW keeps
+// z (exp_avg) and exp_avg_sq like Adam: 28 / 30; schedule-free SGD keeps z only: 20 / 22.  The clip coefficient, the
 // skip decision and the bias corrections come from device memory, so there is no host synchronisation anywhere on the
 // step.
 //
@@ -24,7 +25,8 @@
 // Arithmetic follows torch/optim/adam.py (_single_tensor_adam, the path torch takes on CPU -- the oracle),
 // torch/optim/sgd.py (_single_tensor_sgd), nadam.py (_single_tensor_nadam), radam.py (_single_tensor_radam), adamax.py
 // (_single_tensor_adamax), adadelta.py (_single_tensor_adadelta), rprop.py (_single_tensor_rprop) and asgd.py
-// (_single_tensor_asgd), and Lion follows stoke_b200.optim.Lion.step (torch has no Lion); the clip follows
+// (_single_tensor_asgd); Lion follows stoke_b200.optim.Lion.step (torch has no Lion) and the schedule-free kinds
+// stoke_b200.optim.AdamWScheduleFree.step / SGDScheduleFree.step, each rounded like those steps on CUDA; the clip follows
 // torch/nn/utils/clip_grad.py:165-174 (coef = max_norm / (total_norm + 1e-6), clamped to 1) and :291-292 (clamp).
 #include <cstdlib>
 
@@ -51,7 +53,10 @@ struct GroupHyperS {   // what the inner loop reads (shared memory, one entry pe
     float rho;                                  // Adadelta
     float b1;                                   // Lion
   };
-  float one_m_rho;                              // Adadelta
+  union {
+    float one_m_rho;                            // Adadelta
+    float c3;                                   // schedule-free AdamW: the fourth group scalar, fp32(1 / bc2)
+  };
   float etaminus, etaplus, ss_min, ss_max;      // Rprop
 };
 
@@ -134,7 +139,8 @@ __device__ __forceinline__ float4 step_scalars(int kind, const GroupHyperD& h, d
     }
     return make_float4((float)(h.lr / bc1), 0.f, 0.f, 0.f);
   }
-  if (kind == STK_OPT_LION) return make_float4(0.f, 0.f, 0.f, 0.f);  // none: only the step count advances
+  // none: only the step count advances (the schedule-free scalars come from k_sf_prologue)
+  if (kind >= STK_OPT_LION) return make_float4(0.f, 0.f, 0.f, 0.f);
   return make_float4((float)(h.lr / bc1), 0.f, 0.f, 0.f);  // Adamax: clr = lr / bias_correction
 }
 
@@ -216,8 +222,8 @@ __global__ void __launch_bounds__(256, KIND >= STK_OPT_NADAM ? 2 : 0) k_optim_st
   if (PERSIST && p.prof_ns && blockIdx.x == 0 && threadIdx.x == 0) t_begin = globaltimer_ns();
 
   const bool use_m = (KIND != STK_OPT_SGD) || p.m != nullptr;
-  // ASGD and Lion: one state tensor (ax / exp_avg, in p.m)
-  constexpr bool kHasV = KIND != STK_OPT_SGD && KIND != STK_OPT_ASGD && KIND != STK_OPT_LION;
+  // ASGD, Lion and schedule-free SGD: one state tensor (ax / exp_avg / z, in p.m)
+  constexpr bool kHasV = KIND != STK_OPT_SGD && KIND != STK_OPT_ASGD && KIND != STK_OPT_LION && KIND != STK_OPT_SF_SGD;
   const size_t stride = PERSIST ? size_t(gridDim.x) * blockDim.x * VPT : 0;
   size_t i = (size_t(blockIdx.x) * blockDim.x + threadIdx.x) * VPT;
 
@@ -292,6 +298,7 @@ __global__ void __launch_bounds__(256, KIND >= STK_OPT_NADAM ? 2 : 0) k_optim_st
       o.ss_max = (float)h.step_size_max;
     }
     if constexpr (KIND == STK_OPT_LION) o.b1 = (float)h.beta1;
+    if constexpr (KIND == STK_OPT_SF_ADAMW || KIND == STK_OPT_SF_SGD) o.c3 = c.w;
     s_g[threadIdx.x] = o;
   }
   __syncthreads();
@@ -406,6 +413,20 @@ __global__ void __launch_bounds__(256, KIND >= STK_OPT_NADAM ? 2 : 0) k_optim_st
             const float sg = (float)((c > 0.f) - (c < 0.f));       // .sign_(): NaN and +-0 give 0
             ww = fmaf(-h.lr, sg, ww);                                // param.add_(u, alpha=-lr)
             m[k][e] = fmaf(gg, h.one_m_b2, __fmul_rn(mm, h.b2));    // exp_avg.mul_(beta2).add_(g, alpha=1 - beta2)
+          } else if (KIND == STK_OPT_SF_ADAMW || KIND == STK_OPT_SF_SGD) {
+            // group scalars (k_sf_prologue): c0 = ckp1, c1 = lr (beta1 (1 - ckp1) - 1), c2 = lr, c3 = fp32(1 / bc2)
+            float d = gg;
+            if (KIND == STK_OPT_SF_ADAMW) {
+              // exp_avg_sq.mul_(beta2).addcmul_(g, g, value=1 - beta2): torch's CUDA addcmul rounds g * g first
+              const float vv = fmaf(h.one_m_b2, __fmul_rn(gg, gg), __fmul_rn(v[k][e], h.b2));
+              // exp_avg_sq.mul(1 / bc2).sqrt_().add_(eps), then g / denom
+              d = __fdiv_rn(gg, __fadd_rn(__fsqrt_rn(__fmul_rn(vv, h.c3)), h.eps));
+              v[k][e] = vv;
+            }
+            if (h.wd != 0.f) d = fmaf(ww, h.wd, d);                 // d.add(y, alpha=wd), y before this step's update
+            ww = lerp_torch(ww, m[k][e], h.c0);                      // y.lerp_(z, ckp1)
+            ww = fmaf(h.c1, d, ww);                                  // y.add_(d, alpha=lr (beta1 (1 - ckp1) - 1))
+            m[k][e] = fmaf(-h.c2, d, m[k][e]);                       // z.sub_(d, alpha=lr)
           } else {  // SGD
             if (h.wd != 0.f) gg = fmaf(ww, h.wd, gg);
             if (h.mom != 0.f) {
@@ -471,6 +492,39 @@ __global__ void k_step_prologue(const StepPrologueParams p) {
   if (!advance) return;
   for (int k = 0; k < w; ++k) p.scalar_state[j * w + k] = st[k];
   if (per_range) p.range_steps[j] = (int32_t)(done + 1);
+}
+
+struct SfPrologueParams {
+  stk_sf_hyper_t g[STK_MAX_GROUPS];
+  int n_groups;
+  double* state;   // {lr_max, weight_sum} per group
+  float4* bc;
+  const stk_scaler_state_t* scaler;
+};
+
+// One thread per group: the schedule-free group scalars of step k + 1 (AdamWScheduleFree.step / SGDScheduleFree.step, in
+// python doubles; the explicit roundings keep nvcc from contracting a * b - 1 into one DFMA, which python does not do)
+// and, unless found_inf, the advance of lr_max and weight_sum.  k itself is the optimizer-wide count, advanced by the
+// epilogue only on a step that was applied.
+__global__ void k_sf_prologue(const SfPrologueParams p) {
+  const int j = threadIdx.x;
+  if (j >= p.n_groups) return;
+  const stk_sf_hyper_t& h = p.g[j];
+  const int64_t k = p.scaler->opt_steps;
+  const double kp1 = (double)(k + 1);
+  const double sched = k < h.warmup_steps ? __ddiv_rn(kp1, (double)h.warmup_steps) : 1.0;
+  const double lr = __dmul_rn(h.lr, sched);
+  const double prev_max = p.state[2 * j];
+  const double lr_max = prev_max > lr ? prev_max : lr;                     // python max(lr, lr_max)
+  const double weight = __dmul_rn(pow(kp1, h.r), pow(lr_max, h.weight_lr_power));
+  const double weight_sum = __dadd_rn(p.state[2 * j + 1], weight);
+  const double ckp1 = weight_sum != 0.0 ? __ddiv_rn(weight, weight_sum) : 0.0;
+  const double y_lr = __dmul_rn(lr, __dadd_rn(__dmul_rn(h.beta1, __dadd_rn(1.0, -ckp1)), -1.0));
+  const double bc2 = __dadd_rn(1.0, -pow(h.beta2, kp1));
+  p.bc[j] = make_float4((float)ckp1, (float)y_lr, (float)lr, (float)__ddiv_rn(1.0, bc2));
+  if (p.scaler->found_inf != 0) return;
+  p.state[2 * j] = lr_max;
+  p.state[2 * j + 1] = weight_sum;
 }
 
 // scaler.update() (torch/amp/grad_scaler.py:549-556 -> _amp_update_scale_), step counters, per-step accumulator reset
@@ -574,13 +628,16 @@ int stk_optim_step_ex(stk_ctx* c, const stk_optim_args_t* a, void* stream) {
   STK_REQUIRE(c, a->n_groups >= 1 && a->n_groups <= STK_MAX_GROUPS, "stk_optim_step_ex: n_groups must be in [1, 8]");
   STK_REQUIRE(c, a->n_local % 8 == 0, "stk_optim_step_ex: n_local must be a multiple of 8");
   const stk_optim_hyper_t* h = a->hyper;
-  STK_REQUIRE(c, h->kind >= STK_OPT_ADAM && h->kind <= STK_OPT_LION, "stk_optim_step_ex: bad optimizer kind");
+  STK_REQUIRE(c, h->kind >= STK_OPT_ADAM && h->kind <= STK_OPT_SF_SGD, "stk_optim_step_ex: bad optimizer kind");
+  const bool sf = h->kind == STK_OPT_SF_ADAMW || h->kind == STK_OPT_SF_SGD;
+  STK_REQUIRE(c, !sf || a->group_bc, "stk_optim_step_ex: the schedule-free kinds need group_bc of stk_sf_step_prologue");
   STK_REQUIRE(c, h->kind <= STK_OPT_SGD || h->kind == STK_OPT_LION || a->group_bc || (a->n_ranges > 0 && a->range_bc),
               "stk_optim_step_ex: the kinds after SGD need the scalars of stk_optim_step_prologue (group_bc or range_bc)");
   STK_REQUIRE(c, (reinterpret_cast<uintptr_t>(a->group_bc) & 15) == 0, "stk_optim_step_ex: group_bc must be 16-byte aligned");
   STK_REQUIRE(c, h->kind == STK_OPT_SGD ||
-                     (a->exp_avg && (a->exp_avg_sq || h->kind == STK_OPT_ASGD || h->kind == STK_OPT_LION)),
-              "stk_optim_step_ex: this kind needs exp_avg and exp_avg_sq (ASGD, Lion: exp_avg)");
+                     (a->exp_avg && (a->exp_avg_sq || h->kind == STK_OPT_ASGD || h->kind == STK_OPT_LION ||
+                                     h->kind == STK_OPT_SF_SGD)),
+              "stk_optim_step_ex: this kind needs exp_avg and exp_avg_sq (ASGD, Lion, SF_SGD: exp_avg)");
   bool any_mom = false;
   for (int gi = 0; gi < a->n_groups; ++gi) {
     STK_REQUIRE(c, h[gi].kind == h->kind, "stk_optim_step_ex: all groups must use the same optimizer kind");
@@ -663,7 +720,8 @@ int stk_optim_step_ex(stk_ctx* c, const stk_optim_args_t* a, void* stream) {
   p.n_ranges = a->n_ranges;
   p.range_end = a->range_end_vec;
   p.range_group = a->range_group;
-  p.range_bc = a->n_ranges > 0 ? reinterpret_cast<const float4*>(a->range_bc) : nullptr;
+  // the schedule-free scalars belong to the group (upstream keeps k per group), whatever the range table says
+  p.range_bc = (a->n_ranges > 0 && !sf) ? reinterpret_cast<const float4*>(a->range_bc) : nullptr;
   p.group_bc = reinterpret_cast<const float4*>(a->group_bc);
   if (a->grad_raw) {
     // 1/loss_scale is applied when the scaler is live; the device flag decides (enabled), so no host read
@@ -691,6 +749,8 @@ int stk_optim_step_ex(stk_ctx* c, const stk_optim_args_t* a, void* stream) {
     case STK_OPT_RPROP: err = launch_optim<STK_OPT_RPROP>(c, p, a->lp_dtype, a->grad_dtype, raw, pair_ok, s); break;
     case STK_OPT_ASGD: err = launch_optim<STK_OPT_ASGD>(c, p, a->lp_dtype, a->grad_dtype, raw, pair_ok, s); break;
     case STK_OPT_LION: err = launch_optim<STK_OPT_LION>(c, p, a->lp_dtype, a->grad_dtype, raw, pair_ok, s); break;
+    case STK_OPT_SF_ADAMW: err = launch_optim<STK_OPT_SF_ADAMW>(c, p, a->lp_dtype, a->grad_dtype, raw, pair_ok, s); break;
+    case STK_OPT_SF_SGD: err = launch_optim<STK_OPT_SF_SGD>(c, p, a->lp_dtype, a->grad_dtype, raw, pair_ok, s); break;
     default: err = launch_optim<STK_OPT_SGD>(c, p, a->lp_dtype, a->grad_dtype, raw, pair_ok, s); break;
   }
   if (err == cudaErrorNotSupported)
@@ -726,7 +786,7 @@ int stk_optim_step_prologue(stk_ctx* c, const stk_optim_hyper_t* h, const stk_op
   STK_REQUIRE(c, n_groups >= 1 && n_groups <= STK_MAX_GROUPS, "stk_optim_step_prologue: n_groups must be in [1, 8]");
   STK_REQUIRE(c, n_ranges >= 0, "stk_optim_step_prologue: negative n_ranges");
   STK_REQUIRE(c, n_ranges == 0 || (range_group && range_steps), "stk_optim_step_prologue: range arrays are NULL");
-  STK_REQUIRE(c, h->kind >= STK_OPT_ADAM && h->kind <= STK_OPT_LION, "stk_optim_step_prologue: bad optimizer kind");
+  STK_REQUIRE(c, h->kind >= STK_OPT_ADAM && h->kind <= STK_OPT_SF_SGD, "stk_optim_step_prologue: bad optimizer kind");
   STK_REQUIRE(c, scalar_state_width(h->kind) == 0 || scalar_state,
               "stk_optim_step_prologue: NAdam and ASGD need their scalar state");
   STK_REQUIRE(c, (reinterpret_cast<uintptr_t>(bc) & 15) == 0, "stk_optim_step_prologue: bc must be 16-byte aligned");
@@ -744,6 +804,25 @@ int stk_optim_step_prologue(stk_ctx* c, const stk_optim_hyper_t* h, const stk_op
   p.scaler = c->scaler_dev;
   const int n = n_ranges > 0 ? n_ranges : n_groups;
   k_step_prologue<<<(n + 127) / 128, 128, 0, reinterpret_cast<cudaStream_t>(stream)>>>(p);
+  STK_CUDA(c, cudaGetLastError());
+  return STK_OK;
+}
+
+int stk_sf_step_prologue(stk_ctx* c, const stk_sf_hyper_t* h, int n_groups, double* group_state, float* bc, void* stream) {
+  STK_REQUIRE(c, c && h && group_state && bc, "stk_sf_step_prologue: NULL argument");
+  STK_REQUIRE(c, n_groups >= 1 && n_groups <= STK_MAX_GROUPS, "stk_sf_step_prologue: n_groups must be in [1, 8]");
+  STK_REQUIRE(c, (reinterpret_cast<uintptr_t>(bc) & 15) == 0, "stk_sf_step_prologue: bc must be 16-byte aligned");
+  for (int gi = 0; gi < n_groups; ++gi)
+    STK_REQUIRE(c, h[gi].warmup_steps >= 0, "stk_sf_step_prologue: warmup_steps must be >= 0");
+  std::lock_guard<std::mutex> lk(c->mu);
+  DeviceGuard g(c->device);
+  SfPrologueParams p{};
+  for (int gi = 0; gi < n_groups; ++gi) p.g[gi] = h[gi];
+  p.n_groups = n_groups;
+  p.state = group_state;
+  p.bc = reinterpret_cast<float4*>(bc);
+  p.scaler = c->scaler_dev;
+  k_sf_prologue<<<1, 32, 0, reinterpret_cast<cudaStream_t>(stream)>>>(p);
   STK_CUDA(c, cudaGetLastError());
   return STK_OK;
 }

@@ -7,13 +7,7 @@
 
 namespace stk {
 
-// torch.lerp(a, b, w) on fp32 (ATen/native/Lerp.h) with the FMA contraction nvcc gives torch's CUDA foreach-lerp kernel:
-// |w| < 0.5: a + w (b - a) -> FFMA(w, b - a, a);  else b - (b - a)(1 - w) -> FFMA(-(b - a), 1 - w, b).
-__device__ __forceinline__ float lerp_torch(float a, float b, float w) {
-  const float d = b - a;
-  return fabsf(w) < 0.5f ? fmaf(w, d, a) : fmaf(-d, 1.f - w, b);
-}
-
+// lerp_torch (k1_common.cuh): torch.lerp on fp32 with the contraction of torch's CUDA foreach-lerp kernel
 template <int MODE>
 __global__ void __launch_bounds__(256) k_weight_avg(float* __restrict__ avg, const float* __restrict__ master, size_t n4,
                                                     float w) {

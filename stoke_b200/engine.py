@@ -493,7 +493,7 @@ class GradPath:
                  module: Optional[torch.nn.Module] = None, sync_init: bool = True, needs_second_moment: bool = True,
                  needs_first_moment: bool = True, bucket_mb: Optional[float] = None, state_id: Optional[int] = None,
                  route: Optional[str] = None, group_of: Optional[Sequence[int]] = None, overlap: bool = True,
-                 scalar_state: int = 0, adafactor: bool = False, layerwise: bool = False):
+                 scalar_state: int = 0, adafactor: bool = False, layerwise: bool = False, schedule_free: bool = False):
         self.engine = engine
         self.params = [p for p in params if p.requires_grad]
         if not self.params:
@@ -618,6 +618,13 @@ class GradPath:
         self._group_bc = torch.zeros(n_grp, 4, dtype=torch.float32, device=dev)
         self._touched = np.ones(len(self.params), dtype=bool)
         self._track_touched = False
+        # Schedule-free kinds: z lives in M and starts as the master (upstream clones p at a parameter's first gradient; a
+        # parameter without one is never touched, so cloning at construction is the same); {lr_max, weight_sum} per group
+        # on the device, advanced by stk_sf_step_prologue
+        self._sf_state = None
+        if schedule_free:
+            self.m_flat.copy_(self.master_flat)
+            self._sf_state = torch.tensor([[-1.0, 0.0]] * n_grp, dtype=torch.float64, device=dev)
 
         # ---- re-point the module at the flat buffers ----
         if self.low_precision and module is not None:
@@ -652,6 +659,7 @@ class GradPath:
         if self.layerwise:
             self._layerwise_setup()
         self.avg_flat = None   # AVG, allocated by enable_weight_average
+        self.avg_owner = None  # the WeightAverage over this path: its applied() refuses a schedule-free swap
         self.avg_due = None    # (mode, weight) of the weight-average update the next step carries, set by Stoke.step
         torch.cuda.synchronize(engine.device)
         if W > 1:
@@ -878,11 +886,12 @@ class GradPath:
         """Sets the per-group scalar state (checkpoint load while step counts are optimizer-wide)."""
         self._group_scal.copy_(torch.tensor([list(r) for r in rows], dtype=torch.float32))
 
-    def optimizer_step(self, hypers, exts=None):
+    def optimizer_step(self, hypers, exts=None, sf=None):
         """One fused K2 launch (+ the one-thread epilogue).  ``hypers``: one ``OptimHyper`` or a list (one per group).
         ``exts``: per-group ``OptimHyperExt`` of the kinds after SGD.  stk_optim_step_prologue forms their per-step scalars
         (and the scalar state of NAdam and ASGD) on the device before the step, and every kind's once step counts are
-        per parameter; the optimizer-wide Adam / AdamW / SGD step forms its own."""
+        per parameter; the optimizer-wide Adam / AdamW / SGD step forms its own.  ``sf``: per-group ``SfHyper`` of the
+        schedule-free kinds, whose group scalars stk_sf_step_prologue forms (and whose lr_max / weight_sum it advances)."""
         e = self.engine
         e.state_select(self.state_id)
         if isinstance(hypers, _lib.OptimHyper):
@@ -941,6 +950,13 @@ class GradPath:
                 a.range_bc = bc.data_ptr()
             else:
                 a.group_bc = bc.data_ptr()
+        if sf is not None:
+            sarr = (_lib.SfHyper * ng)(*sf)
+            keep.append(sarr)
+            e._check(e.lib.stk_sf_step_prologue(e.ctx, sarr, ng, self._sf_state.data_ptr(), self._group_bc.data_ptr(),
+                                                e._stream()))
+            e.launches += 1
+            a.group_bc = self._group_bc.data_ptr()
         e.optim_step_ex(a)
         self.weight_avg_after_step()
         e.step_epilogue()
@@ -1070,6 +1086,36 @@ class GradPath:
             self.p_flat.copy_(saved)
         else:
             self.p_flat.copy_(self.gather_master() if self.sharded else self.master_flat)
+
+    # -- schedule-free: the swap between y (where gradients are taken) and x (what is evaluated) ------------------------------
+    def schedule_free_swap(self, weights: Sequence[Optional[float]]):
+        """master = torch.lerp(master, z, w) for every parameter whose ``weights`` entry is a float (None: left as it is),
+        then P <- the master cast to the model dtype.  The lerp is ``stk_weight_avg``'s (mode 2, z in place of the master
+        it averages), one launch per run of adjacent parameters with the same weight.  Sharded: each rank lerps its own
+        shard and P is refilled from the gathered master (collective)."""
+        e = self.engine
+        runs = []   # [global begin, global end, weight] over the padded flat layout
+        for o, pad, w in zip(self.offsets, self.padded, weights):
+            if w is not None and runs and runs[-1][2] == w and runs[-1][1] == o:
+                runs[-1][1] = o + pad
+            elif w is not None:
+                runs.append([o, o + pad, w])
+        pieces = []  # the same runs in local indices: [local begin, local end, weight]
+        for g0, g1, w in runs:
+            for s0, s1, l0, _ in self.segs:
+                a, b = max(g0, s0), min(g1, s1)
+                if a >= b:
+                    continue
+                if pieces and pieces[-1][2] == w and pieces[-1][1] == l0 + (a - s0):
+                    pieces[-1][1] = l0 + (b - s0)
+                else:
+                    pieces.append([l0 + (a - s0), l0 + (b - s0), w])
+        for l0, l1, w in pieces:
+            e._check(e.lib.stk_weight_avg(e.ctx, self.master_ptr + l0 * 4, self.M.ptr + l0 * 4, l1 - l0, 2, w,
+                                          e._stream()))
+            e.launches += 1
+        if self.master_flat is not self.p_flat:
+            self.params_restore(None)
 
     # -- inspection (tests, checkpoints) ----------------------------------------------------------------------------------
     def gather_master(self) -> torch.Tensor:

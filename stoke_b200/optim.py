@@ -5,7 +5,7 @@
 of the reference) whose ``step()`` is the single fused K2 launch over the flat fp32 master / moment buffers; its sharded
 flavour is the ZeRO-1 analogue of fairscale ``OSS`` (/root/reference/stoke/extensions.py:109-141): same ``clip_grad_norm`` /
 ``consolidate_state_dict`` surface.  Adam, AdamW, SGD(-momentum), NAdam, RAdam, Adamax, Adadelta, Rprop, ASGD and the
-package's own ``Lion``, up to 8 parameter groups (per-group lr / betas / eps / weight decay / momentum ... selected inside
+package's own ``Lion``, ``AdamWScheduleFree`` and ``SGDScheduleFree``, up to 8 parameter groups (per-group lr / betas / eps / weight decay / momentum ... selected inside
 the kernel by element range).
 NAdam, RAdam, Adamax, Adadelta and Rprop keep two fp32 state tensors per parameter like Adam (Adamax's ``exp_inf``,
 Adadelta's ``acc_delta`` and Rprop's ``step_size`` in the second-moment buffer); ASGD keeps one (``ax``), as does Lion
@@ -15,6 +15,11 @@ none of them reads a scalar back to the host (torch's single-tensor ASGD calls `
 Adadelta, Rprop, ASGD and Lion create their state lazily like torch: a parameter never stepped has no ``state_dict``
 entry.  Lion is element-wise and independent of the partition, so under DDP / ``fairscale_oss`` it is sharded like the
 other kinds.
+``AdamWScheduleFree`` and ``SGDScheduleFree`` (defined here, after facebookresearch/schedule_free) are two more kinds:
+``z`` in the first-moment buffer (AdamW's ``exp_avg_sq`` in the second), their per-group running state (``lr_max``,
+``weight_sum``; ``k`` is the step count) on the device, advanced by ``stk_sf_step_prologue``, and lazy state without
+``step``.  ``train()`` / ``eval()`` swap the master and the model between y and x; a step in eval mode raises.  They are
+sharded like the other kinds.
 ``torch.optim.Adafactor`` takes its own fused entry point, ``stk_adafactor_step`` (per-parameter reductions: row / column
 means of g^2, the parameter's RMS, the update's RMS), with per-parameter step counts on the device and torch's
 state_dict layout (``row_var`` / ``col_var`` or ``variance``).  Its state is never sharded: the reductions need whole
@@ -43,13 +48,14 @@ _KINDS = {torch.optim.Adam: _lib.OPT_ADAM, torch.optim.AdamW: _lib.OPT_ADAMW, to
 # per-step scalars from stk_optim_step_prologue
 _EXT_KINDS = (_lib.OPT_NADAM, _lib.OPT_RADAM, _lib.OPT_ADAMAX, _lib.OPT_ADADELTA, _lib.OPT_RPROP, _lib.OPT_ASGD)
 # element-wise classes whose state torch creates at a parameter's first step (no state_dict entry before it)
-_LAZY_KINDS = (_lib.OPT_ADADELTA, _lib.OPT_RPROP, _lib.OPT_ASGD, _lib.OPT_LION)
+_LAZY_KINDS = (_lib.OPT_ADADELTA, _lib.OPT_RPROP, _lib.OPT_ASGD, _lib.OPT_LION, _lib.OPT_SF_ADAMW, _lib.OPT_SF_SGD)
 # torch's per-parameter state keys of the two fp32 buffers M and V (None: no V buffer)
 _STATE_KEYS = {_lib.OPT_SGD: ("momentum_buffer", None),
                _lib.OPT_ADAM: ("exp_avg", "exp_avg_sq"), _lib.OPT_ADAMW: ("exp_avg", "exp_avg_sq"),
                _lib.OPT_NADAM: ("exp_avg", "exp_avg_sq"), _lib.OPT_RADAM: ("exp_avg", "exp_avg_sq"),
                _lib.OPT_ADAMAX: ("exp_avg", "exp_inf"), _lib.OPT_ADADELTA: ("square_avg", "acc_delta"),
-               _lib.OPT_RPROP: ("prev", "step_size"), _lib.OPT_ASGD: ("ax", None), _lib.OPT_LION: ("exp_avg", None)}
+               _lib.OPT_RPROP: ("prev", "step_size"), _lib.OPT_ASGD: ("ax", None), _lib.OPT_LION: ("exp_avg", None),
+               _lib.OPT_SF_ADAMW: ("z", "exp_avg_sq"), _lib.OPT_SF_SGD: ("z", None)}
 # per-entry scalar state carried by the step prologue: NAdam's mu_product, ASGD's (eta, mu), torch's 0-dim fp32 tensors
 _SCALAR_KEYS = {_lib.OPT_NADAM: ("mu_product",), _lib.OPT_ASGD: ("eta", "mu")}
 _STOCK_ONLY_TRUE = ("amsgrad", "capturable", "differentiable")
@@ -244,6 +250,176 @@ class Lion(torch.optim.Optimizer):
 
 _KINDS[Lion] = _lib.OPT_LION
 
+
+def _sf_beta1(group) -> float:
+    return group["betas"][0] if "betas" in group else group["momentum"]
+
+
+def _check_train_mode(param_groups):
+    if not all(g["train_mode"] for g in param_groups):
+        raise RuntimeError("Stoke -- a schedule-free optimizer steps only in train mode: call optimizer.train() "
+                           "before training steps and optimizer.eval() before evaluating or saving the evaluated weights")
+
+
+def _sf_scheduled_lr(group, k: int) -> float:
+    """The learning rate of step k + 1 (0-based k): the group's lr times the linear warmup."""
+    warmup = group["warmup_steps"]
+    return group["lr"] * ((k + 1) / warmup if k < warmup else 1.0)
+
+
+class _ScheduleFree(torch.optim.Optimizer):
+    """What AdamWScheduleFree and SGDScheduleFree share: the group scalars of a step, the y / x swap of ``train()`` and
+    ``eval()``, and the refusal to step in eval mode.  Subclasses give ``_direction`` (the update direction d before
+    weight decay) and ``_init_state``."""
+
+    @torch.no_grad()
+    def _swap(self, to_train: bool):
+        for group in self.param_groups:
+            if group["train_mode"] == to_train:
+                continue
+            beta1 = _sf_beta1(group)
+            w = 1 - beta1 if to_train else 1 - 1 / beta1
+            for p in group["params"]:
+                if "z" in self.state[p]:
+                    p.lerp_(self.state[p]["z"], w)
+            group["train_mode"] = to_train
+
+    def train(self):
+        """Parameters to y, the point where gradients are taken: p = lerp(p, z, 1 - beta1)."""
+        self._swap(True)
+
+    def eval(self):
+        """Parameters to x, the averaged point that is evaluated: p = lerp(p, z, 1 - 1 / beta1)."""
+        self._swap(False)
+
+    @torch.no_grad()
+    def step(self, closure=None):
+        _check_train_mode(self.param_groups)
+        loss = None
+        if closure is not None:
+            with torch.enable_grad():
+                loss = closure()
+        for group in self.param_groups:
+            k = group["k"]
+            lr = group["scheduled_lr"] = _sf_scheduled_lr(group, k)
+            lr_max = group["lr_max"] = max(lr, group["lr_max"])
+            weight = ((k + 1) ** group["r"]) * (lr_max ** group["weight_lr_power"])
+            weight_sum = group["weight_sum"] = group["weight_sum"] + weight
+            ckp1 = weight / weight_sum if weight_sum != 0 else 0.0
+            y_lr = lr * (_sf_beta1(group) * (1 - ckp1) - 1)
+            wd = group["weight_decay"]
+            for p in group["params"]:
+                if p.grad is None:
+                    continue
+                state = self.state[p]
+                if not state:
+                    self._init_state(p, state)
+                d = self._direction(p.grad, state, group, k)
+                if wd != 0:
+                    d = d.add(p, alpha=wd)
+                p.lerp_(state["z"], ckp1)
+                p.add_(d, alpha=y_lr)
+                state["z"].sub_(d, alpha=lr)
+            group["k"] = k + 1
+        return loss
+
+
+class AdamWScheduleFree(_ScheduleFree):
+    """Schedule-free AdamW (Defazio et al., "The Road Less Scheduled", 2024; facebookresearch/schedule_free's
+    ``AdamWScheduleFree``, same arguments, group keys and state keys, with the second-moment bias correction inside the
+    denominator as its 1.3+ releases).  No learning-rate schedule and no stopping time: the evaluated weights x are an
+    online average of the iterates z, and gradients are taken at y, an interpolation of the two.  Per group, with its
+    step count k (0-based, python doubles)::
+
+        lr = group_lr * ((k + 1) / warmup_steps if k < warmup_steps else 1)
+        lr_max = max(lr, lr_max);  weight = (k + 1) ** r * lr_max ** weight_lr_power
+        weight_sum = weight_sum + weight;  ckp1 = weight / weight_sum (0 if weight_sum == 0)
+        bc2 = 1 - beta2 ** (k + 1)
+
+    then for every parameter y with a gradient g::
+
+        v = v * beta2 + (1 - beta2) * g * g;  d = g / (sqrt(v / bc2) + eps)
+        if weight_decay != 0: d = d + weight_decay * y          # y before this step's update
+        y = lerp(y, z, ckp1);  y = y + lr * (beta1 * (1 - ckp1) - 1) * d;  z = z - lr * d
+
+    ``train()`` moves the parameters to y (lerp(p, z, 1 - beta1)), ``eval()`` to x (lerp(p, z, 1 - 1 / beta1)); a new
+    optimizer is in eval mode and ``step()`` raises there, modifying nothing.  ``v / bc2`` is computed as
+    ``v * (1 / bc2)``, one rounding the fused kernel reproduces.  State per parameter, created at its first gradient:
+    ``z`` (a copy of the parameter) and ``exp_avg_sq``; no ``step``.  ``step()`` leaves ``p.grad`` unmodified.  This
+    ``step()`` is plain per-parameter torch: what runs outside the engine and on its stock route; inside ``Stoke`` the
+    class runs on the fused sm_90a step (``k_optim_step``, kind ``STK_OPT_SF_ADAMW``).  ``foreach`` is accepted and
+    ignored.  BatchNorm running statistics are gathered at y: recompute them at x if the model has any."""
+
+    def __init__(self, params, lr: float = 0.0025, betas=(0.9, 0.999), eps: float = 1e-8, weight_decay: float = 0.0,
+                 warmup_steps: int = 0, r: float = 0.0, weight_lr_power: float = 2.0, foreach: Optional[bool] = None):
+        if lr < 0.0:
+            raise ValueError(f"Invalid learning rate: {lr}")
+        if eps < 0.0:
+            raise ValueError(f"Invalid epsilon value: {eps}")
+        if not 0.0 < betas[0] < 1.0 or not 0.0 <= betas[1] < 1.0:
+            raise ValueError(f"Invalid beta parameters: {betas}")
+        if weight_decay < 0.0:
+            raise ValueError(f"Invalid weight_decay value: {weight_decay}")
+        if warmup_steps < 0:
+            raise ValueError(f"Invalid warmup_steps: {warmup_steps}")
+        super().__init__(params, dict(lr=lr, betas=tuple(betas), eps=eps, r=r, k=0, warmup_steps=int(warmup_steps),
+                                      train_mode=False, weight_sum=0.0, lr_max=-1.0, scheduled_lr=0.0,
+                                      weight_lr_power=weight_lr_power, weight_decay=weight_decay, foreach=foreach))
+
+    @staticmethod
+    def _init_state(p, state):
+        state["z"] = torch.clone(p, memory_format=torch.preserve_format)
+        state["exp_avg_sq"] = torch.zeros_like(p, memory_format=torch.preserve_format)
+
+    @staticmethod
+    def _direction(g, state, group, k):
+        beta2 = group["betas"][1]
+        v = state["exp_avg_sq"]
+        v.mul_(beta2).addcmul_(g, g, value=1 - beta2)
+        bc2 = 1 - beta2 ** (k + 1)
+        return g / v.mul(1 / bc2).sqrt_().add_(group["eps"])
+
+
+class SGDScheduleFree(_ScheduleFree):
+    """Schedule-free SGD (Defazio et al. 2024; facebookresearch/schedule_free's ``SGDScheduleFree``, same arguments,
+    group keys and state keys).  The group scalars are AdamWScheduleFree's with beta1 = momentum (no bc2); for every
+    parameter y with a gradient g::
+
+        d = g + weight_decay * y if weight_decay != 0 else g   # y before this step's update
+        y = lerp(y, z, ckp1);  y = y + lr * (momentum * (1 - ckp1) - 1) * d;  z = z - lr * d
+
+    ``train()`` / ``eval()`` as AdamWScheduleFree's with beta1 = momentum; ``step()`` raises in eval mode, modifying
+    nothing.  State per parameter, created at its first gradient: ``z`` (a copy of the parameter); no ``step``.
+    ``step()`` leaves ``p.grad`` unmodified.  Plain per-parameter torch here; inside ``Stoke`` the class runs on the fused
+    sm_90a step (``k_optim_step``, kind ``STK_OPT_SF_SGD``).  ``foreach`` is accepted and ignored."""
+
+    def __init__(self, params, lr: float = 1.0, momentum: float = 0.9, weight_decay: float = 0.0, warmup_steps: int = 0,
+                 r: float = 0.0, weight_lr_power: float = 2.0, foreach: Optional[bool] = None):
+        if lr < 0.0:
+            raise ValueError(f"Invalid learning rate: {lr}")
+        if not 0.0 < momentum < 1.0:
+            raise ValueError(f"Invalid momentum value: {momentum}")
+        if weight_decay < 0.0:
+            raise ValueError(f"Invalid weight_decay value: {weight_decay}")
+        if warmup_steps < 0:
+            raise ValueError(f"Invalid warmup_steps: {warmup_steps}")
+        super().__init__(params, dict(lr=lr, momentum=momentum, r=r, k=0, warmup_steps=int(warmup_steps),
+                                      train_mode=False, weight_sum=0.0, lr_max=-1.0, scheduled_lr=0.0,
+                                      weight_lr_power=weight_lr_power, weight_decay=weight_decay, foreach=foreach))
+
+    @staticmethod
+    def _init_state(p, state):
+        state["z"] = torch.clone(p, memory_format=torch.preserve_format)
+
+    @staticmethod
+    def _direction(g, state, group, k):
+        return g
+
+
+_KINDS[AdamWScheduleFree] = _lib.OPT_SF_ADAMW
+_KINDS[SGDScheduleFree] = _lib.OPT_SF_SGD
+_SF_KINDS = (_lib.OPT_SF_ADAMW, _lib.OPT_SF_SGD)
+
 # LAMB and LARS run on their own entry point, stk_layerwise_step (per-parameter trust ratios), not as kinds of K2
 _LAMB, _LARS = "lamb", "lars"
 _KINDS[LAMB] = _LAMB
@@ -288,11 +464,11 @@ def state_dict_index(group_of: List[int], n_groups: int) -> Dict[int, int]:
 
 
 def load_step_counts(kind, entries: List[Dict], group_of: List[int], opt_steps: Optional[int], per_param_on: bool,
-                     momentum: Optional[List[float]] = None):
+                     momentum: Optional[List[float]] = None, group_k: Optional[List[int]] = None):
     """How a loaded state dict's step counts and scalar state (NAdam's ``mu_product``, ASGD's ``eta`` / ``mu``) go onto
     the fused step.  ``entries``: torch's state entry of every parameter in flat order (``{}`` where it has none);
     ``opt_steps``: the checkpoint's ``b200_opt_steps`` (None in a torch-written one); ``per_param_on``: the step already
-    keeps per-parameter counts; ``momentum``: SGD's per-group momentum.
+    keeps per-parameter counts; ``momentum``: SGD's per-group momentum; ``group_k``: the schedule-free groups' ``k``.
 
     torch creates a parameter's state at its first step, so a parameter without an entry has taken 0 steps and has the
     initial scalar state (1.0).  torch's SGD keeps no ``step``: a parameter with a ``momentum_buffer`` has taken
@@ -302,7 +478,21 @@ def load_step_counts(kind, entries: List[Dict], group_of: List[int], opt_steps: 
     Returns ``(opt_steps, steps, scalars)``: the optimizer-wide count, then either per-parameter counts and per-parameter
     scalar state (``steps`` a list) or ``steps = None`` and per-group scalar state.  Counts go per parameter when they
     are not all the optimizer-wide count, when the scalar state differs within a group, or when ``per_param_on``.
-    ``scalars`` is None for the kinds without scalar state."""
+    ``scalars`` is None for the kinds without scalar state.
+
+    The schedule-free kinds keep no ``step``: k is the checkpoint's ``b200_opt_steps``, else the groups' common ``k``
+    (groups whose k differ raise ValueError), and a parameter has taken k steps if its entry has ``z``, 0 if not."""
+    if kind in _SF_KINDS:
+        if opt_steps is None:
+            ks = set(int(k) for k in (group_k or []))
+            if len(ks) > 1:
+                raise ValueError(f"Stoke -- schedule-free parameter groups with different step counts k: {sorted(ks)}")
+            opt_steps = ks.pop() if ks else 0
+        steps = [opt_steps if "z" in e else 0 for e in entries]
+        if per_param_on or any(s != opt_steps for s in steps):
+            return opt_steps, steps, None
+        return opt_steps, None, None
+
     def count(e, g):
         if kind != _lib.OPT_SGD:
             return int(float(e["step"])) if "step" in e else 0
@@ -358,7 +548,7 @@ class B200FusedOptimizer(torch.optim.Optimizer):
                  bucket_mb: Optional[float] = None):
         if optim_cls not in _KINDS:
             raise NotImplementedError(
-                f"Stoke -- the fused step covers torch.optim.Adam, AdamW, SGD, NAdam, RAdam, Adamax, Adadelta, Rprop, ASGD and Adafactor and stoke_b200.optim.LAMB, LARS and Lion; got {getattr(optim_cls, '__name__', optim_cls)}"
+                f"Stoke -- the fused step covers torch.optim.Adam, AdamW, SGD, NAdam, RAdam, Adamax, Adadelta, Rprop, ASGD and Adafactor and stoke_b200.optim.LAMB, LARS, Lion, AdamWScheduleFree and SGDScheduleFree; got {getattr(optim_cls, '__name__', optim_cls)}"
                 f" (use B200StockOptimizer / build_optimizer, which routes other classes to the stock-optimizer path)")
         params, group_of, extra, kw = _group_layout(module, optim_kwargs)
         if len(extra) > _lib.MAX_GROUPS:
@@ -380,7 +570,7 @@ class B200FusedOptimizer(torch.optim.Optimizer):
         ada = self._kind == _ADAFACTOR
         lw = self._kind in _LAYERWISE
         lars = self._kind == _LARS
-        one_state = self._kind in (_lib.OPT_ASGD, _lib.OPT_LION)   # a single fp32 state tensor, in M
+        one_state = self._kind in (_lib.OPT_ASGD, _lib.OPT_LION, _lib.OPT_SF_SGD)   # a single fp32 state tensor, in M
         if (ada or lw) and engine.world > 1:
             # Adafactor's per-parameter reductions and LAMB's / LARS's trust ratios need whole parameters on one rank: their
             # state is replicated (also under fairscale_oss) and every rank runs the same deterministic step on the same
@@ -390,7 +580,7 @@ class B200FusedOptimizer(torch.optim.Optimizer):
                              module=module, needs_second_moment=not (sgd or ada or lars or one_state),
                              needs_first_moment=not (sgd or ada or lars) or any_mom, state_id=state_id, route=route,
                              group_of=group_of, bucket_mb=bucket_mb, scalar_state=len(_SCALAR_KEYS.get(self._kind, ())),
-                             adafactor=ada, layerwise=lw)
+                             adafactor=ada, layerwise=lw, schedule_free=self._kind in _SF_KINDS)
         by_group: List[List[torch.nn.Parameter]] = [[] for _ in extra]
         for p, gi in zip(params, group_of):
             by_group[gi].append(p)
@@ -447,6 +637,17 @@ class B200FusedOptimizer(torch.optim.Optimizer):
     def _hypers(self) -> List[_lib.OptimHyper]:
         return [self._hyper_of(g) for g in self.param_groups]
 
+    def _sf_hypers(self) -> List[_lib.SfHyper]:
+        out = []
+        for g in self.param_groups:
+            x = _lib.SfHyper()
+            x.lr, x.beta1, x.r = float(g["lr"]), float(_sf_beta1(g)), float(g["r"])
+            x.weight_lr_power = float(g["weight_lr_power"])
+            x.beta2 = float(g["betas"][1]) if "betas" in g else 0.0
+            x.warmup_steps = int(g["warmup_steps"])
+            out.append(x)
+        return out
+
     def _exts(self) -> Optional[List[_lib.OptimHyperExt]]:
         if self._kind not in _EXT_KINDS:
             return None
@@ -472,7 +673,42 @@ class B200FusedOptimizer(torch.optim.Optimizer):
         if self._kind in _LAYERWISE:
             self.path.layerwise_step(_LAYERWISE[self._kind], [self._layerwise_hyper_of(g) for g in self.param_groups])
             return
+        if self._kind in _SF_KINDS:
+            self.check_train_mode()
+            self.path.optimizer_step(self._hypers(), None, self._sf_hypers())
+            return
         self.path.optimizer_step(self._hypers(), self._exts())
+
+    # -- schedule-free: train() / eval() ------------------------------------------------------------------------------------
+    def check_train_mode(self):
+        """Raises RuntimeError if a schedule-free optimizer is in eval mode (``Stoke.step`` asks before it runs anything)."""
+        if self._kind in _SF_KINDS:
+            _check_train_mode(self.param_groups)
+
+    def _sf_swap(self, to_train: bool):
+        if self._kind not in _SF_KINDS:
+            raise NotImplementedError("Stoke -- optimizer.train() / eval() swap the weights of AdamWScheduleFree and "
+                                      "SGDScheduleFree only")
+        path = self.path
+        if path.avg_owner is not None:
+            path.avg_owner._check_idle(f"optimizer.{'train' if to_train else 'eval'}()")
+        weights = {}
+        for gi, g in enumerate(self.param_groups):
+            if g["train_mode"] != to_train:
+                beta1 = _sf_beta1(g)
+                weights[gi] = 1 - beta1 if to_train else 1 - 1 / beta1
+        if weights:
+            path.schedule_free_swap([weights.get(gi) for gi in self._group_of])
+        for g in self.param_groups:
+            g["train_mode"] = to_train
+
+    def train(self):
+        """Schedule-free: the master (and the model's parameters) to y, where gradients are taken."""
+        self._sf_swap(True)
+
+    def eval(self):
+        """Schedule-free: the master (and the model's parameters) to x, the averaged point that is evaluated."""
+        self._sf_swap(False)
 
     def zero_grad(self, set_to_none: bool = True):
         """No-op: the gradient bucket is zeroed by the kernel that consumes it, and ``param.grad`` must stay a view of that
@@ -565,7 +801,7 @@ class B200FusedOptimizer(torch.optim.Optimizer):
                 continue
             if steps[i] == 0 and self._kind in _LAZY_KINDS:
                 continue
-            d = {"step": torch.tensor(float(steps[i]))}
+            d = {} if self._kind in _SF_KINDS else {"step": torch.tensor(float(steps[i]))}
             if scal is not None:
                 for key, val in zip(_SCALAR_KEYS[self._kind], scal[i]):
                     d[key] = torch.tensor(val, dtype=torch.float32)
@@ -573,7 +809,15 @@ class B200FusedOptimizer(torch.optim.Optimizer):
             if k_v is not None:
                 d[k_v] = vs[i].clone()
             state[j] = d
-        return self._export(state)
+        out = self._export(state)
+        if self._kind in _SF_KINDS:   # the running group state, read back from the device (one synchronisation)
+            k = out["b200_opt_steps"]
+            for g, src, (lr_max, weight_sum) in zip(out["param_groups"], self.param_groups, path._sf_state.tolist()):
+                vals = dict(k=k, lr_max=lr_max, weight_sum=weight_sum,
+                            scheduled_lr=_sf_scheduled_lr(src, k - 1) if k > 0 else src["scheduled_lr"])
+                g.update(vals)
+                src.update(vals)   # param_groups as of this state_dict(); reading them every step would synchronise
+        return out
 
     def load_state_dict(self, sd):
         """Accepts this class's own export and a plain ``torch.optim`` state dict written by the reference
@@ -587,6 +831,8 @@ class B200FusedOptimizer(torch.optim.Optimizer):
                     g[k] = val
         dev = path.p_flat.device
         entries = [sd["state"].get(self._sd_index[i], {}) for i in range(len(path.params))]
+        # the master this checkpoint continues from: its own, or (reference-written) the model weights already in P
+        master = sd["b200_master"].to(device=dev, dtype=torch.float32) if "b200_master" in sd else path.p_flat.float()
         if self._kind == _ADAFACTOR:
             for src, views in zip(entries, path.adafactor_state_views()):
                 keys = ("row_var", "col_var") if len(views) == 2 else ("variance",)
@@ -601,26 +847,30 @@ class B200FusedOptimizer(torch.optim.Optimizer):
             for local_dst, key in zip((path.m_flat, path.v_flat), keys):
                 if local_dst is None:
                     continue
-                full = torch.zeros(path.n, dtype=torch.float32, device=dev)
+                # schedule-free: a parameter without z has not been stepped, and its z is its master (upstream's clone)
+                full = master.clone() if key == "z" else torch.zeros(path.n, dtype=torch.float32, device=dev)
                 for view, src in zip(path.unflatten(full), entries):
                     if src.get(key) is not None:
                         view.copy_(src[key].to(device=dev, dtype=torch.float32))
                 path.scatter_local(full, local_dst)
         steps, per_param, scalars = load_step_counts(self._kind, entries, self._group_of, sd.get("b200_opt_steps"),
                                                      path._range_steps is not None,
-                                                     [g.get("momentum", 0.0) for g in self.param_groups])
+                                                     [g.get("momentum", 0.0) for g in self.param_groups],
+                                                     [g.get("k", 0) for g in self.param_groups])
+        if self._kind in _SF_KINDS:
+            path._sf_state.copy_(torch.tensor([[float(g["lr_max"]), float(g["weight_sum"])] for g in self.param_groups],
+                                              dtype=torch.float64))
         if per_param is not None:
             path.enable_per_param_steps(per_param, scalars)
         elif scalars is not None:
             path.set_group_scalars(scalars)
         if "b200_master" in sd:
-            master = sd["b200_master"].to(device=dev, dtype=torch.float32)
             if path.master_flat is not path.p_flat:
                 path.scatter_local(master, path.master_flat)
             path.p_flat.copy_(master)
         elif path.master_flat is not path.p_flat:
             # reference-written checkpoint: the model weights are already in P (model dtype); they are the best master
-            path.scatter_local(path.p_flat.float(), path.master_flat)
+            path.scatter_local(master, path.master_flat)
         path.engine.scaler_set(state=path.state_id, opt_steps=steps)
 
     def close(self):
@@ -654,8 +904,33 @@ class B200StockOptimizer(torch.optim.Optimizer):
         self.state = self.inner.state
         engine.scaler_set(state=path.state_id, opt_steps=0, skipped_steps=0, found_inf=0, growth_tracker=0)
 
+    def check_train_mode(self):
+        """Raises RuntimeError if a schedule-free optimizer is in eval mode (``Stoke.step`` asks before it runs anything)."""
+        if isinstance(self.inner, _ScheduleFree):
+            _check_train_mode(self.inner.param_groups)
+
+    def _sf_swap(self, to_train: bool):
+        if not isinstance(self.inner, _ScheduleFree):
+            raise NotImplementedError("Stoke -- optimizer.train() / eval() swap the weights of AdamWScheduleFree and "
+                                      "SGDScheduleFree only")
+        path = self.path
+        if path.avg_owner is not None:
+            path.avg_owner._check_idle(f"optimizer.{'train' if to_train else 'eval'}()")
+        self.inner.train() if to_train else self.inner.eval()
+        if path.master_flat is not path.p_flat:
+            path.p_flat.copy_(path.master_flat)   # fp32 -> model dtype, round-to-nearest-even
+
+    def train(self):
+        """Schedule-free: the inner optimizer's ``train()`` on the master, then the model's parameters from it."""
+        self._sf_swap(True)
+
+    def eval(self):
+        """Schedule-free: the inner optimizer's ``eval()`` on the master, then the model's parameters from it."""
+        self._sf_swap(False)
+
     @torch.no_grad()
     def step(self, closure=None):
+        self.check_train_mode()   # before the clip touches the gradients
         path, e = self.path, self.path.engine
         e.state_select(path.state_id)
         skip = False

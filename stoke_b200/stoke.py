@@ -229,6 +229,10 @@ class Stoke:
             self._weight_average._check_idle("step")
         if not self._check_accum():
             return
+        # a schedule-free optimizer in eval mode refuses the step before anything runs, the weight-average schedule included
+        check_train_mode = getattr(self._optimizer, "check_train_mode", None)
+        if check_train_mode is not None:
+            check_train_mode()
         if self._verbose and self.grad_accum > 0:
             self.print(f"Gradient Accumulation Steps: {self.grad_accum}")
         if self.grad_clip is not None:

@@ -62,6 +62,7 @@ class WeightAverage:
         self.n_averaged = 0
         self.active = False
         path.enable_weight_average()
+        path.avg_owner = self
         self._name_of = {id(p): name for name, p in module.named_parameters()}
         # fp32 copies of the floating buffers (use_buffers); non-floating buffers (num_batches_tracked) are the model's
         self._buffers: Dict[str, torch.Tensor] = {}
