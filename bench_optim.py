@@ -1,17 +1,19 @@
 # -*- coding: utf-8 -*-
 """torch.optim classes on the fused step, on one GPU, at ResNet-50 size (25.6 M elements) and BERT-base size
 (109.5 M elements), with Adam as the yardstick.  By default Adam, NAdam, RAdam and Adamax; ``--kinds`` picks others, e.g.
-``--kinds adadelta,rprop,asgd``, ``--kinds adam,lion`` (stoke_b200.Lion) or ``--kinds adam,sf_adamw,sgd,sf_sgd``
-(stoke_b200.AdamWScheduleFree and SGDScheduleFree against the kinds whose bytes they move):
+``--kinds adadelta,rprop,asgd``, ``--kinds adam,lion`` (stoke_b200.Lion), ``--kinds adam,sf_adamw,sgd,sf_sgd``
+(stoke_b200.AdamWScheduleFree and SGDScheduleFree against the kinds whose bytes they move) or ``--kinds adam,ademamix``
+(stoke_b200.AdEMAMix, Adam's step with a third state tensor):
 
   k_optim_step[raw]    the world-1 route: the step reads and zeroes the raw bf16 bucket and writes the bf16 model copy
                        (30 B/element algorithmic: read g 2, p m v 12; write p m v 12, bf16 copy 2, zeroing 2), with the
                        step prologue in front of it.  ASGD keeps one state tensor and, while mu == 1 (torch's default
                        t0 = 1e6), writes it without reading it: 18 B/element.  Lion keeps one state tensor, reads it
                        and runs without the prologue: 22 B/element.  SGD with momentum and schedule-free SGD keep one
-                       (momentum_buffer / z): 22 B/element; schedule-free AdamW keeps two like Adam: 30
+                       (momentum_buffer / z): 22 B/element; schedule-free AdamW keeps two like Adam: 30.  AdEMAMix
+                       keeps three (exp_avg_fast, exp_avg_slow, exp_avg_sq): 38 B/element
   k_optim_step[main]   fp32 model, fp32 main gradients (28 B/element: read g p m v 16, write p m v 12; ASGD 16, Lion, SGD
-                       and schedule-free SGD 20)
+                       and schedule-free SGD 20, AdEMAMix 36)
   optimizer step       gradient pass + step, the fused route (k_grad_norm + prologue + k_optim_step) against
                        B200StockOptimizer (K1 main-gradient reduce + the class's own update on fp32 views + the cast
                        into the bf16 model), same class, same gradients, timed in alternating rounds in the same run
@@ -55,10 +57,13 @@ CLASSES = {"adam": (torch.optim.Adam, {"lr": 1e-3}), "nadam": (torch.optim.NAdam
            "asgd": (torch.optim.ASGD, {"lr": 1e-2}), "lion": (stoke_b200.Lion, {"lr": 1e-4, "weight_decay": 0.1}),
            "sgd": (torch.optim.SGD, {"lr": 0.1, "momentum": 0.9}),
            "sf_adamw": (stoke_b200.AdamWScheduleFree, {"lr": 2.5e-3, "weight_decay": 0.01}),
-           "sf_sgd": (stoke_b200.SGDScheduleFree, {"lr": 1.0, "weight_decay": 1e-4})}
+           "sf_sgd": (stoke_b200.SGDScheduleFree, {"lr": 1.0, "weight_decay": 1e-4}),
+           "ademamix": (stoke_b200.AdEMAMix, {"lr": 1e-3, "alpha": 5.0, "alpha_warmup": 100_000,
+                                              "beta3_warmup": 100_000, "weight_decay": 0.01})}
 # algorithmic bytes per element (raw bf16 route, main fp32 route) of the kinds with one state tensor; the others: 30, 28
 ONE_STATE_BYTES = {"asgd": (18, 16),   # ax written without being read while mu == 1
                    "lion": (22, 20), "sgd": (22, 20), "sf_sgd": (22, 20)}
+THREE_STATE_BYTES = {"ademamix": (38, 36)}   # the first and second moments plus exp_avg_slow
 SCHEDULE_FREE = ("sf_adamw", "sf_sgd")   # a new optimizer is in eval mode: train() before stepping
 
 
@@ -116,7 +121,7 @@ def main():
         flush_l2 = n < 60_000_000
         for tag, cls, kw in classes:
             # ---- the kernel alone, both gradient sources ----
-            raw_b, main_b = ONE_STATE_BYTES.get(tag, (30, 28))
+            raw_b, main_b = ONE_STATE_BYTES.get(tag, THREE_STATE_BYTES.get(tag, (30, 28)))
             for route, lp, per in (("local", torch.bfloat16, raw_b), ("main", None, main_b)):
                 net = Flat(n).cuda()
                 opt = B200FusedOptimizer(net, cls, kw, engine=eng, route=route, clip=clip, lp_dtype=lp)

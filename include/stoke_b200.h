@@ -90,8 +90,12 @@ typedef enum {
   STK_OPT_SF_ADAMW = 10,  /* stoke_b200.optim.AdamWScheduleFree (Defazio et al. 2024); exp_avg = z, exp_avg_sq = exp_avg_sq.
                              Reads beta2, eps and weight_decay of stk_optim_hyper_t; the rest from group_bc
                              (stk_sf_step_prologue) */
-  STK_OPT_SF_SGD = 11     /* stoke_b200.optim.SGDScheduleFree; exp_avg = z, no exp_avg_sq.  Reads weight_decay of
+  STK_OPT_SF_SGD = 11,    /* stoke_b200.optim.SGDScheduleFree; exp_avg = z, no exp_avg_sq.  Reads weight_decay of
                              stk_optim_hyper_t; the rest from group_bc (stk_sf_step_prologue) */
+  STK_OPT_ADEMAMIX = 12   /* stoke_b200.optim.AdEMAMix (Pagliardini et al. 2024); exp_avg = exp_avg_fast (not read or
+                             written in a group with beta1 == 0), exp_avg_sq = exp_avg_sq, exp_avg_slow = exp_avg_slow.
+                             Reads lr, beta1, beta2, eps and weight_decay of stk_optim_hyper_t; the per-step scalars from
+                             group_bc / range_bc of stk_ademamix_step_prologue */
 } stk_optim_kind;
 
 /* flags of stk_grad_reduce */
@@ -300,6 +304,8 @@ typedef struct {
                              The schedule-free kinds need group_bc from stk_sf_step_prologue and ignore range_bc: their
                              step count and scalars belong to the group, not to the parameter.  SF_SGD takes no
                              exp_avg_sq */
+  float* exp_avg_slow;    /* ADEMAMIX only (required there): the third fp32 state tensor, indexed like exp_avg.  ADEMAMIX
+                             also needs exp_avg_sq, and exp_avg unless every group has beta1 == 0 */
 } stk_optim_args_t;
 int stk_optim_step_ex(stk_ctx* ctx, const stk_optim_args_t* args, void* stream);
 
@@ -365,6 +371,29 @@ typedef struct {
  *   z = fma(-lr, d, z) */
 int stk_sf_step_prologue(stk_ctx* ctx, const stk_sf_hyper_t* hyper, int n_groups, double* group_state, float* bc,
                          void* stream);
+
+/* Per-group hyper-parameters of AdEMAMix that stk_optim_hyper_t has no field for (apple/ml-ademamix's arguments).  A
+ * warm-up of 0 means none (upstream's None). */
+typedef struct {
+  double alpha, beta3;
+  int64_t alpha_warmup, beta3_warmup;
+} stk_ademamix_hyper_t;
+/* The per-step scalars of STK_OPT_ADEMAMIX, with stk_optim_step_prologue's range / group / found_inf semantics (call it
+ * right before stk_optim_step_ex, same stream; pass bc as the step's range_bc when n_ranges > 0, else as its group_bc).
+ * With t the entry's step count after this step, in double in the order of the python formulas (no contraction):
+ *   bc1 = 1 - beta1^t;  bc2 = 1 - beta2^t
+ *   alpha_t = (t / alpha_warmup) alpha if alpha_warmup > 0 and t < alpha_warmup, else alpha
+ *   f(b) = log(0.5) / log(b + 1e-8) - 1;  f_inv(x) = 0.5^(1 / (x + 1));  a = t / beta3_warmup
+ *   beta3_t = f_inv((1 - a) f(beta1) + a f(beta3)) if beta3_warmup > 0 and t < beta3_warmup, else beta3
+ *   bc[4j..4j+3] = fp32 {1 / bc1, 1 / sqrt(bc2), alpha_t, 1 - beta3_t}
+ * beta1 and beta2 come from hyper (stk_optim_hyper_t), the rest from ademamix.  The update of one element with the formed
+ * gradient g, m1 = exp_avg, m2 = exp_avg_slow, v = exp_avg_sq (lerp: torch's fp32 lerp, see stk_weight_avg):
+ *   m1 = lerp(m1, g, 1 - beta1) (beta1 == 0: m1 = g, the buffer untouched);  m2 = lerp(m2, g, bc.w)
+ *   v = fma(1 - beta2, g * g, v * beta2);  u = fma(m2, bc.z, m1 * bc.x) / (sqrt(v) * bc.y + eps)
+ *   u = fma(p, wd, u) if wd != 0;  p = fma(-lr, u, p) */
+int stk_ademamix_step_prologue(stk_ctx* ctx, const stk_optim_hyper_t* hyper, const stk_ademamix_hyper_t* ademamix,
+                               int n_groups, int n_ranges, const uint8_t* range_group, int32_t* range_steps, float* bc,
+                               void* stream);
 
 /* scaler.update(), opt_steps/skipped_steps bookkeeping, reset of the per-step accumulators */
 int stk_step_epilogue(stk_ctx* ctx, void* stream);

@@ -1,6 +1,7 @@
 // k2_optim.cu -- K2: single-pass fused optimizer step (Adam / AdamW / SGD-momentum / NAdam / RAdam / Adamax / Adadelta /
-// Rprop / ASGD / Lion / schedule-free AdamW and SGD), plus the step prologues (per-parameter step counts, NAdam's
-// mu_product, ASGD's eta and mu; the schedule-free group scalars) and epilogue.
+// Rprop / ASGD / Lion / schedule-free AdamW and SGD / AdEMAMix), plus the step prologues (per-parameter step counts,
+// NAdam's mu_product, ASGD's eta and mu; the schedule-free group scalars; AdEMAMix's bias corrections and warm-ups) and
+// epilogue.
 //
 // One sweep over (grad, master, exp_avg, exp_avg_sq) does what the reference spreads over clip_grad_norm_'s scaling pass /
 // clip_grad_value_, GradScaler.step's inf gate, the ~7 foreach kernels of torch.optim.Adam and (mixed precision) the
@@ -10,7 +11,9 @@
 // Rprop keep two fp32 state tensors like Adam; Adamax's exp_inf, Adadelta's acc_delta and Rprop's step_size live in the
 // exp_avg_sq buffer).  ASGD keeps one (ax, in exp_avg): read g,p,ax + write p,ax = 20 / 22, and 16 / 18 while mu == 1,
 // when ax is written without being read.  Lion keeps one (exp_avg) and reads it: 20 / 22.  Schedule-free AdamW keeps
-// z (exp_avg) and exp_avg_sq like Adam: 28 / 30; schedule-free SGD keeps z only: 20 / 22.  The clip coefficient, the
+// z (exp_avg) and exp_avg_sq like Adam: 28 / 30; schedule-free SGD keeps z only: 20 / 22.  AdEMAMix keeps a third
+// tensor (exp_avg_slow, in m2) besides exp_avg_fast and exp_avg_sq: 36 / 38, and 28 / 30 in a group with beta1 == 0,
+// which neither reads nor writes exp_avg_fast.  The clip coefficient, the
 // skip decision and the bias corrections come from device memory, so there is no host synchronisation anywhere on the
 // step.
 //
@@ -25,8 +28,9 @@
 // Arithmetic follows torch/optim/adam.py (_single_tensor_adam, the path torch takes on CPU -- the oracle),
 // torch/optim/sgd.py (_single_tensor_sgd), nadam.py (_single_tensor_nadam), radam.py (_single_tensor_radam), adamax.py
 // (_single_tensor_adamax), adadelta.py (_single_tensor_adadelta), rprop.py (_single_tensor_rprop) and asgd.py
-// (_single_tensor_asgd); Lion follows stoke_b200.optim.Lion.step (torch has no Lion) and the schedule-free kinds
-// stoke_b200.optim.AdamWScheduleFree.step / SGDScheduleFree.step, each rounded like those steps on CUDA; the clip follows
+// (_single_tensor_asgd); Lion follows stoke_b200.optim.Lion.step (torch has no Lion), the schedule-free kinds
+// stoke_b200.optim.AdamWScheduleFree.step / SGDScheduleFree.step and AdEMAMix stoke_b200.optim.AdEMAMix.step, each
+// rounded like those steps on CUDA; the clip follows
 // torch/nn/utils/clip_grad.py:165-174 (coef = max_norm / (total_norm + 1e-6), clamped to 1) and :291-292 (clamp).
 #include <cstdlib>
 
@@ -52,10 +56,12 @@ struct GroupHyperS {   // what the inner loop reads (shared memory, one entry pe
   union {
     float rho;                                  // Adadelta
     float b1;                                   // Lion
+    int no_m1;                                  // AdEMAMix: beta1 == 0, exp_avg_fast is the gradient (no state)
   };
   union {
     float one_m_rho;                            // Adadelta
-    float c3;                                   // schedule-free AdamW: the fourth group scalar, fp32(1 / bc2)
+    float c3;                                   // the fourth per-step scalar: schedule-free AdamW's fp32(1 / bc2),
+                                                // AdEMAMix's 1 - beta3_t
   };
   float etaminus, etaplus, ss_min, ss_max;      // Rprop
 };
@@ -92,6 +98,9 @@ struct OptimParams {
   const uint8_t* range_group;                // device; bit 7: skip
   const float4* range_bc;                    // device, optional: per-range scalars of stk_optim_step_prologue
   const float4* group_bc;                    // device, optional: per-group scalars of stk_optim_step_prologue
+  // appended, so that the fields above keep their offsets (and the other kinds their code)
+  float* m2;                                 // AdEMAMix: exp_avg_slow
+  int m_deferred;                            // AdEMAMix: some group has beta1 == 0, so m is loaded once the range is known
 };
 
 // floats of per-entry scalar state the prologue carries (the stk_optim_step_prologue `scalar_state` array)
@@ -221,13 +230,16 @@ __global__ void __launch_bounds__(256, KIND >= STK_OPT_NADAM ? 2 : 0) k_optim_st
   unsigned long long t_begin = 0;
   if (PERSIST && p.prof_ns && blockIdx.x == 0 && threadIdx.x == 0) t_begin = globaltimer_ns();
 
-  const bool use_m = (KIND != STK_OPT_SGD) || p.m != nullptr;
+  // SGD without momentum and AdEMAMix with beta1 == 0 in every group have no m
+  const bool use_m = (KIND != STK_OPT_SGD && KIND != STK_OPT_ADEMAMIX) || p.m != nullptr;
   // ASGD, Lion and schedule-free SGD: one state tensor (ax / exp_avg / z, in p.m)
   constexpr bool kHasV = KIND != STK_OPT_SGD && KIND != STK_OPT_ASGD && KIND != STK_OPT_LION && KIND != STK_OPT_SF_SGD;
+  constexpr bool kHasM2 = KIND == STK_OPT_ADEMAMIX;
   const size_t stride = PERSIST ? size_t(gridDim.x) * blockDim.x * VPT : 0;
   size_t i = (size_t(blockIdx.x) * blockDim.x + threadIdx.x) * VPT;
 
   float g[VPT][8], w[VPT][8], m[VPT][8], v[VPT][8];
+  float m2[kHasM2 ? VPT : 1][8];
   size_t gv = 0;
   int nv = 0;
   auto load = [&]() {
@@ -242,8 +254,11 @@ __global__ void __launch_bounds__(256, KIND >= STK_OPT_NADAM ? 2 : 0) k_optim_st
         if constexpr (RAW) InVec<GRAD>::load(p.grad, gv + k, g[k]);
         else InVec<STK_F32>::load(p.grad, i + k, g[k]);
         InVec<STK_F32>::load(p.master, i + k, w[k]);
-        if (use_m && KIND != STK_OPT_ASGD) InVec<STK_F32>::load(p.m, i + k, m[k]);  // ASGD: ax only when mu != 1
+        // ASGD: ax only when mu != 1; AdEMAMix with a beta1 == 0 group: m only where beta1 != 0
+        if (use_m && KIND != STK_OPT_ASGD && !(KIND == STK_OPT_ADEMAMIX && p.m_deferred))
+          InVec<STK_F32>::load(p.m, i + k, m[k]);
         if (kHasV) InVec<STK_F32>::load(p.v, i + k, v[k]);
+        if constexpr (kHasM2) InVec<STK_F32>::load(p.m2, i + k, m2[k]);
       }
     if constexpr (RAW) {
       if (p.acc != nullptr) {
@@ -298,7 +313,8 @@ __global__ void __launch_bounds__(256, KIND >= STK_OPT_NADAM ? 2 : 0) k_optim_st
       o.ss_max = (float)h.step_size_max;
     }
     if constexpr (KIND == STK_OPT_LION) o.b1 = (float)h.beta1;
-    if constexpr (KIND == STK_OPT_SF_ADAMW || KIND == STK_OPT_SF_SGD) o.c3 = c.w;
+    if constexpr (KIND == STK_OPT_SF_ADAMW || KIND == STK_OPT_SF_SGD || KIND == STK_OPT_ADEMAMIX) o.c3 = c.w;
+    if constexpr (KIND == STK_OPT_ADEMAMIX) o.no_m1 = h.beta1 == 0.0;
     s_g[threadIdx.x] = o;
   }
   __syncthreads();
@@ -320,6 +336,7 @@ __global__ void __launch_bounds__(256, KIND >= STK_OPT_NADAM ? 2 : 0) k_optim_st
       h.c0 = bc.x;
       h.c1 = bc.y;
       h.c2 = bc.z;
+      if constexpr (KIND == STK_OPT_ADEMAMIX) h.c3 = bc.w;
     }
     const bool skip = skip_all || (rb & 0x80u);
     if (!skip) {
@@ -328,6 +345,9 @@ __global__ void __launch_bounds__(256, KIND >= STK_OPT_NADAM ? 2 : 0) k_optim_st
         if (k >= nv) continue;
         if constexpr (KIND == STK_OPT_ASGD) {  // ax is only read when it is averaged (torch: mu.item() != 1)
           if (h.c2 != 1.f) InVec<STK_F32>::load(p.m, i + k, m[k]);
+        }
+        if constexpr (KIND == STK_OPT_ADEMAMIX) {  // exp_avg_fast does not exist in a beta1 == 0 group
+          if (p.m_deferred && !h.no_m1) InVec<STK_F32>::load(p.m, i + k, m[k]);
         }
 #pragma unroll
         for (int e = 0; e < 8; ++e) {
@@ -427,6 +447,21 @@ __global__ void __launch_bounds__(256, KIND >= STK_OPT_NADAM ? 2 : 0) k_optim_st
             ww = lerp_torch(ww, m[k][e], h.c0);                      // y.lerp_(z, ckp1)
             ww = fmaf(h.c1, d, ww);                                  // y.add_(d, alpha=lr (beta1 (1 - ckp1) - 1))
             m[k][e] = fmaf(-h.c2, d, m[k][e]);                       // z.sub_(d, alpha=lr)
+          } else if (KIND == STK_OPT_ADEMAMIX) {
+            // per-step scalars (k_ademamix_prologue): c0 = 1 / bc1, c1 = 1 / sqrt(bc2), c2 = alpha_t, c3 = 1 - beta3_t
+            const float mf = h.no_m1 ? gg : lerp_torch(m[k][e], gg, h.one_m_b1);  // exp_avg_fast.lerp_(g, 1 - beta1)
+            const float ms = lerp_torch(m2[k][e], gg, h.c3);                     // exp_avg_slow.lerp_(g, 1 - beta3_t)
+            // exp_avg_sq.mul_(beta2).addcmul_(g, g, value=1 - beta2): torch's CUDA addcmul rounds g * g first
+            const float vv = fmaf(h.one_m_b2, __fmul_rn(gg, gg), __fmul_rn(v[k][e], h.b2));
+            // exp_avg_sq.sqrt().mul_(1 / sqrt(bc2)).add_(eps)
+            const float den = __fadd_rn(__fmul_rn(__fsqrt_rn(vv), h.c1), h.eps);
+            // exp_avg_fast.mul(1 / bc1).add_(exp_avg_slow, alpha=alpha_t).div_(denom): add(alpha) is one FFMA
+            float u = __fdiv_rn(fmaf(ms, h.c2, __fmul_rn(mf, h.c0)), den);
+            if (h.wd != 0.f) u = fmaf(ww, h.wd, u);                   // u.add_(p, alpha=weight_decay)
+            ww = fmaf(-h.lr, u, ww);                                 // p.add_(u, alpha=-lr)
+            m[k][e] = mf;
+            m2[k][e] = ms;
+            v[k][e] = vv;
           } else {  // SGD
             if (h.wd != 0.f) gg = fmaf(ww, h.wd, gg);
             if (h.mom != 0.f) {
@@ -443,8 +478,10 @@ __global__ void __launch_bounds__(256, KIND >= STK_OPT_NADAM ? 2 : 0) k_optim_st
       for (int k = 0; k < VPT; ++k)
         if (k < nv) {
           st_stream_f8(p.master + (i + k) * 8, w[k]);
-          if (use_m && (KIND != STK_OPT_SGD || p.any_mom)) st_stream_f8(p.m + (i + k) * 8, m[k]);
+          if (use_m && (KIND != STK_OPT_SGD || p.any_mom) && !(KIND == STK_OPT_ADEMAMIX && h.no_m1))
+            st_stream_f8(p.m + (i + k) * 8, m[k]);
           if (kHasV) st_stream_f8(p.v + (i + k) * 8, v[k]);
+          if constexpr (kHasM2) st_stream_f8(p.m2 + (i + k) * 8, m2[k]);
         }
       store_lp<LP_DT, VPT>(p, gv, w, nv);
     }
@@ -475,23 +512,85 @@ struct StepPrologueParams {
   const stk_scaler_state_t* scaler;
 };
 
-// one thread per range (n_ranges > 0) or per group (n_ranges == 0): the scalars of that entry's NEXT step and, unless it is
-// skipped or the step is (found_inf), the advance of its step count (torch increments state[p]["step"] only for
-// parameters that are stepped) and of its scalar state (NAdam's mu_product, ASGD's eta and mu)
+// The step-count bookkeeping every prologue shares: one thread per range (n_ranges > 0) or per group (n_ranges == 0).
+// The entry's group, the steps it has taken (its own count, or the optimizer-wide one), and whether this step advances it:
+// not when the range is skipped or the step found inf (torch increments state[p]["step"] only for parameters that are
+// stepped).  False when the thread has no entry.
+struct StepEntry {
+  int j;
+  unsigned group;
+  int64_t done;
+  bool advance, per_range;
+};
+__device__ __forceinline__ bool step_entry(int n_groups, int n_ranges, const uint8_t* range_group,
+                                           const int32_t* range_steps, const stk_scaler_state_t* scaler, StepEntry& e) {
+  e.j = blockIdx.x * blockDim.x + threadIdx.x;
+  e.per_range = n_ranges > 0;
+  if (e.j >= (e.per_range ? n_ranges : n_groups)) return false;
+  const unsigned b = e.per_range ? (unsigned)range_group[e.j] : (unsigned)e.j;
+  e.group = b & 0x7f;
+  e.done = e.per_range ? (int64_t)range_steps[e.j] : scaler->opt_steps;
+  e.advance = !(b & 0x80u) && scaler->found_inf == 0;
+  return true;
+}
+// after an advancing step: the entry's own count moves (the optimizer-wide one is the epilogue's)
+__device__ __forceinline__ void step_entry_advance(const StepEntry& e, int32_t* range_steps) {
+  if (e.per_range) range_steps[e.j] = (int32_t)(e.done + 1);
+}
+
+// the scalars of each entry's NEXT step and, when it advances, its step count and scalar state (NAdam's mu_product,
+// ASGD's eta and mu)
 __global__ void k_step_prologue(const StepPrologueParams p) {
-  const int j = blockIdx.x * blockDim.x + threadIdx.x;
-  const bool per_range = p.n_ranges > 0;
-  if (j >= (per_range ? p.n_ranges : p.n_groups)) return;
-  const unsigned b = per_range ? (unsigned)p.range_group[j] : (unsigned)j;
-  const int64_t done = per_range ? (int64_t)p.range_steps[j] : p.scaler->opt_steps;
-  const bool advance = !(b & 0x80u) && p.scaler->found_inf == 0;
+  StepEntry e;
+  if (!step_entry(p.n_groups, p.n_ranges, p.range_group, p.range_steps, p.scaler, e)) return;
+  const int j = e.j;
   const int w = scalar_state_width(p.kind);
   float st[2] = {1.f, 1.f};
   for (int k = 0; k < w; ++k) st[k] = p.scalar_state[j * w + k];
-  p.bc[j] = step_scalars(p.kind, p.g[b & 0x7f], (double)(done + 1), st);
-  if (!advance) return;
+  p.bc[j] = step_scalars(p.kind, p.g[e.group], (double)(e.done + 1), st);
+  if (!e.advance) return;
   for (int k = 0; k < w; ++k) p.scalar_state[j * w + k] = st[k];
-  if (per_range) p.range_steps[j] = (int32_t)(done + 1);
+  step_entry_advance(e, p.range_steps);
+}
+
+struct AdemamixPrologueParams {
+  double beta1[STK_MAX_GROUPS], beta2[STK_MAX_GROUPS];
+  stk_ademamix_hyper_t a[STK_MAX_GROUPS];
+  int n_groups, n_ranges;
+  const uint8_t* range_group;
+  int32_t* range_steps;
+  float4* bc;
+  const stk_scaler_state_t* scaler;
+};
+
+// apple/ml-ademamix's half-life map of the beta3 warm-up: f(b) = log(0.5) / log(b + 1e-8) - 1
+__device__ __forceinline__ double ademamix_f(double b) {
+  return __dadd_rn(__ddiv_rn(log(0.5), log(__dadd_rn(b, 1e-8))), -1.0);
+}
+
+// AdEMAMix.step's per-step scalars of step t, in python doubles and python's order (the explicit roundings keep nvcc
+// from contracting a * b + c into one DFMA, which python does not do):  {1 / bc1, 1 / sqrt(bc2), alpha_t, 1 - beta3_t}
+__device__ __forceinline__ float4 ademamix_scalars(double beta1, double beta2, const stk_ademamix_hyper_t& h, double t) {
+  const double bc1 = __dadd_rn(1.0, -pow(beta1, t));
+  const double bc2 = __dadd_rn(1.0, -pow(beta2, t));
+  double alpha_t = h.alpha;
+  if (h.alpha_warmup > 0 && t < (double)h.alpha_warmup) alpha_t = __dmul_rn(__ddiv_rn(t, (double)h.alpha_warmup), h.alpha);
+  double beta3_t = h.beta3;
+  if (h.beta3_warmup > 0 && t < (double)h.beta3_warmup) {
+    const double a = __ddiv_rn(t, (double)h.beta3_warmup);
+    const double x = __dadd_rn(__dmul_rn(__dadd_rn(1.0, -a), ademamix_f(beta1)), __dmul_rn(a, ademamix_f(h.beta3)));
+    beta3_t = pow(0.5, __ddiv_rn(1.0, __dadd_rn(x, 1.0)));   // f_inv(x) = 0.5 ** (1 / (x + 1))
+  }
+  return make_float4((float)__ddiv_rn(1.0, bc1), (float)__ddiv_rn(1.0, __dsqrt_rn(bc2)), (float)alpha_t,
+                     (float)__dadd_rn(1.0, -beta3_t));
+}
+
+// stk_optim_step_prologue's bookkeeping with AdEMAMix's scalars (no scalar state)
+__global__ void k_ademamix_prologue(const AdemamixPrologueParams p) {
+  StepEntry e;
+  if (!step_entry(p.n_groups, p.n_ranges, p.range_group, p.range_steps, p.scaler, e)) return;
+  p.bc[e.j] = ademamix_scalars(p.beta1[e.group], p.beta2[e.group], p.a[e.group], (double)(e.done + 1));
+  if (e.advance) step_entry_advance(e, p.range_steps);
 }
 
 struct SfPrologueParams {
@@ -628,21 +727,26 @@ int stk_optim_step_ex(stk_ctx* c, const stk_optim_args_t* a, void* stream) {
   STK_REQUIRE(c, a->n_groups >= 1 && a->n_groups <= STK_MAX_GROUPS, "stk_optim_step_ex: n_groups must be in [1, 8]");
   STK_REQUIRE(c, a->n_local % 8 == 0, "stk_optim_step_ex: n_local must be a multiple of 8");
   const stk_optim_hyper_t* h = a->hyper;
-  STK_REQUIRE(c, h->kind >= STK_OPT_ADAM && h->kind <= STK_OPT_SF_SGD, "stk_optim_step_ex: bad optimizer kind");
+  STK_REQUIRE(c, h->kind >= STK_OPT_ADAM && h->kind <= STK_OPT_ADEMAMIX, "stk_optim_step_ex: bad optimizer kind");
   const bool sf = h->kind == STK_OPT_SF_ADAMW || h->kind == STK_OPT_SF_SGD;
+  const bool ademamix = h->kind == STK_OPT_ADEMAMIX;
   STK_REQUIRE(c, !sf || a->group_bc, "stk_optim_step_ex: the schedule-free kinds need group_bc of stk_sf_step_prologue");
   STK_REQUIRE(c, h->kind <= STK_OPT_SGD || h->kind == STK_OPT_LION || a->group_bc || (a->n_ranges > 0 && a->range_bc),
               "stk_optim_step_ex: the kinds after SGD need the scalars of stk_optim_step_prologue (group_bc or range_bc)");
   STK_REQUIRE(c, (reinterpret_cast<uintptr_t>(a->group_bc) & 15) == 0, "stk_optim_step_ex: group_bc must be 16-byte aligned");
-  STK_REQUIRE(c, h->kind == STK_OPT_SGD ||
+  STK_REQUIRE(c, h->kind == STK_OPT_SGD || ademamix ||
                      (a->exp_avg && (a->exp_avg_sq || h->kind == STK_OPT_ASGD || h->kind == STK_OPT_LION ||
                                      h->kind == STK_OPT_SF_SGD)),
               "stk_optim_step_ex: this kind needs exp_avg and exp_avg_sq (ASGD, Lion, SF_SGD: exp_avg)");
-  bool any_mom = false;
+  bool any_mom = false, any_b1 = false, any_b1_zero = false;
   for (int gi = 0; gi < a->n_groups; ++gi) {
     STK_REQUIRE(c, h[gi].kind == h->kind, "stk_optim_step_ex: all groups must use the same optimizer kind");
     any_mom |= h[gi].momentum != 0.0;
+    any_b1 |= h[gi].beta1 != 0.0;
+    any_b1_zero |= h[gi].beta1 == 0.0;
   }
+  STK_REQUIRE(c, !ademamix || (a->exp_avg_slow && a->exp_avg_sq && (a->exp_avg || !any_b1)),
+              "stk_optim_step_ex: ADEMAMIX needs exp_avg_slow, exp_avg_sq and (unless every group has beta1 == 0) exp_avg");
   STK_REQUIRE(c, !(h->kind == STK_OPT_SGD && any_mom && !a->exp_avg), "stk_optim_step_ex: SGD momentum needs a buffer");
   STK_REQUIRE(c, a->lp_ptrs == nullptr || a->lp_world == 1 || a->lp_world == c->world, "stk_optim_step_ex: lp_world must be 1 or world");
   STK_REQUIRE(c, a->lp_ptrs == nullptr || a->lp_dtype == STK_BF16 || a->lp_dtype == STK_F32, "stk_optim_step_ex: lp dtype");
@@ -723,6 +827,8 @@ int stk_optim_step_ex(stk_ctx* c, const stk_optim_args_t* a, void* stream) {
   // the schedule-free scalars belong to the group (upstream keeps k per group), whatever the range table says
   p.range_bc = (a->n_ranges > 0 && !sf) ? reinterpret_cast<const float4*>(a->range_bc) : nullptr;
   p.group_bc = reinterpret_cast<const float4*>(a->group_bc);
+  p.m2 = ademamix ? a->exp_avg_slow : nullptr;
+  p.m_deferred = (ademamix && a->exp_avg && any_b1_zero) ? 1 : 0;
   if (a->grad_raw) {
     // 1/loss_scale is applied when the scaler is live; the device flag decides (enabled), so no host read
     p.unscale = 1;
@@ -751,6 +857,7 @@ int stk_optim_step_ex(stk_ctx* c, const stk_optim_args_t* a, void* stream) {
     case STK_OPT_LION: err = launch_optim<STK_OPT_LION>(c, p, a->lp_dtype, a->grad_dtype, raw, pair_ok, s); break;
     case STK_OPT_SF_ADAMW: err = launch_optim<STK_OPT_SF_ADAMW>(c, p, a->lp_dtype, a->grad_dtype, raw, pair_ok, s); break;
     case STK_OPT_SF_SGD: err = launch_optim<STK_OPT_SF_SGD>(c, p, a->lp_dtype, a->grad_dtype, raw, pair_ok, s); break;
+    case STK_OPT_ADEMAMIX: err = launch_optim<STK_OPT_ADEMAMIX>(c, p, a->lp_dtype, a->grad_dtype, raw, pair_ok, s); break;
     default: err = launch_optim<STK_OPT_SGD>(c, p, a->lp_dtype, a->grad_dtype, raw, pair_ok, s); break;
   }
   if (err == cudaErrorNotSupported)
@@ -804,6 +911,36 @@ int stk_optim_step_prologue(stk_ctx* c, const stk_optim_hyper_t* h, const stk_op
   p.scaler = c->scaler_dev;
   const int n = n_ranges > 0 ? n_ranges : n_groups;
   k_step_prologue<<<(n + 127) / 128, 128, 0, reinterpret_cast<cudaStream_t>(stream)>>>(p);
+  STK_CUDA(c, cudaGetLastError());
+  return STK_OK;
+}
+
+int stk_ademamix_step_prologue(stk_ctx* c, const stk_optim_hyper_t* h, const stk_ademamix_hyper_t* ah, int n_groups,
+                               int n_ranges, const uint8_t* range_group, int32_t* range_steps, float* bc, void* stream) {
+  STK_REQUIRE(c, c && h && ah && bc, "stk_ademamix_step_prologue: NULL argument");
+  STK_REQUIRE(c, n_groups >= 1 && n_groups <= STK_MAX_GROUPS, "stk_ademamix_step_prologue: n_groups must be in [1, 8]");
+  STK_REQUIRE(c, n_ranges >= 0, "stk_ademamix_step_prologue: negative n_ranges");
+  STK_REQUIRE(c, n_ranges == 0 || (range_group && range_steps), "stk_ademamix_step_prologue: range arrays are NULL");
+  STK_REQUIRE(c, (reinterpret_cast<uintptr_t>(bc) & 15) == 0, "stk_ademamix_step_prologue: bc must be 16-byte aligned");
+  for (int gi = 0; gi < n_groups; ++gi)
+    STK_REQUIRE(c, ah[gi].alpha_warmup >= 0 && ah[gi].beta3_warmup >= 0,
+                "stk_ademamix_step_prologue: warm-ups must be >= 0 (0: none)");
+  std::lock_guard<std::mutex> lk(c->mu);
+  DeviceGuard g(c->device);
+  AdemamixPrologueParams p{};
+  for (int gi = 0; gi < n_groups; ++gi) {
+    p.beta1[gi] = h[gi].beta1;
+    p.beta2[gi] = h[gi].beta2;
+    p.a[gi] = ah[gi];
+  }
+  p.n_groups = n_groups;
+  p.n_ranges = n_ranges;
+  p.range_group = range_group;
+  p.range_steps = range_steps;
+  p.bc = reinterpret_cast<float4*>(bc);
+  p.scaler = c->scaler_dev;
+  const int n = n_ranges > 0 ? n_ranges : n_groups;
+  k_ademamix_prologue<<<(n + 127) / 128, 128, 0, reinterpret_cast<cudaStream_t>(stream)>>>(p);
   STK_CUDA(c, cudaGetLastError());
   return STK_OK;
 }

@@ -479,6 +479,8 @@ class GradPath:
                                                                               | absent (local route)
       MASTER fp32 master weights                               local          aliases P when the model is fp32 and unsharded
       M, V   fp32 optimizer state                              local          owned shards (sharded) | all n
+      M2     fp32 third optimizer state (AdEMAMix's            local          indexed like M; only for that kind
+             exp_avg_slow)                                                    (``third_state``)
       AVG    fp32 weight average (EMA / SWA)                   local          indexed like MASTER; only when averaging is
                                                                               configured (``enable_weight_average``)
 
@@ -493,7 +495,8 @@ class GradPath:
                  module: Optional[torch.nn.Module] = None, sync_init: bool = True, needs_second_moment: bool = True,
                  needs_first_moment: bool = True, bucket_mb: Optional[float] = None, state_id: Optional[int] = None,
                  route: Optional[str] = None, group_of: Optional[Sequence[int]] = None, overlap: bool = True,
-                 scalar_state: int = 0, adafactor: bool = False, layerwise: bool = False, schedule_free: bool = False):
+                 scalar_state: int = 0, adafactor: bool = False, layerwise: bool = False, schedule_free: bool = False,
+                 third_state: bool = False):
         self.engine = engine
         self.params = [p for p in params if p.requires_grad]
         if not self.params:
@@ -584,12 +587,14 @@ class GradPath:
         self.MASTER = alloc(nl * 4) if separate_master else None
         self.M = alloc(nl * 4) if needs_first_moment else None
         self.V = alloc(nl * 4) if needs_second_moment else None
+        self.M2 = alloc(nl * 4) if third_state else None
 
         self.p_flat = self.P.tensor(self.model_dtype, self.n)
         self.g_flat = self.G.tensor(self.model_dtype, self.n)
         self.main_flat = self.MAIN.tensor(torch.float32, self.n_local) if self.MAIN else None
         self.m_flat = self.M.tensor(torch.float32, self.n_local) if self.M else None
         self.v_flat = self.V.tensor(torch.float32, self.n_local) if self.V else None
+        self.m2_flat = self.M2.tensor(torch.float32, self.n_local) if self.M2 else None
         self.p_flat.copy_(full32)  # round-to-nearest-even, same as the kernel's cast
         if separate_master:
             self.master_flat = self.MASTER.tensor(torch.float32, self.n_local)
@@ -886,12 +891,14 @@ class GradPath:
         """Sets the per-group scalar state (checkpoint load while step counts are optimizer-wide)."""
         self._group_scal.copy_(torch.tensor([list(r) for r in rows], dtype=torch.float32))
 
-    def optimizer_step(self, hypers, exts=None, sf=None):
+    def optimizer_step(self, hypers, exts=None, sf=None, ademamix=None):
         """One fused K2 launch (+ the one-thread epilogue).  ``hypers``: one ``OptimHyper`` or a list (one per group).
         ``exts``: per-group ``OptimHyperExt`` of the kinds after SGD.  stk_optim_step_prologue forms their per-step scalars
         (and the scalar state of NAdam and ASGD) on the device before the step, and every kind's once step counts are
         per parameter; the optimizer-wide Adam / AdamW / SGD step forms its own.  ``sf``: per-group ``SfHyper`` of the
-        schedule-free kinds, whose group scalars stk_sf_step_prologue forms (and whose lr_max / weight_sum it advances)."""
+        schedule-free kinds, whose group scalars stk_sf_step_prologue forms (and whose lr_max / weight_sum it advances).
+        ``ademamix``: per-group ``AdemamixHyper``; stk_ademamix_step_prologue then takes stk_optim_step_prologue's place
+        (same step counts, AdEMAMix's scalars) and M2 is the step's third state tensor."""
         e = self.engine
         e.state_select(self.state_id)
         if isinstance(hypers, _lib.OptimHyper):
@@ -908,6 +915,7 @@ class GradPath:
         a.master = self.master_ptr
         a.exp_avg = self.M.ptr if self.M else None
         a.exp_avg_sq = self.V.ptr if self.V else None
+        a.exp_avg_slow = self.M2.ptr if self.M2 else None
         a.n_local = self.n_local
         a.grid_n = self.n_local_max
         keep = [harr]
@@ -935,7 +943,20 @@ class GradPath:
         nr, rend, rgrp = self._ranges_for_step()
         a.n_ranges, a.range_end_vec, a.range_group = nr, rend, rgrp
         per_range = bool(nr) and self._range_steps is not None
-        if exts is not None or per_range:
+        if ademamix is not None:
+            aarr = (_lib.AdemamixHyper * ng)(*ademamix)
+            keep.append(aarr)
+            bc = self._range_bc if per_range else self._group_bc
+            e._check(e.lib.stk_ademamix_step_prologue(e.ctx, harr, aarr, ng, nr if per_range else 0,
+                                                      rgrp if per_range else None,
+                                                      self._range_steps.data_ptr() if per_range else None, bc.data_ptr(),
+                                                      e._stream()))
+            e.launches += 1
+            if per_range:
+                a.range_bc = bc.data_ptr()
+            else:
+                a.group_bc = bc.data_ptr()
+        elif exts is not None or per_range:
             xarr = (_lib.OptimHyperExt * ng)(*exts) if exts is not None else None
             keep.append(xarr)
             a.hyper_ext = xarr
@@ -1160,7 +1181,8 @@ class GradPath:
                 p.data = p.data.clone()
                 p.grad = None
         self.grad_views = []
-        self.p_flat = self.g_flat = self.main_flat = self.m_flat = self.v_flat = self.master_flat = self.avg_flat = None
+        self.p_flat = self.g_flat = self.main_flat = self.m_flat = self.v_flat = self.m2_flat = self.master_flat = None
+        self.avg_flat = None
         self.af_state = self._af_ws = self._af_desc = None
         self._lw_ws = self._lw_desc = None
         for b in self._bufs:

@@ -20,6 +20,10 @@ other kinds.
 ``weight_sum``; ``k`` is the step count) on the device, advanced by ``stk_sf_step_prologue``, and lazy state without
 ``step``.  ``train()`` / ``eval()`` swap the master and the model between y and x; a step in eval mode raises.  They are
 sharded like the other kinds.
+``AdEMAMix`` (defined here, after apple/ml-ademamix) is the one kind with three fp32 state tensors: ``exp_avg_fast`` in
+the first-moment buffer, ``exp_avg_sq`` in the second and ``exp_avg_slow`` in a third (``GradPath.M2``), with its
+per-step scalars (bias corrections, the alpha and beta3 warm-ups) formed by ``stk_ademamix_step_prologue``.  It is
+element-wise and sharded like Adam.
 ``torch.optim.Adafactor`` takes its own fused entry point, ``stk_adafactor_step`` (per-parameter reductions: row / column
 means of g^2, the parameter's RMS, the update's RMS), with per-parameter step counts on the device and torch's
 state_dict layout (``row_var`` / ``col_var`` or ``variance``).  Its state is never sharded: the reductions need whole
@@ -35,7 +39,8 @@ groups): the gradient path
 is still the engine's (K1 reduce with fused cast / unscale / inf test / norm, the clip applied by ``k_grad_scale``); the
 update itself is the stock optimizer stepping on per-parameter fp32 views of the flat master / main-grad buffers.
 """
-from typing import Dict, List, Optional, Type
+import math
+from typing import Dict, List, Optional, Tuple, Type
 
 import torch
 
@@ -48,14 +53,18 @@ _KINDS = {torch.optim.Adam: _lib.OPT_ADAM, torch.optim.AdamW: _lib.OPT_ADAMW, to
 # per-step scalars from stk_optim_step_prologue
 _EXT_KINDS = (_lib.OPT_NADAM, _lib.OPT_RADAM, _lib.OPT_ADAMAX, _lib.OPT_ADADELTA, _lib.OPT_RPROP, _lib.OPT_ASGD)
 # element-wise classes whose state torch creates at a parameter's first step (no state_dict entry before it)
-_LAZY_KINDS = (_lib.OPT_ADADELTA, _lib.OPT_RPROP, _lib.OPT_ASGD, _lib.OPT_LION, _lib.OPT_SF_ADAMW, _lib.OPT_SF_SGD)
+_LAZY_KINDS = (_lib.OPT_ADADELTA, _lib.OPT_RPROP, _lib.OPT_ASGD, _lib.OPT_LION, _lib.OPT_SF_ADAMW, _lib.OPT_SF_SGD,
+               _lib.OPT_ADEMAMIX)
 # torch's per-parameter state keys of the two fp32 buffers M and V (None: no V buffer)
 _STATE_KEYS = {_lib.OPT_SGD: ("momentum_buffer", None),
                _lib.OPT_ADAM: ("exp_avg", "exp_avg_sq"), _lib.OPT_ADAMW: ("exp_avg", "exp_avg_sq"),
                _lib.OPT_NADAM: ("exp_avg", "exp_avg_sq"), _lib.OPT_RADAM: ("exp_avg", "exp_avg_sq"),
                _lib.OPT_ADAMAX: ("exp_avg", "exp_inf"), _lib.OPT_ADADELTA: ("square_avg", "acc_delta"),
                _lib.OPT_RPROP: ("prev", "step_size"), _lib.OPT_ASGD: ("ax", None), _lib.OPT_LION: ("exp_avg", None),
-               _lib.OPT_SF_ADAMW: ("z", "exp_avg_sq"), _lib.OPT_SF_SGD: ("z", None)}
+               _lib.OPT_SF_ADAMW: ("z", "exp_avg_sq"), _lib.OPT_SF_SGD: ("z", None),
+               _lib.OPT_ADEMAMIX: ("exp_avg_fast", "exp_avg_sq")}
+# the per-parameter state key of the third fp32 buffer M2, for the kinds that have one
+_THIRD_KEYS = {_lib.OPT_ADEMAMIX: "exp_avg_slow"}
 # per-entry scalar state carried by the step prologue: NAdam's mu_product, ASGD's (eta, mu), torch's 0-dim fp32 tensors
 _SCALAR_KEYS = {_lib.OPT_NADAM: ("mu_product",), _lib.OPT_ASGD: ("eta", "mu")}
 _STOCK_ONLY_TRUE = ("amsgrad", "capturable", "differentiable")
@@ -420,6 +429,113 @@ _KINDS[AdamWScheduleFree] = _lib.OPT_SF_ADAMW
 _KINDS[SGDScheduleFree] = _lib.OPT_SF_SGD
 _SF_KINDS = (_lib.OPT_SF_ADAMW, _lib.OPT_SF_SGD)
 
+
+def ademamix_schedule(group, t: float) -> Tuple[float, float]:
+    """AdEMAMix's ``(alpha_t, beta3_t)`` at step t (after the increment), in python doubles: the linear alpha warm-up
+    from 0 and the beta3 warm-up that is linear in half-life from beta1 (apple/ml-ademamix's schedulers)."""
+    b1, _, b3 = group["betas"]
+    alpha, a_warm, b_warm = group["alpha"], group["alpha_warmup"], group["beta3_warmup"]
+    alpha_t = (t / a_warm) * alpha if a_warm is not None and t < a_warm else alpha
+    if b_warm is not None and t < b_warm:
+        def f(b):
+            return math.log(0.5) / math.log(b + 1e-8) - 1
+
+        a = t / b_warm
+        beta3_t = 0.5 ** (1 / ((1 - a) * f(b1) + a * f(b3) + 1))
+    else:
+        beta3_t = b3
+    return alpha_t, beta3_t
+
+
+class AdEMAMix(torch.optim.Optimizer):
+    """AdEMAMix (Pagliardini, Ablin and Grangier, "The AdEMAMix Optimizer: Better, Faster, Older", 2024;
+    apple/ml-ademamix's arguments, group keys and state keys): Adam with a second, slow EMA of the gradient mixed into
+    the numerator.  For one parameter p with gradient g and its own step count t (after the increment), in python
+    doubles for the scalars::
+
+        bc1 = 1 - beta1 ** t;  bc2 = 1 - beta2 ** t;  alpha_t, beta3_t = ademamix_schedule(group, t)
+        m1 = lerp(m1, g, 1 - beta1)          (beta1 == 0: no exp_avg_fast state, m1 = g)
+        m2 = lerp(m2, g, 1 - beta3_t)
+        v = v * beta2 + (1 - beta2) * g * g
+        u = (m1 * (1 / bc1) + alpha_t * m2) / (sqrt(v) * (1 / sqrt(bc2)) + eps)
+        if weight_decay != 0: u = u + weight_decay * p
+        p = p - lr * u
+
+    alpha_t ramps linearly from 0 to alpha over ``alpha_warmup`` steps, and beta3_t from beta1 to beta3 over
+    ``beta3_warmup`` steps, linearly in half-life; None means no warm-up.  The tensor ops are chosen so that the fused
+    kernel can reproduce their CUDA rounding: ``lerp_`` for the two EMAs, multiplication by ``1 / bc1`` and
+    ``1 / sqrt(bc2)``, ``add(alpha=)`` (one FFMA) and ``addcmul_`` (g * g rounded first).  State per parameter, created
+    at its first step: ``step`` (0-dim fp32 tensor; ``load_state_dict`` also accepts upstream's python int),
+    ``exp_avg_fast`` (None in a group with beta1 == 0), ``exp_avg_slow`` and ``exp_avg_sq``.  This ``step()`` is plain
+    per-parameter torch: what runs outside the engine and on its stock route; inside ``Stoke`` the class runs on the
+    fused sm_90a step (``k_optim_step``, kind ``STK_OPT_ADEMAMIX``)."""
+
+    def __init__(self, params, lr: float = 1e-3, betas=(0.9, 0.999, 0.9999), alpha: float = 2.0,
+                 beta3_warmup: Optional[int] = None, alpha_warmup: Optional[int] = None, eps: float = 1e-8,
+                 weight_decay: float = 0):
+        if lr < 0.0:
+            raise ValueError(f"Invalid learning rate: {lr}")
+        if eps < 0.0:
+            raise ValueError(f"Invalid epsilon value: {eps}")
+        if len(betas) != 3 or not all(0.0 <= b < 1.0 for b in betas):
+            raise ValueError(f"Invalid beta parameters: {betas}")
+        if weight_decay < 0.0:
+            raise ValueError(f"Invalid weight_decay value: {weight_decay}")
+        if alpha < 0.0:
+            raise ValueError(f"Invalid alpha value: {alpha}")
+        for name, w in (("beta3_warmup", beta3_warmup), ("alpha_warmup", alpha_warmup)):
+            if w is not None and (isinstance(w, bool) or not isinstance(w, int) or w <= 0):
+                raise ValueError(f"Invalid {name}: {w} (None or a positive int)")
+        super().__init__(params, dict(lr=lr, betas=tuple(betas), alpha=alpha, beta3_warmup=beta3_warmup,
+                                      alpha_warmup=alpha_warmup, eps=eps, weight_decay=weight_decay))
+
+    def load_state_dict(self, state_dict):
+        super().load_state_dict(state_dict)
+        for st in self.state.values():   # upstream keeps step as a python int
+            if "step" in st and not torch.is_tensor(st["step"]):
+                st["step"] = torch.tensor(float(st["step"]), dtype=torch.float32)
+
+    @torch.no_grad()
+    def step(self, closure=None):
+        loss = None
+        if closure is not None:
+            with torch.enable_grad():
+                loss = closure()
+        for group in self.param_groups:
+            b1, b2, _ = group["betas"]
+            lr, eps, wd = group["lr"], group["eps"], group["weight_decay"]
+            for p in group["params"]:
+                if p.grad is None:
+                    continue
+                g = p.grad
+                state = self.state[p]
+                if not state:
+                    state["step"] = torch.tensor(0.0, dtype=torch.float32)
+                    state["exp_avg_fast"] = torch.zeros_like(p, memory_format=torch.preserve_format) if b1 != 0 else None
+                    state["exp_avg_slow"] = torch.zeros_like(p, memory_format=torch.preserve_format)
+                    state["exp_avg_sq"] = torch.zeros_like(p, memory_format=torch.preserve_format)
+                state["step"] += 1
+                t = float(state["step"])
+                bc1, bc2 = 1 - b1 ** t, 1 - b2 ** t
+                alpha_t, beta3_t = ademamix_schedule(group, t)
+                m1 = state["exp_avg_fast"]
+                if m1 is None:
+                    m1 = g
+                else:
+                    m1.lerp_(g, 1 - b1)
+                m2, v = state["exp_avg_slow"], state["exp_avg_sq"]
+                m2.lerp_(g, 1 - beta3_t)
+                v.mul_(b2).addcmul_(g, g, value=1 - b2)
+                denom = v.sqrt().mul_(1 / math.sqrt(bc2)).add_(eps)
+                u = m1.mul(1 / bc1).add_(m2, alpha=alpha_t).div_(denom)
+                if wd != 0:
+                    u.add_(p, alpha=wd)
+                p.add_(u, alpha=-lr)
+        return loss
+
+
+_KINDS[AdEMAMix] = _lib.OPT_ADEMAMIX
+
 # LAMB and LARS run on their own entry point, stk_layerwise_step (per-parameter trust ratios), not as kinds of K2
 _LAMB, _LARS = "lamb", "lars"
 _KINDS[LAMB] = _LAMB
@@ -548,7 +664,7 @@ class B200FusedOptimizer(torch.optim.Optimizer):
                  bucket_mb: Optional[float] = None):
         if optim_cls not in _KINDS:
             raise NotImplementedError(
-                f"Stoke -- the fused step covers torch.optim.Adam, AdamW, SGD, NAdam, RAdam, Adamax, Adadelta, Rprop, ASGD and Adafactor and stoke_b200.optim.LAMB, LARS, Lion, AdamWScheduleFree and SGDScheduleFree; got {getattr(optim_cls, '__name__', optim_cls)}"
+                f"Stoke -- the fused step covers torch.optim.Adam, AdamW, SGD, NAdam, RAdam, Adamax, Adadelta, Rprop, ASGD and Adafactor and stoke_b200.optim.LAMB, LARS, Lion, AdamWScheduleFree, SGDScheduleFree and AdEMAMix; got {getattr(optim_cls, '__name__', optim_cls)}"
                 f" (use B200StockOptimizer / build_optimizer, which routes other classes to the stock-optimizer path)")
         params, group_of, extra, kw = _group_layout(module, optim_kwargs)
         if len(extra) > _lib.MAX_GROUPS:
@@ -571,6 +687,9 @@ class B200FusedOptimizer(torch.optim.Optimizer):
         lw = self._kind in _LAYERWISE
         lars = self._kind == _LARS
         one_state = self._kind in (_lib.OPT_ASGD, _lib.OPT_LION, _lib.OPT_SF_SGD)   # a single fp32 state tensor, in M
+        needs_m = not (sgd or ada or lars) or any_mom
+        if self._kind == _lib.OPT_ADEMAMIX:   # exp_avg_fast exists only in groups with beta1 != 0
+            needs_m = any(g["betas"][0] != 0 for g in probe.param_groups)
         if (ada or lw) and engine.world > 1:
             # Adafactor's per-parameter reductions and LAMB's / LARS's trust ratios need whole parameters on one rank: their
             # state is replicated (also under fairscale_oss) and every rank runs the same deterministic step on the same
@@ -578,9 +697,10 @@ class B200FusedOptimizer(torch.optim.Optimizer):
             route = "allreduce"
         self.path = GradPath(engine, params, grad_accum=grad_accum, clip=clip, sharded=sharded, lp_dtype=lp_dtype,
                              module=module, needs_second_moment=not (sgd or ada or lars or one_state),
-                             needs_first_moment=not (sgd or ada or lars) or any_mom, state_id=state_id, route=route,
+                             needs_first_moment=needs_m, state_id=state_id, route=route,
                              group_of=group_of, bucket_mb=bucket_mb, scalar_state=len(_SCALAR_KEYS.get(self._kind, ())),
-                             adafactor=ada, layerwise=lw, schedule_free=self._kind in _SF_KINDS)
+                             adafactor=ada, layerwise=lw, schedule_free=self._kind in _SF_KINDS,
+                             third_state=self._kind in _THIRD_KEYS)
         by_group: List[List[torch.nn.Parameter]] = [[] for _ in extra]
         for p, gi in zip(params, group_of):
             by_group[gi].append(p)
@@ -624,8 +744,8 @@ class B200FusedOptimizer(torch.optim.Optimizer):
             h.momentum = float(g.get("momentum", 0.0))
             h.dampening = float(g.get("dampening", 0.0))
             h.nesterov = int(bool(g.get("nesterov", False)))
-        elif "betas" in g:
-            h.beta1, h.beta2 = (float(b) for b in g["betas"])
+        elif "betas" in g:   # AdEMAMix has a third beta, which goes in AdemamixHyper
+            h.beta1, h.beta2 = float(g["betas"][0]), float(g["betas"][1])
             h.eps = float(g.get("eps", 0.0))   # Lion has no eps
         elif "eps" in g:   # Adadelta
             h.eps = float(g["eps"])
@@ -645,6 +765,16 @@ class B200FusedOptimizer(torch.optim.Optimizer):
             x.weight_lr_power = float(g["weight_lr_power"])
             x.beta2 = float(g["betas"][1]) if "betas" in g else 0.0
             x.warmup_steps = int(g["warmup_steps"])
+            out.append(x)
+        return out
+
+    def _ademamix_hypers(self) -> List[_lib.AdemamixHyper]:
+        out = []
+        for g in self.param_groups:
+            x = _lib.AdemamixHyper()
+            x.alpha, x.beta3 = float(g["alpha"]), float(g["betas"][2])
+            x.alpha_warmup = int(g["alpha_warmup"] or 0)   # 0: none
+            x.beta3_warmup = int(g["beta3_warmup"] or 0)
             out.append(x)
         return out
 
@@ -676,6 +806,9 @@ class B200FusedOptimizer(torch.optim.Optimizer):
         if self._kind in _SF_KINDS:
             self.check_train_mode()
             self.path.optimizer_step(self._hypers(), None, self._sf_hypers())
+            return
+        if self._kind == _lib.OPT_ADEMAMIX:
+            self.path.optimizer_step(self._hypers(), ademamix=self._ademamix_hypers())
             return
         self.path.optimizer_step(self._hypers(), self._exts())
 
@@ -782,15 +915,18 @@ class B200FusedOptimizer(torch.optim.Optimizer):
         """torch's per-parameter format: ``step``, the scalar state (NAdam's ``mu_product``, ASGD's ``eta`` and ``mu``) as
         0-dim fp32 tensors, then the class's state tensors.  Adadelta, Rprop, ASGD and Lion omit a parameter that was never
         stepped (torch creates their state at its first gradient); the other kinds emit it.  SGD emits only
-        ``momentum_buffer``, None before a parameter's first step or without momentum."""
+        ``momentum_buffer``, None before a parameter's first step or without momentum.  AdEMAMix emits ``step``,
+        ``exp_avg_fast`` (None in a group with beta1 == 0), ``exp_avg_slow`` and ``exp_avg_sq``."""
         path = self.path
         if self._kind == _ADAFACTOR:
             return self._adafactor_state_dict()
         if self._kind in _LAYERWISE:
             return self._layerwise_state_dict()
         k_m, k_v = _STATE_KEYS[self._kind]
+        k_3 = _THIRD_KEYS.get(self._kind)
         ms = path.unflatten(self._full(path.m_flat)) if path.m_flat is not None else None
         vs = path.unflatten(self._full(path.v_flat)) if k_v is not None else None
+        m2s = path.unflatten(self._full(path.m2_flat)) if k_3 is not None else None
         steps = path.param_steps()
         scal = path.param_scalars() if self._kind in _SCALAR_KEYS else None
         state = {}
@@ -805,7 +941,10 @@ class B200FusedOptimizer(torch.optim.Optimizer):
             if scal is not None:
                 for key, val in zip(_SCALAR_KEYS[self._kind], scal[i]):
                     d[key] = torch.tensor(val, dtype=torch.float32)
-            d[k_m] = ms[i].clone()
+            no_m = self._kind == _lib.OPT_ADEMAMIX and self.param_groups[self._group_of[i]]["betas"][0] == 0
+            d[k_m] = None if no_m else ms[i].clone()
+            if k_3 is not None:
+                d[k_3] = m2s[i].clone()
             if k_v is not None:
                 d[k_v] = vs[i].clone()
             state[j] = d
@@ -844,7 +983,10 @@ class B200FusedOptimizer(torch.optim.Optimizer):
         else:
             keys = _STATE_KEYS[self._kind] if self._kind not in _LAYERWISE else \
                 (("exp_avg", "exp_avg_sq") if self._kind == _LAMB else ("momentum_buffer", None))
-            for local_dst, key in zip((path.m_flat, path.v_flat), keys):
+            dsts = list(zip((path.m_flat, path.v_flat), keys))
+            if self._kind in _THIRD_KEYS:
+                dsts.append((path.m2_flat, _THIRD_KEYS[self._kind]))
+            for local_dst, key in dsts:
                 if local_dst is None:
                     continue
                 # schedule-free: a parameter without z has not been stepped, and its z is its master (upstream's clone)
