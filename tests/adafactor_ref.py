@@ -141,6 +141,23 @@ def step_bound(w, state: Dict, G, step: int, h: Dict, ref_w, ref_state: Dict):
     return SLACK * e_w, e_state
 
 
+def update_ratio(state: Dict, g, step: int, h: Dict) -> float:
+    """||u|| / (sqrt(numel) d) of one step in float64 (state: torch's row_var / col_var or variance before the step).
+    torch divides the update by max(1, this): above 1 the update's RMS clip is active, below it is not."""
+    g = g.to(F64)
+    n = g.numel()
+    eps1 = eps1_of(h)
+    b2 = (step + 1) ** h.get("beta2_decay", -0.8)
+    if g.dim() >= 2:
+        rv = state["row_var"].to(F64).lerp((g * g).mean(dim=-1, keepdim=True), b2)
+        cv = state["col_var"].to(F64).lerp((g * g).mean(dim=-2, keepdim=True), b2)
+        v = rv * cv / rv.mean(dim=-2, keepdim=True).clamp(min=eps1)
+    else:
+        v = state["variance"].to(F64).lerp(g * g, b2)
+    u = g / v.clamp(min=eps1 * eps1).sqrt()
+    return float(u.norm()) / (math.sqrt(n) * h.get("d", 1.0))
+
+
 # ---- deliberately wrong references (negative controls) ------------------------------------------------------------------
 MUTATIONS = ("alpha_after_decay", "eps1_bf16", "rho_no_min", "sum_not_mean", "no_eps1sq_clamp", "denom_no_max1")
 
