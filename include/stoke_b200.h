@@ -92,10 +92,15 @@ typedef enum {
                              (stk_sf_step_prologue) */
   STK_OPT_SF_SGD = 11,    /* stoke_b200.optim.SGDScheduleFree; exp_avg = z, no exp_avg_sq.  Reads weight_decay of
                              stk_optim_hyper_t; the rest from group_bc (stk_sf_step_prologue) */
-  STK_OPT_ADEMAMIX = 12   /* stoke_b200.optim.AdEMAMix (Pagliardini et al. 2024); exp_avg = exp_avg_fast (not read or
+  STK_OPT_ADEMAMIX = 12,  /* stoke_b200.optim.AdEMAMix (Pagliardini et al. 2024); exp_avg = exp_avg_fast (not read or
                              written in a group with beta1 == 0), exp_avg_sq = exp_avg_sq, exp_avg_slow = exp_avg_slow.
                              Reads lr, beta1, beta2, eps and weight_decay of stk_optim_hyper_t; the per-step scalars from
                              group_bc / range_bc of stk_ademamix_step_prologue */
+  STK_OPT_RMSPROP_TF = 13 /* stoke_b200.optim.RMSpropTF (TensorFlow-style RMSprop, timm's RMSpropTF); only through
+                             stk_rmsprop_tf_step.  exp_avg = momentum_buffer (not read or written in a group with
+                             momentum == 0), exp_avg_sq = square_avg, exp_avg_slow = grad_avg (not read or written in a
+                             group that is not centered).  Reads lr, eps, weight_decay and momentum of stk_optim_hyper_t
+                             and the group's stk_rmsprop_tf_hyper_t; no per-step scalars */
 } stk_optim_kind;
 
 /* flags of stk_grad_reduce */
@@ -304,10 +309,33 @@ typedef struct {
                              The schedule-free kinds need group_bc from stk_sf_step_prologue and ignore range_bc: their
                              step count and scalars belong to the group, not to the parameter.  SF_SGD takes no
                              exp_avg_sq */
-  float* exp_avg_slow;    /* ADEMAMIX only (required there): the third fp32 state tensor, indexed like exp_avg.  ADEMAMIX
-                             also needs exp_avg_sq, and exp_avg unless every group has beta1 == 0 */
+  float* exp_avg_slow;    /* the third fp32 state tensor, indexed like exp_avg; ADEMAMIX (required there) and RMSPROP_TF
+                             only.  ADEMAMIX also needs exp_avg_sq, and exp_avg unless every group has beta1 == 0 */
 } stk_optim_args_t;
+/* Every kind but RMSPROP_TF, which is refused here (its per-group hyper-parameters go through stk_rmsprop_tf_step). */
 int stk_optim_step_ex(stk_ctx* ctx, const stk_optim_args_t* args, void* stream);
+
+/* Per-group hyper-parameters of STK_OPT_RMSPROP_TF that stk_optim_hyper_t has no field for (timm's RMSpropTF). */
+typedef struct {
+  double alpha;            /* the square_avg (and grad_avg) decay */
+  int32_t centered, decoupled_decay, lr_in_momentum;
+} stk_rmsprop_tf_hyper_t;
+/* The fused step of STK_OPT_RMSPROP_TF: stk_optim_step_ex's arguments, routes and launch, plus one stk_rmsprop_tf_hyper_t
+ * per group (args->n_groups, host array).  args->hyper[*].kind must be STK_OPT_RMSPROP_TF.  exp_avg_sq (square_avg) is
+ * required; exp_avg (momentum_buffer) when some group has momentum > 0, exp_avg_slow (grad_avg) when some group is
+ * centered.  No per-step scalars: group_bc is not needed, and with per-parameter step counts range_bc is that of
+ * stk_optim_step_prologue (an all-zero row for this kind) and is not read.  One element with the formed gradient g (after
+ * unscale and clip), sq = square_avg, ga = grad_avg, buf = momentum_buffer, all in fp32 (fp32(x): the python double x
+ * rounded to fp32):
+ *   wd != 0:  decoupled_decay: p = p * fp32(1 - lr wd)   else: g = fma(wd, p, g)
+ *   sq = fma(fp32(1 - alpha), g * g - sq, sq)
+ *   centered: ga = fma(fp32(1 - alpha), g - ga, ga);  avg = sqrt((sq - ga * ga) + eps)   else: avg = sqrt(sq + eps)
+ *   momentum > 0: buf = fma(c, g / avg, buf * momentum);  lr_in_momentum: c = lr, p = p - buf
+ *                                                         else:           c = 1,  p = fma(-lr, buf, p)
+ *   else:         p = fma(-lr, g / avg, p)
+ * with every product, difference, sum, sqrt and division rounded on its own (IEEE, round to nearest). */
+int stk_rmsprop_tf_step(stk_ctx* ctx, const stk_optim_args_t* args, const stk_rmsprop_tf_hyper_t* rmsprop_tf,
+                        void* stream);
 
 /* Weight-average update over n fp32 elements (n a multiple of 4, both pointers 16-byte aligned), one launch on `stream`:
  * mode 1: avg = master;  mode 2: avg = torch.lerp(avg, master, weight) on fp32 -- for |weight| < 0.5
@@ -343,6 +371,8 @@ int stk_weight_avg(stk_ctx* ctx, float* avg, const float* master, size_t n, int 
  *           exp_avg beta2)
  *   SF_ADAMW, SF_SGD: {0, 0, 0, 0}: the prologue runs for them only to keep per-parameter step counts (which decide the
  *           state_dict entries); their scalars come from stk_sf_step_prologue
+ *   RMSPROP_TF: {0, 0, 0, 0}: no per-step scalars (see stk_rmsprop_tf_step); the prologue runs for it only to keep
+ *           per-parameter step counts
  * with bc1 = 1 - beta1^t, bc2 = 1 - beta2^t.  The scalar state `scalar_state` (fp32, torch keeps it per parameter) holds per
  * range or per group: NADAM one float, mu_product (torch initialises it to 1); ASGD two floats, {eta, mu}.  It is read and
  * written only for those two kinds and may be NULL for the others; hyper_ext may be NULL (all zero).

@@ -1,5 +1,5 @@
 // k2_optim.cu -- K2: single-pass fused optimizer step (Adam / AdamW / SGD-momentum / NAdam / RAdam / Adamax / Adadelta /
-// Rprop / ASGD / Lion / schedule-free AdamW and SGD / AdEMAMix), plus the step prologues (per-parameter step counts,
+// Rprop / ASGD / Lion / schedule-free AdamW and SGD / AdEMAMix / TensorFlow-style RMSprop), plus the step prologues (per-parameter step counts,
 // NAdam's mu_product, ASGD's eta and mu; the schedule-free group scalars; AdEMAMix's bias corrections and warm-ups) and
 // epilogue.
 //
@@ -13,8 +13,9 @@
 // when ax is written without being read.  Lion keeps one (exp_avg) and reads it: 20 / 22.  Schedule-free AdamW keeps
 // z (exp_avg) and exp_avg_sq like Adam: 28 / 30; schedule-free SGD keeps z only: 20 / 22.  AdEMAMix keeps a third
 // tensor (exp_avg_slow, in m2) besides exp_avg_fast and exp_avg_sq: 36 / 38, and 28 / 30 in a group with beta1 == 0,
-// which neither reads nor writes exp_avg_fast.  The clip coefficient, the
-// skip decision and the bias corrections come from device memory, so there is no host synchronisation anywhere on the
+// which neither reads nor writes exp_avg_fast.  RMSpropTF keeps square_avg (v), momentum_buffer (m) in a group with
+// momentum and grad_avg (m2) in a centered group: 20 / 22 with neither, 28 / 30 with momentum, 36 / 38 with both.  The
+// clip coefficient, the skip decision and the bias corrections come from device memory, so there is no host synchronisation anywhere on the
 // step.
 //
 // Gradient sources:  MAIN  -- fp32 reduced / unscaled gradients written by K1 (cross-rank routes), indexed like the state;
@@ -29,8 +30,8 @@
 // torch/optim/sgd.py (_single_tensor_sgd), nadam.py (_single_tensor_nadam), radam.py (_single_tensor_radam), adamax.py
 // (_single_tensor_adamax), adadelta.py (_single_tensor_adadelta), rprop.py (_single_tensor_rprop) and asgd.py
 // (_single_tensor_asgd); Lion follows stoke_b200.optim.Lion.step (torch has no Lion), the schedule-free kinds
-// stoke_b200.optim.AdamWScheduleFree.step / SGDScheduleFree.step and AdEMAMix stoke_b200.optim.AdEMAMix.step, each
-// rounded like those steps on CUDA; the clip follows
+// stoke_b200.optim.AdamWScheduleFree.step / SGDScheduleFree.step, AdEMAMix stoke_b200.optim.AdEMAMix.step and
+// RMSpropTF stoke_b200.optim.RMSpropTF.step, each rounded like those steps on CUDA; the clip follows
 // torch/nn/utils/clip_grad.py:165-174 (coef = max_norm / (total_norm + 1e-6), clamped to 1) and :291-292 (clamp).
 #include <cstdlib>
 
@@ -42,9 +43,19 @@ struct GroupHyperD {   // host-side doubles, converted exactly like torch conver
   double lr, beta1, beta2, eps, weight_decay, momentum, dampening;
   int nesterov, maximize;
   double momentum_decay;  // NAdam
-  int decoupled;          // NAdam / RAdam: decoupled weight decay
-  double rho;                                    // Adadelta
-  double etaminus, etaplus, step_size_min, step_size_max;  // Rprop
+  int decoupled;          // NAdam / RAdam: decoupled weight decay; RMSpropTF: decoupled_decay
+  int centered;           // RMSpropTF (in the padding before rho, so that no field moves)
+  double rho;                                    // Adadelta; RMSpropTF: alpha (the square_avg decay, like rho)
+  // Rprop's four; RMSpropTF keeps its momentum constants in the first two (stk_rmsprop_tf_step fills them)
+  union {
+    double etaminus;
+    double buf_c;                                // RMSpropTF: momentum_buffer's addcdiv value (lr, or 1)
+  };
+  union {
+    double etaplus;
+    double upd_c;                                // RMSpropTF: the update's coefficient on momentum_buffer (1, or lr)
+  };
+  double step_size_min, step_size_max;
   double lambd, alpha, t0;                       // ASGD
 };
 struct GroupHyperS {   // what the inner loop reads (shared memory, one entry per parameter group)
@@ -57,13 +68,28 @@ struct GroupHyperS {   // what the inner loop reads (shared memory, one entry pe
     float rho;                                  // Adadelta
     float b1;                                   // Lion
     int no_m1;                                  // AdEMAMix: beta1 == 0, exp_avg_fast is the gradient (no state)
+    int centered;                               // RMSpropTF: the group keeps grad_avg
   };
   union {
     float one_m_rho;                            // Adadelta
     float c3;                                   // the fourth per-step scalar: schedule-free AdamW's fp32(1 / bc2),
                                                 // AdEMAMix's 1 - beta3_t
+    float one_m_alpha;                          // RMSpropTF: fp32(1 - alpha)
   };
-  float etaminus, etaplus, ss_min, ss_max;      // Rprop
+  // Rprop's four; RMSpropTF keeps its momentum constants in the first three
+  union {
+    float etaminus;
+    float buf_c;                                // RMSpropTF: momentum_buffer's addcdiv value (lr, or 1)
+  };
+  union {
+    float etaplus;
+    float upd_c;                                // RMSpropTF: the update's coefficient on momentum_buffer (1, or lr)
+  };
+  union {
+    float ss_min;
+    int has_mom;                                // RMSpropTF: momentum > 0, the group keeps momentum_buffer
+  };
+  float ss_max;
 };
 
 struct OptimParams {
@@ -99,8 +125,11 @@ struct OptimParams {
   const float4* range_bc;                    // device, optional: per-range scalars of stk_optim_step_prologue
   const float4* group_bc;                    // device, optional: per-group scalars of stk_optim_step_prologue
   // appended, so that the fields above keep their offsets (and the other kinds their code)
-  float* m2;                                 // AdEMAMix: exp_avg_slow
-  int m_deferred;                            // AdEMAMix: some group has beta1 == 0, so m is loaded once the range is known
+  float* m2;                                 // AdEMAMix: exp_avg_slow; RMSpropTF: grad_avg (nullptr: no centered group)
+  int m_deferred;                            // AdEMAMix: some group has beta1 == 0, so m is loaded once the range is known;
+                                             // RMSpropTF: likewise, some group has no momentum
+  int m2_deferred;                           // RMSpropTF: some group is not centered, so m2 is loaded once the range is
+                                             // known (in the tail padding: the struct keeps its size)
 };
 
 // floats of per-entry scalar state the prologue carries (the stk_optim_step_prologue `scalar_state` array)
@@ -230,11 +259,12 @@ __global__ void __launch_bounds__(256, KIND >= STK_OPT_NADAM ? 2 : 0) k_optim_st
   unsigned long long t_begin = 0;
   if (PERSIST && p.prof_ns && blockIdx.x == 0 && threadIdx.x == 0) t_begin = globaltimer_ns();
 
-  // SGD without momentum and AdEMAMix with beta1 == 0 in every group have no m
-  const bool use_m = (KIND != STK_OPT_SGD && KIND != STK_OPT_ADEMAMIX) || p.m != nullptr;
+  // SGD without momentum, AdEMAMix with beta1 == 0 and RMSpropTF without momentum in every group have no m
+  const bool use_m = (KIND != STK_OPT_SGD && KIND != STK_OPT_ADEMAMIX && KIND != STK_OPT_RMSPROP_TF) || p.m != nullptr;
   // ASGD, Lion and schedule-free SGD: one state tensor (ax / exp_avg / z, in p.m)
   constexpr bool kHasV = KIND != STK_OPT_SGD && KIND != STK_OPT_ASGD && KIND != STK_OPT_LION && KIND != STK_OPT_SF_SGD;
-  constexpr bool kHasM2 = KIND == STK_OPT_ADEMAMIX;
+  constexpr bool kHasM2 = KIND == STK_OPT_ADEMAMIX || KIND == STK_OPT_RMSPROP_TF;
+  constexpr bool kDeferM = KIND == STK_OPT_ADEMAMIX || KIND == STK_OPT_RMSPROP_TF;   // m may exist in some groups only
   const size_t stride = PERSIST ? size_t(gridDim.x) * blockDim.x * VPT : 0;
   size_t i = (size_t(blockIdx.x) * blockDim.x + threadIdx.x) * VPT;
 
@@ -254,11 +284,13 @@ __global__ void __launch_bounds__(256, KIND >= STK_OPT_NADAM ? 2 : 0) k_optim_st
         if constexpr (RAW) InVec<GRAD>::load(p.grad, gv + k, g[k]);
         else InVec<STK_F32>::load(p.grad, i + k, g[k]);
         InVec<STK_F32>::load(p.master, i + k, w[k]);
-        // ASGD: ax only when mu != 1; AdEMAMix with a beta1 == 0 group: m only where beta1 != 0
-        if (use_m && KIND != STK_OPT_ASGD && !(KIND == STK_OPT_ADEMAMIX && p.m_deferred))
-          InVec<STK_F32>::load(p.m, i + k, m[k]);
+        // ASGD: ax only when mu != 1; AdEMAMix with a beta1 == 0 group: m only where beta1 != 0; RMSpropTF likewise m
+        // where the group has momentum and m2 where it is centered
+        if (use_m && KIND != STK_OPT_ASGD && !(kDeferM && p.m_deferred)) InVec<STK_F32>::load(p.m, i + k, m[k]);
         if (kHasV) InVec<STK_F32>::load(p.v, i + k, v[k]);
-        if constexpr (kHasM2) InVec<STK_F32>::load(p.m2, i + k, m2[k]);
+        if constexpr (kHasM2) {
+          if (KIND == STK_OPT_ADEMAMIX || (p.m2 != nullptr && !p.m2_deferred)) InVec<STK_F32>::load(p.m2, i + k, m2[k]);
+        }
       }
     if constexpr (RAW) {
       if (p.acc != nullptr) {
@@ -315,6 +347,14 @@ __global__ void __launch_bounds__(256, KIND >= STK_OPT_NADAM ? 2 : 0) k_optim_st
     if constexpr (KIND == STK_OPT_LION) o.b1 = (float)h.beta1;
     if constexpr (KIND == STK_OPT_SF_ADAMW || KIND == STK_OPT_SF_SGD || KIND == STK_OPT_ADEMAMIX) o.c3 = c.w;
     if constexpr (KIND == STK_OPT_ADEMAMIX) o.no_m1 = h.beta1 == 0.0;
+    if constexpr (KIND == STK_OPT_RMSPROP_TF) {
+      o.one_m_alpha = (float)(1.0 - h.rho);
+      o.centered = h.centered;
+      o.decay_mul = (float)__dadd_rn(1.0, -__dmul_rn(h.lr, h.weight_decay));   // python's 1 - lr * wd, not one DFMA
+      o.has_mom = h.momentum > 0.0;
+      o.buf_c = (float)h.buf_c;
+      o.upd_c = (float)h.upd_c;
+    }
     s_g[threadIdx.x] = o;
   }
   __syncthreads();
@@ -348,6 +388,10 @@ __global__ void __launch_bounds__(256, KIND >= STK_OPT_NADAM ? 2 : 0) k_optim_st
         }
         if constexpr (KIND == STK_OPT_ADEMAMIX) {  // exp_avg_fast does not exist in a beta1 == 0 group
           if (p.m_deferred && !h.no_m1) InVec<STK_F32>::load(p.m, i + k, m[k]);
+        }
+        if constexpr (KIND == STK_OPT_RMSPROP_TF) {  // momentum_buffer / grad_avg exist only with momentum / centered
+          if (p.m_deferred && h.has_mom) InVec<STK_F32>::load(p.m, i + k, m[k]);
+          if (p.m2_deferred && h.centered) InVec<STK_F32>::load(p.m2, i + k, m2[k]);
         }
 #pragma unroll
         for (int e = 0; e < 8; ++e) {
@@ -462,6 +506,32 @@ __global__ void __launch_bounds__(256, KIND >= STK_OPT_NADAM ? 2 : 0) k_optim_st
             m[k][e] = mf;
             m2[k][e] = ms;
             v[k][e] = vv;
+          } else if (KIND == STK_OPT_RMSPROP_TF) {
+            if (h.wd != 0.f) {
+              if (h.decoupled) ww = __fmul_rn(ww, h.decay_mul);      // p.mul_(1 - lr * wd)
+              else gg = fmaf(h.wd, ww, gg);                          // grad = grad.add(p, alpha=wd)
+            }
+            // square_avg.add_(grad.pow(2) - square_avg, alpha=1 - alpha): pow(2) is g * g, add(alpha) one FFMA
+            const float sq = fmaf(h.one_m_alpha, __fsub_rn(__fmul_rn(gg, gg), v[k][e]), v[k][e]);
+            float avg;
+            if (h.centered) {
+              const float ga = fmaf(h.one_m_alpha, __fsub_rn(gg, m2[k][e]), m2[k][e]);  // grad_avg.add_(g - ga, 1 - alpha)
+              // square_avg.addcmul(grad_avg, grad_avg, value=-1).add(eps).sqrt_(): addcmul rounds ga * ga first
+              avg = __fsqrt_rn(__fadd_rn(__fsub_rn(sq, __fmul_rn(ga, ga)), h.eps));
+              m2[k][e] = ga;
+            } else {
+              avg = __fsqrt_rn(__fadd_rn(sq, h.eps));                // square_avg.add(eps).sqrt_()
+            }
+            const float q = __fdiv_rn(gg, avg);
+            if (h.has_mom) {
+              // buf.mul_(momentum).addcdiv_(grad, avg, value=c): addcdiv is one FFMA on the quotient
+              const float buf = fmaf(h.buf_c, q, __fmul_rn(m[k][e], h.mom));
+              ww = fmaf(-h.upd_c, buf, ww);                          // p.add_(-buf) | p.add_(buf, alpha=-lr)
+              m[k][e] = buf;
+            } else {
+              ww = fmaf(-h.lr, q, ww);                               // p.addcdiv_(grad, avg, value=-lr)
+            }
+            v[k][e] = sq;
           } else {  // SGD
             if (h.wd != 0.f) gg = fmaf(ww, h.wd, gg);
             if (h.mom != 0.f) {
@@ -478,10 +548,13 @@ __global__ void __launch_bounds__(256, KIND >= STK_OPT_NADAM ? 2 : 0) k_optim_st
       for (int k = 0; k < VPT; ++k)
         if (k < nv) {
           st_stream_f8(p.master + (i + k) * 8, w[k]);
-          if (use_m && (KIND != STK_OPT_SGD || p.any_mom) && !(KIND == STK_OPT_ADEMAMIX && h.no_m1))
+          if (use_m && (KIND != STK_OPT_SGD || p.any_mom) && !(KIND == STK_OPT_ADEMAMIX && h.no_m1) &&
+              !(KIND == STK_OPT_RMSPROP_TF && !h.has_mom))
             st_stream_f8(p.m + (i + k) * 8, m[k]);
           if (kHasV) st_stream_f8(p.v + (i + k) * 8, v[k]);
-          if constexpr (kHasM2) st_stream_f8(p.m2 + (i + k) * 8, m2[k]);
+          if constexpr (kHasM2) {
+            if (KIND == STK_OPT_ADEMAMIX || h.centered) st_stream_f8(p.m2 + (i + k) * 8, m2[k]);
+          }
         }
       store_lp<LP_DT, VPT>(p, gv, w, nv);
     }
@@ -720,33 +793,45 @@ static cudaError_t launch_optim(stk_ctx* c, const OptimParams& p, int lp_dtype, 
   return launch_one(c, k_optim_step<KIND, STK_F32, false, 1, STK_F32, false>, p, false, 1, s);
 }
 
-extern "C" {
-
-int stk_optim_step_ex(stk_ctx* c, const stk_optim_args_t* a, void* stream) {
+// The body of stk_optim_step_ex and stk_rmsprop_tf_step: rt is the RMSPROP_TF groups' array (nullptr for every other
+// kind, which the callers check)
+static int optim_step(stk_ctx* c, const stk_optim_args_t* a, const stk_rmsprop_tf_hyper_t* rt, void* stream) {
   STK_REQUIRE(c, c && a && a->hyper && a->master && a->grad, "stk_optim_step_ex: NULL argument");
   STK_REQUIRE(c, a->n_groups >= 1 && a->n_groups <= STK_MAX_GROUPS, "stk_optim_step_ex: n_groups must be in [1, 8]");
   STK_REQUIRE(c, a->n_local % 8 == 0, "stk_optim_step_ex: n_local must be a multiple of 8");
   const stk_optim_hyper_t* h = a->hyper;
-  STK_REQUIRE(c, h->kind >= STK_OPT_ADAM && h->kind <= STK_OPT_ADEMAMIX, "stk_optim_step_ex: bad optimizer kind");
+  STK_REQUIRE(c, h->kind >= STK_OPT_ADAM && h->kind <= STK_OPT_RMSPROP_TF, "stk_optim_step_ex: bad optimizer kind");
   const bool sf = h->kind == STK_OPT_SF_ADAMW || h->kind == STK_OPT_SF_SGD;
   const bool ademamix = h->kind == STK_OPT_ADEMAMIX;
+  const bool rmsprop_tf = h->kind == STK_OPT_RMSPROP_TF;
   STK_REQUIRE(c, !sf || a->group_bc, "stk_optim_step_ex: the schedule-free kinds need group_bc of stk_sf_step_prologue");
-  STK_REQUIRE(c, h->kind <= STK_OPT_SGD || h->kind == STK_OPT_LION || a->group_bc || (a->n_ranges > 0 && a->range_bc),
+  STK_REQUIRE(c, h->kind <= STK_OPT_SGD || h->kind == STK_OPT_LION || rmsprop_tf || a->group_bc ||
+                     (a->n_ranges > 0 && a->range_bc),
               "stk_optim_step_ex: the kinds after SGD need the scalars of stk_optim_step_prologue (group_bc or range_bc)");
   STK_REQUIRE(c, (reinterpret_cast<uintptr_t>(a->group_bc) & 15) == 0, "stk_optim_step_ex: group_bc must be 16-byte aligned");
-  STK_REQUIRE(c, h->kind == STK_OPT_SGD || ademamix ||
+  STK_REQUIRE(c, h->kind == STK_OPT_SGD || ademamix || rmsprop_tf ||
                      (a->exp_avg && (a->exp_avg_sq || h->kind == STK_OPT_ASGD || h->kind == STK_OPT_LION ||
                                      h->kind == STK_OPT_SF_SGD)),
               "stk_optim_step_ex: this kind needs exp_avg and exp_avg_sq (ASGD, Lion, SF_SGD: exp_avg)");
-  bool any_mom = false, any_b1 = false, any_b1_zero = false;
+  bool any_mom = false, any_b1 = false, any_b1_zero = false, any_centered = false, any_plain = false;
+  bool any_rms_mom = false, any_rms_no_mom = false;
   for (int gi = 0; gi < a->n_groups; ++gi) {
     STK_REQUIRE(c, h[gi].kind == h->kind, "stk_optim_step_ex: all groups must use the same optimizer kind");
     any_mom |= h[gi].momentum != 0.0;
     any_b1 |= h[gi].beta1 != 0.0;
     any_b1_zero |= h[gi].beta1 == 0.0;
+    if (rmsprop_tf) {
+      any_rms_mom |= h[gi].momentum > 0.0;
+      any_rms_no_mom |= !(h[gi].momentum > 0.0);
+      any_centered |= rt[gi].centered != 0;
+      any_plain |= rt[gi].centered == 0;
+    }
   }
   STK_REQUIRE(c, !ademamix || (a->exp_avg_slow && a->exp_avg_sq && (a->exp_avg || !any_b1)),
               "stk_optim_step_ex: ADEMAMIX needs exp_avg_slow, exp_avg_sq and (unless every group has beta1 == 0) exp_avg");
+  STK_REQUIRE(c, !rmsprop_tf || (a->exp_avg_sq && (a->exp_avg || !any_rms_mom) && (a->exp_avg_slow || !any_centered)),
+              "stk_rmsprop_tf_step: needs exp_avg_sq, exp_avg when some group has momentum > 0 and exp_avg_slow when "
+              "some group is centered");
   STK_REQUIRE(c, !(h->kind == STK_OPT_SGD && any_mom && !a->exp_avg), "stk_optim_step_ex: SGD momentum needs a buffer");
   STK_REQUIRE(c, a->lp_ptrs == nullptr || a->lp_world == 1 || a->lp_world == c->world, "stk_optim_step_ex: lp_world must be 1 or world");
   STK_REQUIRE(c, a->lp_ptrs == nullptr || a->lp_dtype == STK_BF16 || a->lp_dtype == STK_F32, "stk_optim_step_ex: lp dtype");
@@ -829,6 +914,20 @@ int stk_optim_step_ex(stk_ctx* c, const stk_optim_args_t* a, void* stream) {
   p.group_bc = reinterpret_cast<const float4*>(a->group_bc);
   p.m2 = ademamix ? a->exp_avg_slow : nullptr;
   p.m_deferred = (ademamix && a->exp_avg && any_b1_zero) ? 1 : 0;
+  if (rmsprop_tf) {
+    p.m = any_rms_mom ? a->exp_avg : nullptr;
+    p.m2 = any_centered ? a->exp_avg_slow : nullptr;
+    p.m_deferred = (any_rms_mom && any_rms_no_mom) ? 1 : 0;
+    p.m2_deferred = (any_centered && any_plain) ? 1 : 0;
+    for (int gi = 0; gi < a->n_groups; ++gi) {   // the group's alpha and flags in the slots RMSpropTF does not use
+      GroupHyperD& d = p.g[gi];
+      d.rho = rt[gi].alpha;
+      d.centered = rt[gi].centered != 0;
+      d.decoupled = rt[gi].decoupled_decay != 0;
+      d.buf_c = rt[gi].lr_in_momentum ? h[gi].lr : 1.0;
+      d.upd_c = rt[gi].lr_in_momentum ? 1.0 : h[gi].lr;
+    }
+  }
   if (a->grad_raw) {
     // 1/loss_scale is applied when the scaler is live; the device flag decides (enabled), so no host read
     p.unscale = 1;
@@ -858,12 +957,29 @@ int stk_optim_step_ex(stk_ctx* c, const stk_optim_args_t* a, void* stream) {
     case STK_OPT_SF_ADAMW: err = launch_optim<STK_OPT_SF_ADAMW>(c, p, a->lp_dtype, a->grad_dtype, raw, pair_ok, s); break;
     case STK_OPT_SF_SGD: err = launch_optim<STK_OPT_SF_SGD>(c, p, a->lp_dtype, a->grad_dtype, raw, pair_ok, s); break;
     case STK_OPT_ADEMAMIX: err = launch_optim<STK_OPT_ADEMAMIX>(c, p, a->lp_dtype, a->grad_dtype, raw, pair_ok, s); break;
+    case STK_OPT_RMSPROP_TF:
+      err = launch_optim<STK_OPT_RMSPROP_TF>(c, p, a->lp_dtype, a->grad_dtype, raw, pair_ok, s);
+      break;
     default: err = launch_optim<STK_OPT_SGD>(c, p, a->lp_dtype, a->grad_dtype, raw, pair_ok, s); break;
   }
   if (err == cudaErrorNotSupported)
     return stk_fail(c, STK_ERR_UNSUPPORTED, "stk_optim_step_ex: this gradient dtype / parameter dtype pair has no raw route");
   if (err != cudaSuccess) return stk_fail(c, STK_ERR_CUDA, std::string("k_optim_step launch: ") + cudaGetErrorString(err));
   return STK_OK;
+}
+
+extern "C" {
+
+int stk_optim_step_ex(stk_ctx* c, const stk_optim_args_t* a, void* stream) {
+  STK_REQUIRE(c, !(a && a->hyper && a->hyper->kind == STK_OPT_RMSPROP_TF),
+              "stk_optim_step_ex: RMSPROP_TF takes its per-group hyper-parameters through stk_rmsprop_tf_step");
+  return optim_step(c, a, nullptr, stream);
+}
+
+int stk_rmsprop_tf_step(stk_ctx* c, const stk_optim_args_t* a, const stk_rmsprop_tf_hyper_t* rt, void* stream) {
+  STK_REQUIRE(c, c && a && a->hyper && rt, "stk_rmsprop_tf_step: NULL argument");
+  STK_REQUIRE(c, a->hyper->kind == STK_OPT_RMSPROP_TF, "stk_rmsprop_tf_step: hyper->kind must be STK_OPT_RMSPROP_TF");
+  return optim_step(c, a, rt, stream);
 }
 
 int stk_optim_step(stk_ctx* c, const stk_optim_hyper_t* h, float* master, float* exp_avg, float* exp_avg_sq,
@@ -893,7 +1009,8 @@ int stk_optim_step_prologue(stk_ctx* c, const stk_optim_hyper_t* h, const stk_op
   STK_REQUIRE(c, n_groups >= 1 && n_groups <= STK_MAX_GROUPS, "stk_optim_step_prologue: n_groups must be in [1, 8]");
   STK_REQUIRE(c, n_ranges >= 0, "stk_optim_step_prologue: negative n_ranges");
   STK_REQUIRE(c, n_ranges == 0 || (range_group && range_steps), "stk_optim_step_prologue: range arrays are NULL");
-  STK_REQUIRE(c, h->kind >= STK_OPT_ADAM && h->kind <= STK_OPT_SF_SGD, "stk_optim_step_prologue: bad optimizer kind");
+  STK_REQUIRE(c, (h->kind >= STK_OPT_ADAM && h->kind <= STK_OPT_SF_SGD) || h->kind == STK_OPT_RMSPROP_TF,
+              "stk_optim_step_prologue: bad optimizer kind");
   STK_REQUIRE(c, scalar_state_width(h->kind) == 0 || scalar_state,
               "stk_optim_step_prologue: NAdam and ASGD need their scalar state");
   STK_REQUIRE(c, (reinterpret_cast<uintptr_t>(bc) & 15) == 0, "stk_optim_step_prologue: bc must be 16-byte aligned");

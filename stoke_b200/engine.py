@@ -298,6 +298,10 @@ class Engine:
         self._check(self.lib.stk_optim_step_ex(self.ctx, C.byref(args), self._stream()))
         self.launches += 1
 
+    def rmsprop_tf_step(self, args: _lib.OptimArgs, hypers):
+        self._check(self.lib.stk_rmsprop_tf_step(self.ctx, C.byref(args), hypers, self._stream()))
+        self.launches += 1
+
     def step_epilogue(self):
         self._check(self.lib.stk_step_epilogue(self.ctx, self._stream()))
         self.launches += 1
@@ -479,8 +483,8 @@ class GradPath:
                                                                               | absent (local route)
       MASTER fp32 master weights                               local          aliases P when the model is fp32 and unsharded
       M, V   fp32 optimizer state                              local          owned shards (sharded) | all n
-      M2     fp32 third optimizer state (AdEMAMix's            local          indexed like M; only for that kind
-             exp_avg_slow)                                                    (``third_state``)
+      M2     fp32 third optimizer state (AdEMAMix's            local          indexed like M; only for those kinds
+             exp_avg_slow, RMSpropTF's grad_avg)                              (``third_state``)
       AVG    fp32 weight average (EMA / SWA)                   local          indexed like MASTER; only when averaging is
                                                                               configured (``enable_weight_average``)
 
@@ -496,7 +500,7 @@ class GradPath:
                  needs_first_moment: bool = True, bucket_mb: Optional[float] = None, state_id: Optional[int] = None,
                  route: Optional[str] = None, group_of: Optional[Sequence[int]] = None, overlap: bool = True,
                  scalar_state: int = 0, adafactor: bool = False, layerwise: bool = False, schedule_free: bool = False,
-                 third_state: bool = False):
+                 third_state: bool = False, second_moment_init: float = 0.0):
         self.engine = engine
         self.params = [p for p in params if p.requires_grad]
         if not self.params:
@@ -630,6 +634,11 @@ class GradPath:
         if schedule_free:
             self.m_flat.copy_(self.master_flat)
             self._sf_state = torch.tensor([[-1.0, 0.0]] * n_grp, dtype=torch.float64, device=dev)
+        # RMSpropTF: square_avg (V) starts at ones (timm's ones_like at a parameter's first gradient; a parameter without
+        # one is never touched, so filling at construction is the same)
+        if second_moment_init != 0.0:
+            self.scatter_local(torch.full((self.n,), float(second_moment_init), dtype=torch.float32, device=dev),
+                               self.v_flat)
 
         # ---- re-point the module at the flat buffers ----
         if self.low_precision and module is not None:
@@ -891,14 +900,15 @@ class GradPath:
         """Sets the per-group scalar state (checkpoint load while step counts are optimizer-wide)."""
         self._group_scal.copy_(torch.tensor([list(r) for r in rows], dtype=torch.float32))
 
-    def optimizer_step(self, hypers, exts=None, sf=None, ademamix=None):
+    def optimizer_step(self, hypers, exts=None, sf=None, ademamix=None, rmsprop_tf=None):
         """One fused K2 launch (+ the one-thread epilogue).  ``hypers``: one ``OptimHyper`` or a list (one per group).
         ``exts``: per-group ``OptimHyperExt`` of the kinds after SGD.  stk_optim_step_prologue forms their per-step scalars
         (and the scalar state of NAdam and ASGD) on the device before the step, and every kind's once step counts are
         per parameter; the optimizer-wide Adam / AdamW / SGD step forms its own.  ``sf``: per-group ``SfHyper`` of the
         schedule-free kinds, whose group scalars stk_sf_step_prologue forms (and whose lr_max / weight_sum it advances).
         ``ademamix``: per-group ``AdemamixHyper``; stk_ademamix_step_prologue then takes stk_optim_step_prologue's place
-        (same step counts, AdEMAMix's scalars) and M2 is the step's third state tensor."""
+        (same step counts, AdEMAMix's scalars) and M2 is the step's third state tensor.  ``rmsprop_tf``: per-group
+        ``RmspropTfHyper``; the step is stk_rmsprop_tf_step (no per-step scalars), with M2 as grad_avg."""
         e = self.engine
         e.state_select(self.state_id)
         if isinstance(hypers, _lib.OptimHyper):
@@ -978,7 +988,12 @@ class GradPath:
                                                 e._stream()))
             e.launches += 1
             a.group_bc = self._group_bc.data_ptr()
-        e.optim_step_ex(a)
+        if rmsprop_tf is not None:
+            rarr = (_lib.RmspropTfHyper * ng)(*rmsprop_tf)
+            keep.append(rarr)
+            e.rmsprop_tf_step(a, rarr)
+        else:
+            e.optim_step_ex(a)
         self.weight_avg_after_step()
         e.step_epilogue()
         self._track_touched = False

@@ -24,6 +24,10 @@ sharded like the other kinds.
 the first-moment buffer, ``exp_avg_sq`` in the second and ``exp_avg_slow`` in a third (``GradPath.M2``), with its
 per-step scalars (bias corrections, the alpha and beta3 warm-ups) formed by ``stk_ademamix_step_prologue``.  It is
 element-wise and sharded like Adam.
+``RMSpropTF`` (defined here, after timm's TensorFlow-style RMSprop) keeps ``square_avg`` in the second-moment buffer
+(filled with ones at construction), ``momentum_buffer`` in the first (only when some group has momentum) and ``grad_avg``
+in the third (only when some group is centered).  Its per-group alpha and flags go to ``stk_rmsprop_tf_step``; it has no
+per-step scalars.  It is element-wise and sharded like Adam.
 ``torch.optim.Adafactor`` takes its own fused entry point, ``stk_adafactor_step`` (per-parameter reductions: row / column
 means of g^2, the parameter's RMS, the update's RMS), with per-parameter step counts on the device and torch's
 state_dict layout (``row_var`` / ``col_var`` or ``variance``).  Its state is never sharded: the reductions need whole
@@ -54,7 +58,7 @@ _KINDS = {torch.optim.Adam: _lib.OPT_ADAM, torch.optim.AdamW: _lib.OPT_ADAMW, to
 _EXT_KINDS = (_lib.OPT_NADAM, _lib.OPT_RADAM, _lib.OPT_ADAMAX, _lib.OPT_ADADELTA, _lib.OPT_RPROP, _lib.OPT_ASGD)
 # element-wise classes whose state torch creates at a parameter's first step (no state_dict entry before it)
 _LAZY_KINDS = (_lib.OPT_ADADELTA, _lib.OPT_RPROP, _lib.OPT_ASGD, _lib.OPT_LION, _lib.OPT_SF_ADAMW, _lib.OPT_SF_SGD,
-               _lib.OPT_ADEMAMIX)
+               _lib.OPT_ADEMAMIX, _lib.OPT_RMSPROP_TF)
 # torch's per-parameter state keys of the two fp32 buffers M and V (None: no V buffer)
 _STATE_KEYS = {_lib.OPT_SGD: ("momentum_buffer", None),
                _lib.OPT_ADAM: ("exp_avg", "exp_avg_sq"), _lib.OPT_ADAMW: ("exp_avg", "exp_avg_sq"),
@@ -536,6 +540,103 @@ class AdEMAMix(torch.optim.Optimizer):
 
 _KINDS[AdEMAMix] = _lib.OPT_ADEMAMIX
 
+
+class RMSpropTF(torch.optim.Optimizer):
+    """TensorFlow-style RMSprop (timm's ``RMSpropTF``: its arguments, group keys and state keys), the optimizer of the
+    published EfficientNet and MobileNet recipes.  It differs from ``torch.optim.RMSprop`` in three ways: eps goes inside
+    the square root, ``square_avg`` starts at ones, and (``lr_in_momentum``) the learning rate is accumulated into the
+    momentum buffer.  For one parameter p with gradient g, in timm's order of ops::
+
+        if weight_decay != 0:  p = p * (1 - lr * weight_decay) if decoupled_decay else g = g + weight_decay * p
+        square_avg = square_avg + (1 - alpha) * (g * g - square_avg)
+        centered:  grad_avg = grad_avg + (1 - alpha) * (g - grad_avg);  avg = sqrt(square_avg - grad_avg ** 2 + eps)
+        else:      avg = sqrt(square_avg + eps)
+        momentum > 0:  buf = buf * momentum + c * g / avg,  p = p - (1 if lr_in_momentum else lr) * buf,
+                       with c = lr if lr_in_momentum else 1
+        else:          p = p - lr * g / avg
+
+    State per parameter, created at its first step: ``step`` (0-dim fp32 tensor; ``load_state_dict`` also accepts
+    timm's python int), ``square_avg`` (ones), ``momentum_buffer`` (zeros, only in a group with momentum > 0) and
+    ``grad_avg`` (zeros, only in a centered group).  This ``step()`` is plain per-parameter torch: what runs outside the
+    engine and on its stock route; inside ``Stoke`` the class runs on the fused sm_90a step (``k_optim_step``, kind
+    ``STK_OPT_RMSPROP_TF``), which rounds every element as this step does on CUDA."""
+
+    def __init__(self, params, lr: float = 1e-2, alpha: float = 0.9, eps: float = 1e-10, weight_decay: float = 0,
+                 momentum: float = 0.0, centered: bool = False, decoupled_decay: bool = False,
+                 lr_in_momentum: bool = True):
+        if lr < 0.0:
+            raise ValueError(f"Invalid learning rate: {lr}")
+        if eps < 0.0:
+            raise ValueError(f"Invalid epsilon value: {eps}")
+        if momentum < 0.0:
+            raise ValueError(f"Invalid momentum value: {momentum}")
+        if weight_decay < 0.0:
+            raise ValueError(f"Invalid weight_decay value: {weight_decay}")
+        if alpha < 0.0:
+            raise ValueError(f"Invalid alpha value: {alpha}")
+        super().__init__(params, dict(lr=lr, alpha=alpha, eps=eps, weight_decay=weight_decay, momentum=momentum,
+                                      centered=centered, decoupled_decay=decoupled_decay,
+                                      lr_in_momentum=lr_in_momentum))
+
+    def load_state_dict(self, state_dict):
+        super().load_state_dict(state_dict)
+        for st in self.state.values():   # timm keeps step as a python int
+            if "step" in st and not torch.is_tensor(st["step"]):
+                st["step"] = torch.tensor(float(st["step"]), dtype=torch.float32)
+
+    @torch.no_grad()
+    def step(self, closure=None):
+        loss = None
+        if closure is not None:
+            with torch.enable_grad():
+                loss = closure()
+        for group in self.param_groups:
+            lr, alpha, eps, wd, mom = group["lr"], group["alpha"], group["eps"], group["weight_decay"], group["momentum"]
+            for p in group["params"]:
+                if p.grad is None:
+                    continue
+                grad = p.grad
+                state = self.state[p]
+                if not state:
+                    state["step"] = torch.tensor(0.0, dtype=torch.float32)
+                    state["square_avg"] = torch.ones_like(p, memory_format=torch.preserve_format)
+                    if mom > 0:
+                        state["momentum_buffer"] = torch.zeros_like(p, memory_format=torch.preserve_format)
+                    if group["centered"]:
+                        state["grad_avg"] = torch.zeros_like(p, memory_format=torch.preserve_format)
+                state["step"] += 1
+                if wd != 0:
+                    if group["decoupled_decay"]:
+                        p.mul_(1 - lr * wd)
+                    else:
+                        grad = grad.add(p, alpha=wd)
+                square_avg = state["square_avg"]
+                square_avg.add_(grad.pow(2) - square_avg, alpha=1 - alpha)
+                if group["centered"]:
+                    grad_avg = state["grad_avg"]
+                    grad_avg.add_(grad - grad_avg, alpha=1 - alpha)
+                    avg = square_avg.addcmul(grad_avg, grad_avg, value=-1).add(eps).sqrt_()
+                else:
+                    avg = square_avg.add(eps).sqrt_()
+                if mom > 0:
+                    buf = state["momentum_buffer"]
+                    buf.mul_(mom)
+                    if group["lr_in_momentum"]:
+                        buf.addcdiv_(grad, avg, value=lr)
+                        p.add_(-buf)
+                    else:
+                        buf.addcdiv_(grad, avg)
+                        p.add_(buf, alpha=-lr)
+                else:
+                    p.addcdiv_(grad, avg, value=-lr)
+        return loss
+
+
+_KINDS[RMSpropTF] = _lib.OPT_RMSPROP_TF
+# RMSpropTF's per-parameter state keys of M, V and M2 (its own table: M exists only in groups with momentum > 0 and M2
+# only in centered groups, and V starts at ones)
+_RMSPROP_TF_KEYS = ("momentum_buffer", "square_avg", "grad_avg")
+
 # LAMB and LARS run on their own entry point, stk_layerwise_step (per-parameter trust ratios), not as kinds of K2
 _LAMB, _LARS = "lamb", "lars"
 _KINDS[LAMB] = _LAMB
@@ -664,7 +765,7 @@ class B200FusedOptimizer(torch.optim.Optimizer):
                  bucket_mb: Optional[float] = None):
         if optim_cls not in _KINDS:
             raise NotImplementedError(
-                f"Stoke -- the fused step covers torch.optim.Adam, AdamW, SGD, NAdam, RAdam, Adamax, Adadelta, Rprop, ASGD and Adafactor and stoke_b200.optim.LAMB, LARS, Lion, AdamWScheduleFree, SGDScheduleFree and AdEMAMix; got {getattr(optim_cls, '__name__', optim_cls)}"
+                f"Stoke -- the fused step covers torch.optim.Adam, AdamW, SGD, NAdam, RAdam, Adamax, Adadelta, Rprop, ASGD and Adafactor and stoke_b200.optim.LAMB, LARS, Lion, AdamWScheduleFree, SGDScheduleFree, AdEMAMix and RMSpropTF; got {getattr(optim_cls, '__name__', optim_cls)}"
                 f" (use B200StockOptimizer / build_optimizer, which routes other classes to the stock-optimizer path)")
         params, group_of, extra, kw = _group_layout(module, optim_kwargs)
         if len(extra) > _lib.MAX_GROUPS:
@@ -690,6 +791,10 @@ class B200FusedOptimizer(torch.optim.Optimizer):
         needs_m = not (sgd or ada or lars) or any_mom
         if self._kind == _lib.OPT_ADEMAMIX:   # exp_avg_fast exists only in groups with beta1 != 0
             needs_m = any(g["betas"][0] != 0 for g in probe.param_groups)
+        rmsprop_tf = self._kind == _lib.OPT_RMSPROP_TF
+        if rmsprop_tf:   # momentum_buffer and grad_avg exist only in groups with momentum > 0 / centered
+            needs_m = any(g["momentum"] > 0 for g in probe.param_groups)
+        third = self._kind in _THIRD_KEYS or (rmsprop_tf and any(g["centered"] for g in probe.param_groups))
         if (ada or lw) and engine.world > 1:
             # Adafactor's per-parameter reductions and LAMB's / LARS's trust ratios need whole parameters on one rank: their
             # state is replicated (also under fairscale_oss) and every rank runs the same deterministic step on the same
@@ -700,7 +805,7 @@ class B200FusedOptimizer(torch.optim.Optimizer):
                              needs_first_moment=needs_m, state_id=state_id, route=route,
                              group_of=group_of, bucket_mb=bucket_mb, scalar_state=len(_SCALAR_KEYS.get(self._kind, ())),
                              adafactor=ada, layerwise=lw, schedule_free=self._kind in _SF_KINDS,
-                             third_state=self._kind in _THIRD_KEYS)
+                             third_state=third, second_moment_init=1.0 if rmsprop_tf else 0.0)
         by_group: List[List[torch.nn.Parameter]] = [[] for _ in extra]
         for p, gi in zip(params, group_of):
             by_group[gi].append(p)
@@ -744,6 +849,8 @@ class B200FusedOptimizer(torch.optim.Optimizer):
             h.momentum = float(g.get("momentum", 0.0))
             h.dampening = float(g.get("dampening", 0.0))
             h.nesterov = int(bool(g.get("nesterov", False)))
+        elif self._kind == _lib.OPT_RMSPROP_TF:   # alpha and the flags go in RmspropTfHyper
+            h.eps, h.momentum = float(g["eps"]), float(g["momentum"])
         elif "betas" in g:   # AdEMAMix has a third beta, which goes in AdemamixHyper
             h.beta1, h.beta2 = float(g["betas"][0]), float(g["betas"][1])
             h.eps = float(g.get("eps", 0.0))   # Lion has no eps
@@ -778,6 +885,16 @@ class B200FusedOptimizer(torch.optim.Optimizer):
             out.append(x)
         return out
 
+    def _rmsprop_tf_hypers(self) -> List[_lib.RmspropTfHyper]:
+        out = []
+        for g in self.param_groups:
+            x = _lib.RmspropTfHyper()
+            x.alpha = float(g["alpha"])
+            x.centered, x.decoupled_decay = int(bool(g["centered"])), int(bool(g["decoupled_decay"]))
+            x.lr_in_momentum = int(bool(g["lr_in_momentum"]))
+            out.append(x)
+        return out
+
     def _exts(self) -> Optional[List[_lib.OptimHyperExt]]:
         if self._kind not in _EXT_KINDS:
             return None
@@ -809,6 +926,9 @@ class B200FusedOptimizer(torch.optim.Optimizer):
             return
         if self._kind == _lib.OPT_ADEMAMIX:
             self.path.optimizer_step(self._hypers(), ademamix=self._ademamix_hypers())
+            return
+        if self._kind == _lib.OPT_RMSPROP_TF:
+            self.path.optimizer_step(self._hypers(), rmsprop_tf=self._rmsprop_tf_hypers())
             return
         self.path.optimizer_step(self._hypers(), self._exts())
 
@@ -911,6 +1031,26 @@ class B200FusedOptimizer(torch.optim.Optimizer):
             state[self._sd_index[i]] = d
         return self._export(state)
 
+    def _rmsprop_tf_state_dict(self):
+        """timm's format: a parameter that was never stepped has no entry; ``step``, ``square_avg``, then
+        ``momentum_buffer`` in a group with momentum > 0 and ``grad_avg`` in a centered group (absent elsewhere)."""
+        path = self.path
+        steps = path.param_steps()
+        sq, buf, ga = (path.unflatten(self._full(f)) if f is not None else None
+                       for f in (path.v_flat, path.m_flat, path.m2_flat))
+        state = {}
+        for i in range(len(path.params)):
+            if steps[i] == 0:
+                continue
+            g = self.param_groups[self._group_of[i]]
+            d = {"step": torch.tensor(float(steps[i])), "square_avg": sq[i].clone()}
+            if g["momentum"] > 0:
+                d["momentum_buffer"] = buf[i].clone()
+            if g["centered"]:
+                d["grad_avg"] = ga[i].clone()
+            state[self._sd_index[i]] = d
+        return self._export(state)
+
     def state_dict(self):
         """torch's per-parameter format: ``step``, the scalar state (NAdam's ``mu_product``, ASGD's ``eta`` and ``mu``) as
         0-dim fp32 tensors, then the class's state tensors.  Adadelta, Rprop, ASGD and Lion omit a parameter that was never
@@ -922,6 +1062,8 @@ class B200FusedOptimizer(torch.optim.Optimizer):
             return self._adafactor_state_dict()
         if self._kind in _LAYERWISE:
             return self._layerwise_state_dict()
+        if self._kind == _lib.OPT_RMSPROP_TF:
+            return self._rmsprop_tf_state_dict()
         k_m, k_v = _STATE_KEYS[self._kind]
         k_3 = _THIRD_KEYS.get(self._kind)
         ms = path.unflatten(self._full(path.m_flat)) if path.m_flat is not None else None
@@ -981,16 +1123,26 @@ class B200FusedOptimizer(torch.optim.Optimizer):
                     else:
                         v.zero_()
         else:
-            keys = _STATE_KEYS[self._kind] if self._kind not in _LAYERWISE else \
-                (("exp_avg", "exp_avg_sq") if self._kind == _LAMB else ("momentum_buffer", None))
-            dsts = list(zip((path.m_flat, path.v_flat), keys))
-            if self._kind in _THIRD_KEYS:
-                dsts.append((path.m2_flat, _THIRD_KEYS[self._kind]))
+            rmsprop_tf = self._kind == _lib.OPT_RMSPROP_TF
+            if rmsprop_tf:
+                dsts = list(zip((path.m_flat, path.v_flat, path.m2_flat), _RMSPROP_TF_KEYS))
+            else:
+                keys = _STATE_KEYS[self._kind] if self._kind not in _LAYERWISE else \
+                    (("exp_avg", "exp_avg_sq") if self._kind == _LAMB else ("momentum_buffer", None))
+                dsts = list(zip((path.m_flat, path.v_flat), keys))
+                if self._kind in _THIRD_KEYS:
+                    dsts.append((path.m2_flat, _THIRD_KEYS[self._kind]))
             for local_dst, key in dsts:
                 if local_dst is None:
                     continue
-                # schedule-free: a parameter without z has not been stepped, and its z is its master (upstream's clone)
-                full = master.clone() if key == "z" else torch.zeros(path.n, dtype=torch.float32, device=dev)
+                # schedule-free: a parameter without z has not been stepped, and its z is its master (upstream's clone);
+                # RMSpropTF: square_avg starts at ones
+                if key == "z":
+                    full = master.clone()
+                elif rmsprop_tf and key == "square_avg":
+                    full = torch.ones(path.n, dtype=torch.float32, device=dev)
+                else:
+                    full = torch.zeros(path.n, dtype=torch.float32, device=dev)
                 for view, src in zip(path.unflatten(full), entries):
                     if src.get(key) is not None:
                         view.copy_(src[key].to(device=dev, dtype=torch.float32))
