@@ -483,8 +483,9 @@ class GradPath:
                                                                               | absent (local route)
       MASTER fp32 master weights                               local          aliases P when the model is fp32 and unsharded
       M, V   fp32 optimizer state                              local          owned shards (sharded) | all n
-      M2     fp32 third optimizer state (AdEMAMix's            local          indexed like M; only for those kinds
-             exp_avg_slow, RMSpropTF's grad_avg)                              (``third_state``)
+      M2     fp32 third optimizer state (AdEMAMix's            local          indexed like M
+             exp_avg_slow, RMSpropTF's grad_avg)
+             (M, V and M2 exist as ``state`` lists them: buffer -> initial value)
       AVG    fp32 weight average (EMA / SWA)                   local          indexed like MASTER; only when averaging is
                                                                               configured (``enable_weight_average``)
 
@@ -496,11 +497,11 @@ class GradPath:
 
     def __init__(self, engine: Engine, params: Sequence[torch.nn.Parameter], grad_accum: int = 1,
                  clip: Optional[ClipSpec] = None, sharded: bool = False, lp_dtype: Optional[torch.dtype] = None,
-                 module: Optional[torch.nn.Module] = None, sync_init: bool = True, needs_second_moment: bool = True,
-                 needs_first_moment: bool = True, bucket_mb: Optional[float] = None, state_id: Optional[int] = None,
-                 route: Optional[str] = None, group_of: Optional[Sequence[int]] = None, overlap: bool = True,
-                 scalar_state: int = 0, adafactor: bool = False, layerwise: bool = False, schedule_free: bool = False,
-                 third_state: bool = False, second_moment_init: float = 0.0):
+                 module: Optional[torch.nn.Module] = None, sync_init: bool = True,
+                 state: Optional[Dict[str, object]] = None, bucket_mb: Optional[float] = None,
+                 state_id: Optional[int] = None, route: Optional[str] = None, group_of: Optional[Sequence[int]] = None,
+                 overlap: bool = True, scalar_state: int = 0, adafactor: bool = False, layerwise: bool = False,
+                 schedule_free: bool = False):
         self.engine = engine
         self.params = [p for p in params if p.requires_grad]
         if not self.params:
@@ -589,9 +590,8 @@ class GradPath:
         self.MAIN = alloc(nl * 4, multicast=(route == "allreduce")) if route != "local" else None
         separate_master = self.low_precision or self.sharded
         self.MASTER = alloc(nl * 4) if separate_master else None
-        self.M = alloc(nl * 4) if needs_first_moment else None
-        self.V = alloc(nl * 4) if needs_second_moment else None
-        self.M2 = alloc(nl * 4) if third_state else None
+        state = state or {}
+        self.M, self.V, self.M2 = (alloc(nl * 4) if state.get(b) is not None else None for b in ("M", "V", "M2"))
 
         self.p_flat = self.P.tensor(self.model_dtype, self.n)
         self.g_flat = self.G.tensor(self.model_dtype, self.n)
@@ -608,6 +608,15 @@ class GradPath:
             self.master_flat = self.p_flat
             self.master_ptr = self.P.ptr
         del full32
+        # Initial optimizer state (the buffers come zeroed).  The classes create it at a parameter's first gradient (the
+        # schedule-free z as a clone of the parameter, RMSpropTF's square_avg as ones); a parameter without one is never
+        # touched, so filling at construction is the same.
+        for flat, b in ((self.m_flat, "M"), (self.v_flat, "V"), (self.m2_flat, "M2")):
+            init = state.get(b)
+            if init == "master":
+                flat.copy_(self.master_flat)
+            elif init:
+                self.scatter_local(torch.full((self.n,), float(init), dtype=torch.float32, device=dev), flat)
 
         # ---- parameter groups / unused parameters: the range table of the fused step ----
         self.group_of = list(group_of) if group_of is not None else [0] * len(self.params)
@@ -627,18 +636,10 @@ class GradPath:
         self._group_bc = torch.zeros(n_grp, 4, dtype=torch.float32, device=dev)
         self._touched = np.ones(len(self.params), dtype=bool)
         self._track_touched = False
-        # Schedule-free kinds: z lives in M and starts as the master (upstream clones p at a parameter's first gradient; a
-        # parameter without one is never touched, so cloning at construction is the same); {lr_max, weight_sum} per group
-        # on the device, advanced by stk_sf_step_prologue
+        # Schedule-free kinds: {lr_max, weight_sum} per group on the device, advanced by stk_sf_step_prologue
         self._sf_state = None
         if schedule_free:
-            self.m_flat.copy_(self.master_flat)
             self._sf_state = torch.tensor([[-1.0, 0.0]] * n_grp, dtype=torch.float64, device=dev)
-        # RMSpropTF: square_avg (V) starts at ones (timm's ones_like at a parameter's first gradient; a parameter without
-        # one is never touched, so filling at construction is the same)
-        if second_moment_init != 0.0:
-            self.scatter_local(torch.full((self.n,), float(second_moment_init), dtype=torch.float32, device=dev),
-                               self.v_flat)
 
         # ---- re-point the module at the flat buffers ----
         if self.low_precision and module is not None:

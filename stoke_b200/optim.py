@@ -36,6 +36,10 @@ every rank taking the same deterministic step on the same gradients, as the stoc
 ``LAMB`` and ``LARS`` (defined here; torch.optim has neither) take ``stk_layerwise_step``: per-parameter trust ratios from
 two whole-parameter norms, per-parameter step counts on the device, the classes' own state_dict layout, and the same
 replicated all-reduce route at world > 1.
+Each fused kind's per-parameter state is one row of ``_STATE_LAYOUT``: torch's keys in order, the flat buffer that holds
+each tensor (M, V, M2 or Adafactor's own), its initial value, the groups it exists in, and what a never-stepped
+parameter exports.  The buffers ``GradPath`` allocates (``state_buffers``), ``state_dict`` (``export_state``) and
+``load_state_dict`` (``import_state``) all follow from that row, so a new kind adds one row.
 
 ``B200StockOptimizer`` -- every other ``torch.optim`` class (the reference instantiates whatever class the user passes,
 stoke/extensions.py:53-78) and the options the fused step does not cover (amsgrad, capturable, differentiable, more than 8
@@ -44,7 +48,7 @@ is still the engine's (K1 reduce with fused cast / unscale / inf test / norm, th
 update itself is the stock optimizer stepping on per-parameter fp32 views of the flat master / main-grad buffers.
 """
 import math
-from typing import Dict, List, Optional, Tuple, Type
+from typing import Callable, Dict, List, NamedTuple, Optional, Tuple, Type, Union
 
 import torch
 
@@ -56,21 +60,6 @@ _KINDS = {torch.optim.Adam: _lib.OPT_ADAM, torch.optim.AdamW: _lib.OPT_ADAMW, to
           torch.optim.Adadelta: _lib.OPT_ADADELTA, torch.optim.Rprop: _lib.OPT_RPROP, torch.optim.ASGD: _lib.OPT_ASGD}
 # per-step scalars from stk_optim_step_prologue
 _EXT_KINDS = (_lib.OPT_NADAM, _lib.OPT_RADAM, _lib.OPT_ADAMAX, _lib.OPT_ADADELTA, _lib.OPT_RPROP, _lib.OPT_ASGD)
-# element-wise classes whose state torch creates at a parameter's first step (no state_dict entry before it)
-_LAZY_KINDS = (_lib.OPT_ADADELTA, _lib.OPT_RPROP, _lib.OPT_ASGD, _lib.OPT_LION, _lib.OPT_SF_ADAMW, _lib.OPT_SF_SGD,
-               _lib.OPT_ADEMAMIX, _lib.OPT_RMSPROP_TF)
-# torch's per-parameter state keys of the two fp32 buffers M and V (None: no V buffer)
-_STATE_KEYS = {_lib.OPT_SGD: ("momentum_buffer", None),
-               _lib.OPT_ADAM: ("exp_avg", "exp_avg_sq"), _lib.OPT_ADAMW: ("exp_avg", "exp_avg_sq"),
-               _lib.OPT_NADAM: ("exp_avg", "exp_avg_sq"), _lib.OPT_RADAM: ("exp_avg", "exp_avg_sq"),
-               _lib.OPT_ADAMAX: ("exp_avg", "exp_inf"), _lib.OPT_ADADELTA: ("square_avg", "acc_delta"),
-               _lib.OPT_RPROP: ("prev", "step_size"), _lib.OPT_ASGD: ("ax", None), _lib.OPT_LION: ("exp_avg", None),
-               _lib.OPT_SF_ADAMW: ("z", "exp_avg_sq"), _lib.OPT_SF_SGD: ("z", None),
-               _lib.OPT_ADEMAMIX: ("exp_avg_fast", "exp_avg_sq")}
-# the per-parameter state key of the third fp32 buffer M2, for the kinds that have one
-_THIRD_KEYS = {_lib.OPT_ADEMAMIX: "exp_avg_slow"}
-# per-entry scalar state carried by the step prologue: NAdam's mu_product, ASGD's (eta, mu), torch's 0-dim fp32 tensors
-_SCALAR_KEYS = {_lib.OPT_NADAM: ("mu_product",), _lib.OPT_ASGD: ("eta", "mu")}
 _STOCK_ONLY_TRUE = ("amsgrad", "capturable", "differentiable")
 # torch.optim.Adafactor (torch >= 2.5) runs on its own entry point, stk_adafactor_step, not as a kind of K2
 _ADAFACTOR = "adafactor"
@@ -633,15 +622,114 @@ class RMSpropTF(torch.optim.Optimizer):
 
 
 _KINDS[RMSpropTF] = _lib.OPT_RMSPROP_TF
-# RMSpropTF's per-parameter state keys of M, V and M2 (its own table: M exists only in groups with momentum > 0 and M2
-# only in centered groups, and V starts at ones)
-_RMSPROP_TF_KEYS = ("momentum_buffer", "square_avg", "grad_avg")
 
 # LAMB and LARS run on their own entry point, stk_layerwise_step (per-parameter trust ratios), not as kinds of K2
 _LAMB, _LARS = "lamb", "lars"
 _KINDS[LAMB] = _LAMB
 _KINDS[LARS] = _LARS
 _LAYERWISE = {_LAMB: _lib.LW_LAMB, _LARS: _lib.LW_LARS}
+
+
+class StateTensor(NamedTuple):
+    """One per-parameter state tensor of a fused kind."""
+    key: str                                         # torch's state key
+    buf: str                                         # the flat fp32 buffer: "M", "V" or "M2"; "af": Adafactor's own
+    init: Union[float, str] = 0.0                    # its value before the first step: 0.0, 1.0 or "master"
+    where: Optional[Callable[[Dict], bool]] = None   # the group condition under which it exists (None: every group)
+    none: bool = False                               # where it does not exist, a parameter exports None (else no key)
+    alloc: Optional[Callable[[Dict], bool]] = None   # the buffer exists iff some group satisfies this (None: `where`)
+
+
+class StateLayout(NamedTuple):
+    """What a fused kind keeps per parameter, in torch's ``state_dict`` format."""
+    step: bool                          # entries carry ``step`` (a 0-dim fp32 tensor)
+    scalars: Tuple[str, ...]            # scalar state, 0-dim fp32 tensors after ``step``
+    unstepped: str                      # a never-stepped parameter: "omit" (no entry, torch's lazy state), "same"
+                                        # (exported like a stepped one, at step 0) or "none" (every tensor None)
+    tensors: Tuple[StateTensor, ...]    # in torch's key order
+
+
+def _momentum(g):
+    return g["momentum"] != 0
+
+
+_ADAM_STATE = (StateTensor("exp_avg", "M"), StateTensor("exp_avg_sq", "V"))
+# Every fused kind's state.  A new kind adds one row; allocation (state_buffers), state_dict (export_state) and
+# load_state_dict (import_state) follow from it.  SGD exports its momentum buffer in every group once some group has
+# momentum: M exists for all of them.
+_STATE_LAYOUT: Dict[object, StateLayout] = {
+    _lib.OPT_SGD: StateLayout(False, (), "none", (StateTensor("momentum_buffer", "M", none=True, alloc=_momentum),)),
+    _lib.OPT_ADAM: StateLayout(True, (), "same", _ADAM_STATE),
+    _lib.OPT_ADAMW: StateLayout(True, (), "same", _ADAM_STATE),
+    _lib.OPT_RADAM: StateLayout(True, (), "same", _ADAM_STATE),
+    _lib.OPT_NADAM: StateLayout(True, ("mu_product",), "same", _ADAM_STATE),
+    _lib.OPT_ADAMAX: StateLayout(True, (), "same", (StateTensor("exp_avg", "M"), StateTensor("exp_inf", "V"))),
+    _lib.OPT_ADADELTA: StateLayout(True, (), "omit", (StateTensor("square_avg", "M"), StateTensor("acc_delta", "V"))),
+    _lib.OPT_RPROP: StateLayout(True, (), "omit", (StateTensor("prev", "M"), StateTensor("step_size", "V"))),
+    _lib.OPT_ASGD: StateLayout(True, ("eta", "mu"), "omit", (StateTensor("ax", "M"),)),
+    _lib.OPT_LION: StateLayout(True, (), "omit", (StateTensor("exp_avg", "M"),)),
+    _lib.OPT_SF_ADAMW: StateLayout(False, (), "omit", (StateTensor("z", "M", "master"),
+                                                       StateTensor("exp_avg_sq", "V"))),
+    _lib.OPT_SF_SGD: StateLayout(False, (), "omit", (StateTensor("z", "M", "master"),)),
+    _lib.OPT_ADEMAMIX: StateLayout(True, (), "omit", (
+        StateTensor("exp_avg_fast", "M", where=lambda g: g["betas"][0] != 0, none=True),
+        StateTensor("exp_avg_slow", "M2"), StateTensor("exp_avg_sq", "V"))),
+    _lib.OPT_RMSPROP_TF: StateLayout(True, (), "omit", (
+        StateTensor("square_avg", "V", 1.0), StateTensor("momentum_buffer", "M", where=lambda g: g["momentum"] > 0),
+        StateTensor("grad_avg", "M2", where=lambda g: g["centered"]))),
+    _LAMB: StateLayout(True, (), "omit", _ADAM_STATE),
+    _LARS: StateLayout(True, (), "omit", (StateTensor("momentum_buffer", "M", where=_momentum),)),
+    # row_var / col_var of a factored parameter, variance of the others: views of GradPath.af_state
+    _ADAFACTOR: StateLayout(True, (), "omit", (StateTensor("row_var", "af"), StateTensor("col_var", "af"),
+                                               StateTensor("variance", "af"))),
+}
+
+
+def state_buffers(layout: StateLayout, groups: List[Dict]) -> Dict[str, object]:
+    """The flat fp32 buffers a kind needs for these parameter groups: ``{"M", "V", "M2"} -> initial value`` (0.0, 1.0
+    or "master"), None for a buffer that is not allocated."""
+    out = {"M": None, "V": None, "M2": None}
+    for t in layout.tensors:
+        cond = t.alloc or t.where
+        if t.buf in out and (cond is None or any(cond(g) for g in groups)):
+            out[t.buf] = t.init
+    return out
+
+
+def export_state(layout: StateLayout, groups: List[Dict], group_of: List[int], sd_index: Dict[int, int],
+                 steps: List[int], scalars: Optional[List[List[float]]],
+                 views: Dict[str, List[Optional[torch.Tensor]]]) -> Dict[int, Dict]:
+    """torch's ``state`` mapping.  ``steps`` / ``scalars``: every parameter's step count and scalar state (flat order);
+    ``views``: per state key, every parameter's view of the full-length vector that holds it (None, or no key, where it
+    has none).  A tensor is exported as a clone where the parameter has a view and its group meets ``where``."""
+    state = {}
+    for i, gi in enumerate(group_of):
+        if steps[i] == 0 and layout.unstepped == "omit":
+            continue
+        if steps[i] == 0 and layout.unstepped == "none":
+            state[sd_index[i]] = {t.key: None for t in layout.tensors}
+            continue
+        d = {"step": torch.tensor(float(steps[i]))} if layout.step else {}
+        for key, val in zip(layout.scalars, scalars[i] if layout.scalars else ()):
+            d[key] = torch.tensor(val, dtype=torch.float32)
+        for t in layout.tensors:
+            view = views[t.key][i] if t.key in views else None
+            if view is not None and (t.where is None or t.where(groups[gi])):
+                d[t.key] = view.clone()
+            elif t.none:
+                d[t.key] = None
+        state[sd_index[i]] = d
+    return state
+
+
+def import_state(layout: StateLayout, entries: List[Dict], views: Dict[str, List[Optional[torch.Tensor]]]):
+    """Copies a state dict's tensors into ``views`` (as ``export_state``'s, already at their initial values).
+    ``entries``: torch's state entry of every parameter in flat order (``{}`` where it has none); a key that is missing
+    or None leaves the parameter at the initial value."""
+    for t in layout.tensors:
+        for src, view in zip(entries, views.get(t.key, ())):
+            if view is not None and src.get(t.key) is not None:
+                view.copy_(src[t.key].reshape(view.shape))
 
 
 def _module_params(module: torch.nn.Module):
@@ -719,7 +807,7 @@ def load_step_counts(kind, entries: List[Dict], group_of: List[int], opt_steps: 
             return 0
         return 1 if opt_steps is None else opt_steps
 
-    keys = _SCALAR_KEYS.get(kind, ())
+    keys = _STATE_LAYOUT[kind].scalars
     steps = [count(e, g) for e, g in zip(entries, group_of)]
     if opt_steps is None:
         opt_steps = max([s for s in steps if s is not None], default=0)
@@ -782,30 +870,19 @@ class B200FusedOptimizer(torch.optim.Optimizer):
         if self._kind == _lib.OPT_ADAM and probe.defaults.get("decoupled_weight_decay"):
             self._kind = _lib.OPT_ADAMW
         self._torch_cls = optim_cls
-        sgd = self._kind == _lib.OPT_SGD
-        any_mom = any(g.get("momentum", 0) != 0 for g in probe.param_groups)
+        self._layout = _STATE_LAYOUT[self._kind]
+        self._buffers = state_buffers(self._layout, probe.param_groups)
         ada = self._kind == _ADAFACTOR
         lw = self._kind in _LAYERWISE
-        lars = self._kind == _LARS
-        one_state = self._kind in (_lib.OPT_ASGD, _lib.OPT_LION, _lib.OPT_SF_SGD)   # a single fp32 state tensor, in M
-        needs_m = not (sgd or ada or lars) or any_mom
-        if self._kind == _lib.OPT_ADEMAMIX:   # exp_avg_fast exists only in groups with beta1 != 0
-            needs_m = any(g["betas"][0] != 0 for g in probe.param_groups)
-        rmsprop_tf = self._kind == _lib.OPT_RMSPROP_TF
-        if rmsprop_tf:   # momentum_buffer and grad_avg exist only in groups with momentum > 0 / centered
-            needs_m = any(g["momentum"] > 0 for g in probe.param_groups)
-        third = self._kind in _THIRD_KEYS or (rmsprop_tf and any(g["centered"] for g in probe.param_groups))
         if (ada or lw) and engine.world > 1:
             # Adafactor's per-parameter reductions and LAMB's / LARS's trust ratios need whole parameters on one rank: their
             # state is replicated (also under fairscale_oss) and every rank runs the same deterministic step on the same
             # all-reduced fp32 gradients
             route = "allreduce"
         self.path = GradPath(engine, params, grad_accum=grad_accum, clip=clip, sharded=sharded, lp_dtype=lp_dtype,
-                             module=module, needs_second_moment=not (sgd or ada or lars or one_state),
-                             needs_first_moment=needs_m, state_id=state_id, route=route,
-                             group_of=group_of, bucket_mb=bucket_mb, scalar_state=len(_SCALAR_KEYS.get(self._kind, ())),
-                             adafactor=ada, layerwise=lw, schedule_free=self._kind in _SF_KINDS,
-                             third_state=third, second_moment_init=1.0 if rmsprop_tf else 0.0)
+                             module=module, state=self._buffers, state_id=state_id, route=route,
+                             group_of=group_of, bucket_mb=bucket_mb, scalar_state=len(self._layout.scalars),
+                             adafactor=ada, layerwise=lw, schedule_free=self._kind in _SF_KINDS)
         by_group: List[List[torch.nn.Parameter]] = [[] for _ in extra]
         for p, gi in zip(params, group_of):
             by_group[gi].append(p)
@@ -980,10 +1057,20 @@ class B200FusedOptimizer(torch.optim.Optimizer):
         return None
 
     # -- state dict in torch's per-parameter format ----------------------------------------------------------------------
-    def _full(self, flat: Optional[torch.Tensor]) -> Optional[torch.Tensor]:
-        if flat is None:
-            return None
-        return self.path._gather_shards(flat) if self.path.sharded else flat
+    def _flats(self) -> Dict[str, torch.Tensor]:
+        """This rank's allocated state buffers, by name."""
+        path = self.path
+        flats = {"M": path.m_flat, "V": path.v_flat, "M2": path.m2_flat}
+        return {b: f for b, f in flats.items() if f is not None}
+
+    def _views(self, full: Dict[str, torch.Tensor]) -> Dict[str, List[Optional[torch.Tensor]]]:
+        """Per state key, every parameter's view of it: into the full-length vectors ``full`` (by buffer), or for
+        Adafactor into its own state buffer (row_var / col_var of a factored parameter, variance of the others)."""
+        if self._kind == _ADAFACTOR:
+            per_param = [dict(zip(("row_var", "col_var") if len(vs) == 2 else ("variance",), vs))
+                         for vs in self.path.adafactor_state_views()]
+            return {t.key: [d.get(t.key) for d in per_param] for t in self._layout.tensors}
+        return {t.key: self.path.unflatten(full[t.buf]) for t in self._layout.tensors if t.buf in full}
 
     def _groups_sd(self):
         groups, start = [], 0
@@ -999,98 +1086,15 @@ class B200FusedOptimizer(torch.optim.Optimizer):
         return {"state": state, "param_groups": self._groups_sd(), "b200_master": path.gather_master(),
                 "b200_opt_steps": int(path.engine.scaler_get(path.state_id).opt_steps)}
 
-    def _adafactor_state_dict(self):
-        """torch's format: a parameter that was never stepped has no entry (torch creates its state at its first gradient)."""
-        path = self.path
-        steps = path.param_steps()
-        state = {}
-        for i, views in enumerate(path.adafactor_state_views()):
-            if steps[i] == 0:
-                continue
-            keys = ("row_var", "col_var") if len(views) == 2 else ("variance",)
-            state[self._sd_index[i]] = dict({"step": torch.tensor(float(steps[i]))},
-                                            **{k: v.clone() for k, v in zip(keys, views)})
-        return self._export(state)
-
-    def _layerwise_state_dict(self):
-        """The classes' own format: a parameter that was never stepped has no entry; ``step``, then LAMB's ``exp_avg`` /
-        ``exp_avg_sq`` or, in a LARS group with momentum, ``momentum_buffer``."""
-        path = self.path
-        steps = path.param_steps()
-        ms = path.unflatten(path.m_flat) if path.m_flat is not None else None
-        vs = path.unflatten(path.v_flat) if path.v_flat is not None else None
-        state = {}
-        for i in range(len(path.params)):
-            if steps[i] == 0:
-                continue
-            d = {"step": torch.tensor(float(steps[i]))}
-            if self._kind == _LAMB:
-                d["exp_avg"], d["exp_avg_sq"] = ms[i].clone(), vs[i].clone()
-            elif self.param_groups[self._group_of[i]]["momentum"] != 0:
-                d["momentum_buffer"] = ms[i].clone()
-            state[self._sd_index[i]] = d
-        return self._export(state)
-
-    def _rmsprop_tf_state_dict(self):
-        """timm's format: a parameter that was never stepped has no entry; ``step``, ``square_avg``, then
-        ``momentum_buffer`` in a group with momentum > 0 and ``grad_avg`` in a centered group (absent elsewhere)."""
-        path = self.path
-        steps = path.param_steps()
-        sq, buf, ga = (path.unflatten(self._full(f)) if f is not None else None
-                       for f in (path.v_flat, path.m_flat, path.m2_flat))
-        state = {}
-        for i in range(len(path.params)):
-            if steps[i] == 0:
-                continue
-            g = self.param_groups[self._group_of[i]]
-            d = {"step": torch.tensor(float(steps[i])), "square_avg": sq[i].clone()}
-            if g["momentum"] > 0:
-                d["momentum_buffer"] = buf[i].clone()
-            if g["centered"]:
-                d["grad_avg"] = ga[i].clone()
-            state[self._sd_index[i]] = d
-        return self._export(state)
-
     def state_dict(self):
-        """torch's per-parameter format: ``step``, the scalar state (NAdam's ``mu_product``, ASGD's ``eta`` and ``mu``) as
-        0-dim fp32 tensors, then the class's state tensors.  Adadelta, Rprop, ASGD and Lion omit a parameter that was never
-        stepped (torch creates their state at its first gradient); the other kinds emit it.  SGD emits only
-        ``momentum_buffer``, None before a parameter's first step or without momentum.  AdEMAMix emits ``step``,
-        ``exp_avg_fast`` (None in a group with beta1 == 0), ``exp_avg_slow`` and ``exp_avg_sq``."""
+        """torch's per-parameter format, as ``_STATE_LAYOUT`` describes this kind: ``step``, the scalar state (NAdam's
+        ``mu_product``, ASGD's ``eta`` and ``mu``) as 0-dim fp32 tensors, then the class's state tensors.  Sharded
+        buffers are all-gathered (collective)."""
         path = self.path
-        if self._kind == _ADAFACTOR:
-            return self._adafactor_state_dict()
-        if self._kind in _LAYERWISE:
-            return self._layerwise_state_dict()
-        if self._kind == _lib.OPT_RMSPROP_TF:
-            return self._rmsprop_tf_state_dict()
-        k_m, k_v = _STATE_KEYS[self._kind]
-        k_3 = _THIRD_KEYS.get(self._kind)
-        ms = path.unflatten(self._full(path.m_flat)) if path.m_flat is not None else None
-        vs = path.unflatten(self._full(path.v_flat)) if k_v is not None else None
-        m2s = path.unflatten(self._full(path.m2_flat)) if k_3 is not None else None
-        steps = path.param_steps()
-        scal = path.param_scalars() if self._kind in _SCALAR_KEYS else None
-        state = {}
-        for i in range(len(path.params)):
-            j = self._sd_index[i]
-            if self._kind == _lib.OPT_SGD:
-                state[j] = {k_m: ms[i].clone() if ms is not None and steps[i] > 0 else None}
-                continue
-            if steps[i] == 0 and self._kind in _LAZY_KINDS:
-                continue
-            d = {} if self._kind in _SF_KINDS else {"step": torch.tensor(float(steps[i]))}
-            if scal is not None:
-                for key, val in zip(_SCALAR_KEYS[self._kind], scal[i]):
-                    d[key] = torch.tensor(val, dtype=torch.float32)
-            no_m = self._kind == _lib.OPT_ADEMAMIX and self.param_groups[self._group_of[i]]["betas"][0] == 0
-            d[k_m] = None if no_m else ms[i].clone()
-            if k_3 is not None:
-                d[k_3] = m2s[i].clone()
-            if k_v is not None:
-                d[k_v] = vs[i].clone()
-            state[j] = d
-        out = self._export(state)
+        full = {b: path._gather_shards(f) if path.sharded else f for b, f in self._flats().items()}
+        scalars = path.param_scalars() if self._layout.scalars else None
+        out = self._export(export_state(self._layout, self.param_groups, self._group_of, self._sd_index,
+                                        path.param_steps(), scalars, self._views(full)))
         if self._kind in _SF_KINDS:   # the running group state, read back from the device (one synchronisation)
             k = out["b200_opt_steps"]
             for g, src, (lr_max, weight_sum) in zip(out["param_groups"], self.param_groups, path._sf_state.tolist()):
@@ -1103,8 +1107,9 @@ class B200FusedOptimizer(torch.optim.Optimizer):
     def load_state_dict(self, sd):
         """Accepts this class's own export and a plain ``torch.optim`` state dict written by the reference
         (stoke/io_ops.py:224-236): without ``b200_master`` the fp32 master weights are rebuilt from the model parameters
-        that ``model.load_state_dict`` has just filled (load order of BaseStokeIO.load).  Step counts and scalar state
-        follow torch's lazy state creation (``load_step_counts``)."""
+        that ``model.load_state_dict`` has just filled (load order of BaseStokeIO.load).  A state tensor the checkpoint
+        lacks starts at its initial value.  Step counts and scalar state follow torch's lazy state creation
+        (``load_step_counts``)."""
         path = self.path
         for g, src in zip(self.param_groups, sd["param_groups"]):
             for k, val in src.items():
@@ -1114,39 +1119,13 @@ class B200FusedOptimizer(torch.optim.Optimizer):
         entries = [sd["state"].get(self._sd_index[i], {}) for i in range(len(path.params))]
         # the master this checkpoint continues from: its own, or (reference-written) the model weights already in P
         master = sd["b200_master"].to(device=dev, dtype=torch.float32) if "b200_master" in sd else path.p_flat.float()
+        full = {b: master.clone() if self._buffers[b] == "master" else
+                torch.full((path.n,), float(self._buffers[b]), dtype=torch.float32, device=dev) for b in self._flats()}
         if self._kind == _ADAFACTOR:
-            for src, views in zip(entries, path.adafactor_state_views()):
-                keys = ("row_var", "col_var") if len(views) == 2 else ("variance",)
-                for k, v in zip(keys, views):
-                    if k in src:
-                        v.copy_(src[k].to(device=dev, dtype=torch.float32).reshape(v.shape))
-                    else:
-                        v.zero_()
-        else:
-            rmsprop_tf = self._kind == _lib.OPT_RMSPROP_TF
-            if rmsprop_tf:
-                dsts = list(zip((path.m_flat, path.v_flat, path.m2_flat), _RMSPROP_TF_KEYS))
-            else:
-                keys = _STATE_KEYS[self._kind] if self._kind not in _LAYERWISE else \
-                    (("exp_avg", "exp_avg_sq") if self._kind == _LAMB else ("momentum_buffer", None))
-                dsts = list(zip((path.m_flat, path.v_flat), keys))
-                if self._kind in _THIRD_KEYS:
-                    dsts.append((path.m2_flat, _THIRD_KEYS[self._kind]))
-            for local_dst, key in dsts:
-                if local_dst is None:
-                    continue
-                # schedule-free: a parameter without z has not been stepped, and its z is its master (upstream's clone);
-                # RMSpropTF: square_avg starts at ones
-                if key == "z":
-                    full = master.clone()
-                elif rmsprop_tf and key == "square_avg":
-                    full = torch.ones(path.n, dtype=torch.float32, device=dev)
-                else:
-                    full = torch.zeros(path.n, dtype=torch.float32, device=dev)
-                for view, src in zip(path.unflatten(full), entries):
-                    if src.get(key) is not None:
-                        view.copy_(src[key].to(device=dev, dtype=torch.float32))
-                path.scatter_local(full, local_dst)
+            path.af_state.zero_()
+        import_state(self._layout, entries, self._views(full))
+        for b, local in self._flats().items():
+            path.scatter_local(full[b], local)
         steps, per_param, scalars = load_step_counts(self._kind, entries, self._group_of, sd.get("b200_opt_steps"),
                                                      path._range_steps is not None,
                                                      [g.get("momentum", 0.0) for g in self.param_groups],
@@ -1180,8 +1159,8 @@ class B200StockOptimizer(torch.optim.Optimizer):
                  lp_dtype: Optional[torch.dtype] = None, state_id: Optional[int] = None, bucket_mb: Optional[float] = None):
         params, group_of, extra, kw = _group_layout(module, optim_kwargs)
         self.path = GradPath(engine, params, grad_accum=grad_accum, clip=clip, sharded=False, lp_dtype=lp_dtype,
-                             module=module, needs_second_moment=False, needs_first_moment=False, state_id=state_id,
-                             route="allreduce" if engine.world > 1 else "main", group_of=None, bucket_mb=bucket_mb)
+                             module=module, state_id=state_id, route="allreduce" if engine.world > 1 else "main",
+                             group_of=None, bucket_mb=bucket_mb)
         path = self.path
         self.user_sharded = bool(sharded)
         # fp32 master parameters: per-parameter views of the flat master buffer, their .grad views of the main grads

@@ -159,8 +159,8 @@ def test_state_layout_and_int_step():
         assert torch.equal(x.detach(), y.detach())
 
 
-def test_constants_structs_and_routing():
-    from stoke_b200.optim import _EXT_KINDS, _KINDS, _LAZY_KINDS, _SCALAR_KEYS, _STATE_KEYS, _THIRD_KEYS, fused_supported
+def test_constants_structs_routing_and_state_layout():
+    from stoke_b200.optim import _EXT_KINDS, _KINDS, _STATE_LAYOUT, fused_supported
 
     assert _lib.OPT_ADEMAMIX == 12
     with open(os.path.join(ROOT, "include", "stoke_b200.h")) as f:
@@ -168,10 +168,11 @@ def test_constants_structs_and_routing():
     assert "STK_OPT_ADEMAMIX = 12" in header
     assert sb.AdEMAMix is AdEMAMix and "AdEMAMix" in sb.__all__
     assert _KINDS[AdEMAMix] == _lib.OPT_ADEMAMIX
-    assert _STATE_KEYS[_lib.OPT_ADEMAMIX] == ("exp_avg_fast", "exp_avg_sq")
-    assert _THIRD_KEYS == {_lib.OPT_ADEMAMIX: "exp_avg_slow"}
-    assert _lib.OPT_ADEMAMIX in _LAZY_KINDS and _lib.OPT_ADEMAMIX not in _EXT_KINDS
-    assert _lib.OPT_ADEMAMIX not in _SCALAR_KEYS
+    lay = _STATE_LAYOUT[_lib.OPT_ADEMAMIX]
+    assert [(t.key, t.buf) for t in lay.tensors] == [("exp_avg_fast", "M"), ("exp_avg_slow", "M2"), ("exp_avg_sq", "V")]
+    assert lay.tensors[0].none and not lay.tensors[0].where({"betas": (0.0, 0.9, 0.99)})   # None where beta1 == 0
+    assert lay.unstepped == "omit" and _lib.OPT_ADEMAMIX not in _EXT_KINDS
+    assert lay.scalars == ()
     # stk_ademamix_hyper_t: two doubles, two int64
     assert C.sizeof(_lib.AdemamixHyper) == 32
     assert [(n, getattr(_lib.AdemamixHyper, n).offset) for n, _ in _lib.AdemamixHyper._fields_] == \

@@ -110,14 +110,15 @@ def test_lazy_state_and_step_counter():
     assert torch.equal(a.detach(), a2.detach()) and torch.equal(b.detach(), b2.detach())
 
 
-def test_constants_and_export():
-    from stoke_b200.optim import _EXT_KINDS, _KINDS, _LAZY_KINDS, _SCALAR_KEYS, _STATE_KEYS
+def test_constants_and_state_layout():
+    from stoke_b200.optim import _EXT_KINDS, _KINDS, _STATE_LAYOUT
 
     assert _lib.OPT_LION == 9
     assert "Lion" in sb.__all__ and sb.Lion is Lion
     assert _KINDS[Lion] == _lib.OPT_LION
-    assert _STATE_KEYS[_lib.OPT_LION] == ("exp_avg", None)
-    assert _lib.OPT_LION in _LAZY_KINDS and _lib.OPT_LION not in _SCALAR_KEYS
+    lay = _STATE_LAYOUT[_lib.OPT_LION]
+    assert [(t.key, t.buf) for t in lay.tensors] == [("exp_avg", "M")]   # one state tensor: no V
+    assert lay.step and lay.unstepped == "omit" and lay.scalars == ()
     assert _lib.OPT_LION not in _EXT_KINDS   # no per-step scalars: the prologue runs only for per-parameter counts
     with open(os.path.join(ROOT, "include", "stoke_b200.h")) as f:
         assert "STK_OPT_LION = 9" in f.read()

@@ -174,9 +174,9 @@ def test_fused_supported_routing():
         assert not fused_supported(cls, {"lr": 1e-3}, net)
 
 
-def test_kind_of_each_class():
+def test_kind_and_state_layout_of_each_class():
     from stoke_b200 import _lib
-    from stoke_b200.optim import _KINDS, _SCALAR_KEYS, _STATE_KEYS
+    from stoke_b200.optim import _KINDS, _STATE_LAYOUT
 
     assert (_lib.OPT_ADADELTA, _lib.OPT_RPROP, _lib.OPT_ASGD) == (6, 7, 8)
     assert _KINDS[torch.optim.Adadelta] == _lib.OPT_ADADELTA
@@ -189,9 +189,10 @@ def test_kind_of_each_class():
         opt = cls([p], lr=1e-2, foreach=False)
         p.grad = torch.ones(3)
         opt.step()
-        want = {k for k in _STATE_KEYS[kind] if k} | set(_SCALAR_KEYS.get(kind, ())) | {"step"}
+        lay = _STATE_LAYOUT[kind]
+        want = {t.key for t in lay.tensors} | set(lay.scalars) | {"step"}
         assert set(opt.state[p]) == want, cls
-    assert _STATE_KEYS[_lib.OPT_ASGD][1] is None
+    assert [t.buf for t in _STATE_LAYOUT[_lib.OPT_ASGD].tensors] == ["M"]   # ASGD has no V
 
 
 def test_ext_struct_appends_fields():

@@ -142,9 +142,8 @@ def test_state_layout_and_int_step():
         assert torch.equal(x.detach(), y.detach())
 
 
-def test_constants_struct_and_routing():
-    from stoke_b200.optim import _EXT_KINDS, _KINDS, _LAZY_KINDS, _RMSPROP_TF_KEYS, _SCALAR_KEYS, _STATE_KEYS, \
-        _THIRD_KEYS, fused_supported
+def test_constants_struct_routing_and_state_layout():
+    from stoke_b200.optim import _EXT_KINDS, _KINDS, _STATE_LAYOUT, fused_supported
 
     assert _lib.OPT_RMSPROP_TF == 13
     with open(os.path.join(ROOT, "include", "stoke_b200.h")) as f:
@@ -152,10 +151,11 @@ def test_constants_struct_and_routing():
     assert "STK_OPT_RMSPROP_TF = 13" in header and "int stk_rmsprop_tf_step(" in header
     assert sb.RMSpropTF is RMSpropTF and "RMSpropTF" in sb.__all__
     assert _KINDS[RMSpropTF] == _lib.OPT_RMSPROP_TF
-    assert _RMSPROP_TF_KEYS == ("momentum_buffer", "square_avg", "grad_avg")   # M, V, M2
-    assert _lib.OPT_RMSPROP_TF not in _STATE_KEYS and _lib.OPT_RMSPROP_TF not in _THIRD_KEYS
-    assert _lib.OPT_RMSPROP_TF in _LAZY_KINDS and _lib.OPT_RMSPROP_TF not in _EXT_KINDS
-    assert _lib.OPT_RMSPROP_TF not in _SCALAR_KEYS
+    lay = _STATE_LAYOUT[_lib.OPT_RMSPROP_TF]
+    assert [(t.key, t.buf, t.init) for t in lay.tensors] == \
+        [("square_avg", "V", 1.0), ("momentum_buffer", "M", 0.0), ("grad_avg", "M2", 0.0)]
+    assert lay.unstepped == "omit" and _lib.OPT_RMSPROP_TF not in _EXT_KINDS
+    assert lay.scalars == ()
     # stk_rmsprop_tf_hyper_t: one double, three int32 (and 4 bytes of tail padding)
     assert C.sizeof(_lib.RmspropTfHyper) == 24
     assert [(n, getattr(_lib.RmspropTfHyper, n).offset) for n, _ in _lib.RmspropTfHyper._fields_] == \

@@ -188,16 +188,21 @@ def test_validation():
         (1.0, 0.9, 0.0, 0, 0.0, 2.0)
 
 
-def test_constants_struct_and_routing():
-    from stoke_b200.optim import _EXT_KINDS, _KINDS, _LAZY_KINDS, _SCALAR_KEYS, _STATE_KEYS, fused_supported
+def test_constants_struct_routing_and_state_layout():
+    from stoke_b200.optim import _EXT_KINDS, _KINDS, _STATE_LAYOUT, fused_supported
 
     assert (_lib.OPT_SF_ADAMW, _lib.OPT_SF_SGD) == (10, 11)
     assert sb.AdamWScheduleFree is AdamWScheduleFree and sb.SGDScheduleFree is SGDScheduleFree
     assert "AdamWScheduleFree" in sb.__all__ and "SGDScheduleFree" in sb.__all__
     assert _KINDS[AdamWScheduleFree] == _lib.OPT_SF_ADAMW and _KINDS[SGDScheduleFree] == _lib.OPT_SF_SGD
-    assert _STATE_KEYS[_lib.OPT_SF_ADAMW] == ("z", "exp_avg_sq") and _STATE_KEYS[_lib.OPT_SF_SGD] == ("z", None)
+    def tensors(k):
+        return [(t.key, t.buf, t.init) for t in _STATE_LAYOUT[k].tensors]
+
+    assert tensors(_lib.OPT_SF_ADAMW) == [("z", "M", "master"), ("exp_avg_sq", "V", 0.0)]
+    assert tensors(_lib.OPT_SF_SGD) == [("z", "M", "master")]
     for k in (_lib.OPT_SF_ADAMW, _lib.OPT_SF_SGD):
-        assert k in _LAZY_KINDS and k not in _EXT_KINDS and k not in _SCALAR_KEYS
+        lay = _STATE_LAYOUT[k]
+        assert lay.unstepped == "omit" and not lay.step and k not in _EXT_KINDS and lay.scalars == ()
     with open(os.path.join(ROOT, "include", "stoke_b200.h")) as f:
         header = f.read()
     assert "STK_OPT_SF_ADAMW = 10" in header and "STK_OPT_SF_SGD = 11" in header
