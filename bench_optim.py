@@ -3,8 +3,9 @@
 (109.5 M elements), with Adam as the yardstick.  By default Adam, NAdam, RAdam and Adamax; ``--kinds`` picks others, e.g.
 ``--kinds adadelta,rprop,asgd``, ``--kinds adam,lion`` (stoke_b200.Lion), ``--kinds adam,sf_adamw,sgd,sf_sgd``
 (stoke_b200.AdamWScheduleFree and SGDScheduleFree against the kinds whose bytes they move), ``--kinds adam,ademamix``
-(stoke_b200.AdEMAMix, Adam's step with a third state tensor) or ``--kinds adam,rmsprop_tf,rmsprop_tf_centered,ademamix``
-(stoke_b200.RMSpropTF with the EfficientNet recipe's settings, and centered, against the kinds whose bytes they move):
+(stoke_b200.AdEMAMix, Adam's step with a third state tensor), ``--kinds adam,rmsprop_tf,rmsprop_tf_centered,ademamix``
+(stoke_b200.RMSpropTF with the EfficientNet recipe's settings, and centered, against the kinds whose bytes they move) or
+``--kinds adam,ademamix,adan`` (stoke_b200.Adan, with a fourth state tensor):
 
   k_optim_step[raw]    the world-1 route: the step reads and zeroes the raw bf16 bucket and writes the bf16 model copy
                        (30 B/element algorithmic: read g 2, p m v 12; write p m v 12, bf16 copy 2, zeroing 2), with the
@@ -14,9 +15,9 @@
                        (momentum_buffer / z): 22 B/element; schedule-free AdamW keeps two like Adam: 30.  AdEMAMix
                        keeps three (exp_avg_fast, exp_avg_slow, exp_avg_sq): 38 B/element.  RMSpropTF with momentum
                        keeps two (square_avg, momentum_buffer) and runs without the prologue: 30 B/element; centered it
-                       keeps grad_avg too: 38
+                       keeps grad_avg too: 38.  Adan keeps four (exp_avg, exp_avg_sq, exp_avg_diff, neg_pre_grad): 46
   k_optim_step[main]   fp32 model, fp32 main gradients (28 B/element: read g p m v 16, write p m v 12; ASGD 16, Lion, SGD
-                       and schedule-free SGD 20, AdEMAMix and centered RMSpropTF 36)
+                       and schedule-free SGD 20, AdEMAMix and centered RMSpropTF 36, Adan 44)
   optimizer step       gradient pass + step, the fused route (k_grad_norm + prologue + k_optim_step) against
                        B200StockOptimizer (K1 main-gradient reduce + the class's own update on fp32 views + the cast
                        into the bf16 model), same class, same gradients, timed in alternating rounds in the same run
@@ -67,12 +68,14 @@ CLASSES = {"adam": (torch.optim.Adam, {"lr": 1e-3}), "nadam": (torch.optim.NAdam
            "rmsprop_tf": (stoke_b200.RMSpropTF, {"lr": 0.016, "alpha": 0.9, "eps": 1e-3, "momentum": 0.9,
                                                  "weight_decay": 1e-5}),
            "rmsprop_tf_centered": (stoke_b200.RMSpropTF, {"lr": 0.016, "alpha": 0.9, "eps": 1e-3, "momentum": 0.9,
-                                                          "weight_decay": 1e-5, "centered": True})}
+                                                          "weight_decay": 1e-5, "centered": True}),
+           "adan": (stoke_b200.Adan, {"lr": 1e-3, "weight_decay": 0.02})}
 # algorithmic bytes per element (raw bf16 route, main fp32 route) of the kinds with one state tensor; the others: 30, 28
 ONE_STATE_BYTES = {"asgd": (18, 16),   # ax written without being read while mu == 1
                    "lion": (22, 20), "sgd": (22, 20), "sf_sgd": (22, 20)}
 THREE_STATE_BYTES = {"ademamix": (38, 36),   # the first and second moments plus exp_avg_slow
-                     "rmsprop_tf_centered": (38, 36)}   # square_avg, momentum_buffer and grad_avg
+                     "rmsprop_tf_centered": (38, 36),   # square_avg, momentum_buffer and grad_avg
+                     "adan": (46, 44)}   # four: exp_avg, exp_avg_sq, exp_avg_diff and neg_pre_grad
 SCHEDULE_FREE = ("sf_adamw", "sf_sgd")   # a new optimizer is in eval mode: train() before stepping
 
 

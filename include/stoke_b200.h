@@ -96,11 +96,15 @@ typedef enum {
                              written in a group with beta1 == 0), exp_avg_sq = exp_avg_sq, exp_avg_slow = exp_avg_slow.
                              Reads lr, beta1, beta2, eps and weight_decay of stk_optim_hyper_t; the per-step scalars from
                              group_bc / range_bc of stk_ademamix_step_prologue */
-  STK_OPT_RMSPROP_TF = 13 /* stoke_b200.optim.RMSpropTF (TensorFlow-style RMSprop, timm's RMSpropTF); only through
+  STK_OPT_RMSPROP_TF = 13, /* stoke_b200.optim.RMSpropTF (TensorFlow-style RMSprop, timm's RMSpropTF); only through
                              stk_rmsprop_tf_step.  exp_avg = momentum_buffer (not read or written in a group with
                              momentum == 0), exp_avg_sq = square_avg, exp_avg_slow = grad_avg (not read or written in a
                              group that is not centered).  Reads lr, eps, weight_decay and momentum of stk_optim_hyper_t
                              and the group's stk_rmsprop_tf_hyper_t; no per-step scalars */
+  STK_OPT_ADAN = 14       /* stoke_b200.optim.Adan (Xie et al. 2022); only through stk_adan_step.  exp_avg = exp_avg,
+                             exp_avg_sq = exp_avg_sq, exp_avg_slow = exp_avg_diff, and a fourth stream neg_pre_grad.
+                             Reads beta1, beta2, eps and weight_decay of stk_optim_hyper_t and the group's
+                             stk_adan_hyper_t; the per-step scalars from group_bc / range_bc of stk_adan_step_prologue */
 } stk_optim_kind;
 
 /* flags of stk_grad_reduce */
@@ -312,7 +316,8 @@ typedef struct {
   float* exp_avg_slow;    /* the third fp32 state tensor, indexed like exp_avg; ADEMAMIX (required there) and RMSPROP_TF
                              only.  ADEMAMIX also needs exp_avg_sq, and exp_avg unless every group has beta1 == 0 */
 } stk_optim_args_t;
-/* Every kind but RMSPROP_TF, which is refused here (its per-group hyper-parameters go through stk_rmsprop_tf_step). */
+/* Every kind but RMSPROP_TF and ADAN, which are refused here (their per-group hyper-parameters go through
+ * stk_rmsprop_tf_step and stk_adan_step). */
 int stk_optim_step_ex(stk_ctx* ctx, const stk_optim_args_t* args, void* stream);
 
 /* Per-group hyper-parameters of STK_OPT_RMSPROP_TF that stk_optim_hyper_t has no field for (timm's RMSpropTF). */
@@ -336,6 +341,32 @@ typedef struct {
  * with every product, difference, sum, sqrt and division rounded on its own (IEEE, round to nearest). */
 int stk_rmsprop_tf_step(stk_ctx* ctx, const stk_optim_args_t* args, const stk_rmsprop_tf_hyper_t* rmsprop_tf,
                         void* stream);
+
+/* Per-group hyper-parameters of STK_OPT_ADAN that stk_optim_hyper_t has no field for (the official Adan's arguments). */
+typedef struct {
+  double beta3;            /* the exp_avg_sq decay */
+  int32_t no_prox;         /* 1: weight decay multiplies p by (1 - lr wd) before the update; 0: divides it by (1 + lr wd)
+                              after */
+} stk_adan_hyper_t;
+/* The fused step of STK_OPT_ADAN: stk_optim_step_ex's arguments, routes and launch, plus one stk_adan_hyper_t per group
+ * (args->n_groups, host array) and the fourth fp32 state tensor neg_pre_grad (DEVICE, indexed like exp_avg).
+ * args->hyper[*].kind must be STK_OPT_ADAN.  exp_avg, exp_avg_sq, exp_avg_slow (exp_avg_diff) and neg_pre_grad are
+ * required, and so are the scalars of stk_adan_step_prologue (group_bc, or range_bc with per-parameter step counts):
+ * bc = {s, s_d, r, first}.  One element with the formed gradient g (after unscale, accumulation and clip), m = exp_avg,
+ * d = exp_avg_diff, n = exp_avg_sq, P = neg_pre_grad, all in fp32 (fp32(x): the python double x rounded to fp32):
+ *   P = -g if first;  x = P + g
+ *   m = fma(g, fp32(1 - beta1), m * fp32(beta1));  d = fma(x, fp32(1 - beta2), d * fp32(beta2))
+ *   u = x * fp32(beta2) + g;  n = fma(fp32(1 - beta3), u * u, n * fp32(beta3));  den = sqrt(n) * r + eps
+ *   no_prox: p = p * fp32(1 - lr wd);  p = fma(-s, m / den, p);  p = fma(-s_d, d / den, p)
+ *   else:    p = fma(-s, m / den, p);  p = fma(-s_d, d / den, p);  p = p * fp32(1 / (1 + lr wd))
+ *   P = 0 + (-g)
+ * with every product, sum, sqrt and division rounded on its own (IEEE, round to nearest).  That is Adan.step on CUDA
+ * fp32 tensors: torch's CUDA true division by a python scalar b multiplies by fp32(1 / b), the reciprocal taken in
+ * double (not fp32(1 / fp32(b)), which differs for some b, e.g. sqrt(1 - 0.99^2)), so `/ sqrt(bc3)` and
+ * `div_(1 + lr wd)` are multiplications by that reciprocal.  A skipped step (found_inf, or a skipped range) writes no
+ * state, neg_pre_grad included; the raw bucket is still zeroed. */
+int stk_adan_step(stk_ctx* ctx, const stk_optim_args_t* args, const stk_adan_hyper_t* adan, float* neg_pre_grad,
+                  void* stream);
 
 /* Weight-average update over n fp32 elements (n a multiple of 4, both pointers 16-byte aligned), one launch on `stream`:
  * mode 1: avg = master;  mode 2: avg = torch.lerp(avg, master, weight) on fp32 -- for |weight| < 0.5
@@ -424,6 +455,18 @@ typedef struct {
 int stk_ademamix_step_prologue(stk_ctx* ctx, const stk_optim_hyper_t* hyper, const stk_ademamix_hyper_t* ademamix,
                                int n_groups, int n_ranges, const uint8_t* range_group, int32_t* range_steps, float* bc,
                                void* stream);
+
+/* The per-step scalars of STK_OPT_ADAN, with stk_ademamix_step_prologue's range / group / found_inf semantics (call it
+ * right before stk_adan_step, same stream; pass bc as the step's range_bc when n_ranges > 0, else as its group_bc).
+ * Adan keeps its step count in the group, so the bias corrections use t = the selected state's optimizer-wide counter
+ * + 1 for every entry.  In double, in the order of the python formulas (no contraction):
+ *   bc1 = 1 - beta1^t;  bc2 = 1 - beta2^t;  bc3 = 1 - beta3^t
+ *   bc[4j..4j+3] = fp32 {lr / bc1, lr beta2 / bc2, 1 / sqrt(bc3), first}
+ * with first = 1 when t == 1 or (n_ranges > 0) the range has taken no step yet: its neg_pre_grad is taken as -g, so the
+ * first gradient difference is 0.  lr, beta1 and beta2 come from hyper, beta3 from adan.  Unless the range is skipped or
+ * the step found inf, range_steps[j] advances. */
+int stk_adan_step_prologue(stk_ctx* ctx, const stk_optim_hyper_t* hyper, const stk_adan_hyper_t* adan, int n_groups,
+                           int n_ranges, const uint8_t* range_group, int32_t* range_steps, float* bc, void* stream);
 
 /* scaler.update(), opt_steps/skipped_steps bookkeeping, reset of the per-step accumulators */
 int stk_step_epilogue(stk_ctx* ctx, void* stream);

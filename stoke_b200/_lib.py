@@ -16,7 +16,7 @@ NORM_NONE, NORM_L2, NORM_INF, NORM_P = 0, 1, 2, 3
 CLIP_NONE, CLIP_NORM, CLIP_VALUE = 0, 1, 2
 OPT_ADAM, OPT_ADAMW, OPT_SGD, OPT_NADAM, OPT_RADAM, OPT_ADAMAX = 0, 1, 2, 3, 4, 5
 OPT_ADADELTA, OPT_RPROP, OPT_ASGD, OPT_LION = 6, 7, 8, 9
-OPT_SF_ADAMW, OPT_SF_SGD, OPT_ADEMAMIX, OPT_RMSPROP_TF = 10, 11, 12, 13
+OPT_SF_ADAMW, OPT_SF_SGD, OPT_ADEMAMIX, OPT_RMSPROP_TF, OPT_ADAN = 10, 11, 12, 13, 14
 ACT_RELU, ACT_SILU, ACT_HARDSWISH, ACT_RELU6 = 0, 1, 2, 3
 RF_FINAL, RF_ZERO_INPUT, RF_UNSCALE = 1, 2, 4
 OPT_K1_ALGO, OPT_MEM_MODE, OPT_K1_MAX_BLOCKS, OPT_COOP_LAUNCH, OPT_NVLS_MAX_BLOCKS, OPT_K2_AG_MC = 1, 2, 3, 4, 5, 6
@@ -80,6 +80,10 @@ class AdemamixHyper(C.Structure):
 class RmspropTfHyper(C.Structure):
     _fields_ = [("alpha", C.c_double), ("centered", C.c_int32), ("decoupled_decay", C.c_int32),
                 ("lr_in_momentum", C.c_int32)]
+
+
+class AdanHyper(C.Structure):
+    _fields_ = [("beta3", C.c_double), ("no_prox", C.c_int32)]
 
 
 class AdafactorParam(C.Structure):
@@ -185,6 +189,9 @@ _SIGNATURES = {
     "stk_ademamix_step_prologue": (C.c_int, [_P, C.POINTER(OptimHyper), C.POINTER(AdemamixHyper), C.c_int, C.c_int, _P,
                                              _P, _P, _P]),
     "stk_rmsprop_tf_step": (C.c_int, [_P, C.POINTER(OptimArgs), C.POINTER(RmspropTfHyper), _P]),
+    "stk_adan_step": (C.c_int, [_P, C.POINTER(OptimArgs), C.POINTER(AdanHyper), _P, _P]),
+    "stk_adan_step_prologue": (C.c_int, [_P, C.POINTER(OptimHyper), C.POINTER(AdanHyper), C.c_int, C.c_int, _P, _P, _P,
+                                         _P]),
     "stk_step_epilogue": (C.c_int, [_P, _P]),
     "stk_adafactor_plan": (C.c_int, [C.POINTER(AdafactorParam), C.c_int, C.POINTER(AdafactorPlan)]),
     "stk_adafactor_step": (C.c_int, [_P, C.POINTER(AdafactorArgs), _P]),

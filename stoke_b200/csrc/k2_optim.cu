@@ -1,7 +1,7 @@
 // k2_optim.cu -- K2: single-pass fused optimizer step (Adam / AdamW / SGD-momentum / NAdam / RAdam / Adamax / Adadelta /
-// Rprop / ASGD / Lion / schedule-free AdamW and SGD / AdEMAMix / TensorFlow-style RMSprop), plus the step prologues (per-parameter step counts,
-// NAdam's mu_product, ASGD's eta and mu; the schedule-free group scalars; AdEMAMix's bias corrections and warm-ups) and
-// epilogue.
+// Rprop / ASGD / Lion / schedule-free AdamW and SGD / AdEMAMix / TensorFlow-style RMSprop / Adan), plus the step prologues
+// (per-parameter step counts, NAdam's mu_product, ASGD's eta and mu; the schedule-free group scalars; AdEMAMix's bias
+// corrections and warm-ups; Adan's step sizes and first-step flags) and epilogue.
 //
 // One sweep over (grad, master, exp_avg, exp_avg_sq) does what the reference spreads over clip_grad_norm_'s scaling pass /
 // clip_grad_value_, GradScaler.step's inf gate, the ~7 foreach kernels of torch.optim.Adam and (mixed precision) the
@@ -14,8 +14,8 @@
 // z (exp_avg) and exp_avg_sq like Adam: 28 / 30; schedule-free SGD keeps z only: 20 / 22.  AdEMAMix keeps a third
 // tensor (exp_avg_slow, in m2) besides exp_avg_fast and exp_avg_sq: 36 / 38, and 28 / 30 in a group with beta1 == 0,
 // which neither reads nor writes exp_avg_fast.  RMSpropTF keeps square_avg (v), momentum_buffer (m) in a group with
-// momentum and grad_avg (m2) in a centered group: 20 / 22 with neither, 28 / 30 with momentum, 36 / 38 with both.  The
-// clip coefficient, the skip decision and the bias corrections come from device memory, so there is no host synchronisation anywhere on the
+// momentum and grad_avg (m2) in a centered group: 20 / 22 with neither, 28 / 30 with momentum, 36 / 38 with both.  Adan
+// keeps four (exp_avg, exp_avg_sq, exp_avg_diff in m2 and neg_pre_grad in m3): 44 / 46.  The clip coefficient, the skip decision and the bias corrections come from device memory, so there is no host synchronisation anywhere on the
 // step.
 //
 // Gradient sources:  MAIN  -- fp32 reduced / unscaled gradients written by K1 (cross-rank routes), indexed like the state;
@@ -30,8 +30,8 @@
 // torch/optim/sgd.py (_single_tensor_sgd), nadam.py (_single_tensor_nadam), radam.py (_single_tensor_radam), adamax.py
 // (_single_tensor_adamax), adadelta.py (_single_tensor_adadelta), rprop.py (_single_tensor_rprop) and asgd.py
 // (_single_tensor_asgd); Lion follows stoke_b200.optim.Lion.step (torch has no Lion), the schedule-free kinds
-// stoke_b200.optim.AdamWScheduleFree.step / SGDScheduleFree.step, AdEMAMix stoke_b200.optim.AdEMAMix.step and
-// RMSpropTF stoke_b200.optim.RMSpropTF.step, each rounded like those steps on CUDA; the clip follows
+// stoke_b200.optim.AdamWScheduleFree.step / SGDScheduleFree.step, AdEMAMix stoke_b200.optim.AdEMAMix.step,
+// RMSpropTF stoke_b200.optim.RMSpropTF.step and Adan stoke_b200.optim.Adan.step, each rounded like those steps on CUDA; the clip follows
 // torch/nn/utils/clip_grad.py:165-174 (coef = max_norm / (total_norm + 1e-6), clamped to 1) and :291-292 (clamp).
 #include <cstdlib>
 
@@ -43,9 +43,9 @@ struct GroupHyperD {   // host-side doubles, converted exactly like torch conver
   double lr, beta1, beta2, eps, weight_decay, momentum, dampening;
   int nesterov, maximize;
   double momentum_decay;  // NAdam
-  int decoupled;          // NAdam / RAdam: decoupled weight decay; RMSpropTF: decoupled_decay
+  int decoupled;          // NAdam / RAdam: decoupled weight decay; RMSpropTF: decoupled_decay; Adan: no_prox
   int centered;           // RMSpropTF (in the padding before rho, so that no field moves)
-  double rho;                                    // Adadelta; RMSpropTF: alpha (the square_avg decay, like rho)
+  double rho;                                    // Adadelta; RMSpropTF: alpha (the square_avg decay, like rho); Adan: beta3
   // Rprop's four; RMSpropTF keeps its momentum constants in the first two (stk_rmsprop_tf_step fills them)
   union {
     double etaminus;
@@ -73,17 +73,19 @@ struct GroupHyperS {   // what the inner loop reads (shared memory, one entry pe
   union {
     float one_m_rho;                            // Adadelta
     float c3;                                   // the fourth per-step scalar: schedule-free AdamW's fp32(1 / bc2),
-                                                // AdEMAMix's 1 - beta3_t
+                                                // AdEMAMix's 1 - beta3_t, Adan's first-step flag
     float one_m_alpha;                          // RMSpropTF: fp32(1 - alpha)
   };
-  // Rprop's four; RMSpropTF keeps its momentum constants in the first three
+  // Rprop's four; RMSpropTF keeps its momentum constants in the first three, Adan its beta3 in the first two
   union {
     float etaminus;
     float buf_c;                                // RMSpropTF: momentum_buffer's addcdiv value (lr, or 1)
+    float b3;                                   // Adan: fp32(beta3)
   };
   union {
     float etaplus;
     float upd_c;                                // RMSpropTF: the update's coefficient on momentum_buffer (1, or lr)
+    float one_m_b3;                             // Adan: fp32(1 - beta3)
   };
   union {
     float ss_min;
@@ -130,6 +132,7 @@ struct OptimParams {
                                              // RMSpropTF: likewise, some group has no momentum
   int m2_deferred;                           // RMSpropTF: some group is not centered, so m2 is loaded once the range is
                                              // known (in the tail padding: the struct keeps its size)
+  float* m3;                                 // Adan: neg_pre_grad (the block grows from 1984 to 1992 bytes)
 };
 
 // floats of per-entry scalar state the prologue carries (the stk_optim_step_prologue `scalar_state` array)
@@ -263,13 +266,15 @@ __global__ void __launch_bounds__(256, KIND >= STK_OPT_NADAM ? 2 : 0) k_optim_st
   const bool use_m = (KIND != STK_OPT_SGD && KIND != STK_OPT_ADEMAMIX && KIND != STK_OPT_RMSPROP_TF) || p.m != nullptr;
   // ASGD, Lion and schedule-free SGD: one state tensor (ax / exp_avg / z, in p.m)
   constexpr bool kHasV = KIND != STK_OPT_SGD && KIND != STK_OPT_ASGD && KIND != STK_OPT_LION && KIND != STK_OPT_SF_SGD;
-  constexpr bool kHasM2 = KIND == STK_OPT_ADEMAMIX || KIND == STK_OPT_RMSPROP_TF;
+  constexpr bool kHasM2 = KIND == STK_OPT_ADEMAMIX || KIND == STK_OPT_RMSPROP_TF || KIND == STK_OPT_ADAN;
+  constexpr bool kHasM3 = KIND == STK_OPT_ADAN;
   constexpr bool kDeferM = KIND == STK_OPT_ADEMAMIX || KIND == STK_OPT_RMSPROP_TF;   // m may exist in some groups only
   const size_t stride = PERSIST ? size_t(gridDim.x) * blockDim.x * VPT : 0;
   size_t i = (size_t(blockIdx.x) * blockDim.x + threadIdx.x) * VPT;
 
   float g[VPT][8], w[VPT][8], m[VPT][8], v[VPT][8];
   float m2[kHasM2 ? VPT : 1][8];
+  float m3[kHasM3 ? VPT : 1][8];
   size_t gv = 0;
   int nv = 0;
   auto load = [&]() {
@@ -289,8 +294,10 @@ __global__ void __launch_bounds__(256, KIND >= STK_OPT_NADAM ? 2 : 0) k_optim_st
         if (use_m && KIND != STK_OPT_ASGD && !(kDeferM && p.m_deferred)) InVec<STK_F32>::load(p.m, i + k, m[k]);
         if (kHasV) InVec<STK_F32>::load(p.v, i + k, v[k]);
         if constexpr (kHasM2) {
-          if (KIND == STK_OPT_ADEMAMIX || (p.m2 != nullptr && !p.m2_deferred)) InVec<STK_F32>::load(p.m2, i + k, m2[k]);
+          if (KIND == STK_OPT_ADEMAMIX || KIND == STK_OPT_ADAN || (p.m2 != nullptr && !p.m2_deferred))
+            InVec<STK_F32>::load(p.m2, i + k, m2[k]);
         }
+        if constexpr (kHasM3) InVec<STK_F32>::load(p.m3, i + k, m3[k]);
       }
     if constexpr (RAW) {
       if (p.acc != nullptr) {
@@ -345,7 +352,8 @@ __global__ void __launch_bounds__(256, KIND >= STK_OPT_NADAM ? 2 : 0) k_optim_st
       o.ss_max = (float)h.step_size_max;
     }
     if constexpr (KIND == STK_OPT_LION) o.b1 = (float)h.beta1;
-    if constexpr (KIND == STK_OPT_SF_ADAMW || KIND == STK_OPT_SF_SGD || KIND == STK_OPT_ADEMAMIX) o.c3 = c.w;
+    if constexpr (KIND == STK_OPT_SF_ADAMW || KIND == STK_OPT_SF_SGD || KIND == STK_OPT_ADEMAMIX || KIND == STK_OPT_ADAN)
+      o.c3 = c.w;
     if constexpr (KIND == STK_OPT_ADEMAMIX) o.no_m1 = h.beta1 == 0.0;
     if constexpr (KIND == STK_OPT_RMSPROP_TF) {
       o.one_m_alpha = (float)(1.0 - h.rho);
@@ -354,6 +362,15 @@ __global__ void __launch_bounds__(256, KIND >= STK_OPT_NADAM ? 2 : 0) k_optim_st
       o.has_mom = h.momentum > 0.0;
       o.buf_c = (float)h.buf_c;
       o.upd_c = (float)h.upd_c;
+    }
+    if constexpr (KIND == STK_OPT_ADAN) {
+      o.b1 = (float)h.beta1;
+      o.b3 = (float)h.rho;
+      o.one_m_b3 = (float)(1.0 - h.rho);
+      // python's 1 - lr * wd (no_prox, a multiplier) or 1 + lr * wd (a divisor: torch's CUDA division by a python
+      // scalar b multiplies by fp32(1 / b), the reciprocal taken in double), without a DFMA
+      const double lr_wd = __dmul_rn(h.lr, h.weight_decay);
+      o.decay_mul = (float)(h.decoupled ? __dadd_rn(1.0, -lr_wd) : __ddiv_rn(1.0, __dadd_rn(1.0, lr_wd)));
     }
     s_g[threadIdx.x] = o;
   }
@@ -376,7 +393,7 @@ __global__ void __launch_bounds__(256, KIND >= STK_OPT_NADAM ? 2 : 0) k_optim_st
       h.c0 = bc.x;
       h.c1 = bc.y;
       h.c2 = bc.z;
-      if constexpr (KIND == STK_OPT_ADEMAMIX) h.c3 = bc.w;
+      if constexpr (KIND == STK_OPT_ADEMAMIX || KIND == STK_OPT_ADAN) h.c3 = bc.w;
     }
     const bool skip = skip_all || (rb & 0x80u);
     if (!skip) {
@@ -532,6 +549,24 @@ __global__ void __launch_bounds__(256, KIND >= STK_OPT_NADAM ? 2 : 0) k_optim_st
               ww = fmaf(-h.lr, q, ww);                               // p.addcdiv_(grad, avg, value=-lr)
             }
             v[k][e] = sq;
+          } else if (KIND == STK_OPT_ADAN) {
+            // per-step scalars (k_adan_prologue): c0 = lr / bc1, c1 = lr beta2 / bc2, c2 = 1 / sqrt(bc3),
+            // c3 = first (neg_pre_grad = -g, so the first difference is 0)
+            const float x = __fadd_rn(h.c3 != 0.f ? -gg : m3[k][e], gg);       // P.add_(g): g - g_prev
+            const float mm = fmaf(gg, h.one_m_b1, __fmul_rn(m[k][e], h.b1));   // exp_avg.mul_(b1).add_(g, alpha=1 - b1)
+            const float dd = fmaf(x, h.one_m_b2, __fmul_rn(m2[k][e], h.b2));   // exp_avg_diff likewise with P, beta2
+            const float u = __fadd_rn(__fmul_rn(x, h.b2), gg);                 // P.mul_(beta2).add_(g)
+            // exp_avg_sq.mul_(beta3).addcmul_(P, P, value=1 - beta3): addcmul rounds P * P first
+            const float nn = fmaf(h.one_m_b3, __fmul_rn(u, u), __fmul_rn(v[k][e], h.b3));
+            const float den = __fadd_rn(__fmul_rn(__fsqrt_rn(nn), h.c2), h.eps);  // (sqrt(n) / sqrt(bc3)).add_(eps)
+            if (h.decoupled) ww = __fmul_rn(ww, h.decay_mul);                   // no_prox: p.mul_(1 - lr wd)
+            ww = fmaf(-h.c0, __fdiv_rn(mm, den), ww);                           // addcdiv is one FFMA on the quotient
+            ww = fmaf(-h.c1, __fdiv_rn(dd, den), ww);
+            if (!h.decoupled) ww = __fmul_rn(ww, h.decay_mul);                  // p.div_(1 + lr wd)
+            m[k][e] = mm;
+            m2[k][e] = dd;
+            v[k][e] = nn;
+            m3[k][e] = __fadd_rn(0.f, -gg);                                     // P.zero_().add_(g, alpha=-1)
           } else {  // SGD
             if (h.wd != 0.f) gg = fmaf(ww, h.wd, gg);
             if (h.mom != 0.f) {
@@ -553,8 +588,9 @@ __global__ void __launch_bounds__(256, KIND >= STK_OPT_NADAM ? 2 : 0) k_optim_st
             st_stream_f8(p.m + (i + k) * 8, m[k]);
           if (kHasV) st_stream_f8(p.v + (i + k) * 8, v[k]);
           if constexpr (kHasM2) {
-            if (KIND == STK_OPT_ADEMAMIX || h.centered) st_stream_f8(p.m2 + (i + k) * 8, m2[k]);
+            if (KIND == STK_OPT_ADEMAMIX || KIND == STK_OPT_ADAN || h.centered) st_stream_f8(p.m2 + (i + k) * 8, m2[k]);
           }
+          if constexpr (kHasM3) st_stream_f8(p.m3 + (i + k) * 8, m3[k]);
         }
       store_lp<LP_DT, VPT>(p, gv, w, nv);
     }
@@ -663,6 +699,35 @@ __global__ void k_ademamix_prologue(const AdemamixPrologueParams p) {
   StepEntry e;
   if (!step_entry(p.n_groups, p.n_ranges, p.range_group, p.range_steps, p.scaler, e)) return;
   p.bc[e.j] = ademamix_scalars(p.beta1[e.group], p.beta2[e.group], p.a[e.group], (double)(e.done + 1));
+  if (e.advance) step_entry_advance(e, p.range_steps);
+}
+
+struct AdanPrologueParams {
+  double lr[STK_MAX_GROUPS], beta1[STK_MAX_GROUPS], beta2[STK_MAX_GROUPS];
+  stk_adan_hyper_t a[STK_MAX_GROUPS];
+  int n_groups, n_ranges;
+  const uint8_t* range_group;
+  int32_t* range_steps;
+  float4* bc;
+  const stk_scaler_state_t* scaler;
+};
+
+// stk_optim_step_prologue's bookkeeping with Adan.step's scalars.  The bias corrections use the optimizer-wide count (Adan
+// keeps `step` in the group); an entry's own count only says whether it has a previous gradient.  In python doubles and
+// python's order (the explicit roundings keep nvcc from contracting, which python does not do):
+// {lr / bc1, lr * beta2 / bc2, 1 / sqrt(bc3), first}
+__global__ void k_adan_prologue(const AdanPrologueParams p) {
+  StepEntry e;
+  if (!step_entry(p.n_groups, p.n_ranges, p.range_group, p.range_steps, p.scaler, e)) return;
+  const unsigned gi = e.group;
+  const int64_t done = p.scaler->opt_steps;
+  const double t = (double)(done + 1);
+  const double bc1 = __dadd_rn(1.0, -pow(p.beta1[gi], t));
+  const double bc2 = __dadd_rn(1.0, -pow(p.beta2[gi], t));
+  const double bc3 = __dadd_rn(1.0, -pow(p.a[gi].beta3, t));
+  const bool first = done == 0 || e.done == 0;   // upstream: "neg_pre_grad" not in state or group["step"] == 1
+  p.bc[e.j] = make_float4((float)__ddiv_rn(p.lr[gi], bc1), (float)__ddiv_rn(__dmul_rn(p.lr[gi], p.beta2[gi]), bc2),
+                          (float)__ddiv_rn(1.0, __dsqrt_rn(bc3)), first ? 1.f : 0.f);
   if (e.advance) step_entry_advance(e, p.range_steps);
 }
 
@@ -783,7 +848,10 @@ static cudaError_t launch_optim(stk_ctx* c, const OptimParams& p, int lp_dtype, 
   }
   if (p.cross_rank) {
     if (lp_dtype == STK_BF16) {
-      if (pair && p.lp_mc == nullptr) return launch_one(c, k_optim_step<KIND, STK_BF16, true, 2, STK_F32, false>, p, true, 2, s);
+      // Adan's four state streams spill in two vectors per thread under __launch_bounds__(256, 2): one vector only
+      if constexpr (KIND != STK_OPT_ADAN) {
+        if (pair && p.lp_mc == nullptr) return launch_one(c, k_optim_step<KIND, STK_BF16, true, 2, STK_F32, false>, p, true, 2, s);
+      }
       return launch_one(c, k_optim_step<KIND, STK_BF16, true, 1, STK_F32, false>, p, true, 1, s);
     }
     return launch_one(c, k_optim_step<KIND, STK_F32, true, 1, STK_F32, false>, p, true, 1, s);
@@ -793,17 +861,23 @@ static cudaError_t launch_optim(stk_ctx* c, const OptimParams& p, int lp_dtype, 
   return launch_one(c, k_optim_step<KIND, STK_F32, false, 1, STK_F32, false>, p, false, 1, s);
 }
 
-// The body of stk_optim_step_ex and stk_rmsprop_tf_step: rt is the RMSPROP_TF groups' array (nullptr for every other
-// kind, which the callers check)
-static int optim_step(stk_ctx* c, const stk_optim_args_t* a, const stk_rmsprop_tf_hyper_t* rt, void* stream) {
+// The body of stk_optim_step_ex, stk_rmsprop_tf_step and stk_adan_step: rt is the RMSPROP_TF groups' array, ad the ADAN
+// groups' array and m3 ADAN's neg_pre_grad (nullptr for every other kind, which the callers check)
+static int optim_step(stk_ctx* c, const stk_optim_args_t* a, const stk_rmsprop_tf_hyper_t* rt,
+                      const stk_adan_hyper_t* ad, float* m3, void* stream) {
   STK_REQUIRE(c, c && a && a->hyper && a->master && a->grad, "stk_optim_step_ex: NULL argument");
   STK_REQUIRE(c, a->n_groups >= 1 && a->n_groups <= STK_MAX_GROUPS, "stk_optim_step_ex: n_groups must be in [1, 8]");
   STK_REQUIRE(c, a->n_local % 8 == 0, "stk_optim_step_ex: n_local must be a multiple of 8");
   const stk_optim_hyper_t* h = a->hyper;
-  STK_REQUIRE(c, h->kind >= STK_OPT_ADAM && h->kind <= STK_OPT_RMSPROP_TF, "stk_optim_step_ex: bad optimizer kind");
+  STK_REQUIRE(c, h->kind >= STK_OPT_ADAM && h->kind <= STK_OPT_ADAN, "stk_optim_step_ex: bad optimizer kind");
   const bool sf = h->kind == STK_OPT_SF_ADAMW || h->kind == STK_OPT_SF_SGD;
   const bool ademamix = h->kind == STK_OPT_ADEMAMIX;
   const bool rmsprop_tf = h->kind == STK_OPT_RMSPROP_TF;
+  const bool adan = h->kind == STK_OPT_ADAN;
+  STK_REQUIRE(c, !adan || a->group_bc || (a->n_ranges > 0 && a->range_bc),
+              "stk_adan_step: needs the scalars of stk_adan_step_prologue (group_bc or range_bc)");
+  STK_REQUIRE(c, !adan || (a->exp_avg && a->exp_avg_sq && a->exp_avg_slow && m3),
+              "stk_adan_step: needs exp_avg, exp_avg_sq, exp_avg_slow (exp_avg_diff) and neg_pre_grad");
   STK_REQUIRE(c, !sf || a->group_bc, "stk_optim_step_ex: the schedule-free kinds need group_bc of stk_sf_step_prologue");
   STK_REQUIRE(c, h->kind <= STK_OPT_SGD || h->kind == STK_OPT_LION || rmsprop_tf || a->group_bc ||
                      (a->n_ranges > 0 && a->range_bc),
@@ -912,7 +986,8 @@ static int optim_step(stk_ctx* c, const stk_optim_args_t* a, const stk_rmsprop_t
   // the schedule-free scalars belong to the group (upstream keeps k per group), whatever the range table says
   p.range_bc = (a->n_ranges > 0 && !sf) ? reinterpret_cast<const float4*>(a->range_bc) : nullptr;
   p.group_bc = reinterpret_cast<const float4*>(a->group_bc);
-  p.m2 = ademamix ? a->exp_avg_slow : nullptr;
+  p.m2 = (ademamix || adan) ? a->exp_avg_slow : nullptr;
+  p.m3 = adan ? m3 : nullptr;
   p.m_deferred = (ademamix && a->exp_avg && any_b1_zero) ? 1 : 0;
   if (rmsprop_tf) {
     p.m = any_rms_mom ? a->exp_avg : nullptr;
@@ -926,6 +1001,12 @@ static int optim_step(stk_ctx* c, const stk_optim_args_t* a, const stk_rmsprop_t
       d.decoupled = rt[gi].decoupled_decay != 0;
       d.buf_c = rt[gi].lr_in_momentum ? h[gi].lr : 1.0;
       d.upd_c = rt[gi].lr_in_momentum ? 1.0 : h[gi].lr;
+    }
+  }
+  if (adan) {
+    for (int gi = 0; gi < a->n_groups; ++gi) {   // beta3 and no_prox in the slots Adan does not use
+      p.g[gi].rho = ad[gi].beta3;
+      p.g[gi].decoupled = ad[gi].no_prox != 0;
     }
   }
   if (a->grad_raw) {
@@ -960,6 +1041,7 @@ static int optim_step(stk_ctx* c, const stk_optim_args_t* a, const stk_rmsprop_t
     case STK_OPT_RMSPROP_TF:
       err = launch_optim<STK_OPT_RMSPROP_TF>(c, p, a->lp_dtype, a->grad_dtype, raw, pair_ok, s);
       break;
+    case STK_OPT_ADAN: err = launch_optim<STK_OPT_ADAN>(c, p, a->lp_dtype, a->grad_dtype, raw, pair_ok, s); break;
     default: err = launch_optim<STK_OPT_SGD>(c, p, a->lp_dtype, a->grad_dtype, raw, pair_ok, s); break;
   }
   if (err == cudaErrorNotSupported)
@@ -973,13 +1055,21 @@ extern "C" {
 int stk_optim_step_ex(stk_ctx* c, const stk_optim_args_t* a, void* stream) {
   STK_REQUIRE(c, !(a && a->hyper && a->hyper->kind == STK_OPT_RMSPROP_TF),
               "stk_optim_step_ex: RMSPROP_TF takes its per-group hyper-parameters through stk_rmsprop_tf_step");
-  return optim_step(c, a, nullptr, stream);
+  STK_REQUIRE(c, !(a && a->hyper && a->hyper->kind == STK_OPT_ADAN),
+              "stk_optim_step_ex: ADAN takes its per-group hyper-parameters and neg_pre_grad through stk_adan_step");
+  return optim_step(c, a, nullptr, nullptr, nullptr, stream);
 }
 
 int stk_rmsprop_tf_step(stk_ctx* c, const stk_optim_args_t* a, const stk_rmsprop_tf_hyper_t* rt, void* stream) {
   STK_REQUIRE(c, c && a && a->hyper && rt, "stk_rmsprop_tf_step: NULL argument");
   STK_REQUIRE(c, a->hyper->kind == STK_OPT_RMSPROP_TF, "stk_rmsprop_tf_step: hyper->kind must be STK_OPT_RMSPROP_TF");
-  return optim_step(c, a, rt, stream);
+  return optim_step(c, a, rt, nullptr, nullptr, stream);
+}
+
+int stk_adan_step(stk_ctx* c, const stk_optim_args_t* a, const stk_adan_hyper_t* ad, float* neg_pre_grad, void* stream) {
+  STK_REQUIRE(c, c && a && a->hyper && ad, "stk_adan_step: NULL argument");
+  STK_REQUIRE(c, a->hyper->kind == STK_OPT_ADAN, "stk_adan_step: hyper->kind must be STK_OPT_ADAN");
+  return optim_step(c, a, nullptr, ad, neg_pre_grad, stream);
 }
 
 int stk_optim_step(stk_ctx* c, const stk_optim_hyper_t* h, float* master, float* exp_avg, float* exp_avg_sq,
@@ -1058,6 +1148,34 @@ int stk_ademamix_step_prologue(stk_ctx* c, const stk_optim_hyper_t* h, const stk
   p.scaler = c->scaler_dev;
   const int n = n_ranges > 0 ? n_ranges : n_groups;
   k_ademamix_prologue<<<(n + 127) / 128, 128, 0, reinterpret_cast<cudaStream_t>(stream)>>>(p);
+  STK_CUDA(c, cudaGetLastError());
+  return STK_OK;
+}
+
+int stk_adan_step_prologue(stk_ctx* c, const stk_optim_hyper_t* h, const stk_adan_hyper_t* ah, int n_groups, int n_ranges,
+                           const uint8_t* range_group, int32_t* range_steps, float* bc, void* stream) {
+  STK_REQUIRE(c, c && h && ah && bc, "stk_adan_step_prologue: NULL argument");
+  STK_REQUIRE(c, n_groups >= 1 && n_groups <= STK_MAX_GROUPS, "stk_adan_step_prologue: n_groups must be in [1, 8]");
+  STK_REQUIRE(c, n_ranges >= 0, "stk_adan_step_prologue: negative n_ranges");
+  STK_REQUIRE(c, n_ranges == 0 || (range_group && range_steps), "stk_adan_step_prologue: range arrays are NULL");
+  STK_REQUIRE(c, (reinterpret_cast<uintptr_t>(bc) & 15) == 0, "stk_adan_step_prologue: bc must be 16-byte aligned");
+  std::lock_guard<std::mutex> lk(c->mu);
+  DeviceGuard g(c->device);
+  AdanPrologueParams p{};
+  for (int gi = 0; gi < n_groups; ++gi) {
+    p.lr[gi] = h[gi].lr;
+    p.beta1[gi] = h[gi].beta1;
+    p.beta2[gi] = h[gi].beta2;
+    p.a[gi] = ah[gi];
+  }
+  p.n_groups = n_groups;
+  p.n_ranges = n_ranges;
+  p.range_group = range_group;
+  p.range_steps = range_steps;
+  p.bc = reinterpret_cast<float4*>(bc);
+  p.scaler = c->scaler_dev;
+  const int n = n_ranges > 0 ? n_ranges : n_groups;
+  k_adan_prologue<<<(n + 127) / 128, 128, 0, reinterpret_cast<cudaStream_t>(stream)>>>(p);
   STK_CUDA(c, cudaGetLastError());
   return STK_OK;
 }

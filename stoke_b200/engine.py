@@ -302,6 +302,10 @@ class Engine:
         self._check(self.lib.stk_rmsprop_tf_step(self.ctx, C.byref(args), hypers, self._stream()))
         self.launches += 1
 
+    def adan_step(self, args: _lib.OptimArgs, hypers, neg_pre_grad: int):
+        self._check(self.lib.stk_adan_step(self.ctx, C.byref(args), hypers, neg_pre_grad, self._stream()))
+        self.launches += 1
+
     def step_epilogue(self):
         self._check(self.lib.stk_step_epilogue(self.ctx, self._stream()))
         self.launches += 1
@@ -484,8 +488,11 @@ class GradPath:
       MASTER fp32 master weights                               local          aliases P when the model is fp32 and unsharded
       M, V   fp32 optimizer state                              local          owned shards (sharded) | all n
       M2     fp32 third optimizer state (AdEMAMix's            local          indexed like M
-             exp_avg_slow, RMSpropTF's grad_avg)
-             (M, V and M2 exist as ``state`` lists them: buffer -> initial value)
+             exp_avg_slow, RMSpropTF's grad_avg, Adan's
+             exp_avg_diff)
+      M3     fp32 fourth optimizer state (Adan's               local          indexed like M
+             neg_pre_grad)
+             (M, V, M2 and M3 exist as ``state`` lists them: buffer -> initial value)
       AVG    fp32 weight average (EMA / SWA)                   local          indexed like MASTER; only when averaging is
                                                                               configured (``enable_weight_average``)
 
@@ -591,7 +598,8 @@ class GradPath:
         separate_master = self.low_precision or self.sharded
         self.MASTER = alloc(nl * 4) if separate_master else None
         state = state or {}
-        self.M, self.V, self.M2 = (alloc(nl * 4) if state.get(b) is not None else None for b in ("M", "V", "M2"))
+        self.M, self.V, self.M2, self.M3 = (alloc(nl * 4) if state.get(b) is not None else None
+                                            for b in ("M", "V", "M2", "M3"))
 
         self.p_flat = self.P.tensor(self.model_dtype, self.n)
         self.g_flat = self.G.tensor(self.model_dtype, self.n)
@@ -599,6 +607,7 @@ class GradPath:
         self.m_flat = self.M.tensor(torch.float32, self.n_local) if self.M else None
         self.v_flat = self.V.tensor(torch.float32, self.n_local) if self.V else None
         self.m2_flat = self.M2.tensor(torch.float32, self.n_local) if self.M2 else None
+        self.m3_flat = self.M3.tensor(torch.float32, self.n_local) if self.M3 else None
         self.p_flat.copy_(full32)  # round-to-nearest-even, same as the kernel's cast
         if separate_master:
             self.master_flat = self.MASTER.tensor(torch.float32, self.n_local)
@@ -611,7 +620,7 @@ class GradPath:
         # Initial optimizer state (the buffers come zeroed).  The classes create it at a parameter's first gradient (the
         # schedule-free z as a clone of the parameter, RMSpropTF's square_avg as ones); a parameter without one is never
         # touched, so filling at construction is the same.
-        for flat, b in ((self.m_flat, "M"), (self.v_flat, "V"), (self.m2_flat, "M2")):
+        for flat, b in ((self.m_flat, "M"), (self.v_flat, "V"), (self.m2_flat, "M2"), (self.m3_flat, "M3")):
             init = state.get(b)
             if init == "master":
                 flat.copy_(self.master_flat)
@@ -901,7 +910,7 @@ class GradPath:
         """Sets the per-group scalar state (checkpoint load while step counts are optimizer-wide)."""
         self._group_scal.copy_(torch.tensor([list(r) for r in rows], dtype=torch.float32))
 
-    def optimizer_step(self, hypers, exts=None, sf=None, ademamix=None, rmsprop_tf=None):
+    def optimizer_step(self, hypers, exts=None, sf=None, ademamix=None, rmsprop_tf=None, adan=None):
         """One fused K2 launch (+ the one-thread epilogue).  ``hypers``: one ``OptimHyper`` or a list (one per group).
         ``exts``: per-group ``OptimHyperExt`` of the kinds after SGD.  stk_optim_step_prologue forms their per-step scalars
         (and the scalar state of NAdam and ASGD) on the device before the step, and every kind's once step counts are
@@ -909,7 +918,9 @@ class GradPath:
         schedule-free kinds, whose group scalars stk_sf_step_prologue forms (and whose lr_max / weight_sum it advances).
         ``ademamix``: per-group ``AdemamixHyper``; stk_ademamix_step_prologue then takes stk_optim_step_prologue's place
         (same step counts, AdEMAMix's scalars) and M2 is the step's third state tensor.  ``rmsprop_tf``: per-group
-        ``RmspropTfHyper``; the step is stk_rmsprop_tf_step (no per-step scalars), with M2 as grad_avg."""
+        ``RmspropTfHyper``; the step is stk_rmsprop_tf_step (no per-step scalars), with M2 as grad_avg.  ``adan``: per-group
+        ``AdanHyper``; stk_adan_step_prologue takes stk_optim_step_prologue's place and the step is stk_adan_step, with M2
+        as exp_avg_diff and M3 as neg_pre_grad."""
         e = self.engine
         e.state_select(self.state_id)
         if isinstance(hypers, _lib.OptimHyper):
@@ -954,14 +965,14 @@ class GradPath:
         nr, rend, rgrp = self._ranges_for_step()
         a.n_ranges, a.range_end_vec, a.range_group = nr, rend, rgrp
         per_range = bool(nr) and self._range_steps is not None
-        if ademamix is not None:
-            aarr = (_lib.AdemamixHyper * ng)(*ademamix)
+        if ademamix is not None or adan is not None:
+            cls, prologue = ((_lib.AdemamixHyper, e.lib.stk_ademamix_step_prologue) if adan is None else
+                             (_lib.AdanHyper, e.lib.stk_adan_step_prologue))
+            aarr = (cls * ng)(*(ademamix if adan is None else adan))
             keep.append(aarr)
             bc = self._range_bc if per_range else self._group_bc
-            e._check(e.lib.stk_ademamix_step_prologue(e.ctx, harr, aarr, ng, nr if per_range else 0,
-                                                      rgrp if per_range else None,
-                                                      self._range_steps.data_ptr() if per_range else None, bc.data_ptr(),
-                                                      e._stream()))
+            e._check(prologue(e.ctx, harr, aarr, ng, nr if per_range else 0, rgrp if per_range else None,
+                              self._range_steps.data_ptr() if per_range else None, bc.data_ptr(), e._stream()))
             e.launches += 1
             if per_range:
                 a.range_bc = bc.data_ptr()
@@ -993,6 +1004,8 @@ class GradPath:
             rarr = (_lib.RmspropTfHyper * ng)(*rmsprop_tf)
             keep.append(rarr)
             e.rmsprop_tf_step(a, rarr)
+        elif adan is not None:
+            e.adan_step(a, aarr, self.M3.ptr)
         else:
             e.optim_step_ex(a)
         self.weight_avg_after_step()
@@ -1197,7 +1210,8 @@ class GradPath:
                 p.data = p.data.clone()
                 p.grad = None
         self.grad_views = []
-        self.p_flat = self.g_flat = self.main_flat = self.m_flat = self.v_flat = self.m2_flat = self.master_flat = None
+        self.p_flat = self.g_flat = self.main_flat = self.m_flat = self.v_flat = self.m2_flat = self.m3_flat = None
+        self.master_flat = None
         self.avg_flat = None
         self.af_state = self._af_ws = self._af_desc = None
         self._lw_ws = self._lw_desc = None

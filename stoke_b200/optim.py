@@ -28,6 +28,11 @@ element-wise and sharded like Adam.
 (filled with ones at construction), ``momentum_buffer`` in the first (only when some group has momentum) and ``grad_avg``
 in the third (only when some group is centered).  Its per-group alpha and flags go to ``stk_rmsprop_tf_step``; it has no
 per-step scalars.  It is element-wise and sharded like Adam.
+``Adan`` (defined here, after the official Adan and timm's) is the one kind with four fp32 state tensors: ``exp_avg`` in
+the first-moment buffer, ``exp_avg_sq`` in the second, ``exp_avg_diff`` in the third (M2) and ``neg_pre_grad`` in a
+fourth (``GradPath.M3``).  Its step count lives in the group (``group["step"]``), like the schedule-free k;
+``stk_adan_step_prologue`` forms the step sizes and each parameter's first-step flag, and ``stk_adan_step`` takes beta3,
+no_prox and the fourth buffer.  It is element-wise and sharded like Adam.
 ``torch.optim.Adafactor`` takes its own fused entry point, ``stk_adafactor_step`` (per-parameter reductions: row / column
 means of g^2, the parameter's RMS, the update's RMS), with per-parameter step counts on the device and torch's
 state_dict layout (``row_var`` / ``col_var`` or ``variance``).  Its state is never sharded: the reductions need whole
@@ -623,6 +628,82 @@ class RMSpropTF(torch.optim.Optimizer):
 
 _KINDS[RMSpropTF] = _lib.OPT_RMSPROP_TF
 
+
+class Adan(torch.optim.Optimizer):
+    """Adan (Xie, Zhou, Li, Lin and Yan, "Adan: Adaptive Nesterov Momentum Algorithm for Faster Optimizing Deep Models",
+    2022; the official implementation's and timm's arguments, group keys and state keys): Adam-style moments of the
+    gradient and of the gradient difference, with Nesterov momentum folded into the second moment.  With the code's
+    convention (beta = 1 - the paper's beta), t = ``group["step"]`` after its increment and bc_i = 1 - beta_i ** t, for
+    one parameter p with gradient g and previous gradient g_prev (g itself at the parameter's first step)::
+
+        m = beta1 m + (1 - beta1) g;  d = beta2 d + (1 - beta2) (g - g_prev)
+        n = beta3 n + (1 - beta3) (g + beta2 (g - g_prev)) ** 2;  den = sqrt(n) / sqrt(bc3) + eps
+        no_prox:  p = p (1 - lr wd) - lr / bc1 * m / den - lr beta2 / bc2 * d / den
+        else:     p = (p - lr / bc1 * m / den - lr beta2 / bc2 * d / den) / (1 + lr wd)
+
+    That is the paper's Algorithm 1 with bias correction.  ``step()`` is plain per-parameter torch in the official
+    single-tensor order of ops, which the fused kernel rounds like this step on CUDA.  The step count is a python int in
+    the group, absent before the first step.  State per parameter, created at its first gradient: ``exp_avg``,
+    ``exp_avg_sq``, ``exp_avg_diff`` (zeros) and ``neg_pre_grad`` (-g); no ``step``.  Upstream's ``max_grad_norm``
+    (use Stoke's ``grad_clip``) and timm's ``caution`` are not arguments.  ``foreach`` is accepted and ignored.  Inside
+    ``Stoke`` the class runs on the fused sm_90a step (``k_optim_step``, kind ``STK_OPT_ADAN``)."""
+
+    def __init__(self, params, lr: float = 1e-3, betas=(0.98, 0.92, 0.99), eps: float = 1e-8, weight_decay: float = 0.0,
+                 no_prox: bool = False, foreach: Optional[bool] = None):
+        if lr < 0.0:
+            raise ValueError(f"Invalid learning rate: {lr}")
+        if eps < 0.0:
+            raise ValueError(f"Invalid epsilon value: {eps}")
+        if len(betas) != 3 or not all(0.0 <= b < 1.0 for b in betas):
+            raise ValueError(f"Invalid beta parameters: {betas}")
+        super().__init__(params, dict(lr=lr, betas=tuple(betas), eps=eps, weight_decay=weight_decay, no_prox=no_prox,
+                                      foreach=foreach))
+
+    @torch.no_grad()
+    def step(self, closure=None):
+        loss = None
+        if closure is not None:
+            with torch.enable_grad():
+                loss = closure()
+        for group in self.param_groups:
+            group["step"] = t = group.get("step", 0) + 1
+            b1, b2, b3 = group["betas"]
+            lr, eps, wd = group["lr"], group["eps"], group["weight_decay"]
+            bc1, bc2, bc3 = 1 - b1 ** t, 1 - b2 ** t, 1 - b3 ** t
+            step_size, step_size_diff, bc3_sqrt = lr / bc1, lr * b2 / bc2, math.sqrt(bc3)
+            for p in group["params"]:
+                if p.grad is None:
+                    continue
+                grad = p.grad
+                state = self.state[p]
+                if not state:
+                    state["exp_avg"] = torch.zeros_like(p, memory_format=torch.preserve_format)
+                    state["exp_avg_sq"] = torch.zeros_like(p, memory_format=torch.preserve_format)
+                    state["exp_avg_diff"] = torch.zeros_like(p, memory_format=torch.preserve_format)
+                if "neg_pre_grad" not in state or t == 1:
+                    state["neg_pre_grad"] = -grad   # so the first difference is 0
+                exp_avg, exp_avg_sq, exp_avg_diff = state["exp_avg"], state["exp_avg_sq"], state["exp_avg_diff"]
+                P = state["neg_pre_grad"]
+                P.add_(grad)                                             # g - g_prev
+                exp_avg.mul_(b1).add_(grad, alpha=1 - b1)
+                exp_avg_diff.mul_(b2).add_(P, alpha=1 - b2)
+                P.mul_(b2).add_(grad)                                    # g + beta2 (g - g_prev)
+                exp_avg_sq.mul_(b3).addcmul_(P, P, value=1 - b3)
+                denom = (exp_avg_sq.sqrt() / bc3_sqrt).add_(eps)
+                if group["no_prox"]:
+                    p.mul_(1 - lr * wd)
+                    p.addcdiv_(exp_avg, denom, value=-step_size)
+                    p.addcdiv_(exp_avg_diff, denom, value=-step_size_diff)
+                else:
+                    p.addcdiv_(exp_avg, denom, value=-step_size)
+                    p.addcdiv_(exp_avg_diff, denom, value=-step_size_diff)
+                    p.div_(1 + lr * wd)
+                P.zero_().add_(grad, alpha=-1.0)
+        return loss
+
+
+_KINDS[Adan] = _lib.OPT_ADAN
+
 # LAMB and LARS run on their own entry point, stk_layerwise_step (per-parameter trust ratios), not as kinds of K2
 _LAMB, _LARS = "lamb", "lars"
 _KINDS[LAMB] = _LAMB
@@ -633,7 +714,7 @@ _LAYERWISE = {_LAMB: _lib.LW_LAMB, _LARS: _lib.LW_LARS}
 class StateTensor(NamedTuple):
     """One per-parameter state tensor of a fused kind."""
     key: str                                         # torch's state key
-    buf: str                                         # the flat fp32 buffer: "M", "V" or "M2"; "af": Adafactor's own
+    buf: str                                         # the flat fp32 buffer: "M", "V", "M2" or "M3"; "af": Adafactor's
     init: Union[float, str] = 0.0                    # its value before the first step: 0.0, 1.0 or "master"
     where: Optional[Callable[[Dict], bool]] = None   # the group condition under which it exists (None: every group)
     none: bool = False                               # where it does not exist, a parameter exports None (else no key)
@@ -647,6 +728,9 @@ class StateLayout(NamedTuple):
     unstepped: str                      # a never-stepped parameter: "omit" (no entry, torch's lazy state), "same"
                                         # (exported like a stepped one, at step 0) or "none" (every tensor None)
     tensors: Tuple[StateTensor, ...]    # in torch's key order
+    # the step count lives in the parameter groups, not in ``state``: (the group key, the state key whose presence marks
+    # a parameter that has stepped); None: per-parameter ``step`` (or SGD's momentum_buffer rule)
+    group_count: Optional[Tuple[str, str]] = None
 
 
 def _momentum(g):
@@ -669,14 +753,17 @@ _STATE_LAYOUT: Dict[object, StateLayout] = {
     _lib.OPT_ASGD: StateLayout(True, ("eta", "mu"), "omit", (StateTensor("ax", "M"),)),
     _lib.OPT_LION: StateLayout(True, (), "omit", (StateTensor("exp_avg", "M"),)),
     _lib.OPT_SF_ADAMW: StateLayout(False, (), "omit", (StateTensor("z", "M", "master"),
-                                                       StateTensor("exp_avg_sq", "V"))),
-    _lib.OPT_SF_SGD: StateLayout(False, (), "omit", (StateTensor("z", "M", "master"),)),
+                                                       StateTensor("exp_avg_sq", "V")), ("k", "z")),
+    _lib.OPT_SF_SGD: StateLayout(False, (), "omit", (StateTensor("z", "M", "master"),), ("k", "z")),
     _lib.OPT_ADEMAMIX: StateLayout(True, (), "omit", (
         StateTensor("exp_avg_fast", "M", where=lambda g: g["betas"][0] != 0, none=True),
         StateTensor("exp_avg_slow", "M2"), StateTensor("exp_avg_sq", "V"))),
     _lib.OPT_RMSPROP_TF: StateLayout(True, (), "omit", (
         StateTensor("square_avg", "V", 1.0), StateTensor("momentum_buffer", "M", where=lambda g: g["momentum"] > 0),
         StateTensor("grad_avg", "M2", where=lambda g: g["centered"]))),
+    _lib.OPT_ADAN: StateLayout(False, (), "omit", (
+        StateTensor("exp_avg", "M"), StateTensor("exp_avg_sq", "V"), StateTensor("exp_avg_diff", "M2"),
+        StateTensor("neg_pre_grad", "M3")), ("step", "exp_avg")),
     _LAMB: StateLayout(True, (), "omit", _ADAM_STATE),
     _LARS: StateLayout(True, (), "omit", (StateTensor("momentum_buffer", "M", where=_momentum),)),
     # row_var / col_var of a factored parameter, variance of the others: views of GradPath.af_state
@@ -687,8 +774,10 @@ _STATE_LAYOUT: Dict[object, StateLayout] = {
 
 def state_buffers(layout: StateLayout, groups: List[Dict]) -> Dict[str, object]:
     """The flat fp32 buffers a kind needs for these parameter groups: ``{"M", "V", "M2"} -> initial value`` (0.0, 1.0
-    or "master"), None for a buffer that is not allocated."""
+    or "master"), None for a buffer that is not allocated, plus ``"M3"`` for a kind that keeps a tensor there."""
     out = {"M": None, "V": None, "M2": None}
+    if any(t.buf == "M3" for t in layout.tensors):
+        out["M3"] = None
     for t in layout.tensors:
         cond = t.alloc or t.where
         if t.buf in out and (cond is None or any(cond(g) for g in groups)):
@@ -773,7 +862,8 @@ def load_step_counts(kind, entries: List[Dict], group_of: List[int], opt_steps: 
     """How a loaded state dict's step counts and scalar state (NAdam's ``mu_product``, ASGD's ``eta`` / ``mu``) go onto
     the fused step.  ``entries``: torch's state entry of every parameter in flat order (``{}`` where it has none);
     ``opt_steps``: the checkpoint's ``b200_opt_steps`` (None in a torch-written one); ``per_param_on``: the step already
-    keeps per-parameter counts; ``momentum``: SGD's per-group momentum; ``group_k``: the schedule-free groups' ``k``.
+    keeps per-parameter counts; ``momentum``: SGD's per-group momentum; ``group_k``: every group's count, for the kinds
+    that keep it in the group (``StateLayout.group_count``: the schedule-free ``k``, Adan's ``step``).
 
     torch creates a parameter's state at its first step, so a parameter without an entry has taken 0 steps and has the
     initial scalar state (1.0).  torch's SGD keeps no ``step``: a parameter with a ``momentum_buffer`` has taken
@@ -785,15 +875,18 @@ def load_step_counts(kind, entries: List[Dict], group_of: List[int], opt_steps: 
     are not all the optimizer-wide count, when the scalar state differs within a group, or when ``per_param_on``.
     ``scalars`` is None for the kinds without scalar state.
 
-    The schedule-free kinds keep no ``step``: k is the checkpoint's ``b200_opt_steps``, else the groups' common ``k``
-    (groups whose k differ raise ValueError), and a parameter has taken k steps if its entry has ``z``, 0 if not."""
-    if kind in _SF_KINDS:
+    The kinds with ``group_count`` keep no per-parameter ``step``: the count is the checkpoint's ``b200_opt_steps``, else
+    the groups' common count (groups whose counts differ raise ValueError), and a parameter has taken that many steps if
+    its entry has the marker tensor (schedule-free ``z``, Adan's ``exp_avg``), 0 if not."""
+    group_count = _STATE_LAYOUT[kind].group_count
+    if group_count is not None:
+        key, marker = group_count
         if opt_steps is None:
             ks = set(int(k) for k in (group_k or []))
             if len(ks) > 1:
-                raise ValueError(f"Stoke -- schedule-free parameter groups with different step counts k: {sorted(ks)}")
+                raise ValueError(f"Stoke -- parameter groups with different step counts {key}: {sorted(ks)}")
             opt_steps = ks.pop() if ks else 0
-        steps = [opt_steps if "z" in e else 0 for e in entries]
+        steps = [opt_steps if marker in e else 0 for e in entries]
         if per_param_on or any(s != opt_steps for s in steps):
             return opt_steps, steps, None
         return opt_steps, None, None
@@ -853,7 +946,7 @@ class B200FusedOptimizer(torch.optim.Optimizer):
                  bucket_mb: Optional[float] = None):
         if optim_cls not in _KINDS:
             raise NotImplementedError(
-                f"Stoke -- the fused step covers torch.optim.Adam, AdamW, SGD, NAdam, RAdam, Adamax, Adadelta, Rprop, ASGD and Adafactor and stoke_b200.optim.LAMB, LARS, Lion, AdamWScheduleFree, SGDScheduleFree, AdEMAMix and RMSpropTF; got {getattr(optim_cls, '__name__', optim_cls)}"
+                f"Stoke -- the fused step covers torch.optim.Adam, AdamW, SGD, NAdam, RAdam, Adamax, Adadelta, Rprop, ASGD and Adafactor and stoke_b200.optim.LAMB, LARS, Lion, AdamWScheduleFree, SGDScheduleFree, AdEMAMix, RMSpropTF and Adan; got {getattr(optim_cls, '__name__', optim_cls)}"
                 f" (use B200StockOptimizer / build_optimizer, which routes other classes to the stock-optimizer path)")
         params, group_of, extra, kw = _group_layout(module, optim_kwargs)
         if len(extra) > _lib.MAX_GROUPS:
@@ -928,7 +1021,7 @@ class B200FusedOptimizer(torch.optim.Optimizer):
             h.nesterov = int(bool(g.get("nesterov", False)))
         elif self._kind == _lib.OPT_RMSPROP_TF:   # alpha and the flags go in RmspropTfHyper
             h.eps, h.momentum = float(g["eps"]), float(g["momentum"])
-        elif "betas" in g:   # AdEMAMix has a third beta, which goes in AdemamixHyper
+        elif "betas" in g:   # AdEMAMix and Adan have a third beta, which goes in AdemamixHyper / AdanHyper
             h.beta1, h.beta2 = float(g["betas"][0]), float(g["betas"][1])
             h.eps = float(g.get("eps", 0.0))   # Lion has no eps
         elif "eps" in g:   # Adadelta
@@ -972,6 +1065,14 @@ class B200FusedOptimizer(torch.optim.Optimizer):
             out.append(x)
         return out
 
+    def _adan_hypers(self) -> List[_lib.AdanHyper]:
+        out = []
+        for g in self.param_groups:
+            x = _lib.AdanHyper()
+            x.beta3, x.no_prox = float(g["betas"][2]), int(bool(g["no_prox"]))
+            out.append(x)
+        return out
+
     def _exts(self) -> Optional[List[_lib.OptimHyperExt]]:
         if self._kind not in _EXT_KINDS:
             return None
@@ -1006,6 +1107,9 @@ class B200FusedOptimizer(torch.optim.Optimizer):
             return
         if self._kind == _lib.OPT_RMSPROP_TF:
             self.path.optimizer_step(self._hypers(), rmsprop_tf=self._rmsprop_tf_hypers())
+            return
+        if self._kind == _lib.OPT_ADAN:
+            self.path.optimizer_step(self._hypers(), adan=self._adan_hypers())
             return
         self.path.optimizer_step(self._hypers(), self._exts())
 
@@ -1060,7 +1164,7 @@ class B200FusedOptimizer(torch.optim.Optimizer):
     def _flats(self) -> Dict[str, torch.Tensor]:
         """This rank's allocated state buffers, by name."""
         path = self.path
-        flats = {"M": path.m_flat, "V": path.v_flat, "M2": path.m2_flat}
+        flats = {"M": path.m_flat, "V": path.v_flat, "M2": path.m2_flat, "M3": path.m3_flat}
         return {b: f for b, f in flats.items() if f is not None}
 
     def _views(self, full: Dict[str, torch.Tensor]) -> Dict[str, List[Optional[torch.Tensor]]]:
@@ -1102,6 +1206,9 @@ class B200FusedOptimizer(torch.optim.Optimizer):
                             scheduled_lr=_sf_scheduled_lr(src, k - 1) if k > 0 else src["scheduled_lr"])
                 g.update(vals)
                 src.update(vals)   # param_groups as of this state_dict(); reading them every step would synchronise
+        if self._kind == _lib.OPT_ADAN and out["b200_opt_steps"] > 0:   # the class creates group["step"] at its first step
+            for g, src in zip(out["param_groups"], self.param_groups):
+                g["step"] = src["step"] = out["b200_opt_steps"]
         return out
 
     def load_state_dict(self, sd):
@@ -1129,7 +1236,8 @@ class B200FusedOptimizer(torch.optim.Optimizer):
         steps, per_param, scalars = load_step_counts(self._kind, entries, self._group_of, sd.get("b200_opt_steps"),
                                                      path._range_steps is not None,
                                                      [g.get("momentum", 0.0) for g in self.param_groups],
-                                                     [g.get("k", 0) for g in self.param_groups])
+                                                     [g.get(self._layout.group_count[0], 0) for g in self.param_groups]
+                                                     if self._layout.group_count else None)
         if self._kind in _SF_KINDS:
             path._sf_state.copy_(torch.tensor([[float(g["lr_max"]), float(g["weight_sum"])] for g in self.param_groups],
                                               dtype=torch.float64))
