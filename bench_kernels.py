@@ -84,7 +84,7 @@ def main():
                                          clip=ClipSpec(_lib.CLIP_NORM, max_norm=1.0, norm_type=2.0), lp_dtype=lp)
                 path = opt.path
                 npad = path.n
-                hyper = opt._hypers()
+                hyper = opt._hyper_of(opt.param_groups[0])
 
                 def fill():
                     path.g_flat.copy_((torch.randn(path.n, device="cuda") * 1e-3).to(path.g_flat.dtype))

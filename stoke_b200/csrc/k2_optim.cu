@@ -1050,6 +1050,36 @@ static int optim_step(stk_ctx* c, const stk_optim_args_t* a, const stk_rmsprop_t
   return STK_OK;
 }
 
+// What stk_optim_step_prologue, stk_ademamix_step_prologue and stk_adan_step_prologue share: the argument checks (`fn`
+// names the entry point in their messages; `args_ok`: its own pointer arguments are set), the step-count bookkeeping
+// fields, and the launch of one thread per range or per group.  `own(p)` checks and fills the rest of the parameters,
+// returning STK_OK or the entry point's error.
+template <typename Params, typename Own>
+static int range_prologue(stk_ctx* c, const char* fn, bool args_ok, int n_groups, int n_ranges,
+                          const uint8_t* range_group, int32_t* range_steps, float* bc, void (*kernel)(Params), Own own,
+                          void* stream) {
+  const std::string f(fn);
+  STK_REQUIRE(c, c && args_ok && bc, f + ": NULL argument");
+  STK_REQUIRE(c, n_groups >= 1 && n_groups <= STK_MAX_GROUPS, f + ": n_groups must be in [1, 8]");
+  STK_REQUIRE(c, n_ranges >= 0, f + ": negative n_ranges");
+  STK_REQUIRE(c, n_ranges == 0 || (range_group && range_steps), f + ": range arrays are NULL");
+  STK_REQUIRE(c, (reinterpret_cast<uintptr_t>(bc) & 15) == 0, f + ": bc must be 16-byte aligned");
+  Params p{};
+  if (const int rc = own(p)) return rc;
+  std::lock_guard<std::mutex> lk(c->mu);
+  DeviceGuard g(c->device);
+  p.n_groups = n_groups;
+  p.n_ranges = n_ranges;
+  p.range_group = range_group;
+  p.range_steps = range_steps;
+  p.bc = reinterpret_cast<float4*>(bc);
+  p.scaler = c->scaler_dev;
+  const int n = n_ranges > 0 ? n_ranges : n_groups;
+  kernel<<<(n + 127) / 128, 128, 0, reinterpret_cast<cudaStream_t>(stream)>>>(p);
+  STK_CUDA(c, cudaGetLastError());
+  return STK_OK;
+}
+
 extern "C" {
 
 int stk_optim_step_ex(stk_ctx* c, const stk_optim_args_t* a, void* stream) {
@@ -1095,89 +1125,46 @@ int stk_optim_step(stk_ctx* c, const stk_optim_hyper_t* h, float* master, float*
 int stk_optim_step_prologue(stk_ctx* c, const stk_optim_hyper_t* h, const stk_optim_hyper_ext_t* ext, int n_groups,
                             int n_ranges, const uint8_t* range_group, int32_t* range_steps, float* scalar_state, float* bc,
                             void* stream) {
-  STK_REQUIRE(c, c && h && bc, "stk_optim_step_prologue: NULL argument");
-  STK_REQUIRE(c, n_groups >= 1 && n_groups <= STK_MAX_GROUPS, "stk_optim_step_prologue: n_groups must be in [1, 8]");
-  STK_REQUIRE(c, n_ranges >= 0, "stk_optim_step_prologue: negative n_ranges");
-  STK_REQUIRE(c, n_ranges == 0 || (range_group && range_steps), "stk_optim_step_prologue: range arrays are NULL");
-  STK_REQUIRE(c, (h->kind >= STK_OPT_ADAM && h->kind <= STK_OPT_SF_SGD) || h->kind == STK_OPT_RMSPROP_TF,
-              "stk_optim_step_prologue: bad optimizer kind");
-  STK_REQUIRE(c, scalar_state_width(h->kind) == 0 || scalar_state,
-              "stk_optim_step_prologue: NAdam and ASGD need their scalar state");
-  STK_REQUIRE(c, (reinterpret_cast<uintptr_t>(bc) & 15) == 0, "stk_optim_step_prologue: bc must be 16-byte aligned");
-  std::lock_guard<std::mutex> lk(c->mu);
-  DeviceGuard g(c->device);
-  StepPrologueParams p{};
-  fill_groups(p.g, h, ext, n_groups);
-  p.n_groups = n_groups;
-  p.n_ranges = n_ranges;
-  p.kind = h->kind;
-  p.range_group = range_group;
-  p.range_steps = range_steps;
-  p.scalar_state = scalar_state;
-  p.bc = reinterpret_cast<float4*>(bc);
-  p.scaler = c->scaler_dev;
-  const int n = n_ranges > 0 ? n_ranges : n_groups;
-  k_step_prologue<<<(n + 127) / 128, 128, 0, reinterpret_cast<cudaStream_t>(stream)>>>(p);
-  STK_CUDA(c, cudaGetLastError());
-  return STK_OK;
+  return range_prologue(c, "stk_optim_step_prologue", h, n_groups, n_ranges, range_group, range_steps, bc,
+                        k_step_prologue, [&](StepPrologueParams& p) {
+    STK_REQUIRE(c, (h->kind >= STK_OPT_ADAM && h->kind <= STK_OPT_SF_SGD) || h->kind == STK_OPT_RMSPROP_TF,
+                "stk_optim_step_prologue: bad optimizer kind");
+    STK_REQUIRE(c, scalar_state_width(h->kind) == 0 || scalar_state,
+                "stk_optim_step_prologue: NAdam and ASGD need their scalar state");
+    fill_groups(p.g, h, ext, n_groups);
+    p.kind = h->kind;
+    p.scalar_state = scalar_state;
+    return (int)STK_OK;
+  }, stream);
 }
 
 int stk_ademamix_step_prologue(stk_ctx* c, const stk_optim_hyper_t* h, const stk_ademamix_hyper_t* ah, int n_groups,
                                int n_ranges, const uint8_t* range_group, int32_t* range_steps, float* bc, void* stream) {
-  STK_REQUIRE(c, c && h && ah && bc, "stk_ademamix_step_prologue: NULL argument");
-  STK_REQUIRE(c, n_groups >= 1 && n_groups <= STK_MAX_GROUPS, "stk_ademamix_step_prologue: n_groups must be in [1, 8]");
-  STK_REQUIRE(c, n_ranges >= 0, "stk_ademamix_step_prologue: negative n_ranges");
-  STK_REQUIRE(c, n_ranges == 0 || (range_group && range_steps), "stk_ademamix_step_prologue: range arrays are NULL");
-  STK_REQUIRE(c, (reinterpret_cast<uintptr_t>(bc) & 15) == 0, "stk_ademamix_step_prologue: bc must be 16-byte aligned");
-  for (int gi = 0; gi < n_groups; ++gi)
-    STK_REQUIRE(c, ah[gi].alpha_warmup >= 0 && ah[gi].beta3_warmup >= 0,
-                "stk_ademamix_step_prologue: warm-ups must be >= 0 (0: none)");
-  std::lock_guard<std::mutex> lk(c->mu);
-  DeviceGuard g(c->device);
-  AdemamixPrologueParams p{};
-  for (int gi = 0; gi < n_groups; ++gi) {
-    p.beta1[gi] = h[gi].beta1;
-    p.beta2[gi] = h[gi].beta2;
-    p.a[gi] = ah[gi];
-  }
-  p.n_groups = n_groups;
-  p.n_ranges = n_ranges;
-  p.range_group = range_group;
-  p.range_steps = range_steps;
-  p.bc = reinterpret_cast<float4*>(bc);
-  p.scaler = c->scaler_dev;
-  const int n = n_ranges > 0 ? n_ranges : n_groups;
-  k_ademamix_prologue<<<(n + 127) / 128, 128, 0, reinterpret_cast<cudaStream_t>(stream)>>>(p);
-  STK_CUDA(c, cudaGetLastError());
-  return STK_OK;
+  return range_prologue(c, "stk_ademamix_step_prologue", h && ah, n_groups, n_ranges, range_group, range_steps, bc,
+                        k_ademamix_prologue, [&](AdemamixPrologueParams& p) {
+    for (int gi = 0; gi < n_groups; ++gi) {
+      STK_REQUIRE(c, ah[gi].alpha_warmup >= 0 && ah[gi].beta3_warmup >= 0,
+                  "stk_ademamix_step_prologue: warm-ups must be >= 0 (0: none)");
+      p.beta1[gi] = h[gi].beta1;
+      p.beta2[gi] = h[gi].beta2;
+      p.a[gi] = ah[gi];
+    }
+    return (int)STK_OK;
+  }, stream);
 }
 
 int stk_adan_step_prologue(stk_ctx* c, const stk_optim_hyper_t* h, const stk_adan_hyper_t* ah, int n_groups, int n_ranges,
                            const uint8_t* range_group, int32_t* range_steps, float* bc, void* stream) {
-  STK_REQUIRE(c, c && h && ah && bc, "stk_adan_step_prologue: NULL argument");
-  STK_REQUIRE(c, n_groups >= 1 && n_groups <= STK_MAX_GROUPS, "stk_adan_step_prologue: n_groups must be in [1, 8]");
-  STK_REQUIRE(c, n_ranges >= 0, "stk_adan_step_prologue: negative n_ranges");
-  STK_REQUIRE(c, n_ranges == 0 || (range_group && range_steps), "stk_adan_step_prologue: range arrays are NULL");
-  STK_REQUIRE(c, (reinterpret_cast<uintptr_t>(bc) & 15) == 0, "stk_adan_step_prologue: bc must be 16-byte aligned");
-  std::lock_guard<std::mutex> lk(c->mu);
-  DeviceGuard g(c->device);
-  AdanPrologueParams p{};
-  for (int gi = 0; gi < n_groups; ++gi) {
-    p.lr[gi] = h[gi].lr;
-    p.beta1[gi] = h[gi].beta1;
-    p.beta2[gi] = h[gi].beta2;
-    p.a[gi] = ah[gi];
-  }
-  p.n_groups = n_groups;
-  p.n_ranges = n_ranges;
-  p.range_group = range_group;
-  p.range_steps = range_steps;
-  p.bc = reinterpret_cast<float4*>(bc);
-  p.scaler = c->scaler_dev;
-  const int n = n_ranges > 0 ? n_ranges : n_groups;
-  k_adan_prologue<<<(n + 127) / 128, 128, 0, reinterpret_cast<cudaStream_t>(stream)>>>(p);
-  STK_CUDA(c, cudaGetLastError());
-  return STK_OK;
+  return range_prologue(c, "stk_adan_step_prologue", h && ah, n_groups, n_ranges, range_group, range_steps, bc,
+                        k_adan_prologue, [&](AdanPrologueParams& p) {
+    for (int gi = 0; gi < n_groups; ++gi) {
+      p.lr[gi] = h[gi].lr;
+      p.beta1[gi] = h[gi].beta1;
+      p.beta2[gi] = h[gi].beta2;
+      p.a[gi] = ah[gi];
+    }
+    return (int)STK_OK;
+  }, stream);
 }
 
 int stk_sf_step_prologue(stk_ctx* c, const stk_sf_hyper_t* h, int n_groups, double* group_state, float* bc, void* stream) {

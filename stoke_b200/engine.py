@@ -910,42 +910,78 @@ class GradPath:
         """Sets the per-group scalar state (checkpoint load while step counts are optimizer-wide)."""
         self._group_scal.copy_(torch.tensor([list(r) for r in rows], dtype=torch.float32))
 
-    def optimizer_step(self, hypers, exts=None, sf=None, ademamix=None, rmsprop_tf=None, adan=None):
-        """One fused K2 launch (+ the one-thread epilogue).  ``hypers``: one ``OptimHyper`` or a list (one per group).
-        ``exts``: per-group ``OptimHyperExt`` of the kinds after SGD.  stk_optim_step_prologue forms their per-step scalars
-        (and the scalar state of NAdam and ASGD) on the device before the step, and every kind's once step counts are
-        per parameter; the optimizer-wide Adam / AdamW / SGD step forms its own.  ``sf``: per-group ``SfHyper`` of the
-        schedule-free kinds, whose group scalars stk_sf_step_prologue forms (and whose lr_max / weight_sum it advances).
-        ``ademamix``: per-group ``AdemamixHyper``; stk_ademamix_step_prologue then takes stk_optim_step_prologue's place
-        (same step counts, AdEMAMix's scalars) and M2 is the step's third state tensor.  ``rmsprop_tf``: per-group
-        ``RmspropTfHyper``; the step is stk_rmsprop_tf_step (no per-step scalars), with M2 as grad_avg.  ``adan``: per-group
-        ``AdanHyper``; stk_adan_step_prologue takes stk_optim_step_prologue's place and the step is stk_adan_step, with M2
-        as exp_avg_diff and M3 as neg_pre_grad."""
+    def _begin_step(self, a, hyper_cls, hypers):
+        """Selects this path's state and fills what every fused step's args share: the per-group hyper-parameters, the
+        master, and the gradient source (the local raw bucket with the accumulator it may still hold, else the reduced
+        fp32 main gradients).  Returns the engine and the hyper array."""
         e = self.engine
         e.state_select(self.state_id)
-        if isinstance(hypers, _lib.OptimHyper):
-            hypers = [hypers]
         ng = len(hypers)
         if ng > _lib.MAX_GROUPS:
             raise NotImplementedError(f"Stoke -- the fused step handles up to {_lib.MAX_GROUPS} parameter groups")
-        harr = (_lib.OptimHyper * ng)(*hypers)
-        harr[0].clip_kind = self.clip.kind
-        harr[0].clip_max_norm = self.clip.max_norm
-        harr[0].clip_value = self.clip.clip_value
-        a = _lib.OptimArgs()
-        a.hyper, a.n_groups = harr, ng
-        a.master = self.master_ptr
-        a.exp_avg = self.M.ptr if self.M else None
-        a.exp_avg_sq = self.V.ptr if self.V else None
-        a.exp_avg_slow = self.M2.ptr if self.M2 else None
-        a.n_local = self.n_local
-        a.grid_n = self.n_local_max
-        keep = [harr]
+        harr = (hyper_cls * ng)(*hypers)
+        a.hyper, a.n_groups, a.master = harr, ng, self.master_ptr
         if self.route == "local":
             a.grad, a.grad_dtype, a.grad_raw, a.grad_mul = self.G.ptr, _DT[self.model_dtype], 1, 1.0
             a.acc = self.ACC.ptr if self._raw_has_acc else None
         else:
             a.grad, a.grad_dtype, a.grad_raw = self.MAIN.ptr, _lib.F32, 0
+        return e, harr
+
+    def _per_param_args(self, a):
+        """What the per-parameter steps (Adafactor, LAMB / LARS) add to their args: the clip, the group table with this
+        window's skip bits, the per-parameter step counts, and the model-dtype parameters to refresh."""
+        a.clip_kind, a.clip_max_norm, a.clip_value = self.clip.kind, self.clip.max_norm, self.clip.clip_value
+        self._ranges_for_step()   # refreshes the skip bits of the per-parameter group table
+        a.param_group, a.steps = self._range_group.data_ptr(), self._range_steps.data_ptr()
+        if self.low_precision:
+            a.lp, a.lp_dtype = self.P.ptr, _DT[self.model_dtype]
+
+    def _end_step(self):
+        """After every fused step: the due weight-average update, the epilogue, and a new accumulation window."""
+        e = self.engine
+        self.weight_avg_after_step()
+        e.step_epilogue()
+        self._track_touched = False
+        self._raw_has_acc = False
+        e.comm_poll()  # a peer that went missing during this step surfaces here (no synchronisation)
+
+    def optimizer_step(self, hypers, ext=None):
+        """One fused K2 launch, its prologues and the one-thread epilogue.  ``hypers``: one ``OptimHyper`` or a list
+        (one per group), all of one kind.  ``ext``: the kind's per-group struct beside them (one per group), or None.
+        The kind chooses the launches::
+
+            kind                          ext             prologues                              step
+            NAdam RAdam Adamax Adadelta   OptimHyperExt   stk_optim_step_prologue                stk_optim_step_ex
+              Rprop ASGD
+            AdamW / SGD schedule-free     SfHyper         [stk_optim_step_prologue],             stk_optim_step_ex
+                                                            then stk_sf_step_prologue
+            AdEMAMix                      AdemamixHyper   stk_ademamix_step_prologue             stk_optim_step_ex
+            RMSpropTF                     RmspropTfHyper  [stk_optim_step_prologue]              stk_rmsprop_tf_step
+            Adan                          AdanHyper       stk_adan_step_prologue                 stk_adan_step
+            Adam AdamW SGD Lion           None            [stk_optim_step_prologue]              stk_optim_step_ex
+
+        [...]: only once step counts are per parameter, which the prologue then keeps; the optimizer-wide step of these
+        kinds forms its own scalars.  The range-table prologues (stk_optim_step_prologue, or AdEMAMix's / Adan's own)
+        form the per-step scalars and NAdam's / ASGD's scalar state on the device; stk_sf_step_prologue forms the
+        schedule-free group scalars and advances lr_max / weight_sum.  M2 is the step's third state tensor (AdEMAMix's
+        exp_avg_slow, RMSpropTF's grad_avg, Adan's exp_avg_diff) and M3 Adan's neg_pre_grad."""
+        if isinstance(hypers, _lib.OptimHyper):
+            hypers = [hypers]
+        kind = hypers[0].kind
+        a = _lib.OptimArgs()
+        e, harr = self._begin_step(a, _lib.OptimHyper, hypers)
+        ng = len(harr)
+        harr[0].clip_kind = self.clip.kind
+        harr[0].clip_max_norm = self.clip.max_norm
+        harr[0].clip_value = self.clip.clip_value
+        xarr = (type(ext[0]) * ng)(*ext) if ext is not None else None
+        hyper_ext = xarr if ext is not None and isinstance(ext[0], _lib.OptimHyperExt) else None
+        a.exp_avg = self.M.ptr if self.M else None
+        a.exp_avg_sq = self.V.ptr if self.V else None
+        a.exp_avg_slow = self.M2.ptr if self.M2 else None
+        a.n_local = self.n_local
+        a.grid_n = self.n_local_max
         if self.sharded:
             lp = _lib.ptr_array(self.P.peer_ptrs())
             a.lp_ptrs, a.lp_world, a.lp_dtype = lp, e.world, _DT[self.model_dtype]
@@ -953,133 +989,74 @@ class GradPath:
             sl = (C.c_size_t * (ns + 1))(*([s[2] for s in self.segs] + [self.n_local]))
             sg = (C.c_size_t * max(ns, 1))(*[s[0] for s in self.segs]) if ns else (C.c_size_t * 1)(0)
             a.n_seg, a.seg_local, a.seg_global = ns, sl, sg
-            keep += [lp, sl, sg]
-            if ns == 0:
-                a.n_seg = 0
         elif self.low_precision:
-            lp = _lib.ptr_array([self.P.ptr])
-            a.lp_ptrs, a.lp_world, a.lp_dtype = lp, 1, _DT[self.model_dtype]
-            keep.append(lp)
+            a.lp_ptrs, a.lp_world, a.lp_dtype = _lib.ptr_array([self.P.ptr]), 1, _DT[self.model_dtype]
         else:
             a.lp_ptrs, a.lp_world, a.lp_dtype = None, 0, _lib.F32
         nr, rend, rgrp = self._ranges_for_step()
         a.n_ranges, a.range_end_vec, a.range_group = nr, rend, rgrp
         per_range = bool(nr) and self._range_steps is not None
-        if ademamix is not None or adan is not None:
-            cls, prologue = ((_lib.AdemamixHyper, e.lib.stk_ademamix_step_prologue) if adan is None else
-                             (_lib.AdanHyper, e.lib.stk_adan_step_prologue))
-            aarr = (cls * ng)(*(ademamix if adan is None else adan))
-            keep.append(aarr)
+        # AdEMAMix and Adan have range-table prologues of their own, which form their scalars
+        own = (e.lib.stk_ademamix_step_prologue if kind == _lib.OPT_ADEMAMIX else
+               e.lib.stk_adan_step_prologue if kind == _lib.OPT_ADAN else None)
+        if own is not None or hyper_ext is not None or per_range:
             bc = self._range_bc if per_range else self._group_bc
-            e._check(prologue(e.ctx, harr, aarr, ng, nr if per_range else 0, rgrp if per_range else None,
-                              self._range_steps.data_ptr() if per_range else None, bc.data_ptr(), e._stream()))
+            counts = (ng, nr, rgrp, self._range_steps.data_ptr()) if per_range else (ng, 0, None, None)
+            if own is not None:
+                e._check(own(e.ctx, harr, xarr, *counts, bc.data_ptr(), e._stream()))
+            else:
+                a.hyper_ext = hyper_ext
+                scal = self._range_scal if per_range else self._group_scal
+                e._check(e.lib.stk_optim_step_prologue(e.ctx, harr, hyper_ext, *counts,
+                                                       scal.data_ptr() if scal is not None else None, bc.data_ptr(),
+                                                       e._stream()))
             e.launches += 1
             if per_range:
                 a.range_bc = bc.data_ptr()
             else:
                 a.group_bc = bc.data_ptr()
-        elif exts is not None or per_range:
-            xarr = (_lib.OptimHyperExt * ng)(*exts) if exts is not None else None
-            keep.append(xarr)
-            a.hyper_ext = xarr
-            scal = self._range_scal if per_range else self._group_scal
-            bc = self._range_bc if per_range else self._group_bc
-            e._check(e.lib.stk_optim_step_prologue(e.ctx, harr, xarr, ng, nr if per_range else 0, rgrp if per_range else None,
-                                                   self._range_steps.data_ptr() if per_range else None,
-                                                   scal.data_ptr() if scal is not None else None, bc.data_ptr(),
-                                                   e._stream()))
-            e.launches += 1
-            if per_range:
-                a.range_bc = bc.data_ptr()
-            else:
-                a.group_bc = bc.data_ptr()
-        if sf is not None:
-            sarr = (_lib.SfHyper * ng)(*sf)
-            keep.append(sarr)
-            e._check(e.lib.stk_sf_step_prologue(e.ctx, sarr, ng, self._sf_state.data_ptr(), self._group_bc.data_ptr(),
+        if kind in (_lib.OPT_SF_ADAMW, _lib.OPT_SF_SGD):
+            e._check(e.lib.stk_sf_step_prologue(e.ctx, xarr, ng, self._sf_state.data_ptr(), self._group_bc.data_ptr(),
                                                 e._stream()))
             e.launches += 1
             a.group_bc = self._group_bc.data_ptr()
-        if rmsprop_tf is not None:
-            rarr = (_lib.RmspropTfHyper * ng)(*rmsprop_tf)
-            keep.append(rarr)
-            e.rmsprop_tf_step(a, rarr)
-        elif adan is not None:
-            e.adan_step(a, aarr, self.M3.ptr)
+        if kind == _lib.OPT_RMSPROP_TF:
+            e.rmsprop_tf_step(a, xarr)
+        elif kind == _lib.OPT_ADAN:
+            e.adan_step(a, xarr, self.M3.ptr)
         else:
             e.optim_step_ex(a)
-        self.weight_avg_after_step()
-        e.step_epilogue()
-        self._track_touched = False
-        self._raw_has_acc = False
-        e.comm_poll()  # a peer that went missing during this step surfaces here (no synchronisation)
+        self._end_step()
 
     def adafactor_step(self, hypers: Sequence[_lib.AdafactorHyper]):
         """One fused Adafactor step (``stk_adafactor_step``: eight launches over the descriptor table), then the epilogue.
         ``hypers``: one ``AdafactorHyper`` per group.  Parameters without a gradient in this window are skipped through
         the skip bits of the range table; their step counts and state do not move."""
-        e = self.engine
-        e.state_select(self.state_id)
-        ng = len(hypers)
-        if ng > _lib.MAX_GROUPS:
-            raise NotImplementedError(f"Stoke -- the fused step handles up to {_lib.MAX_GROUPS} parameter groups")
-        harr = (_lib.AdafactorHyper * ng)(*hypers)
         a = _lib.AdafactorArgs()
-        a.hyper, a.n_groups = harr, ng
-        a.clip_kind, a.clip_max_norm, a.clip_value = self.clip.kind, self.clip.max_norm, self.clip.clip_value
+        e, _ = self._begin_step(a, _lib.AdafactorHyper, hypers)
         a.params, a.plan = self._af_desc.data_ptr(), C.pointer(self.af_plan)
-        self._ranges_for_step()   # refreshes the skip bits of the per-parameter group table
-        a.param_group, a.steps = self._range_group.data_ptr(), self._range_steps.data_ptr()
-        a.master, a.state, a.workspace = self.master_ptr, self.af_state.data_ptr(), self._af_ws.data_ptr()
-        if self.route == "local":
-            a.grad, a.grad_dtype, a.grad_raw, a.grad_mul = self.G.ptr, _DT[self.model_dtype], 1, 1.0
-            a.acc = self.ACC.ptr if self._raw_has_acc else None
-        else:
-            a.grad, a.grad_dtype, a.grad_raw = self.MAIN.ptr, _lib.F32, 0
-        if self.low_precision:
-            a.lp, a.lp_dtype = self.P.ptr, _DT[self.model_dtype]
+        a.state, a.workspace = self.af_state.data_ptr(), self._af_ws.data_ptr()
+        self._per_param_args(a)
         e._check(e.lib.stk_adafactor_step(e.ctx, C.byref(a), e._stream()))
         e.launches += 8 if self.af_plan.n_line else 5
-        self.weight_avg_after_step()
-        e.step_epilogue()
-        self._track_touched = False
-        self._raw_has_acc = False
-        e.comm_poll()
+        self._end_step()
 
     def layerwise_step(self, kind: int, hypers: Sequence[_lib.LayerwiseHyper]):
         """One fused LAMB / LARS step (``stk_layerwise_step``: tile pass, per-parameter fold, update), then the epilogue.
         ``kind``: ``_lib.LW_LAMB`` or ``_lib.LW_LARS``; ``hypers``: one ``LayerwiseHyper`` per group.  Parameters without a
         gradient in this window are skipped through the skip bits of the range table; their step counts and state do
         not move."""
-        e = self.engine
-        e.state_select(self.state_id)
-        ng = len(hypers)
-        if ng > _lib.MAX_GROUPS:
-            raise NotImplementedError(f"Stoke -- the fused step handles up to {_lib.MAX_GROUPS} parameter groups")
-        harr = (_lib.LayerwiseHyper * ng)(*hypers)
         a = _lib.LayerwiseArgs()
-        a.kind, a.hyper, a.n_groups = kind, harr, ng
-        a.clip_kind, a.clip_max_norm, a.clip_value = self.clip.kind, self.clip.max_norm, self.clip.clip_value
+        e, _ = self._begin_step(a, _lib.LayerwiseHyper, hypers)
+        a.kind = kind
         a.params, a.n_params, a.n_tiles = self._lw_desc.data_ptr(), len(self.params), self.lw_tiles
-        self._ranges_for_step()   # refreshes the skip bits of the per-parameter group table
-        a.param_group, a.steps = self._range_group.data_ptr(), self._range_steps.data_ptr()
-        a.master, a.workspace = self.master_ptr, self._lw_ws.data_ptr()
+        a.workspace = self._lw_ws.data_ptr()
         a.exp_avg = self.M.ptr if self.M else None
         a.exp_avg_sq = self.V.ptr if self.V else None
-        if self.route == "local":
-            a.grad, a.grad_dtype, a.grad_raw, a.grad_mul = self.G.ptr, _DT[self.model_dtype], 1, 1.0
-            a.acc = self.ACC.ptr if self._raw_has_acc else None
-        else:
-            a.grad, a.grad_dtype, a.grad_raw = self.MAIN.ptr, _lib.F32, 0
-        if self.low_precision:
-            a.lp, a.lp_dtype = self.P.ptr, _DT[self.model_dtype]
+        self._per_param_args(a)
         e._check(e.lib.stk_layerwise_step(e.ctx, C.byref(a), e._stream()))
         e.launches += 3
-        self.weight_avg_after_step()
-        e.step_epilogue()
-        self._track_touched = False
-        self._raw_has_acc = False
-        e.comm_poll()
+        self._end_step()
 
     def adafactor_state_views(self) -> List[Tuple[torch.Tensor, ...]]:
         """Per parameter, views of the state buffer in torch's shapes: (row_var [..., R, 1], col_var [..., 1, C]) or

@@ -44,7 +44,10 @@ replicated all-reduce route at world > 1.
 Each fused kind's per-parameter state is one row of ``_STATE_LAYOUT``: torch's keys in order, the flat buffer that holds
 each tensor (M, V, M2 or Adafactor's own), its initial value, the groups it exists in, and what a never-stepped
 parameter exports.  The buffers ``GradPath`` allocates (``state_buffers``), ``state_dict`` (``export_state``) and
-``load_state_dict`` (``import_state``) all follow from that row, so a new kind adds one row.
+``load_state_dict`` (``import_state``) all follow from that row.  The per-group struct a kind's step takes besides
+``OptimHyper`` (``_hyper_of``), or in its place for Adafactor, LAMB and LARS, is built by the kind's row of
+``_GROUP_HYPER``; ``GradPath.optimizer_step`` chooses the prologues and the entry point of a K2 kind by its kind.  A new
+kind therefore adds a state row, a struct builder and its ``_GROUP_HYPER`` row, and at most one case in that choice.
 
 ``B200StockOptimizer`` -- every other ``torch.optim`` class (the reference instantiates whatever class the user passes,
 stoke/extensions.py:53-78) and the options the fused step does not cover (amsgrad, capturable, differentiable, more than 8
@@ -63,7 +66,7 @@ from .engine import ClipSpec, Engine, GradPath
 _KINDS = {torch.optim.Adam: _lib.OPT_ADAM, torch.optim.AdamW: _lib.OPT_ADAMW, torch.optim.SGD: _lib.OPT_SGD,
           torch.optim.NAdam: _lib.OPT_NADAM, torch.optim.RAdam: _lib.OPT_RADAM, torch.optim.Adamax: _lib.OPT_ADAMAX,
           torch.optim.Adadelta: _lib.OPT_ADADELTA, torch.optim.Rprop: _lib.OPT_RPROP, torch.optim.ASGD: _lib.OPT_ASGD}
-# per-step scalars from stk_optim_step_prologue
+# per-step scalars from stk_optim_step_prologue, which takes their OptimHyperExt (_ext_hyper)
 _EXT_KINDS = (_lib.OPT_NADAM, _lib.OPT_RADAM, _lib.OPT_ADAMAX, _lib.OPT_ADADELTA, _lib.OPT_RPROP, _lib.OPT_ASGD)
 _STOCK_ONLY_TRUE = ("amsgrad", "capturable", "differentiable")
 # torch.optim.Adafactor (torch >= 2.5) runs on its own entry point, stk_adafactor_step, not as a kind of K2
@@ -772,6 +775,85 @@ _STATE_LAYOUT: Dict[object, StateLayout] = {
 }
 
 
+def _ext_hyper(g) -> _lib.OptimHyperExt:
+    x = _lib.OptimHyperExt()
+    x.momentum_decay = float(g.get("momentum_decay", 0.0))
+    x.decoupled_weight_decay = int(bool(g.get("decoupled_weight_decay", False)))
+    x.rho = float(g.get("rho", 0.0))
+    x.etaminus, x.etaplus = (float(e) for e in g.get("etas", (0.0, 0.0)))
+    x.step_size_min, x.step_size_max = (float(e) for e in g.get("step_sizes", (0.0, 0.0)))
+    x.lambd, x.alpha, x.t0 = float(g.get("lambd", 0.0)), float(g.get("alpha", 0.0)), float(g.get("t0", 0.0))
+    return x
+
+
+def _sf_hyper(g) -> _lib.SfHyper:
+    x = _lib.SfHyper()
+    x.lr, x.beta1, x.r = float(g["lr"]), float(_sf_beta1(g)), float(g["r"])
+    x.weight_lr_power = float(g["weight_lr_power"])
+    x.beta2 = float(g["betas"][1]) if "betas" in g else 0.0
+    x.warmup_steps = int(g["warmup_steps"])
+    return x
+
+
+def _ademamix_hyper(g) -> _lib.AdemamixHyper:
+    x = _lib.AdemamixHyper()
+    x.alpha, x.beta3 = float(g["alpha"]), float(g["betas"][2])
+    x.alpha_warmup = int(g["alpha_warmup"] or 0)   # 0: none
+    x.beta3_warmup = int(g["beta3_warmup"] or 0)
+    return x
+
+
+def _rmsprop_tf_hyper(g) -> _lib.RmspropTfHyper:
+    x = _lib.RmspropTfHyper()
+    x.alpha = float(g["alpha"])
+    x.centered, x.decoupled_decay = int(bool(g["centered"])), int(bool(g["decoupled_decay"]))
+    x.lr_in_momentum = int(bool(g["lr_in_momentum"]))
+    return x
+
+
+def _adan_hyper(g) -> _lib.AdanHyper:
+    x = _lib.AdanHyper()
+    x.beta3, x.no_prox = float(g["betas"][2]), int(bool(g["no_prox"]))
+    return x
+
+
+def _adafactor_hyper(g) -> _lib.AdafactorHyper:
+    h = _lib.AdafactorHyper()
+    eps1, eps2 = g["eps"]
+    h.lr, h.beta2_decay, h.eps2, h.d = float(g["lr"]), float(g["beta2_decay"]), float(eps2), float(g["d"])
+    h.weight_decay = float(g["weight_decay"])
+    h.eps1_none, h.eps1 = int(eps1 is None), float(eps1 if eps1 is not None else 0.0)
+    h.maximize = int(bool(g.get("maximize", False)))
+    return h
+
+
+def _layerwise_hyper(g) -> _lib.LayerwiseHyper:
+    h = _lib.LayerwiseHyper()
+    h.lr, h.eps, h.weight_decay = float(g["lr"]), float(g["eps"]), float(g["weight_decay"])
+    h.always_adapt = int(bool(g["always_adapt"]))
+    if "betas" in g:   # LAMB
+        h.beta1, h.beta2 = (float(b) for b in g["betas"])
+        h.bias_correction = int(bool(g["bias_correction"]))
+    else:              # LARS
+        h.momentum, h.dampening = float(g["momentum"]), float(g["dampening"])
+        h.trust_coefficient, h.nesterov = float(g["trust_coefficient"]), int(bool(g["nesterov"]))
+    return h
+
+
+# The per-group struct each fused kind's step takes, built from one param group.  The K2 kinds pass it beside their
+# OptimHyper array (GradPath.optimizer_step chooses the prologues and the entry point by kind); a K2 kind without a row
+# passes OptimHyper alone.  Adafactor, LAMB and LARS pass it alone to their own entry points.
+_GROUP_HYPER: Dict[object, Callable[[Dict], object]] = {
+    **{k: _ext_hyper for k in _EXT_KINDS},
+    _lib.OPT_SF_ADAMW: _sf_hyper, _lib.OPT_SF_SGD: _sf_hyper,
+    _lib.OPT_ADEMAMIX: _ademamix_hyper,
+    _lib.OPT_RMSPROP_TF: _rmsprop_tf_hyper,
+    _lib.OPT_ADAN: _adan_hyper,
+    _ADAFACTOR: _adafactor_hyper,
+    _LAMB: _layerwise_hyper, _LARS: _layerwise_hyper,
+}
+
+
 def state_buffers(layout: StateLayout, groups: List[Dict]) -> Dict[str, object]:
     """The flat fp32 buffers a kind needs for these parameter groups: ``{"M", "V", "M2"} -> initial value`` (0.0, 1.0
     or "master"), None for a buffer that is not allocated, plus ``"M3"`` for a kind that keeps a tensor there."""
@@ -986,29 +1068,6 @@ class B200FusedOptimizer(torch.optim.Optimizer):
         engine.scaler_set(state=self.path.state_id, opt_steps=0, skipped_steps=0, found_inf=0, growth_tracker=0)
 
     # -- the step -------------------------------------------------------------------------------------------------------
-    @staticmethod
-    def _adafactor_hyper_of(g) -> _lib.AdafactorHyper:
-        h = _lib.AdafactorHyper()
-        eps1, eps2 = g["eps"]
-        h.lr, h.beta2_decay, h.eps2, h.d = float(g["lr"]), float(g["beta2_decay"]), float(eps2), float(g["d"])
-        h.weight_decay = float(g["weight_decay"])
-        h.eps1_none, h.eps1 = int(eps1 is None), float(eps1 if eps1 is not None else 0.0)
-        h.maximize = int(bool(g.get("maximize", False)))
-        return h
-
-    @staticmethod
-    def _layerwise_hyper_of(g) -> _lib.LayerwiseHyper:
-        h = _lib.LayerwiseHyper()
-        h.lr, h.eps, h.weight_decay = float(g["lr"]), float(g["eps"]), float(g["weight_decay"])
-        h.always_adapt = int(bool(g["always_adapt"]))
-        if "betas" in g:   # LAMB
-            h.beta1, h.beta2 = (float(b) for b in g["betas"])
-            h.bias_correction = int(bool(g["bias_correction"]))
-        else:              # LARS
-            h.momentum, h.dampening = float(g["momentum"]), float(g["dampening"])
-            h.trust_coefficient, h.nesterov = float(g["trust_coefficient"]), int(bool(g["nesterov"]))
-        return h
-
     def _hyper_of(self, g) -> _lib.OptimHyper:
         h = _lib.OptimHyper()
         h.kind = self._kind
@@ -1028,90 +1087,19 @@ class B200FusedOptimizer(torch.optim.Optimizer):
             h.eps = float(g["eps"])
         return h
 
-    def _hyper(self) -> _lib.OptimHyper:
-        return self._hyper_of(self.param_groups[0])
-
-    def _hypers(self) -> List[_lib.OptimHyper]:
-        return [self._hyper_of(g) for g in self.param_groups]
-
-    def _sf_hypers(self) -> List[_lib.SfHyper]:
-        out = []
-        for g in self.param_groups:
-            x = _lib.SfHyper()
-            x.lr, x.beta1, x.r = float(g["lr"]), float(_sf_beta1(g)), float(g["r"])
-            x.weight_lr_power = float(g["weight_lr_power"])
-            x.beta2 = float(g["betas"][1]) if "betas" in g else 0.0
-            x.warmup_steps = int(g["warmup_steps"])
-            out.append(x)
-        return out
-
-    def _ademamix_hypers(self) -> List[_lib.AdemamixHyper]:
-        out = []
-        for g in self.param_groups:
-            x = _lib.AdemamixHyper()
-            x.alpha, x.beta3 = float(g["alpha"]), float(g["betas"][2])
-            x.alpha_warmup = int(g["alpha_warmup"] or 0)   # 0: none
-            x.beta3_warmup = int(g["beta3_warmup"] or 0)
-            out.append(x)
-        return out
-
-    def _rmsprop_tf_hypers(self) -> List[_lib.RmspropTfHyper]:
-        out = []
-        for g in self.param_groups:
-            x = _lib.RmspropTfHyper()
-            x.alpha = float(g["alpha"])
-            x.centered, x.decoupled_decay = int(bool(g["centered"])), int(bool(g["decoupled_decay"]))
-            x.lr_in_momentum = int(bool(g["lr_in_momentum"]))
-            out.append(x)
-        return out
-
-    def _adan_hypers(self) -> List[_lib.AdanHyper]:
-        out = []
-        for g in self.param_groups:
-            x = _lib.AdanHyper()
-            x.beta3, x.no_prox = float(g["betas"][2]), int(bool(g["no_prox"]))
-            out.append(x)
-        return out
-
-    def _exts(self) -> Optional[List[_lib.OptimHyperExt]]:
-        if self._kind not in _EXT_KINDS:
-            return None
-        out = []
-        for g in self.param_groups:
-            x = _lib.OptimHyperExt()
-            x.momentum_decay = float(g.get("momentum_decay", 0.0))
-            x.decoupled_weight_decay = int(bool(g.get("decoupled_weight_decay", False)))
-            x.rho = float(g.get("rho", 0.0))
-            x.etaminus, x.etaplus = (float(e) for e in g.get("etas", (0.0, 0.0)))
-            x.step_size_min, x.step_size_max = (float(e) for e in g.get("step_sizes", (0.0, 0.0)))
-            x.lambd, x.alpha, x.t0 = float(g.get("lambd", 0.0)), float(g.get("alpha", 0.0)), float(g.get("t0", 0.0))
-            out.append(x)
-        return out
-
     @torch.no_grad()
     def step(self, closure=None):
         if closure is not None:
             raise NotImplementedError("Stoke -- closures are not supported by the fused step")
+        self.check_train_mode()
+        build = _GROUP_HYPER.get(self._kind)
+        per_group = [build(g) for g in self.param_groups] if build is not None else None
         if self._kind == _ADAFACTOR:
-            self.path.adafactor_step([self._adafactor_hyper_of(g) for g in self.param_groups])
-            return
-        if self._kind in _LAYERWISE:
-            self.path.layerwise_step(_LAYERWISE[self._kind], [self._layerwise_hyper_of(g) for g in self.param_groups])
-            return
-        if self._kind in _SF_KINDS:
-            self.check_train_mode()
-            self.path.optimizer_step(self._hypers(), None, self._sf_hypers())
-            return
-        if self._kind == _lib.OPT_ADEMAMIX:
-            self.path.optimizer_step(self._hypers(), ademamix=self._ademamix_hypers())
-            return
-        if self._kind == _lib.OPT_RMSPROP_TF:
-            self.path.optimizer_step(self._hypers(), rmsprop_tf=self._rmsprop_tf_hypers())
-            return
-        if self._kind == _lib.OPT_ADAN:
-            self.path.optimizer_step(self._hypers(), adan=self._adan_hypers())
-            return
-        self.path.optimizer_step(self._hypers(), self._exts())
+            self.path.adafactor_step(per_group)
+        elif self._kind in _LAYERWISE:
+            self.path.layerwise_step(_LAYERWISE[self._kind], per_group)
+        else:
+            self.path.optimizer_step([self._hyper_of(g) for g in self.param_groups], per_group)
 
     # -- schedule-free: train() / eval() ------------------------------------------------------------------------------------
     def check_train_mode(self):

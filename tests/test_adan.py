@@ -216,7 +216,7 @@ def test_load_step_counts_from_the_groups():
 
 def test_hypers_without_a_gpu():
     """What the fused optimizer hands stk_adan_step_prologue and stk_adan_step."""
-    from stoke_b200.optim import B200FusedOptimizer
+    from stoke_b200.optim import _GROUP_HYPER, B200FusedOptimizer
 
     obj = B200FusedOptimizer.__new__(B200FusedOptimizer)
     obj._kind = _lib.OPT_ADAN
@@ -225,5 +225,5 @@ def test_hypers_without_a_gpu():
                         dict(Adan(p, no_prox=True).defaults)]
     h = obj._hyper_of(obj.param_groups[0])
     assert (h.kind, h.lr, h.beta1, h.beta2, h.eps, h.weight_decay, h.maximize) == (14, 0.3, 0.9, 0.8, 1e-6, 0.02, 0)
-    x, y = obj._adan_hypers()
+    x, y = (_GROUP_HYPER[_lib.OPT_ADAN](g) for g in obj.param_groups)
     assert (x.beta3, x.no_prox) == (0.7, 0) and (y.beta3, y.no_prox) == (0.99, 1)

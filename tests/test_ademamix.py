@@ -206,7 +206,7 @@ def test_load_step_counts_for_ademamix_state():
 
 def test_hypers_without_a_gpu():
     """What the fused optimizer hands stk_optim_step_ex and stk_ademamix_step_prologue."""
-    from stoke_b200.optim import B200FusedOptimizer
+    from stoke_b200.optim import _GROUP_HYPER, B200FusedOptimizer
 
     obj = B200FusedOptimizer.__new__(B200FusedOptimizer)
     obj._kind = _lib.OPT_ADEMAMIX
@@ -216,7 +216,7 @@ def test_hypers_without_a_gpu():
                         dict(AdEMAMix(p, betas=(0.0, 0.9, 0.99), beta3_warmup=11).defaults)]
     h = obj._hyper_of(obj.param_groups[0])
     assert (h.kind, h.lr, h.beta1, h.beta2, h.eps, h.weight_decay) == (12, 0.3, 0.8, 0.95, 1e-6, 0.1)
-    x, y = obj._ademamix_hypers()
+    x, y = (_GROUP_HYPER[_lib.OPT_ADEMAMIX](g) for g in obj.param_groups)
     assert (x.alpha, x.beta3, x.alpha_warmup, x.beta3_warmup) == (6.0, 0.999, 7, 0)
     assert (y.alpha, y.beta3, y.alpha_warmup, y.beta3_warmup) == (2.0, 0.99, 0, 11)
     assert obj._hyper_of(obj.param_groups[1]).beta1 == 0.0

@@ -150,7 +150,7 @@ def test_fused_supported():
 def test_hyper_of_lion_and_the_existing_classes():
     """Lion's betas, weight decay and maximize reach stk_optim_hyper_t (Lion has no eps); the classes with betas and eps
     keep theirs."""
-    from stoke_b200.optim import B200FusedOptimizer
+    from stoke_b200.optim import _GROUP_HYPER, B200FusedOptimizer
 
     obj = B200FusedOptimizer.__new__(B200FusedOptimizer)
     obj._kind = _lib.OPT_LION
@@ -158,7 +158,7 @@ def test_hyper_of_lion_and_the_existing_classes():
     obj.param_groups = [g]
     h = obj._hyper_of(g)
     assert (h.kind, h.lr, h.beta1, h.beta2, h.weight_decay, h.maximize, h.eps) == (9, 3e-4, 0.95, 0.98, 0.1, 1, 0.0)
-    assert obj._exts() is None
+    assert _lib.OPT_LION not in _GROUP_HYPER   # OptimHyper alone
     obj._kind = _lib.OPT_ADAM
     g = {"lr": 1e-3, "betas": (0.8, 0.9), "eps": 1e-7, "weight_decay": 0.0, "maximize": False}
     h = obj._hyper_of(g)

@@ -211,9 +211,10 @@ def test_ext_struct_appends_fields():
 
 
 def test_exts_and_hypers_per_group():
-    """_hyper_of / _exts fill each class's fields from its param_groups (no GPU: the optimizer object is not built)."""
+    """_hyper_of and the OptimHyperExt builder fill each class's fields from its param_groups (no GPU: the optimizer
+    object is not built)."""
     from stoke_b200 import _lib
-    from stoke_b200.optim import B200FusedOptimizer
+    from stoke_b200.optim import _EXT_KINDS, _GROUP_HYPER, B200FusedOptimizer, _ext_hyper
 
     obj = B200FusedOptimizer.__new__(B200FusedOptimizer)
     groups = {
@@ -224,7 +225,7 @@ def test_exts_and_hypers_per_group():
     for kind, g in groups.items():
         obj._kind = kind
         obj.param_groups = [g]
-        h, (x,) = obj._hyper_of(g), obj._exts()
+        h, x = obj._hyper_of(g), _GROUP_HYPER[kind](g)
         assert h.kind == kind and h.lr == g["lr"] and h.maximize == int(g["maximize"])
         assert h.weight_decay == g.get("weight_decay", 0.0)
         if kind == _lib.OPT_ADADELTA:
@@ -233,3 +234,4 @@ def test_exts_and_hypers_per_group():
             assert (x.etaminus, x.etaplus, x.step_size_min, x.step_size_max) == (0.4, 1.3, 1e-5, 10.0)
         if kind == _lib.OPT_ASGD:
             assert (x.lambd, x.alpha, x.t0) == (1e-3, 0.5, 100.0)
+    assert {k for k, f in _GROUP_HYPER.items() if f is _ext_hyper} == set(_EXT_KINDS)

@@ -182,7 +182,7 @@ def test_load_step_counts_for_rmsprop_tf_state():
 
 def test_hypers_without_a_gpu():
     """What the fused optimizer hands stk_rmsprop_tf_step."""
-    from stoke_b200.optim import B200FusedOptimizer
+    from stoke_b200.optim import _GROUP_HYPER, B200FusedOptimizer
 
     obj = B200FusedOptimizer.__new__(B200FusedOptimizer)
     obj._kind = _lib.OPT_RMSPROP_TF
@@ -192,6 +192,6 @@ def test_hypers_without_a_gpu():
     h = obj._hyper_of(obj.param_groups[0])
     assert (h.kind, h.lr, h.eps, h.weight_decay, h.momentum, h.maximize) == (13, 0.3, 1e-3, 1e-5, 0.9, 0)
     assert obj._hyper_of(obj.param_groups[1]).momentum == 0.0
-    x, y = obj._rmsprop_tf_hypers()
+    x, y = (_GROUP_HYPER[_lib.OPT_RMSPROP_TF](g) for g in obj.param_groups)
     assert (x.alpha, x.centered, x.decoupled_decay, x.lr_in_momentum) == (0.95, 0, 0, 1)
     assert (y.alpha, y.centered, y.decoupled_decay, y.lr_in_momentum) == (0.9, 1, 1, 0)

@@ -236,13 +236,13 @@ def test_load_step_counts_for_schedule_free_state():
 
 def test_sf_hypers_and_swap_guard_without_a_gpu():
     """What the fused optimizer hands stk_sf_step_prologue; train() / eval() on another kind is refused."""
-    from stoke_b200.optim import B200FusedOptimizer
+    from stoke_b200.optim import _GROUP_HYPER, B200FusedOptimizer
 
     obj = B200FusedOptimizer.__new__(B200FusedOptimizer)
     obj._kind = _lib.OPT_SF_SGD
     obj.param_groups = [dict(SGDScheduleFree([torch.nn.Parameter(torch.zeros(1))], lr=0.3, momentum=0.8, r=0.5,
                                              warmup_steps=7, weight_decay=0.1).defaults)]
-    x = obj._sf_hypers()[0]
+    x = _GROUP_HYPER[_lib.OPT_SF_SGD](obj.param_groups[0])
     assert (x.lr, x.beta1, x.beta2, x.r, x.weight_lr_power, x.warmup_steps) == (0.3, 0.8, 0.0, 0.5, 2.0, 7)
     h = obj._hyper_of(obj.param_groups[0])
     assert (h.kind, h.lr, h.weight_decay) == (11, 0.3, 0.1)
