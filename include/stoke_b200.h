@@ -41,6 +41,8 @@
  *                                    the clip and the GradScaler.step gate, without its two .item() per parameter
  *   stk_layerwise_step               the step of the LAMB / LARS classes of stoke_b200.optim (per-parameter trust ratios;
  *                                    torch.optim has neither), plus the clip and the GradScaler.step gate
+ *   stk_adam8bit_step                the step of AdamW8bit / Adam8bit of stoke_b200.optim (bitsandbytes' 8-bit AdamW:
+ *                                    block-wise quantized moments), plus the clip and the GradScaler.step gate
  *   stk_weight_avg                   torch.optim.swa_utils.AveragedModel.update_parameters (EMA / SWA) over the fp32
  *                                    master weights; the reference has no weight averaging
  */
@@ -594,6 +596,58 @@ typedef struct {
   void* lp; int lp_dtype;      /* low-precision parameter copy written after the update (bf16 | f32), or NULL */
 } stk_layerwise_args_t;
 int stk_layerwise_step(stk_ctx* ctx, const stk_layerwise_args_t* args, void* stream);
+
+/* ---- 8-bit AdamW: block-wise quantized moments (stoke_b200.optim.AdamW8bit / Adam8bit) --------------------------------
+ * AdamW with m and v stored as 8-bit codes (Dettmers et al. 2022), plus the clip and the GradScaler.step gate.  Per
+ * parameter with a gradient, g the gradient after unscale, accumulation and clip, t = its own step count after the
+ * increment, every op one fp32 rounding in this order:
+ *   c1 = 1 - beta1^t;  c2 = sqrt(1 - beta2^t)                  (double)
+ *   m = deq(m) b1 + g (1 - b1);  v = deq(v) b2 + (g g) (1 - b2)
+ *   weight_decay != 0: w = w fp32(1 - lr wd)
+ *   w = w - (m / (sqrt(v) + fp32(eps c2))) fp32(lr c2 / c1)
+ *   m, v = quant(m), quant(v)                                    (the update uses the unquantized m, v)
+ * Quantization is over STK_Q8_BLOCK-element blocks of each parameter in flat order: absmax = max |x| over the block (NaN
+ * if the block holds a NaN), n = x * (absmax == 0 ? 0 : 1 / absmax), the code is the index of the qmap entry nearest to n
+ * (fp32 distances |n - q|, ties to the lower index, a NaN n takes the code of 0), deq(code) = qmap[code] absmax.  qmap1
+ * (m) and qmap2 (v): 256 ascending fp32 entries each.  A parameter with `small` >= 0 keeps fp32 m and v in the compact
+ * buffer and skips the quantization.  Two stream-ordered launches: a per-parameter prologue (verdict, step count, step
+ * scalars in `workspace`), then one warp per block.  Deterministic, no floating-point atomics.  found_inf skips every
+ * parameter and a set bit 7 of its group byte skips one: master, codes, absmax, fp32 state and count are left as they
+ * are (the raw bucket is still zeroed).  Nothing is synchronised. */
+#define STK_Q8_BLOCK 256
+
+typedef struct {          /* one per parameter */
+  uint64_t offset;        /* first element in the flat master / gradient / code / lp buffers: a multiple of 16 */
+  int32_t numel;          /* 0 .. 2^31 - 1 */
+  int32_t block0;         /* first block: the sum of ceil(numel / STK_Q8_BLOCK) over the parameters before it */
+  int64_t small;          /* -1: 8-bit state; else the first element of its fp32 state in `small` (a multiple of 16) */
+} stk_adam8bit_param_t;
+
+typedef struct {          /* one per parameter group */
+  double lr, beta1, beta2, eps, weight_decay;
+} stk_adam8bit_hyper_t;
+
+typedef struct {
+  const stk_adam8bit_hyper_t* hyper; int n_groups;   /* host array, <= STK_MAX_GROUPS */
+  int clip_kind; double clip_max_norm, clip_value;
+  const stk_adam8bit_param_t* params;  /* DEVICE table, ascending offsets */
+  const int32_t* block_param;          /* DEVICE, one per block: the index of its parameter */
+  int n_params, n_blocks;              /* n_blocks: the sum of ceil(numel / STK_Q8_BLOCK) */
+  const uint8_t* param_group;  /* DEVICE, one per parameter: group index, bit 7 = no gradient this step (not stepped) */
+  int32_t* steps;              /* DEVICE, one per parameter: steps taken; advanced here unless skipped or found_inf */
+  float* master;               /* fp32 masters (flat indexing) */
+  uint8_t* code1; uint8_t* code2;      /* m and v codes (flat indexing, 8-byte aligned) */
+  float* absmax1; float* absmax2;      /* one per block */
+  const float* qmap1; const float* qmap2;  /* DEVICE, 256 ascending entries each */
+  float* small; size_t n_small;        /* fp32 m at [0, n_small), v at [n_small, 2 n_small); n_small % 8 == 0 */
+  void* workspace;             /* 16 n_params bytes, 16-byte aligned, no initialisation */
+  const void* grad; int grad_dtype; int grad_raw;  /* raw = 1: model-dtype bucket (bf16 | f32) scaled by grad_mul and
+                                                      1/loss_scale, ZEROED after the step (also when skipped);
+                                                      raw = 0: fp32 reduced main gradients */
+  const float* acc; double grad_mul;  /* raw route: optional fp32 accumulator, multiplier */
+  void* lp; int lp_dtype;      /* low-precision parameter copy written after the update (bf16 | f32), or NULL */
+} stk_adam8bit_args_t;
+int stk_adam8bit_step(stk_ctx* ctx, const stk_adam8bit_args_t* args, void* stream);
 
 /* ---- small collectives on the signal pads -------------------------------------------------------------------------- */
 /* mean over ranks of *loss_dev (float32/bf16/f16 scalar) -> *out_host (pinned, mapped) ; synchronises `stream` */

@@ -135,6 +135,29 @@ class LayerwiseArgs(C.Structure):
                 ("grad_mul", C.c_double), ("lp", C.c_void_p), ("lp_dtype", C.c_int)]
 
 
+Q8_BLOCK = 256
+
+
+class Adam8bitParam(C.Structure):
+    _fields_ = [("offset", C.c_uint64), ("numel", C.c_int32), ("block0", C.c_int32), ("small", C.c_int64)]
+
+
+class Adam8bitHyper(C.Structure):
+    _fields_ = [("lr", C.c_double), ("beta1", C.c_double), ("beta2", C.c_double), ("eps", C.c_double),
+                ("weight_decay", C.c_double)]
+
+
+class Adam8bitArgs(C.Structure):
+    _fields_ = [("hyper", C.POINTER(Adam8bitHyper)), ("n_groups", C.c_int), ("clip_kind", C.c_int),
+                ("clip_max_norm", C.c_double), ("clip_value", C.c_double), ("params", C.c_void_p),
+                ("block_param", C.c_void_p), ("n_params", C.c_int), ("n_blocks", C.c_int), ("param_group", C.c_void_p),
+                ("steps", C.c_void_p), ("master", C.c_void_p), ("code1", C.c_void_p), ("code2", C.c_void_p),
+                ("absmax1", C.c_void_p), ("absmax2", C.c_void_p), ("qmap1", C.c_void_p), ("qmap2", C.c_void_p),
+                ("small", C.c_void_p), ("n_small", C.c_size_t), ("workspace", C.c_void_p), ("grad", C.c_void_p),
+                ("grad_dtype", C.c_int), ("grad_raw", C.c_int), ("acc", C.c_void_p), ("grad_mul", C.c_double),
+                ("lp", C.c_void_p), ("lp_dtype", C.c_int)]
+
+
 class SamplerPlan(C.Structure):
     _fields_ = [("n", C.c_int64), ("buckets", C.c_int64), ("batch_size", C.c_int64), ("world", C.c_int64),
                 ("rank", C.c_int64), ("drop_last", C.c_int32), ("allow_bucket_overlap", C.c_int32),
@@ -196,6 +219,7 @@ _SIGNATURES = {
     "stk_adafactor_plan": (C.c_int, [C.POINTER(AdafactorParam), C.c_int, C.POINTER(AdafactorPlan)]),
     "stk_adafactor_step": (C.c_int, [_P, C.POINTER(AdafactorArgs), _P]),
     "stk_layerwise_step": (C.c_int, [_P, C.POINTER(LayerwiseArgs), _P]),
+    "stk_adam8bit_step": (C.c_int, [_P, C.POINTER(Adam8bitArgs), _P]),
     "stk_weight_avg": (C.c_int, [_P, _P, _P, C.c_size_t, C.c_int, C.c_float, _P]),
     "stk_loss_sync": (C.c_int, [_P, _P, C.c_int, C.POINTER(C.c_double), _P]),
     "stk_loss_sync_begin": (C.c_int, [_P, _P, C.c_int, C.POINTER(C.c_int64), _P]),

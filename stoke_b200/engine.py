@@ -493,6 +493,11 @@ class GradPath:
       M3     fp32 fourth optimizer state (Adan's               local          indexed like M
              neg_pre_grad)
              (M, V, M2 and M3 exist as ``state`` lists them: buffer -> initial value)
+      Q8     the 8-bit AdamW's state (``adam8bit``):        local          all n (never sharded)
+             uint8 m / v codes over the flat layout, an
+             fp32 absmax per 256-element block, the two
+             maps, compact fp32 m / v of the parameters
+             below min_8bit_size; no M / V
       AVG    fp32 weight average (EMA / SWA)                   local          indexed like MASTER; only when averaging is
                                                                               configured (``enable_weight_average``)
 
@@ -508,7 +513,7 @@ class GradPath:
                  state: Optional[Dict[str, object]] = None, bucket_mb: Optional[float] = None,
                  state_id: Optional[int] = None, route: Optional[str] = None, group_of: Optional[Sequence[int]] = None,
                  overlap: bool = True, scalar_state: int = 0, adafactor: bool = False, layerwise: bool = False,
-                 schedule_free: bool = False):
+                 schedule_free: bool = False, adam8bit: Optional[Sequence[bool]] = None):
         self.engine = engine
         self.params = [p for p in params if p.requires_grad]
         if not self.params:
@@ -682,6 +687,9 @@ class GradPath:
         self.layerwise = bool(layerwise)
         if self.layerwise:
             self._layerwise_setup()
+        self.adam8bit = adam8bit is not None   # per parameter: 8-bit state (else fp32, below min_8bit_size)
+        if self.adam8bit:
+            self._adam8bit_setup(adam8bit)
         self.avg_flat = None   # AVG, allocated by enable_weight_average
         self.avg_owner = None  # the WeightAverage over this path: its applied() refuses a schedule-free swap
         self.avg_due = None    # (mode, weight) of the weight-average update the next step carries, set by Stoke.step
@@ -730,6 +738,51 @@ class GradPath:
         self._lw_desc = torch.frombuffer(bytearray(C.string_at(descs, C.sizeof(descs))), dtype=torch.uint8).to(dev)
         self._lw_ws = torch.empty(16 * len(self.params) + 8 * self.lw_tiles, dtype=torch.uint8, device=dev)
         self._range_steps = torch.zeros(len(self.params), dtype=torch.int32, device=dev)
+
+    def _adam8bit_setup(self, quantized: Sequence[bool]):
+        """State, descriptor tables and workspace of the fused 8-bit AdamW step, built once.  The state: two uint8 code
+        buffers over the flat layout (m, v), one fp32 absmax per 256-element block of each parameter for each of them,
+        the two maps, and one compact fp32 buffer for the parameters below min_8bit_size (their m, then their v, each
+        parameter at a 16-element aligned offset).  No fp32 moment buffers.  The blocks need whole parameters on one
+        rank, so there is no sharded route."""
+        if self.sharded:
+            raise ValueError("Stoke -- the fused 8-bit AdamW step needs whole parameters on one rank (no sharded route)")
+        dev = self._range_end.device
+        descs = (_lib.Adam8bitParam * len(self.params))()
+        nblocks, self.q8_block0, self.q8_small_at = [], [], []
+        blocks = small = 0
+        for d, p, o, pad, q in zip(descs, self.params, self.offsets, self.padded, quantized):
+            nb = -(-p.numel() // _lib.Q8_BLOCK)
+            d.offset, d.numel, d.block0, d.small = o, p.numel(), blocks, -1 if q else small
+            self.q8_block0.append(blocks)
+            self.q8_small_at.append(None if q else small)
+            nblocks.append(nb)
+            blocks += nb
+            small += 0 if q else pad
+        self.q8_quantized = [bool(q) for q in quantized]
+        self.q8_blocks, self.q8_n_small = max(blocks, 1), small
+        self._q8_desc = torch.frombuffer(bytearray(C.string_at(descs, C.sizeof(descs))), dtype=torch.uint8).to(dev)
+        self._q8_block_param = torch.repeat_interleave(torch.arange(len(self.params), dtype=torch.int32),
+                                                       torch.tensor(nblocks, dtype=torch.int64)).to(dev)
+        self.q8_code1 = torch.zeros(max(self.n, ALIGN_ELEMS), dtype=torch.uint8, device=dev)
+        self.q8_code2 = torch.zeros_like(self.q8_code1)
+        self.q8_absmax1 = torch.zeros(self.q8_blocks, dtype=torch.float32, device=dev)
+        self.q8_absmax2 = torch.zeros_like(self.q8_absmax1)
+        self.q8_small = torch.zeros(max(2 * small, ALIGN_ELEMS), dtype=torch.float32, device=dev)
+        self.q8_qmap1 = torch.empty(256, dtype=torch.float32, device=dev)
+        self.q8_qmap2 = torch.empty_like(self.q8_qmap1)
+        self._q8_ws = torch.empty(16 * len(self.params), dtype=torch.uint8, device=dev)
+        self._range_steps = torch.zeros(len(self.params), dtype=torch.int32, device=dev)
+        self.adam8bit_reset()
+
+    def adam8bit_reset(self):
+        """The 8-bit state as before a first step: codes, absmax and fp32 state zero, the default maps."""
+        from .optim import create_dynamic_map
+
+        for t in (self.q8_code1, self.q8_code2, self.q8_absmax1, self.q8_absmax2, self.q8_small):
+            t.zero_()
+        self.q8_qmap1.copy_(create_dynamic_map(True))
+        self.q8_qmap2.copy_(create_dynamic_map(False))
 
     # -- layout helpers -----------------------------------------------------------------------------------------------
     @staticmethod
@@ -1058,6 +1111,41 @@ class GradPath:
         e.launches += 3
         self._end_step()
 
+    def adam8bit_step(self, hypers: Sequence[_lib.Adam8bitHyper]):
+        """One fused 8-bit AdamW step (``stk_adam8bit_step``: per-parameter prologue, then one warp per 256-element
+        block), then the epilogue.  ``hypers``: one ``Adam8bitHyper`` per group.  Parameters without a gradient in this
+        window are skipped through the skip bits of the range table; their step counts and state do not move."""
+        a = _lib.Adam8bitArgs()
+        e, _ = self._begin_step(a, _lib.Adam8bitHyper, hypers)
+        a.params, a.block_param = self._q8_desc.data_ptr(), self._q8_block_param.data_ptr()
+        a.n_params, a.n_blocks = len(self.params), self._q8_block_param.numel()
+        a.code1, a.code2 = self.q8_code1.data_ptr(), self.q8_code2.data_ptr()
+        a.absmax1, a.absmax2 = self.q8_absmax1.data_ptr(), self.q8_absmax2.data_ptr()
+        a.qmap1, a.qmap2 = self.q8_qmap1.data_ptr(), self.q8_qmap2.data_ptr()
+        a.small, a.n_small = self.q8_small.data_ptr(), self.q8_n_small
+        a.workspace = self._q8_ws.data_ptr()
+        self._per_param_args(a)
+        e._check(e.lib.stk_adam8bit_step(e.ctx, C.byref(a), e._stream()))
+        e.launches += 2
+        self._end_step()
+
+    def adam8bit_state_views(self) -> List[Dict[str, torch.Tensor]]:
+        """Per parameter, its 8-bit state in AdamW8bit's keys: ``state1`` / ``state2`` (uint8 codes shaped and strided
+        like the parameter), ``qmap1`` / ``qmap2`` (the shared maps) and ``absmax1`` / ``absmax2``; or, below
+        min_8bit_size, fp32 ``state1`` / ``state2`` views of the compact buffer."""
+        out = []
+        for i, (p, o) in enumerate(zip(self.params, self.offsets)):
+            if self.q8_quantized[i]:
+                b0, b1 = self.q8_block0[i], self.q8_block0[i] + -(-p.numel() // _lib.Q8_BLOCK)
+                out.append(dict(state1=self._strided(self.q8_code1, p, o), qmap1=self.q8_qmap1,
+                                state2=self._strided(self.q8_code2, p, o), qmap2=self.q8_qmap2,
+                                absmax1=self.q8_absmax1[b0:b1], absmax2=self.q8_absmax2[b0:b1]))
+            else:
+                s = self.q8_small_at[i]
+                out.append(dict(state1=self._strided(self.q8_small, p, s),
+                                state2=self._strided(self.q8_small, p, self.q8_n_small + s)))
+        return out
+
     def adafactor_state_views(self) -> List[Tuple[torch.Tensor, ...]]:
         """Per parameter, views of the state buffer in torch's shapes: (row_var [..., R, 1], col_var [..., 1, C]) or
         (variance,) shaped like the parameter."""
@@ -1192,6 +1280,9 @@ class GradPath:
         self.avg_flat = None
         self.af_state = self._af_ws = self._af_desc = None
         self._lw_ws = self._lw_desc = None
+        if getattr(self, "adam8bit", False):
+            self.q8_code1 = self.q8_code2 = self.q8_absmax1 = self.q8_absmax2 = self.q8_small = None
+            self._q8_ws = self._q8_desc = self._q8_block_param = None
         for b in self._bufs:
             try:
                 e.free(b)

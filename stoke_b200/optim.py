@@ -41,6 +41,9 @@ every rank taking the same deterministic step on the same gradients, as the stoc
 ``LAMB`` and ``LARS`` (defined here; torch.optim has neither) take ``stk_layerwise_step``: per-parameter trust ratios from
 two whole-parameter norms, per-parameter step counts on the device, the classes' own state_dict layout, and the same
 replicated all-reduce route at world > 1.
+``AdamW8bit`` and ``Adam8bit`` (defined here, after bitsandbytes) take ``stk_adam8bit_step``: Adam's moments as 8-bit
+codes, block-wise quantized over 256 elements, with per-parameter step counts on the device, bitsandbytes' state keys
+and no fp32 moment buffers; replicated on the all-reduce route at world > 1 (the blocks do not follow shard boundaries).
 Each fused kind's per-parameter state is one row of ``_STATE_LAYOUT``: torch's keys in order, the flat buffer that holds
 each tensor (M, V, M2 or Adafactor's own), its initial value, the groups it exists in, and what a never-stepped
 parameter exports.  The buffers ``GradPath`` allocates (``state_buffers``), ``state_dict`` (``export_state``) and
@@ -707,6 +710,222 @@ class Adan(torch.optim.Optimizer):
 
 _KINDS[Adan] = _lib.OPT_ADAN
 
+
+def create_dynamic_map(signed: bool = True) -> torch.Tensor:
+    """The 8-bit dynamic tree quantization map of Dettmers et al. (7 exponent bits, 8 bits in all): 256 ascending fp32
+    entries in [-1, 1] (signed) or [0, 1] (unsigned), one of them 0.  For i in 0..6 the midpoints of
+    ``linspace(0.1, 1, n_i)`` (fp32; n_i = 2 ** i + 1 signed, 2 ** (i + 1) + 1 unsigned) scaled by 10 ** (i - 6), with
+    their negatives in the signed map, then 0 and 1."""
+    data = []
+    for i in range(7):
+        b = torch.linspace(0.1, 1, 2 ** i + 1 if signed else 2 ** (i + 1) + 1)
+        mid = (10 ** (i - 6)) * ((b[:-1] + b[1:]) / 2.0)
+        data += mid.tolist() + ((-mid).tolist() if signed else [])
+    data += [0.0, 1.0]
+    return torch.tensor(sorted(data), dtype=torch.float32)
+
+
+def _memory_view(t: torch.Tensor) -> torch.Tensor:
+    """A 1-D view of a dense tensor in its memory order (a channels-last weight in its physical order)."""
+    x = t.permute(sorted(range(t.dim()), key=lambda d: -t.stride(d)))
+    if not x.is_contiguous():
+        raise ValueError("AdamW8bit: parameters and their state must be dense")
+    return x.view(-1)
+
+
+def _sqrt_rn(x: torch.Tensor) -> torch.Tensor:
+    """The correctly rounded fp32 square root on every device (taken in double, then rounded once: exact for fp32
+    inputs).  torch's CPU ``sqrt`` of fp32 is not always correctly rounded; its CUDA ``sqrt`` and the kernel's are."""
+    return x.double().sqrt_().float()
+
+
+def quantize_blockwise(x: torch.Tensor, qmap: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
+    """(uint8 codes, fp32 absmax per block) of a 1-D fp32 tensor: see ``AdamW8bit``."""
+    n = x.numel()
+    nb = -(-n // _lib.Q8_BLOCK)
+    absmax = torch.nn.functional.pad(x, (0, nb * _lib.Q8_BLOCK - n)).view(nb, _lib.Q8_BLOCK).abs().amax(1)
+    inv = torch.where(absmax == 0, torch.zeros_like(absmax), absmax.reciprocal())
+    y = x * inv.repeat_interleave(_lib.Q8_BLOCK)[:n]
+    y = torch.where(torch.isnan(y), torch.zeros_like(y), y)
+    hi = torch.searchsorted(qmap, y)   # the number of map entries below y
+    lo = (hi - 1).clamp_(min=0)
+    hi = hi.clamp_(max=qmap.numel() - 1)
+    code = torch.where((y - qmap[lo]).abs() <= (y - qmap[hi]).abs(), lo, hi)
+    return code.to(torch.uint8), absmax
+
+
+def dequantize_blockwise(code: torch.Tensor, qmap: torch.Tensor, absmax: torch.Tensor) -> torch.Tensor:
+    """qmap[code] * absmax of the code's block, fp32, 1-D."""
+    return qmap[code.long()] * absmax.repeat_interleave(_lib.Q8_BLOCK)[: code.numel()]
+
+
+def check_8bit_entries(entries: List[Dict], quantized: List[bool]):
+    """Refuses, with ValueError, 8-bit optimizer state a step could not continue from: a ``state1`` / ``state2`` dtype
+    that does not match the parameter's ``min_8bit_size`` class (``quantized``: uint8, else fp32), maps that are not
+    256 ascending entries, and maps that differ between parameters.  ``entries``: each parameter's state entry
+    (``{}`` where it has none).  Returns the checkpoint's ``(qmap1, qmap2)``, or None if it holds none."""
+    maps = None
+    for i, (e, quant) in enumerate(zip(entries, quantized)):
+        for key in ("state1", "state2"):
+            s = e.get(key)
+            want = torch.uint8 if quant else torch.float32
+            if s is not None and s.dtype != want:
+                raise ValueError(f"AdamW8bit: {key} of parameter {i} is {s.dtype}, expected {want} "
+                                 f"({'at or above' if quant else 'below'} min_8bit_size)")
+        if not quant or e.get("qmap1") is None or e.get("qmap2") is None:
+            continue
+        qm = (e["qmap1"].detach().float().cpu(), e["qmap2"].detach().float().cpu())
+        for key, q in zip(("qmap1", "qmap2"), qm):
+            if q.numel() != 256 or not bool((q[1:] > q[:-1]).all()):
+                raise ValueError(f"AdamW8bit: {key} must hold 256 ascending entries")
+        if maps is None:
+            maps = qm
+        elif not (torch.equal(maps[0], qm[0]) and torch.equal(maps[1], qm[1])):
+            raise ValueError("AdamW8bit: the quantization maps differ between parameters (the fused step keeps one pair)")
+    return maps
+
+
+class AdamW8bit(torch.optim.Optimizer):
+    """AdamW with 8-bit moments (bitsandbytes' ``AdamW8bit``: its arguments and state keys; Dettmers et al., "8-bit
+    Optimizers via Block-wise Quantization", 2022), about 2 B of optimizer state per parameter instead of 8.  For one
+    parameter w with gradient g and its own step count t (after the increment), every op one fp32 rounding in this order::
+
+        c1 = 1 - beta1 ** t;  c2 = sqrt(1 - beta2 ** t)                     (python doubles)
+        m = deq(m) * beta1 + g * (1 - beta1);  v = deq(v) * beta2 + (g * g) * (1 - beta2)
+        if weight_decay != 0: w = w * (1 - lr * weight_decay)
+        w = w - (m / (sqrt(v) + eps * c2)) * (lr * c2 / c1)
+        m, v = quant(m), quant(v)                                            (the update uses the unquantized m, v)
+
+    sqrt(v) is the correctly rounded fp32 square root on every device.  Quantization is block-wise over the parameter's
+    elements in memory order (a channels-last weight in its physical
+    order), 256 elements per block, the last one possibly short.  Per block absmax = amax(|x|) and
+    n = x * (absmax == 0 ? 0 : 1 / absmax); the code is the index of the map entry nearest to n (fp32 distances
+    |n - q|, equal distances to the lower index), and deq(code) = qmap[code] * absmax.  m takes the signed map
+    ``qmap1``, v the unsigned ``qmap2`` (``create_dynamic_map``).
+
+    Non-finite values: a NaN in a block makes its absmax NaN, an inf (and no NaN) makes it inf.  A NaN n -- a NaN or inf
+    element, or any element of a block whose absmax is NaN -- takes the code of 0 (the entry nearest to 0), and every
+    element of a block whose absmax is not finite decodes to NaN at the next step (qmap[code] * inf is NaN for the code
+    of 0 and +-inf otherwise; a finite element of an inf block has n = 0).
+
+    A parameter with fewer than ``min_8bit_size`` elements keeps fp32 ``state1`` / ``state2`` and takes the same update
+    without quantization.  State per parameter, created at its first step: ``step`` (0-dim fp32 tensor;
+    ``load_state_dict`` also accepts upstream's python int), ``state1``, ``qmap1``, ``state2``, ``qmap2``, ``absmax1``,
+    ``absmax2`` (no maps or absmax for a small parameter).  ``optim_bits`` is accepted and ignored; ``amsgrad``,
+    ``percentile_clipping != 100``, ``block_wise=False``, ``is_paged`` and ``args`` raise ValueError.  This ``step()``
+    is plain per-parameter torch: what runs outside the engine and on its stock route; inside ``Stoke`` the class runs
+    on the fused sm_90a step (``stk_adam8bit_step``)."""
+
+    def __init__(self, params, lr: float = 1e-3, betas=(0.9, 0.999), eps: float = 1e-8, weight_decay: float = 1e-2,
+                 amsgrad: bool = False, optim_bits: int = 32, args=None, min_8bit_size: int = 4096,
+                 percentile_clipping: int = 100, block_wise: bool = True, is_paged: bool = False):
+        for name, value, bad in (("amsgrad", amsgrad, amsgrad), ("args", args, args is not None),
+                                 ("percentile_clipping", percentile_clipping, percentile_clipping != 100),
+                                 ("block_wise", block_wise, not block_wise), ("is_paged", is_paged, is_paged)):
+            if bad:
+                raise ValueError(f"{type(self).__name__}: {name}={value!r} is not supported")
+        if lr < 0.0:
+            raise ValueError(f"Invalid learning rate: {lr}")
+        if eps < 0.0:
+            raise ValueError(f"Invalid epsilon value: {eps}")
+        if not 0.0 <= betas[0] < 1.0 or not 0.0 <= betas[1] < 1.0:
+            raise ValueError(f"Invalid beta parameters: {betas}")
+        if weight_decay < 0.0:
+            raise ValueError(f"Invalid weight_decay value: {weight_decay}")
+        super().__init__(params, dict(lr=lr, betas=tuple(betas), eps=eps, weight_decay=weight_decay,
+                                      min_8bit_size=int(min_8bit_size)))
+        self._maps: Dict[torch.device, Tuple[torch.Tensor, torch.Tensor]] = {}
+
+    def _init_state(self, p, state, quant: bool):
+        state["step"] = torch.tensor(0.0, dtype=torch.float32)
+        if not quant:
+            state["state1"] = torch.zeros_like(p, dtype=torch.float32, memory_format=torch.preserve_format)
+            state["state2"] = torch.zeros_like(p, dtype=torch.float32, memory_format=torch.preserve_format)
+            return
+        if p.device not in self._maps:
+            self._maps[p.device] = (create_dynamic_map(True).to(p.device), create_dynamic_map(False).to(p.device))
+        q1, q2 = self._maps[p.device]
+        nb = -(-p.numel() // _lib.Q8_BLOCK)
+        state["state1"] = torch.zeros_like(p, dtype=torch.uint8, memory_format=torch.preserve_format)
+        state["qmap1"] = q1
+        state["state2"] = torch.zeros_like(p, dtype=torch.uint8, memory_format=torch.preserve_format)
+        state["qmap2"] = q2
+        state["absmax1"] = torch.zeros(nb, dtype=torch.float32, device=p.device)
+        state["absmax2"] = torch.zeros(nb, dtype=torch.float32, device=p.device)
+
+    def load_state_dict(self, state_dict):
+        ids = [i for g in state_dict["param_groups"] for i in g["params"]]
+        quantized = [p.numel() >= sg.get("min_8bit_size", g["min_8bit_size"])
+                     for sg, g in zip(state_dict["param_groups"], self.param_groups) for p in g["params"]]
+        params = [p for g in self.param_groups for p in g["params"]]
+        check_8bit_entries([state_dict["state"].get(i, {}) for i in ids], quantized)
+        super().load_state_dict(state_dict)
+        for p in params:   # torch casts floating-point state to the parameter's dtype; the codes stay uint8
+            st = self.state.get(p)
+            if not st:
+                continue
+            if "step" in st and not torch.is_tensor(st["step"]):   # upstream keeps step as a python int
+                st["step"] = torch.tensor(float(st["step"]), dtype=torch.float32)
+            if "qmap1" in st:
+                st["state1"], st["state2"] = st["state1"].to(torch.uint8), st["state2"].to(torch.uint8)
+
+    @torch.no_grad()
+    def step(self, closure=None):
+        loss = None
+        if closure is not None:
+            with torch.enable_grad():
+                loss = closure()
+        for group in self.param_groups:
+            b1, b2 = group["betas"]
+            lr, eps, wd = group["lr"], group["eps"], group["weight_decay"]
+            for p in group["params"]:
+                if p.grad is None:
+                    continue
+                state = self.state[p]
+                if not state:
+                    self._init_state(p, state, p.numel() >= group["min_8bit_size"])
+                state["step"] += 1
+                t = float(state["step"])
+                c1, c2 = 1 - b1 ** t, math.sqrt(1 - b2 ** t)
+                g = p.grad if p.grad.stride() == p.stride() else torch.empty_like(p).copy_(p.grad)
+                g, w = _memory_view(g), _memory_view(p)
+                quant = "qmap1" in state
+                s1, s2 = _memory_view(state["state1"]), _memory_view(state["state2"])
+                if quant:
+                    m = dequantize_blockwise(s1, state["qmap1"], state["absmax1"])
+                    v = dequantize_blockwise(s2, state["qmap2"], state["absmax2"])
+                else:
+                    m, v = s1, s2
+                m.mul_(b1).add_(g * (1 - b1))
+                v.mul_(b2).add_(g.mul(g).mul_(1 - b2))
+                if wd != 0:
+                    w.mul_(1 - lr * wd)
+                w.sub_(m.div(_sqrt_rn(v).add_(eps * c2)).mul_(lr * c2 / c1))
+                if quant:
+                    for s, x, q, a in ((s1, m, state["qmap1"], state["absmax1"]), (s2, v, state["qmap2"], state["absmax2"])):
+                        code, absmax = quantize_blockwise(x, q)
+                        s.copy_(code)
+                        a.copy_(absmax)
+        return loss
+
+
+class Adam8bit(AdamW8bit):
+    """bitsandbytes' ``Adam8bit``: ``AdamW8bit`` with ``weight_decay=0`` by default (the decay, when given, is decoupled
+    as in AdamW8bit)."""
+
+    def __init__(self, params, lr: float = 1e-3, betas=(0.9, 0.999), eps: float = 1e-8, weight_decay: float = 0.0,
+                 amsgrad: bool = False, optim_bits: int = 32, args=None, min_8bit_size: int = 4096,
+                 percentile_clipping: int = 100, block_wise: bool = True, is_paged: bool = False):
+        super().__init__(params, lr=lr, betas=betas, eps=eps, weight_decay=weight_decay, amsgrad=amsgrad,
+                         optim_bits=optim_bits, args=args, min_8bit_size=min_8bit_size,
+                         percentile_clipping=percentile_clipping, block_wise=block_wise, is_paged=is_paged)
+
+
+# AdamW8bit and Adam8bit run on their own entry point, stk_adam8bit_step (block-wise quantized state), not as a kind of K2
+_ADAM8BIT = "adam8bit"
+_KINDS[AdamW8bit] = _ADAM8BIT
+_KINDS[Adam8bit] = _ADAM8BIT
+
 # LAMB and LARS run on their own entry point, stk_layerwise_step (per-parameter trust ratios), not as kinds of K2
 _LAMB, _LARS = "lamb", "lars"
 _KINDS[LAMB] = _LAMB
@@ -717,7 +936,8 @@ _LAYERWISE = {_LAMB: _lib.LW_LAMB, _LARS: _lib.LW_LARS}
 class StateTensor(NamedTuple):
     """One per-parameter state tensor of a fused kind."""
     key: str                                         # torch's state key
-    buf: str                                         # the flat fp32 buffer: "M", "V", "M2" or "M3"; "af": Adafactor's
+    buf: str                                         # the flat fp32 buffer: "M", "V", "M2" or "M3"; "af": Adafactor's;
+                                                     # "q8": the 8-bit step's codes, maps, absmax and fp32 state
     init: Union[float, str] = 0.0                    # its value before the first step: 0.0, 1.0 or "master"
     where: Optional[Callable[[Dict], bool]] = None   # the group condition under which it exists (None: every group)
     none: bool = False                               # where it does not exist, a parameter exports None (else no key)
@@ -772,6 +992,10 @@ _STATE_LAYOUT: Dict[object, StateLayout] = {
     # row_var / col_var of a factored parameter, variance of the others: views of GradPath.af_state
     _ADAFACTOR: StateLayout(True, (), "omit", (StateTensor("row_var", "af"), StateTensor("col_var", "af"),
                                                StateTensor("variance", "af"))),
+    # uint8 codes (fp32 for a parameter below min_8bit_size), the maps and the block absmax: views of GradPath's 8-bit
+    # state (adam8bit_state_views); no fp32 moment buffers
+    _ADAM8BIT: StateLayout(True, (), "omit", tuple(StateTensor(k, "q8") for k in (
+        "state1", "qmap1", "state2", "qmap2", "absmax1", "absmax2"))),
 }
 
 
@@ -827,6 +1051,13 @@ def _adafactor_hyper(g) -> _lib.AdafactorHyper:
     return h
 
 
+def _adam8bit_hyper(g) -> _lib.Adam8bitHyper:
+    h = _lib.Adam8bitHyper()
+    h.lr, h.eps, h.weight_decay = float(g["lr"]), float(g["eps"]), float(g["weight_decay"])
+    h.beta1, h.beta2 = (float(b) for b in g["betas"])
+    return h
+
+
 def _layerwise_hyper(g) -> _lib.LayerwiseHyper:
     h = _lib.LayerwiseHyper()
     h.lr, h.eps, h.weight_decay = float(g["lr"]), float(g["eps"]), float(g["weight_decay"])
@@ -842,7 +1073,7 @@ def _layerwise_hyper(g) -> _lib.LayerwiseHyper:
 
 # The per-group struct each fused kind's step takes, built from one param group.  The K2 kinds pass it beside their
 # OptimHyper array (GradPath.optimizer_step chooses the prologues and the entry point by kind); a K2 kind without a row
-# passes OptimHyper alone.  Adafactor, LAMB and LARS pass it alone to their own entry points.
+# passes OptimHyper alone.  Adafactor, LAMB, LARS and the 8-bit AdamW pass it alone to their own entry points.
 _GROUP_HYPER: Dict[object, Callable[[Dict], object]] = {
     **{k: _ext_hyper for k in _EXT_KINDS},
     _lib.OPT_SF_ADAMW: _sf_hyper, _lib.OPT_SF_SGD: _sf_hyper,
@@ -851,6 +1082,7 @@ _GROUP_HYPER: Dict[object, Callable[[Dict], object]] = {
     _lib.OPT_ADAN: _adan_hyper,
     _ADAFACTOR: _adafactor_hyper,
     _LAMB: _layerwise_hyper, _LARS: _layerwise_hyper,
+    _ADAM8BIT: _adam8bit_hyper,
 }
 
 
@@ -1028,7 +1260,7 @@ class B200FusedOptimizer(torch.optim.Optimizer):
                  bucket_mb: Optional[float] = None):
         if optim_cls not in _KINDS:
             raise NotImplementedError(
-                f"Stoke -- the fused step covers torch.optim.Adam, AdamW, SGD, NAdam, RAdam, Adamax, Adadelta, Rprop, ASGD and Adafactor and stoke_b200.optim.LAMB, LARS, Lion, AdamWScheduleFree, SGDScheduleFree, AdEMAMix, RMSpropTF and Adan; got {getattr(optim_cls, '__name__', optim_cls)}"
+                f"Stoke -- the fused step covers torch.optim.Adam, AdamW, SGD, NAdam, RAdam, Adamax, Adadelta, Rprop, ASGD and Adafactor and stoke_b200.optim.LAMB, LARS, Lion, AdamWScheduleFree, SGDScheduleFree, AdEMAMix, RMSpropTF, Adan, AdamW8bit and Adam8bit; got {getattr(optim_cls, '__name__', optim_cls)}"
                 f" (use B200StockOptimizer / build_optimizer, which routes other classes to the stock-optimizer path)")
         params, group_of, extra, kw = _group_layout(module, optim_kwargs)
         if len(extra) > _lib.MAX_GROUPS:
@@ -1049,15 +1281,18 @@ class B200FusedOptimizer(torch.optim.Optimizer):
         self._buffers = state_buffers(self._layout, probe.param_groups)
         ada = self._kind == _ADAFACTOR
         lw = self._kind in _LAYERWISE
-        if (ada or lw) and engine.world > 1:
-            # Adafactor's per-parameter reductions and LAMB's / LARS's trust ratios need whole parameters on one rank: their
-            # state is replicated (also under fairscale_oss) and every rank runs the same deterministic step on the same
-            # all-reduced fp32 gradients
+        q8 = None
+        if self._kind == _ADAM8BIT:   # which parameters keep 8-bit state (the others: fp32, below min_8bit_size)
+            q8 = [p.numel() >= probe.param_groups[gi]["min_8bit_size"] for p, gi in zip(params, group_of)]
+        if (ada or lw or q8 is not None) and engine.world > 1:
+            # Adafactor's per-parameter reductions and LAMB's / LARS's trust ratios need whole parameters on one rank, and
+            # the 8-bit state's 256-element blocks do not follow the shard boundaries: their state is replicated (also
+            # under fairscale_oss) and every rank runs the same deterministic step on the same all-reduced fp32 gradients
             route = "allreduce"
         self.path = GradPath(engine, params, grad_accum=grad_accum, clip=clip, sharded=sharded, lp_dtype=lp_dtype,
                              module=module, state=self._buffers, state_id=state_id, route=route,
                              group_of=group_of, bucket_mb=bucket_mb, scalar_state=len(self._layout.scalars),
-                             adafactor=ada, layerwise=lw, schedule_free=self._kind in _SF_KINDS)
+                             adafactor=ada, layerwise=lw, schedule_free=self._kind in _SF_KINDS, adam8bit=q8)
         by_group: List[List[torch.nn.Parameter]] = [[] for _ in extra]
         for p, gi in zip(params, group_of):
             by_group[gi].append(p)
@@ -1098,6 +1333,8 @@ class B200FusedOptimizer(torch.optim.Optimizer):
             self.path.adafactor_step(per_group)
         elif self._kind in _LAYERWISE:
             self.path.layerwise_step(_LAYERWISE[self._kind], per_group)
+        elif self._kind == _ADAM8BIT:
+            self.path.adam8bit_step(per_group)
         else:
             self.path.optimizer_step([self._hyper_of(g) for g in self.param_groups], per_group)
 
@@ -1162,6 +1399,9 @@ class B200FusedOptimizer(torch.optim.Optimizer):
             per_param = [dict(zip(("row_var", "col_var") if len(vs) == 2 else ("variance",), vs))
                          for vs in self.path.adafactor_state_views()]
             return {t.key: [d.get(t.key) for d in per_param] for t in self._layout.tensors}
+        if self._kind == _ADAM8BIT:
+            per_param = self.path.adam8bit_state_views()
+            return {t.key: [d.get(t.key) for d in per_param] for t in self._layout.tensors}
         return {t.key: self.path.unflatten(full[t.buf]) for t in self._layout.tensors if t.buf in full}
 
     def _groups_sd(self):
@@ -1218,6 +1458,9 @@ class B200FusedOptimizer(torch.optim.Optimizer):
                 torch.full((path.n,), float(self._buffers[b]), dtype=torch.float32, device=dev) for b in self._flats()}
         if self._kind == _ADAFACTOR:
             path.af_state.zero_()
+        if self._kind == _ADAM8BIT:   # refuses what the step could not continue from, then starts from the initial state
+            check_8bit_entries(entries, path.q8_quantized)
+            path.adam8bit_reset()
         import_state(self._layout, entries, self._views(full))
         for b, local in self._flats().items():
             path.scatter_local(full[b], local)
