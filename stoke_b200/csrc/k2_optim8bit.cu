@@ -80,11 +80,15 @@ __device__ __forceinline__ float q8_tree_entry(const float* q, int idx) {
 }
 
 // The index of the map entry nearest to n: distances are fp32 subtractions |n - q[i]|, equal distances go to the lower
-// index, and a NaN n takes the code of 0.  Eight comparisons down the tree give P, the number of entries among
-// q[0..254] below n (the branchless lower bound); the last entry found below n is q[P - 1] and the last found at or above
-// it q[P] (q[255] when P = 255), so the nearest is one of the two without reading the map again.
+// index, and a NaN n takes the code of 0.  n is first clamped into [q[0], q[255]] (lo and hi arrive as those two), so
+// an n above the map -- +inf from an overflowing 1 / absmax, or 1.0 under a checkpoint's map that tops out below 1 --
+// takes code 255 and one below it code 0, even where the two top (bottom) entries are equally far from n in fp32.
+// Eight comparisons down the tree give P, the number of entries among q[0..254] below n (the branchless lower bound);
+// the last entry found below n is q[P - 1] and the last found at or above it q[P] (q[255] when P = 255), so the nearest
+// is one of the two without reading the map again.
 __device__ __forceinline__ uint32_t q8_nearest(const float* tree, float lo, float hi, float n) {
   if (n != n) n = 0.f;
+  n = fminf(fmaxf(n, lo), hi);
   int node = 0;
 #pragma unroll
   for (int k = 0; k < 8; ++k) {

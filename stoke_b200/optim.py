@@ -800,7 +800,9 @@ class AdamW8bit(torch.optim.Optimizer):
     elements in memory order (a channels-last weight in its physical
     order), 256 elements per block, the last one possibly short.  Per block absmax = amax(|x|) and
     n = x * (absmax == 0 ? 0 : 1 / absmax); the code is the index of the map entry nearest to n (fp32 distances
-    |n - q|, equal distances to the lower index), and deq(code) = qmap[code] * absmax.  m takes the signed map
+    |n - q|, equal distances to the lower index), and deq(code) = qmap[code] * absmax.  n is clamped into
+    [qmap[0], qmap[255]] first, so an n beyond the map (+inf where 1 / absmax overflows, for a subnormal absmax at or
+    below 2 ** -128) takes the code of its nearer end.  m takes the signed map
     ``qmap1``, v the unsigned ``qmap2`` (``create_dynamic_map``).
 
     Non-finite values: a NaN in a block makes its absmax NaN, an inf (and no NaN) makes it inf.  A NaN n -- a NaN or inf

@@ -65,14 +65,17 @@ def _kinds():
                                                                "bias_correction": False}),
         "lars": (so.LARS, {"lr": 0.5, "weight_decay": 5e-4}, {"lr": 0.2, "weight_decay": 0.0, "always_adapt": True,
                                                               "momentum": 0.8, "nesterov": True}),
+        # the 64x64x3x3 conv weight and the 130x129 matrix reach min_8bit_size (4096): 8-bit codes; the rest fp32
+        "adamw8bit": (so.AdamW8bit, {"lr": 1e-3, "weight_decay": 0.01}, {"lr": 3e-3, "betas": (0.8, 0.95),
+                                                                        "weight_decay": 0.0}),
     }
 
 
 KINDS = ["adam", "adamw", "sgd_momentum", "sgd_nesterov", "nadam", "radam", "adamax", "adadelta", "rprop", "asgd", "lion",
-         "sf_adamw", "sf_sgd", "ademamix", "adafactor", "lamb", "lars"]
+         "sf_adamw", "sf_sgd", "ademamix", "adafactor", "lamb", "lars", "adamw8bit"]
 # fused launches of one opt.step() (the step epilogue included): the stock route launches other kernels
 LAUNCHES = dict({k: 2 for k in KINDS}, nadam=3, radam=3, adamax=3, adadelta=3, rprop=3, asgd=3, sf_adamw=3, sf_sgd=3,
-                ademamix=3, adafactor=9, lamb=4, lars=4)
+                ademamix=3, adafactor=9, lamb=4, lars=4, adamw8bit=3)
 
 # variant: (model dtype, route, grad_accum, loss scaler, clip)
 VARIANTS = {

@@ -25,7 +25,8 @@ f32 = np.float32
 
 # ---- the numpy transcription ---------------------------------------------------------------------------------------------
 def np_quant(x, q):
-    """codes, absmax of a 1-D fp32 array: the nearest map entry by a full scan (fp32 |n - q|, first minimum)."""
+    """codes, absmax of a 1-D fp32 array: n clamped into [q[0], q[255]], then the nearest map entry by a full scan (fp32
+    |n - q|, first minimum)."""
     n = x.size
     nb = -(-n // 256)
     absmax = np.zeros(nb, f32)
@@ -34,10 +35,11 @@ def np_quant(x, q):
         blk = x[256 * b: 256 * (b + 1)]
         a = f32(np.max(np.abs(blk))) if not np.isnan(blk).any() else f32(np.nan)
         absmax[b] = a
-        with np.errstate(divide="ignore", invalid="ignore"):
+        with np.errstate(divide="ignore", invalid="ignore", over="ignore"):
             inv = f32(0) if a == 0 else f32(f32(1) / a)
             y = (blk * inv).astype(f32)
         y[np.isnan(y)] = 0
+        y = np.clip(y, q[0], q[-1])
         d = np.abs((y[:, None] - q[None, :]).astype(f32))
         codes[256 * b: 256 * (b + 1)] = np.argmin(d, axis=1)
     return codes, absmax
@@ -202,6 +204,64 @@ def test_round_trip_bound(signed):
     half = torch.maximum(gaps, torch.cat([torch.zeros(1), gaps[:-1]]))[code.long()] / 2
     a = absmax.repeat_interleave(256)[: x.numel()]
     assert bool(((y - x).abs() <= a * half * (1 + 1e-5) + 1e-30).all())
+
+
+def _subnormal_blocks():
+    """The subnormal-absmax blocks of optim8bit_edges_ref, one per 256-element block (zero-padded): as m, and as the v of
+    the small gradients at beta2 = 0 and at the default beta2."""
+    import optim8bit_edges_ref as er
+
+    def pad(b):
+        return np.pad(b, (0, 256 - b.size))
+
+    m = np.concatenate([pad(er.subnormal_block(a)) for _, a in er.SUBNORMAL_ABSMAX])
+    g0, g1 = er.v_subnormal_grads(4e-20), er.v_subnormal_grads(1e-18)
+    v = np.concatenate([pad((g0 * g0).astype(f32)), pad(((g1 * g1).astype(f32) * f32(1 - 0.999)).astype(f32))])
+    return m, v
+
+
+def test_quantizer_edges_agree():
+    """The class's quantize_blockwise, np_quant above and optim8bit_edges_ref.nearest_code give the same code for every
+    crafted value: each default map's entries, its exact fp32 ties and their neighbours (in blocks of absmax 1, so n is
+    the value), and blocks whose absmax is subnormal, where 1 / absmax overflows and n is +-inf: a positive element
+    takes code 255, a negative one code 0, a zero the code of 0.  Under the default maps the clamp changes no code for a
+    finite n, and the tie-to-upper mutant differs from the rule on the tie elements (150 of qmap1's gaps hold an exact
+    fp32 tie, 92 of qmap2's one reachable as an fp32 square)."""
+    import optim8bit_edges_ref as er
+
+    q1, q2 = create_dynamic_map(True).numpy(), create_dynamic_map(False).numpy()
+    assert er.nearest_code([np.inf, -np.inf, np.nan], q1).tolist() == [255, 0, 127]
+    assert er.nearest_code([np.inf, -np.inf, np.nan], q2).tolist() == [255, 0, 0]
+    rng = np.random.default_rng(11)
+    x1 = er.blocks_with_unit_max(er.qmap1_values(q1), rng)
+    g2 = er.blocks_with_unit_max(er.signed_shuffle(er.qmap2_values(q2), rng), rng)
+    x2 = (g2 * g2).astype(f32)
+    sub_m, sub_v = _subnormal_blocks()
+    for q, x, sub, ties in ((q1, x1, sub_m, 150), (q2, x2, sub_v, 90)):
+        for blocks in (x, sub):
+            want, want_absmax = er.block_codes(blocks, q)
+            code, absmax = quantize_blockwise(torch.from_numpy(blocks), torch.from_numpy(q))
+            np_code, np_absmax = np_quant(blocks, q)
+            np.testing.assert_array_equal(code.numpy(), want)
+            np.testing.assert_array_equal(np_code, want)
+            np.testing.assert_array_equal(absmax.numpy(), want_absmax)
+            np.testing.assert_array_equal(np_absmax, want_absmax)
+        assert (np.abs(x.reshape(-1, 256)).max(1) == 1).all()   # absmax 1: n is the value itself
+        # the subnormal blocks: n = +-inf wherever 1 / absmax overflows
+        absmax = quantize_blockwise(torch.from_numpy(sub), torch.from_numpy(q))[1].numpy()
+        inf = np.repeat(er.overflows(absmax), 256)
+        assert inf.sum() >= 256 * (3 if q is q1 else 2)
+        code = quantize_blockwise(torch.from_numpy(sub), torch.from_numpy(q))[0].numpy()
+        zero = int(er.nearest_code([0.0], q)[0])
+        assert (code[inf & (sub > 0)] == 255).all() and (code[inf & (sub < 0)] == 0).all()
+        assert (code[inf & (sub == 0)] == zero).all() and (inf & (sub > 0)).any()
+        # the clamp changes nothing for a finite n under the default maps
+        lo = -1.0 if q is q1 else 0.0
+        y = np.concatenate([x, rng.uniform(lo, 1.0, 500_000).astype(f32),
+                            np.array([np.nextafter(f32(1), f32(2)), f32(1.5), f32(lo - 0.5)], f32)])
+        np.testing.assert_array_equal(er.nearest_code(y, q, clamp=False), er.nearest_code(y, q))
+        # the tie rule is exercised
+        assert int((er.nearest_code_upper(x, q) != er.nearest_code(x, q)).sum()) >= ties
 
 
 @pytest.mark.parametrize("kw, name", [(dict(amsgrad=True), "amsgrad"), (dict(percentile_clipping=5), "percentile_clipping"),
