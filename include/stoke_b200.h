@@ -43,6 +43,8 @@
  *                                    torch.optim has neither), plus the clip and the GradScaler.step gate
  *   stk_adam8bit_step                the step of AdamW8bit / Adam8bit of stoke_b200.optim (bitsandbytes' 8-bit AdamW:
  *                                    block-wise quantized moments), plus the clip and the GradScaler.step gate
+ *   stk_lion8bit_step / stk_ademamix8bit_step   the steps of Lion8bit / AdEMAMix8bit of stoke_b200.optim (bitsandbytes'
+ *                                    Lion8bit; AdEMAMix with 8-bit state), on the same quantized state and gate
  *   stk_weight_avg                   torch.optim.swa_utils.AveragedModel.update_parameters (EMA / SWA) over the fp32
  *                                    master weights; the reference has no weight averaging
  */
@@ -648,6 +650,32 @@ typedef struct {
   void* lp; int lp_dtype;      /* low-precision parameter copy written after the update (bf16 | f32), or NULL */
 } stk_adam8bit_args_t;
 int stk_adam8bit_step(stk_ctx* ctx, const stk_adam8bit_args_t* args, void* stream);
+
+/* ---- 8-bit Lion and 8-bit AdEMAMix on the same step (stoke_b200.optim.Lion8bit / AdEMAMix8bit) ------------------------
+ * stk_adam8bit_step's arguments, quantization, skip and found_inf rules, with the update of another optimizer.  `small`
+ * holds state k (k = 1, 2, 3) of a parameter below min_8bit_size at [(k - 1) n_small, k n_small).
+ *
+ * stk_lion8bit_step: one state, m = `code1` / `absmax1` on qmap1 (code2, absmax2 and qmap2 are not used and may be NULL);
+ * hyper[g] gives lr, beta1, beta2 and weight_decay (eps is not used).  Per element, every op one fp32 rounding:
+ *   weight_decay != 0: w = w fp32(1 - lr wd)
+ *   c = m b1 + g (1 - b1);  s = (c > 0) - (c < 0)            (NaN and +-0 give 0)
+ *   w = w - s fp32(lr)
+ *   m = m b2 + g (1 - b2);  m = quant(m)                      (m: the dequantized state before this step)
+ * The step count advances as in stk_adam8bit_step; the update does not use it.  workspace: 16 n_params bytes.
+ *
+ * stk_ademamix8bit_step: three states, m1 = code1 / absmax1 and m2 = code3 / absmax3 on qmap1, nu = code2 / absmax2 on
+ * qmap2 (absmax3: one per block, like absmax1).  hyper[g] gives lr, beta1, beta2, eps and weight_decay, ademamix[g]
+ * (host array, n_groups entries) alpha, beta3 and the warm-ups.  Per parameter, with t its step count after the
+ * increment, the scalars of stk_ademamix_step_prologue in double: 1 / bc1, 1 / sqrt(bc2), alpha_t and beta3_t, each
+ * rounded once to fp32.  Per element, every op one fp32 rounding:
+ *   m1 = m1 b1 + g (1 - b1);  m2 = m2 beta3_t + g (1 - beta3_t);  nu = nu b2 + (g g) (1 - b2)
+ *   den = sqrt(nu) fp32(1 / sqrt(bc2)) + fp32(eps)
+ *   u = (m1 fp32(1 / bc1) + m2 alpha_t) / den;  weight_decay != 0: u = u + w fp32(wd)
+ *   w = w - u fp32(lr);  m1, m2, nu = quant(m1), quant(m2), quant(nu)   (the update uses the unquantized state)
+ * workspace: 32 n_params bytes, 16-byte aligned. */
+int stk_lion8bit_step(stk_ctx* ctx, const stk_adam8bit_args_t* args, void* stream);
+int stk_ademamix8bit_step(stk_ctx* ctx, const stk_adam8bit_args_t* args, const stk_ademamix_hyper_t* ademamix,
+                          uint8_t* code3, float* absmax3, void* stream);
 
 /* ---- small collectives on the signal pads -------------------------------------------------------------------------- */
 /* mean over ranks of *loss_dev (float32/bf16/f16 scalar) -> *out_host (pinned, mapped) ; synchronises `stream` */

@@ -220,6 +220,8 @@ _SIGNATURES = {
     "stk_adafactor_step": (C.c_int, [_P, C.POINTER(AdafactorArgs), _P]),
     "stk_layerwise_step": (C.c_int, [_P, C.POINTER(LayerwiseArgs), _P]),
     "stk_adam8bit_step": (C.c_int, [_P, C.POINTER(Adam8bitArgs), _P]),
+    "stk_lion8bit_step": (C.c_int, [_P, C.POINTER(Adam8bitArgs), _P]),
+    "stk_ademamix8bit_step": (C.c_int, [_P, C.POINTER(Adam8bitArgs), C.POINTER(AdemamixHyper), _P, _P, _P]),
     "stk_weight_avg": (C.c_int, [_P, _P, _P, C.c_size_t, C.c_int, C.c_float, _P]),
     "stk_loss_sync": (C.c_int, [_P, _P, C.c_int, C.POINTER(C.c_double), _P]),
     "stk_loss_sync_begin": (C.c_int, [_P, _P, C.c_int, C.POINTER(C.c_int64), _P]),

@@ -13,7 +13,7 @@ PKG = os.path.dirname(HERE)
 LIB = os.path.join(PKG, "libstoke_b200.so")
 SOURCES = ["ctx.cu", "vmm.cu", "k1_reduce.cu", "k1_bulk.cu", "k1_nvls.cu", "k1_norm.cu", "k2_optim.cu", "k2_adafactor.cu",
            "k2_layerwise.cu", "k2_optim8bit.cu", "collectives.cu", "sampler.cu", "bn_act.cu", "weight_avg.cu"]
-HEADERS = ["common.cuh", "ctx.cuh", "k1_common.cuh", os.path.join("..", "..", "include", "stoke_b200.h")]
+HEADERS = ["common.cuh", "ctx.cuh", "k1_common.cuh", "ademamix.cuh",os.path.join("..", "..", "include", "stoke_b200.h")]
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = ARCH + [
     "-lineinfo", "-O3", "-std=c++17", "--use_fast_math", "-Xcompiler", "-fPIC", "-cudart", "static",

@@ -493,11 +493,12 @@ class GradPath:
       M3     fp32 fourth optimizer state (Adan's               local          indexed like M
              neg_pre_grad)
              (M, V, M2 and M3 exist as ``state`` lists them: buffer -> initial value)
-      Q8     the 8-bit AdamW's state (``adam8bit``):        local          all n (never sharded)
-             uint8 m / v codes over the flat layout, an
-             fp32 absmax per 256-element block, the two
-             maps, compact fp32 m / v of the parameters
-             below min_8bit_size; no M / V
+      Q8     the 8-bit optimizers' state (``adam8bit``):    local          all n (never sharded)
+             uint8 codes over the flat layout (AdamW:
+             m / v; Lion: m; AdEMAMix: m1 / nu / m2), an
+             fp32 absmax per 256-element block of each,
+             the maps, compact fp32 state of the
+             parameters below min_8bit_size; no M / V
       AVG    fp32 weight average (EMA / SWA)                   local          indexed like MASTER; only when averaging is
                                                                               configured (``enable_weight_average``)
 
@@ -513,7 +514,7 @@ class GradPath:
                  state: Optional[Dict[str, object]] = None, bucket_mb: Optional[float] = None,
                  state_id: Optional[int] = None, route: Optional[str] = None, group_of: Optional[Sequence[int]] = None,
                  overlap: bool = True, scalar_state: int = 0, adafactor: bool = False, layerwise: bool = False,
-                 schedule_free: bool = False, adam8bit: Optional[Sequence[bool]] = None):
+                 schedule_free: bool = False, adam8bit: Optional[Sequence[bool]] = None, q8_states: int = 2):
         self.engine = engine
         self.params = [p for p in params if p.requires_grad]
         if not self.params:
@@ -689,7 +690,7 @@ class GradPath:
             self._layerwise_setup()
         self.adam8bit = adam8bit is not None   # per parameter: 8-bit state (else fp32, below min_8bit_size)
         if self.adam8bit:
-            self._adam8bit_setup(adam8bit)
+            self._adam8bit_setup(adam8bit, q8_states)
         self.avg_flat = None   # AVG, allocated by enable_weight_average
         self.avg_owner = None  # the WeightAverage over this path: its applied() refuses a schedule-free swap
         self.avg_due = None    # (mode, weight) of the weight-average update the next step carries, set by Stoke.step
@@ -739,14 +740,17 @@ class GradPath:
         self._lw_ws = torch.empty(16 * len(self.params) + 8 * self.lw_tiles, dtype=torch.uint8, device=dev)
         self._range_steps = torch.zeros(len(self.params), dtype=torch.int32, device=dev)
 
-    def _adam8bit_setup(self, quantized: Sequence[bool]):
-        """State, descriptor tables and workspace of the fused 8-bit AdamW step, built once.  The state: two uint8 code
-        buffers over the flat layout (m, v), one fp32 absmax per 256-element block of each parameter for each of them,
-        the two maps, and one compact fp32 buffer for the parameters below min_8bit_size (their m, then their v, each
-        parameter at a 16-element aligned offset).  No fp32 moment buffers.  The blocks need whole parameters on one
-        rank, so there is no sharded route."""
+    def _adam8bit_setup(self, quantized: Sequence[bool], states: int = 2):
+        """State, descriptor tables and workspace of the fused 8-bit step, built once.  ``states``: the quantized states
+        per element, 2 for AdamW (m, v), 1 for Lion (m), 3 for AdEMAMix (m1, nu, m2).  The state: one uint8 code
+        buffer per state over the flat layout (``q8_code1``, ``q8_code2``, ``q8_code3``), one fp32 absmax per 256-element
+        block of each parameter for each of them, the maps (``q8_qmap1`` signed; ``q8_qmap2`` unsigned, not for Lion),
+        and one compact fp32 buffer for the parameters below min_8bit_size (state k of all of them after state k - 1's,
+        each parameter at a 16-element aligned offset).  AdEMAMix's m1 and m2 codes (and absmax) are the two halves of
+        one buffer, so that a parameter's ``state1`` is one (2, *shape) view.  No fp32 moment buffers.  The blocks need
+        whole parameters on one rank, so there is no sharded route."""
         if self.sharded:
-            raise ValueError("Stoke -- the fused 8-bit AdamW step needs whole parameters on one rank (no sharded route)")
+            raise ValueError("Stoke -- the fused 8-bit step needs whole parameters on one rank (no sharded route)")
         dev = self._range_end.device
         descs = (_lib.Adam8bitParam * len(self.params))()
         nblocks, self.q8_block0, self.q8_small_at = [], [], []
@@ -759,19 +763,25 @@ class GradPath:
             nblocks.append(nb)
             blocks += nb
             small += 0 if q else pad
+        self.q8_states = states
         self.q8_quantized = [bool(q) for q in quantized]
         self.q8_blocks, self.q8_n_small = max(blocks, 1), small
         self._q8_desc = torch.frombuffer(bytearray(C.string_at(descs, C.sizeof(descs))), dtype=torch.uint8).to(dev)
         self._q8_block_param = torch.repeat_interleave(torch.arange(len(self.params), dtype=torch.int32),
                                                        torch.tensor(nblocks, dtype=torch.int64)).to(dev)
-        self.q8_code1 = torch.zeros(max(self.n, ALIGN_ELEMS), dtype=torch.uint8, device=dev)
-        self.q8_code2 = torch.zeros_like(self.q8_code1)
-        self.q8_absmax1 = torch.zeros(self.q8_blocks, dtype=torch.float32, device=dev)
-        self.q8_absmax2 = torch.zeros_like(self.q8_absmax1)
-        self.q8_small = torch.zeros(max(2 * small, ALIGN_ELEMS), dtype=torch.float32, device=dev)
+        n = max(self.n, ALIGN_ELEMS)
+        pair = 2 if states == 3 else 1   # AdEMAMix: m1 and m2 in one buffer
+        self.q8_codes = torch.zeros(pair * n, dtype=torch.uint8, device=dev)
+        self.q8_absmaxes = torch.zeros(pair * self.q8_blocks, dtype=torch.float32, device=dev)
+        self.q8_code1, self.q8_absmax1 = self.q8_codes[:n], self.q8_absmaxes[:self.q8_blocks]
+        self.q8_code3 = self.q8_codes[n:] if states == 3 else None
+        self.q8_absmax3 = self.q8_absmaxes[self.q8_blocks:] if states == 3 else None
+        self.q8_code2 = torch.zeros_like(self.q8_code1) if states != 1 else None
+        self.q8_absmax2 = torch.zeros_like(self.q8_absmax1) if states != 1 else None
+        self.q8_small = torch.zeros(max(states * small, ALIGN_ELEMS), dtype=torch.float32, device=dev)
         self.q8_qmap1 = torch.empty(256, dtype=torch.float32, device=dev)
-        self.q8_qmap2 = torch.empty_like(self.q8_qmap1)
-        self._q8_ws = torch.empty(16 * len(self.params), dtype=torch.uint8, device=dev)
+        self.q8_qmap2 = torch.empty_like(self.q8_qmap1) if states != 1 else None
+        self._q8_ws = torch.empty((32 if states == 3 else 16) * len(self.params), dtype=torch.uint8, device=dev)
         self._range_steps = torch.zeros(len(self.params), dtype=torch.int32, device=dev)
         self.adam8bit_reset()
 
@@ -779,10 +789,12 @@ class GradPath:
         """The 8-bit state as before a first step: codes, absmax and fp32 state zero, the default maps."""
         from .optim import create_dynamic_map
 
-        for t in (self.q8_code1, self.q8_code2, self.q8_absmax1, self.q8_absmax2, self.q8_small):
-            t.zero_()
+        for t in (self.q8_codes, self.q8_code2, self.q8_absmaxes, self.q8_absmax2, self.q8_small):
+            if t is not None:
+                t.zero_()
         self.q8_qmap1.copy_(create_dynamic_map(True))
-        self.q8_qmap2.copy_(create_dynamic_map(False))
+        if self.q8_qmap2 is not None:
+            self.q8_qmap2.copy_(create_dynamic_map(False))
 
     # -- layout helpers -----------------------------------------------------------------------------------------------
     @staticmethod
@@ -1111,40 +1123,81 @@ class GradPath:
         e.launches += 3
         self._end_step()
 
-    def adam8bit_step(self, hypers: Sequence[_lib.Adam8bitHyper]):
-        """One fused 8-bit AdamW step (``stk_adam8bit_step``: per-parameter prologue, then one warp per 256-element
-        block), then the epilogue.  ``hypers``: one ``Adam8bitHyper`` per group.  Parameters without a gradient in this
-        window are skipped through the skip bits of the range table; their step counts and state do not move."""
+    def _q8_args(self, hypers: Sequence[_lib.Adam8bitHyper]):
+        """(engine, the ``Adam8bitArgs`` of an 8-bit step); the caller launches it and ends the step."""
         a = _lib.Adam8bitArgs()
         e, _ = self._begin_step(a, _lib.Adam8bitHyper, hypers)
         a.params, a.block_param = self._q8_desc.data_ptr(), self._q8_block_param.data_ptr()
         a.n_params, a.n_blocks = len(self.params), self._q8_block_param.numel()
-        a.code1, a.code2 = self.q8_code1.data_ptr(), self.q8_code2.data_ptr()
-        a.absmax1, a.absmax2 = self.q8_absmax1.data_ptr(), self.q8_absmax2.data_ptr()
-        a.qmap1, a.qmap2 = self.q8_qmap1.data_ptr(), self.q8_qmap2.data_ptr()
+        ptr = lambda t: t.data_ptr() if t is not None else None   # noqa: E731
+        a.code1, a.code2 = ptr(self.q8_code1), ptr(self.q8_code2)
+        a.absmax1, a.absmax2 = ptr(self.q8_absmax1), ptr(self.q8_absmax2)
+        a.qmap1, a.qmap2 = ptr(self.q8_qmap1), ptr(self.q8_qmap2)
         a.small, a.n_small = self.q8_small.data_ptr(), self.q8_n_small
         a.workspace = self._q8_ws.data_ptr()
         self._per_param_args(a)
+        return e, a
+
+    def adam8bit_step(self, hypers: Sequence[_lib.Adam8bitHyper]):
+        """One fused 8-bit AdamW step (``stk_adam8bit_step``: per-parameter prologue, then one warp per 256-element
+        block), then the epilogue.  ``hypers``: one ``Adam8bitHyper`` per group.  Parameters without a gradient in this
+        window are skipped through the skip bits of the range table; their step counts and state do not move."""
+        e, a = self._q8_args(hypers)
         e._check(e.lib.stk_adam8bit_step(e.ctx, C.byref(a), e._stream()))
         e.launches += 2
         self._end_step()
 
-    def adam8bit_state_views(self) -> List[Dict[str, torch.Tensor]]:
-        """Per parameter, its 8-bit state in AdamW8bit's keys: ``state1`` / ``state2`` (uint8 codes shaped and strided
-        like the parameter), ``qmap1`` / ``qmap2`` (the shared maps) and ``absmax1`` / ``absmax2``; or, below
-        min_8bit_size, fp32 ``state1`` / ``state2`` views of the compact buffer."""
+    def lion8bit_step(self, hypers: Sequence[_lib.Adam8bitHyper]):
+        """One fused 8-bit Lion step (``stk_lion8bit_step``), as ``adam8bit_step`` (eps is not used)."""
+        e, a = self._q8_args(hypers)
+        e._check(e.lib.stk_lion8bit_step(e.ctx, C.byref(a), e._stream()))
+        e.launches += 2
+        self._end_step()
+
+    def ademamix8bit_step(self, hypers: Sequence[_lib.Adam8bitHyper], ademamix: Sequence[_lib.AdemamixHyper]):
+        """One fused 8-bit AdEMAMix step (``stk_ademamix8bit_step``), as ``adam8bit_step``; ``ademamix``: one
+        ``AdemamixHyper`` per group (alpha, beta3, the warm-ups)."""
+        e, a = self._q8_args(hypers)
+        xarr = (_lib.AdemamixHyper * len(ademamix))(*ademamix)
+        e._check(e.lib.stk_ademamix8bit_step(e.ctx, C.byref(a), xarr, self.q8_code3.data_ptr(),
+                                             self.q8_absmax3.data_ptr(), e._stream()))
+        e.launches += 2
+        self._end_step()
+
+    def q8_state_views(self) -> List[Dict[str, torch.Tensor]]:
+        """Per parameter, its 8-bit state in the class's keys: ``state1`` (``state2``) as uint8 codes shaped and strided
+        like the parameter, ``qmap1`` (``qmap2``) the shared maps, ``absmax1`` (``absmax2``); or, below min_8bit_size,
+        fp32 ``state1`` (``state2``) views of the compact buffer.  AdEMAMix8bit's ``state1`` and ``absmax1`` stack m1 and
+        m2: (2, *p.shape) and (2, n_blocks) views."""
         out = []
+        three = self.q8_states == 3
         for i, (p, o) in enumerate(zip(self.params, self.offsets)):
             if self.q8_quantized[i]:
                 b0, b1 = self.q8_block0[i], self.q8_block0[i] + -(-p.numel() // _lib.Q8_BLOCK)
-                out.append(dict(state1=self._strided(self.q8_code1, p, o), qmap1=self.q8_qmap1,
-                                state2=self._strided(self.q8_code2, p, o), qmap2=self.q8_qmap2,
-                                absmax1=self.q8_absmax1[b0:b1], absmax2=self.q8_absmax2[b0:b1]))
+                if three:
+                    n = self.q8_code1.numel()
+                    d = dict(state1=torch.as_strided(self.q8_codes, (2, *p.shape), (n, *p.stride()), o),
+                             absmax1=torch.as_strided(self.q8_absmaxes, (2, b1 - b0), (self.q8_blocks, 1), b0))
+                else:
+                    d = dict(state1=self._strided(self.q8_code1, p, o), absmax1=self.q8_absmax1[b0:b1])
+                d["qmap1"] = self.q8_qmap1
+                if self.q8_states >= 2:
+                    d.update(state2=self._strided(self.q8_code2, p, o), qmap2=self.q8_qmap2,
+                             absmax2=self.q8_absmax2[b0:b1])
             else:
-                s = self.q8_small_at[i]
-                out.append(dict(state1=self._strided(self.q8_small, p, s),
-                                state2=self._strided(self.q8_small, p, self.q8_n_small + s)))
+                s, ns = self.q8_small_at[i], self.q8_n_small
+                if three:   # m1 at [0, ns), nu at [ns, 2 ns), m2 at [2 ns, 3 ns)
+                    d = dict(state1=torch.as_strided(self.q8_small, (2, *p.shape), (2 * ns, *p.stride()), s))
+                else:
+                    d = dict(state1=self._strided(self.q8_small, p, s))
+                if self.q8_states >= 2:
+                    d["state2"] = self._strided(self.q8_small, p, ns + s)
+            out.append(d)
         return out
+
+    def adam8bit_state_views(self) -> List[Dict[str, torch.Tensor]]:
+        """``q8_state_views`` (the name the 8-bit AdamW's callers use)."""
+        return self.q8_state_views()
 
     def adafactor_state_views(self) -> List[Tuple[torch.Tensor, ...]]:
         """Per parameter, views of the state buffer in torch's shapes: (row_var [..., R, 1], col_var [..., 1, C]) or
@@ -1282,6 +1335,7 @@ class GradPath:
         self._lw_ws = self._lw_desc = None
         if getattr(self, "adam8bit", False):
             self.q8_code1 = self.q8_code2 = self.q8_absmax1 = self.q8_absmax2 = self.q8_small = None
+            self.q8_codes = self.q8_absmaxes = self.q8_code3 = self.q8_absmax3 = None
             self._q8_ws = self._q8_desc = self._q8_block_param = None
         for b in self._bufs:
             try:

@@ -44,6 +44,8 @@ replicated all-reduce route at world > 1.
 ``AdamW8bit`` and ``Adam8bit`` (defined here, after bitsandbytes) take ``stk_adam8bit_step``: Adam's moments as 8-bit
 codes, block-wise quantized over 256 elements, with per-parameter step counts on the device, bitsandbytes' state keys
 and no fp32 moment buffers; replicated on the all-reduce route at world > 1 (the blocks do not follow shard boundaries).
+``Lion8bit`` and ``AdEMAMix8bit`` keep Lion's momentum and AdEMAMix's three moments the same way, on
+``stk_lion8bit_step`` and ``stk_ademamix8bit_step`` (one and three quantized states per element), with the same routes.
 Each fused kind's per-parameter state is one row of ``_STATE_LAYOUT``: torch's keys in order, the flat buffer that holds
 each tensor (M, V, M2 or Adafactor's own), its initial value, the groups it exists in, and what a never-stepped
 parameter exports.  The buffers ``GradPath`` allocates (``state_buffers``), ``state_dict`` (``export_state``) and
@@ -451,6 +453,22 @@ def ademamix_schedule(group, t: float) -> Tuple[float, float]:
     return alpha_t, beta3_t
 
 
+def _check_ademamix_args(lr, betas, alpha, beta3_warmup, alpha_warmup, eps, weight_decay):
+    if lr < 0.0:
+        raise ValueError(f"Invalid learning rate: {lr}")
+    if eps < 0.0:
+        raise ValueError(f"Invalid epsilon value: {eps}")
+    if len(betas) != 3 or not all(0.0 <= b < 1.0 for b in betas):
+        raise ValueError(f"Invalid beta parameters: {betas}")
+    if weight_decay < 0.0:
+        raise ValueError(f"Invalid weight_decay value: {weight_decay}")
+    if alpha < 0.0:
+        raise ValueError(f"Invalid alpha value: {alpha}")
+    for name, w in (("beta3_warmup", beta3_warmup), ("alpha_warmup", alpha_warmup)):
+        if w is not None and (isinstance(w, bool) or not isinstance(w, int) or w <= 0):
+            raise ValueError(f"Invalid {name}: {w} (None or a positive int)")
+
+
 class AdEMAMix(torch.optim.Optimizer):
     """AdEMAMix (Pagliardini, Ablin and Grangier, "The AdEMAMix Optimizer: Better, Faster, Older", 2024;
     apple/ml-ademamix's arguments, group keys and state keys): Adam with a second, slow EMA of the gradient mixed into
@@ -477,19 +495,7 @@ class AdEMAMix(torch.optim.Optimizer):
     def __init__(self, params, lr: float = 1e-3, betas=(0.9, 0.999, 0.9999), alpha: float = 2.0,
                  beta3_warmup: Optional[int] = None, alpha_warmup: Optional[int] = None, eps: float = 1e-8,
                  weight_decay: float = 0):
-        if lr < 0.0:
-            raise ValueError(f"Invalid learning rate: {lr}")
-        if eps < 0.0:
-            raise ValueError(f"Invalid epsilon value: {eps}")
-        if len(betas) != 3 or not all(0.0 <= b < 1.0 for b in betas):
-            raise ValueError(f"Invalid beta parameters: {betas}")
-        if weight_decay < 0.0:
-            raise ValueError(f"Invalid weight_decay value: {weight_decay}")
-        if alpha < 0.0:
-            raise ValueError(f"Invalid alpha value: {alpha}")
-        for name, w in (("beta3_warmup", beta3_warmup), ("alpha_warmup", alpha_warmup)):
-            if w is not None and (isinstance(w, bool) or not isinstance(w, int) or w <= 0):
-                raise ValueError(f"Invalid {name}: {w} (None or a positive int)")
+        _check_ademamix_args(lr, betas, alpha, beta3_warmup, alpha_warmup, eps, weight_decay)
         super().__init__(params, dict(lr=lr, betas=tuple(betas), alpha=alpha, beta3_warmup=beta3_warmup,
                                       alpha_warmup=alpha_warmup, eps=eps, weight_decay=weight_decay))
 
@@ -759,30 +765,34 @@ def dequantize_blockwise(code: torch.Tensor, qmap: torch.Tensor, absmax: torch.T
     return qmap[code.long()] * absmax.repeat_interleave(_lib.Q8_BLOCK)[: code.numel()]
 
 
-def check_8bit_entries(entries: List[Dict], quantized: List[bool]):
-    """Refuses, with ValueError, 8-bit optimizer state a step could not continue from: a ``state1`` / ``state2`` dtype
-    that does not match the parameter's ``min_8bit_size`` class (``quantized``: uint8, else fp32), maps that are not
+def check_8bit_entries(entries: List[Dict], quantized: List[bool], states: Tuple[str, ...] = ("state1", "state2"),
+                       maps: Tuple[str, ...] = ("qmap1", "qmap2"), name: str = "AdamW8bit"):
+    """Refuses, with ValueError, 8-bit optimizer state a step could not continue from: a dtype of one of ``states``
+    that does not match the parameter's ``min_8bit_size`` class (``quantized``: uint8, else fp32), ``maps`` that are not
     256 ascending entries, and maps that differ between parameters.  ``entries``: each parameter's state entry
-    (``{}`` where it has none).  Returns the checkpoint's ``(qmap1, qmap2)``, or None if it holds none."""
-    maps = None
+    (``{}`` where it has none); ``states`` / ``maps``: the class's keys (AdamW8bit's by default; Lion8bit has
+    ``state1`` and ``qmap1`` only); ``name``: the class named in the messages.  Returns the checkpoint's maps in the order
+    of ``maps``, or None if it holds none."""
+    found = None
     for i, (e, quant) in enumerate(zip(entries, quantized)):
-        for key in ("state1", "state2"):
+        for key in states:
             s = e.get(key)
             want = torch.uint8 if quant else torch.float32
             if s is not None and s.dtype != want:
-                raise ValueError(f"AdamW8bit: {key} of parameter {i} is {s.dtype}, expected {want} "
+                raise ValueError(f"{name}: {key} of parameter {i} is {s.dtype}, expected {want} "
                                  f"({'at or above' if quant else 'below'} min_8bit_size)")
-        if not quant or e.get("qmap1") is None or e.get("qmap2") is None:
+        if not quant or any(e.get(key) is None for key in maps):
             continue
-        qm = (e["qmap1"].detach().float().cpu(), e["qmap2"].detach().float().cpu())
-        for key, q in zip(("qmap1", "qmap2"), qm):
+        qm = tuple(e[key].detach().float().cpu() for key in maps)
+        for key, q in zip(maps, qm):
             if q.numel() != 256 or not bool((q[1:] > q[:-1]).all()):
-                raise ValueError(f"AdamW8bit: {key} must hold 256 ascending entries")
-        if maps is None:
-            maps = qm
-        elif not (torch.equal(maps[0], qm[0]) and torch.equal(maps[1], qm[1])):
-            raise ValueError("AdamW8bit: the quantization maps differ between parameters (the fused step keeps one pair)")
-    return maps
+                raise ValueError(f"{name}: {key} must hold 256 ascending entries")
+        if found is None:
+            found = qm
+        elif not all(torch.equal(a, b) for a, b in zip(found, qm)):
+            raise ValueError(f"{name}: the quantization maps differ between parameters (the fused step keeps one "
+                             f"{'pair' if len(maps) == 2 else 'map'})")
+    return found
 
 
 class AdamW8bit(torch.optim.Optimizer):
@@ -821,11 +831,9 @@ class AdamW8bit(torch.optim.Optimizer):
     def __init__(self, params, lr: float = 1e-3, betas=(0.9, 0.999), eps: float = 1e-8, weight_decay: float = 1e-2,
                  amsgrad: bool = False, optim_bits: int = 32, args=None, min_8bit_size: int = 4096,
                  percentile_clipping: int = 100, block_wise: bool = True, is_paged: bool = False):
-        for name, value, bad in (("amsgrad", amsgrad, amsgrad), ("args", args, args is not None),
-                                 ("percentile_clipping", percentile_clipping, percentile_clipping != 100),
-                                 ("block_wise", block_wise, not block_wise), ("is_paged", is_paged, is_paged)):
-            if bad:
-                raise ValueError(f"{type(self).__name__}: {name}={value!r} is not supported")
+        _refuse_8bit_options(type(self).__name__, amsgrad=(amsgrad, amsgrad), args=(args, args is not None),
+                             percentile_clipping=(percentile_clipping, percentile_clipping != 100),
+                             block_wise=(block_wise, not block_wise), is_paged=(is_paged, is_paged))
         if lr < 0.0:
             raise ValueError(f"Invalid learning rate: {lr}")
         if eps < 0.0:
@@ -923,10 +931,229 @@ class Adam8bit(AdamW8bit):
                          percentile_clipping=percentile_clipping, block_wise=block_wise, is_paged=is_paged)
 
 
-# AdamW8bit and Adam8bit run on their own entry point, stk_adam8bit_step (block-wise quantized state), not as a kind of K2
-_ADAM8BIT = "adam8bit"
+def _refuse_8bit_options(cls_name: str, **bad):
+    """ValueError for the first bitsandbytes option given as ``name=(value, refused)`` with ``refused`` true."""
+    for name, (value, refused) in bad.items():
+        if refused:
+            raise ValueError(f"{cls_name}: {name}={value!r} is not supported")
+
+
+def _q8_zeros(p: torch.Tensor, dtype: torch.dtype, lead: int = 0) -> torch.Tensor:
+    """Zero state for p: shaped and strided like p, or with ``lead`` > 0 shaped ``(lead, *p.shape)``, each ``[k]`` laid
+    out like p (so ``_memory_view`` of it walks p's memory order)."""
+    if not lead:
+        return torch.zeros_like(p, dtype=dtype, memory_format=torch.preserve_format)
+    flat = torch.zeros(lead * p.numel(), dtype=dtype, device=p.device)
+    return flat.as_strided((lead, *p.shape), (p.numel(), *p.stride()))
+
+
+class _Blockwise8bit(torch.optim.Optimizer):
+    """What Lion8bit and AdEMAMix8bit share: the maps cached per device, state creation from ``_STATES`` and loading.
+    ``_STATES``: per state key, (its map key, its absmax key, its leading dimension: 0 or the number of tensors it
+    stacks); ``_MAPS``: the map keys with their signedness, in order."""
+    _STATES: Tuple[Tuple[str, str, str, int], ...] = ()
+    _MAPS: Tuple[Tuple[str, bool], ...] = ()
+
+    def __init__(self, params, defaults):
+        super().__init__(params, defaults)
+        self._maps: Dict[torch.device, Dict[str, torch.Tensor]] = {}
+
+    def _init_state(self, p, state, quant: bool):
+        state["step"] = torch.tensor(0.0, dtype=torch.float32)
+        if not quant:
+            for key, _, _, lead in self._STATES:
+                state[key] = _q8_zeros(p, torch.float32, lead)
+            return
+        if p.device not in self._maps:
+            self._maps[p.device] = {k: create_dynamic_map(signed).to(p.device) for k, signed in self._MAPS}
+        nb = -(-p.numel() // _lib.Q8_BLOCK)
+        for key, qkey, _, lead in self._STATES:
+            state[key] = _q8_zeros(p, torch.uint8, lead)
+            state[qkey] = self._maps[p.device][qkey]
+        for _, _, akey, lead in self._STATES:
+            state[akey] = torch.zeros((lead, nb) if lead else (nb,), dtype=torch.float32, device=p.device)
+
+    def load_state_dict(self, state_dict):
+        ids = [i for g in state_dict["param_groups"] for i in g["params"]]
+        quantized = [p.numel() >= sg.get("min_8bit_size", g["min_8bit_size"])
+                     for sg, g in zip(state_dict["param_groups"], self.param_groups) for p in g["params"]]
+        params = [p for g in self.param_groups for p in g["params"]]
+        check_8bit_entries([state_dict["state"].get(i, {}) for i in ids], quantized,
+                           tuple(s[0] for s in self._STATES), tuple(m[0] for m in self._MAPS), type(self).__name__)
+        super().load_state_dict(state_dict)
+        for p in params:
+            st = self.state.get(p)
+            if not st:
+                continue
+            if "step" in st and not torch.is_tensor(st["step"]):   # upstream keeps step as a python int
+                st["step"] = torch.tensor(float(st["step"]), dtype=torch.float32)
+            # torch casts floating-point state to the parameter's dtype (the codes back to uint8 here), and a checkpoint
+            # may hold the tensors in any strides: each goes back to the layout _init_state gives it
+            for key, _, _, lead in self._STATES:
+                if key in st:
+                    src = st[key]
+                    st[key] = _q8_zeros(p, torch.uint8 if "qmap1" in st else torch.float32, lead)
+                    st[key].copy_(src.reshape(st[key].shape))
+
+    def _views(self, p, state):
+        """(quantized, per state key: its memory-order views, one per stacked tensor)"""
+        return "qmap1" in state, {key: [_memory_view(state[key][k]) for k in range(lead)] if lead else
+                                  [_memory_view(state[key])] for key, _, _, lead in self._STATES}
+
+    @staticmethod
+    def _deq(state, key, qkey, akey, lead, views):
+        absmax = state[akey]
+        return [dequantize_blockwise(v, state[qkey], absmax[k] if lead else absmax) for k, v in enumerate(views)]
+
+    def _store(self, state, key, qkey, akey, lead, views, xs):
+        absmax = state[akey]
+        for k, (v, x) in enumerate(zip(views, xs)):
+            code, a = quantize_blockwise(x, state[qkey])
+            v.copy_(code)
+            (absmax[k] if lead else absmax).copy_(a)
+
+    @torch.no_grad()
+    def step(self, closure=None):
+        loss = None
+        if closure is not None:
+            with torch.enable_grad():
+                loss = closure()
+        for group in self.param_groups:
+            for p in group["params"]:
+                if p.grad is None:
+                    continue
+                state = self.state[p]
+                if not state:
+                    self._init_state(p, state, p.numel() >= group["min_8bit_size"])
+                state["step"] += 1
+                g = p.grad if p.grad.stride() == p.stride() else torch.empty_like(p).copy_(p.grad)
+                g, w = _memory_view(g), _memory_view(p)
+                quant, views = self._views(p, state)
+                # the unquantized state of this step: dequantized copies, or the fp32 state itself (updated in place)
+                xs = {s[0]: self._deq(state, *s, views[s[0]]) if quant else views[s[0]] for s in self._STATES}
+                self._update(group, float(state["step"]), w, g, xs)
+                if quant:
+                    for s in self._STATES:
+                        self._store(state, *s, views[s[0]], xs[s[0]])
+        return loss
+
+    def _update(self, group, t: float, w, g, xs):
+        raise NotImplementedError
+
+
+class Lion8bit(_Blockwise8bit):
+    """Lion with 8-bit momentum (bitsandbytes' ``Lion8bit``: its arguments and state keys), about 1 B of optimizer state
+    per parameter instead of 4.  For one parameter w with gradient g, every op one fp32 rounding in this order::
+
+        if weight_decay != 0: w = w * (1 - lr * weight_decay)
+        c = deq(m) * beta1 + g * (1 - beta1);  s = (c > 0) - (c < 0)       (torch.sign: NaN and +-0 give 0)
+        w = w - s * lr
+        m = deq(m) * beta2 + g * (1 - beta2);  m = quant(m)
+
+    Quantization is ``AdamW8bit``'s (block-wise over 256 elements in memory order, its clamping, tie and NaN rules) on
+    the signed map ``qmap1``.  A parameter with fewer than ``min_8bit_size`` elements keeps an fp32 ``state1`` and takes
+    the same update without quantization.  State per parameter, created at its first step: ``step`` (0-dim fp32 tensor;
+    the update does not use it; ``load_state_dict`` also accepts a python int), ``state1`` (uint8 codes of exp_avg),
+    ``qmap1``, ``absmax1``.  ``args``, ``percentile_clipping != 100``, ``block_wise=False`` and ``is_paged`` raise
+    ValueError.  No parity with bitsandbytes is claimed.  This ``step()`` is plain per-parameter torch: what runs
+    outside the engine and on its stock route; inside ``Stoke`` the class runs on the fused sm_90a step
+    (``stk_lion8bit_step``)."""
+    _STATES = (("state1", "qmap1", "absmax1", 0),)
+    _MAPS = (("qmap1", True),)
+
+    def __init__(self, params, lr: float = 1e-4, betas=(0.9, 0.99), weight_decay: float = 0.0, args=None,
+                 min_8bit_size: int = 4096, percentile_clipping: int = 100, block_wise: bool = True,
+                 is_paged: bool = False):
+        _refuse_8bit_options(type(self).__name__, args=(args, args is not None),
+                             percentile_clipping=(percentile_clipping, percentile_clipping != 100),
+                             block_wise=(block_wise, not block_wise), is_paged=(is_paged, is_paged))
+        if lr < 0.0:
+            raise ValueError(f"Invalid learning rate: {lr}")
+        if not 0.0 <= betas[0] < 1.0 or not 0.0 <= betas[1] < 1.0:
+            raise ValueError(f"Invalid beta parameters: {betas}")
+        if weight_decay < 0.0:
+            raise ValueError(f"Invalid weight_decay value: {weight_decay}")
+        super().__init__(params, dict(lr=lr, betas=tuple(betas), weight_decay=weight_decay,
+                                      min_8bit_size=int(min_8bit_size)))
+
+    def _update(self, group, t, w, g, xs):
+        b1, b2 = group["betas"]
+        lr, wd = group["lr"], group["weight_decay"]
+        m = xs["state1"][0]
+        if wd != 0:
+            w.mul_(1 - lr * wd)
+        w.sub_(m.mul(b1).add_(g.mul(1 - b1)).sign_().mul_(lr))
+        m.mul_(b2).add_(g.mul(1 - b2))
+
+
+def ademamix8bit_scalars(group, t: float) -> Tuple[float, float, float, float]:
+    """AdEMAMix8bit's per-step scalars at step t (after the increment), in python doubles: ``(1 / bc1, 1 / sqrt(bc2),
+    alpha_t, beta3_t)``, the numbers ``AdEMAMix.step`` uses."""
+    b1, b2, _ = group["betas"]
+    alpha_t, beta3_t = ademamix_schedule(group, t)
+    return 1 / (1 - b1 ** t), 1 / math.sqrt(1 - b2 ** t), alpha_t, beta3_t
+
+
+class AdEMAMix8bit(_Blockwise8bit):
+    """AdEMAMix with 8-bit state: ``AdEMAMix``'s arguments and warm-ups, with its three moments stored as 8-bit codes,
+    about 3 B of optimizer state per parameter instead of 12.  For one parameter w with gradient g and its own step count
+    t (after the increment), the scalars ``ademamix8bit_scalars`` in python doubles, then every op one fp32 rounding in
+    this order::
+
+        m1 = deq(m1) * beta1 + g * (1 - beta1)
+        m2 = deq(m2) * beta3_t + g * (1 - beta3_t)
+        nu = deq(nu) * beta2 + (g * g) * (1 - beta2)
+        den = sqrt(nu) * (1 / sqrt(bc2)) + eps
+        u = (m1 * (1 / bc1) + m2 * alpha_t) / den
+        if weight_decay != 0: u = u + w * weight_decay
+        w = w - u * lr
+        m1, m2, nu = quant(m1), quant(m2), quant(nu)                     (the update uses the unquantized state)
+
+    sqrt is the correctly rounded fp32 square root on every device.  Quantization is ``AdamW8bit``'s (block-wise over
+    256 elements in memory order, its clamping, tie and NaN rules): m1 (fast) and m2 (slow) on the signed map ``qmap1``,
+    nu on the unsigned ``qmap2``.  A parameter with fewer than ``min_8bit_size`` elements keeps fp32 state and takes the
+    same update without quantization.  State per parameter, created at its first step: ``step`` (0-dim fp32 tensor;
+    ``load_state_dict`` also accepts a python int), ``state1`` (uint8, shaped ``(2, *p.shape)``: the codes of m1 then
+    m2), ``qmap1``, ``state2`` (the codes of nu), ``qmap2``, ``absmax1`` (shaped ``(2, n_blocks)``) and ``absmax2``; a
+    small parameter has fp32 ``state1`` ``(2, *p.shape)`` and ``state2``.  ``betas[0] == 0`` raises ValueError.  This
+    ``step()`` is plain per-parameter torch: what runs outside the engine and on its stock route; inside ``Stoke`` the
+    class runs on the fused sm_90a step (``stk_ademamix8bit_step``)."""
+    _STATES = (("state1", "qmap1", "absmax1", 2), ("state2", "qmap2", "absmax2", 0))
+    _MAPS = (("qmap1", True), ("qmap2", False))
+
+    def __init__(self, params, lr: float = 1e-3, betas=(0.9, 0.999, 0.9999), alpha: float = 2.0,
+                 beta3_warmup: Optional[int] = None, alpha_warmup: Optional[int] = None, eps: float = 1e-8,
+                 weight_decay: float = 0, min_8bit_size: int = 4096):
+        _check_ademamix_args(lr, betas, alpha, beta3_warmup, alpha_warmup, eps, weight_decay)
+        if betas[0] == 0:
+            raise ValueError(f"{type(self).__name__}: betas[0] = 0 is not supported")
+        super().__init__(params, dict(lr=lr, betas=tuple(betas), alpha=alpha, beta3_warmup=beta3_warmup,
+                                      alpha_warmup=alpha_warmup, eps=eps, weight_decay=weight_decay,
+                                      min_8bit_size=int(min_8bit_size)))
+
+    def _update(self, group, t, w, g, xs):
+        b1, b2, _ = group["betas"]
+        lr, eps, wd = group["lr"], group["eps"], group["weight_decay"]
+        c1, c2, alpha_t, beta3_t = ademamix8bit_scalars(group, t)
+        (m1, m2), (nu,) = xs["state1"], xs["state2"]
+        m1.mul_(b1).add_(g.mul(1 - b1))
+        m2.mul_(beta3_t).add_(g.mul(1 - beta3_t))
+        nu.mul_(b2).add_(g.mul(g).mul_(1 - b2))
+        den = _sqrt_rn(nu).mul_(c2).add_(eps)
+        u = m1.mul(c1).add_(m2.mul(alpha_t)).div_(den)
+        if wd != 0:
+            u.add_(w.mul(wd))
+        w.sub_(u.mul_(lr))
+
+
+# The 8-bit classes run on their own entry points (block-wise quantized state), not as kinds of K2: AdamW8bit and
+# Adam8bit on stk_adam8bit_step, Lion8bit on stk_lion8bit_step, AdEMAMix8bit on stk_ademamix8bit_step
+_ADAM8BIT, _LION8BIT, _ADEMAMIX8BIT = "adam8bit", "lion8bit", "ademamix8bit"
 _KINDS[AdamW8bit] = _ADAM8BIT
 _KINDS[Adam8bit] = _ADAM8BIT
+_KINDS[Lion8bit] = _LION8BIT
+_KINDS[AdEMAMix8bit] = _ADEMAMIX8BIT
+_Q8_KINDS = {_ADAM8BIT: 2, _LION8BIT: 1, _ADEMAMIX8BIT: 3}   # kind -> quantized states per element
 
 # LAMB and LARS run on their own entry point, stk_layerwise_step (per-parameter trust ratios), not as kinds of K2
 _LAMB, _LARS = "lamb", "lars"
@@ -995,8 +1222,12 @@ _STATE_LAYOUT: Dict[object, StateLayout] = {
     _ADAFACTOR: StateLayout(True, (), "omit", (StateTensor("row_var", "af"), StateTensor("col_var", "af"),
                                                StateTensor("variance", "af"))),
     # uint8 codes (fp32 for a parameter below min_8bit_size), the maps and the block absmax: views of GradPath's 8-bit
-    # state (adam8bit_state_views); no fp32 moment buffers
+    # state (q8_state_views); no fp32 moment buffers
     _ADAM8BIT: StateLayout(True, (), "omit", tuple(StateTensor(k, "q8") for k in (
+        "state1", "qmap1", "state2", "qmap2", "absmax1", "absmax2"))),
+    _LION8BIT: StateLayout(True, (), "omit", tuple(StateTensor(k, "q8") for k in ("state1", "qmap1", "absmax1"))),
+    # state1 / absmax1 stack m1 and m2: shaped (2, *p.shape) / (2, n_blocks)
+    _ADEMAMIX8BIT: StateLayout(True, (), "omit", tuple(StateTensor(k, "q8") for k in (
         "state1", "qmap1", "state2", "qmap2", "absmax1", "absmax2"))),
 }
 
@@ -1054,10 +1285,16 @@ def _adafactor_hyper(g) -> _lib.AdafactorHyper:
 
 
 def _adam8bit_hyper(g) -> _lib.Adam8bitHyper:
+    """The per-group struct of every 8-bit step: AdamW8bit's fields; Lion8bit has no eps (0), AdEMAMix8bit's third beta
+    goes in its AdemamixHyper."""
     h = _lib.Adam8bitHyper()
-    h.lr, h.eps, h.weight_decay = float(g["lr"]), float(g["eps"]), float(g["weight_decay"])
-    h.beta1, h.beta2 = (float(b) for b in g["betas"])
+    h.lr, h.eps, h.weight_decay = float(g["lr"]), float(g.get("eps", 0.0)), float(g["weight_decay"])
+    h.beta1, h.beta2 = (float(b) for b in g["betas"][:2])
     return h
+
+
+def _ademamix8bit_hyper(g) -> Tuple[_lib.Adam8bitHyper, _lib.AdemamixHyper]:
+    return _adam8bit_hyper(g), _ademamix_hyper(g)
 
 
 def _layerwise_hyper(g) -> _lib.LayerwiseHyper:
@@ -1075,7 +1312,8 @@ def _layerwise_hyper(g) -> _lib.LayerwiseHyper:
 
 # The per-group struct each fused kind's step takes, built from one param group.  The K2 kinds pass it beside their
 # OptimHyper array (GradPath.optimizer_step chooses the prologues and the entry point by kind); a K2 kind without a row
-# passes OptimHyper alone.  Adafactor, LAMB, LARS and the 8-bit AdamW pass it alone to their own entry points.
+# passes OptimHyper alone.  Adafactor, LAMB, LARS and the 8-bit kinds pass it alone to their own entry points
+# (AdEMAMix8bit: an (Adam8bitHyper, AdemamixHyper) pair).
 _GROUP_HYPER: Dict[object, Callable[[Dict], object]] = {
     **{k: _ext_hyper for k in _EXT_KINDS},
     _lib.OPT_SF_ADAMW: _sf_hyper, _lib.OPT_SF_SGD: _sf_hyper,
@@ -1084,7 +1322,8 @@ _GROUP_HYPER: Dict[object, Callable[[Dict], object]] = {
     _lib.OPT_ADAN: _adan_hyper,
     _ADAFACTOR: _adafactor_hyper,
     _LAMB: _layerwise_hyper, _LARS: _layerwise_hyper,
-    _ADAM8BIT: _adam8bit_hyper,
+    _ADAM8BIT: _adam8bit_hyper, _LION8BIT: _adam8bit_hyper,
+    _ADEMAMIX8BIT: _ademamix8bit_hyper,
 }
 
 
@@ -1262,7 +1501,7 @@ class B200FusedOptimizer(torch.optim.Optimizer):
                  bucket_mb: Optional[float] = None):
         if optim_cls not in _KINDS:
             raise NotImplementedError(
-                f"Stoke -- the fused step covers torch.optim.Adam, AdamW, SGD, NAdam, RAdam, Adamax, Adadelta, Rprop, ASGD and Adafactor and stoke_b200.optim.LAMB, LARS, Lion, AdamWScheduleFree, SGDScheduleFree, AdEMAMix, RMSpropTF, Adan, AdamW8bit and Adam8bit; got {getattr(optim_cls, '__name__', optim_cls)}"
+                f"Stoke -- the fused step covers torch.optim.Adam, AdamW, SGD, NAdam, RAdam, Adamax, Adadelta, Rprop, ASGD and Adafactor and stoke_b200.optim.LAMB, LARS, Lion, AdamWScheduleFree, SGDScheduleFree, AdEMAMix, RMSpropTF, Adan, AdamW8bit, Adam8bit, Lion8bit and AdEMAMix8bit; got {getattr(optim_cls, '__name__', optim_cls)}"
                 f" (use B200StockOptimizer / build_optimizer, which routes other classes to the stock-optimizer path)")
         params, group_of, extra, kw = _group_layout(module, optim_kwargs)
         if len(extra) > _lib.MAX_GROUPS:
@@ -1284,7 +1523,7 @@ class B200FusedOptimizer(torch.optim.Optimizer):
         ada = self._kind == _ADAFACTOR
         lw = self._kind in _LAYERWISE
         q8 = None
-        if self._kind == _ADAM8BIT:   # which parameters keep 8-bit state (the others: fp32, below min_8bit_size)
+        if self._kind in _Q8_KINDS:   # which parameters keep 8-bit state (the others: fp32, below min_8bit_size)
             q8 = [p.numel() >= probe.param_groups[gi]["min_8bit_size"] for p, gi in zip(params, group_of)]
         if (ada or lw or q8 is not None) and engine.world > 1:
             # Adafactor's per-parameter reductions and LAMB's / LARS's trust ratios need whole parameters on one rank, and
@@ -1294,7 +1533,8 @@ class B200FusedOptimizer(torch.optim.Optimizer):
         self.path = GradPath(engine, params, grad_accum=grad_accum, clip=clip, sharded=sharded, lp_dtype=lp_dtype,
                              module=module, state=self._buffers, state_id=state_id, route=route,
                              group_of=group_of, bucket_mb=bucket_mb, scalar_state=len(self._layout.scalars),
-                             adafactor=ada, layerwise=lw, schedule_free=self._kind in _SF_KINDS, adam8bit=q8)
+                             adafactor=ada, layerwise=lw, schedule_free=self._kind in _SF_KINDS, adam8bit=q8,
+                             q8_states=_Q8_KINDS.get(self._kind, 2))
         by_group: List[List[torch.nn.Parameter]] = [[] for _ in extra]
         for p, gi in zip(params, group_of):
             by_group[gi].append(p)
@@ -1337,6 +1577,10 @@ class B200FusedOptimizer(torch.optim.Optimizer):
             self.path.layerwise_step(_LAYERWISE[self._kind], per_group)
         elif self._kind == _ADAM8BIT:
             self.path.adam8bit_step(per_group)
+        elif self._kind == _LION8BIT:
+            self.path.lion8bit_step(per_group)
+        elif self._kind == _ADEMAMIX8BIT:
+            self.path.ademamix8bit_step(*zip(*per_group))
         else:
             self.path.optimizer_step([self._hyper_of(g) for g in self.param_groups], per_group)
 
@@ -1401,8 +1645,8 @@ class B200FusedOptimizer(torch.optim.Optimizer):
             per_param = [dict(zip(("row_var", "col_var") if len(vs) == 2 else ("variance",), vs))
                          for vs in self.path.adafactor_state_views()]
             return {t.key: [d.get(t.key) for d in per_param] for t in self._layout.tensors}
-        if self._kind == _ADAM8BIT:
-            per_param = self.path.adam8bit_state_views()
+        if self._kind in _Q8_KINDS:
+            per_param = self.path.q8_state_views()
             return {t.key: [d.get(t.key) for d in per_param] for t in self._layout.tensors}
         return {t.key: self.path.unflatten(full[t.buf]) for t in self._layout.tensors if t.buf in full}
 
@@ -1460,8 +1704,10 @@ class B200FusedOptimizer(torch.optim.Optimizer):
                 torch.full((path.n,), float(self._buffers[b]), dtype=torch.float32, device=dev) for b in self._flats()}
         if self._kind == _ADAFACTOR:
             path.af_state.zero_()
-        if self._kind == _ADAM8BIT:   # refuses what the step could not continue from, then starts from the initial state
-            check_8bit_entries(entries, path.q8_quantized)
+        if self._kind in _Q8_KINDS:   # refuses what the step could not continue from, then starts from the initial state
+            keys = [t.key for t in self._layout.tensors]
+            check_8bit_entries(entries, path.q8_quantized, tuple(k for k in keys if k.startswith("state")),
+                               tuple(k for k in keys if k.startswith("qmap")), self._torch_cls.__name__)
             path.adam8bit_reset()
         import_state(self._layout, entries, self._views(full))
         for b, local in self._flats().items():
