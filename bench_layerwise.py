@@ -1,5 +1,5 @@
 # -*- coding: utf-8 -*-
-"""stoke_b200.optim.LAMB and LARS on one GPU: the fused step (stk_layerwise_step, three launches, no host synchronisation)
+"""stoke_b200.optim.LAMB, LARS and StableAdamW on one GPU: the fused step (stk_layerwise_step, three launches, no host synchronisation)
 against B200StockOptimizer running the class's own step (K1 main-gradient reduce + per-parameter torch ops on fp32 views,
 two norm reductions per tensor, + the cast into the bf16 model), on the parameter sets of ResNet-50 (torchvision,
 channels-last, bf16; 25.6 M elements, 161 tensors) and BERT-base (BertForSequenceClassification(BertConfig()), bf16;
@@ -14,9 +14,11 @@ with weight decay, so every tensor takes the trust ratio.
 Medians over the timed iterations of every round, after a warm-up.  Algorithmic bytes per element on the raw bf16 route
 (k2_layerwise.cu): LAMB 42 (pass 1: g, w, m, v read, m, v written, g zeroed = 24; pass 3: w, m, v read, w and the bf16
 copy written = 18), LARS with momentum 28 (pass 1: g, w read = 6; pass 3: g, w, buf read, w, buf, bf16 copy written, g
-zeroed = 22).  The card's name and power limit are read in the same run.
+zeroed = 22), StableAdamW 38 (pass 1: g read and zeroed, m, v read and written = 20; pass 3: w, m, v read, w and the
+bf16 copy written = 18; asked for with --kinds lamb,stable_adamw).  The card's name and power limit are read in the same
+run.
 
-    python bench_layerwise.py [--out layerwise.json] [--iters 20] [--rounds 3] [--kinds lamb,lars]
+    python bench_layerwise.py [--out layerwise.json] [--iters 20] [--rounds 3] [--kinds lamb,lars,stable_adamw]
 """
 import argparse
 import json
@@ -53,21 +55,23 @@ def model_of(name):
     return BertForSequenceClassification(BertConfig())
 
 
-BYTES_PER_ELEMENT = {"lamb": 42, "lars": 28}
-KWARGS = {"lamb": {"lr": 1e-3, "weight_decay": 0.01}, "lars": {"lr": 1.0, "momentum": 0.9, "weight_decay": 5e-5}}
+BYTES_PER_ELEMENT = {"lamb": 42, "lars": 28, "stable_adamw": 38}
+KWARGS = {"lamb": {"lr": 1e-3, "weight_decay": 0.01}, "lars": {"lr": 1.0, "momentum": 0.9, "weight_decay": 5e-5},
+          "stable_adamw": {"lr": 1e-3, "weight_decay": 0.01}}
 
 
 def run(name, kind, iters, rounds):
     from stoke_b200 import synthetic
     from stoke_b200.engine import get_engine
-    from stoke_b200.optim import LAMB, LARS, B200FusedOptimizer, B200StockOptimizer
+    from stoke_b200.optim import LAMB, LARS, B200FusedOptimizer, B200StockOptimizer, StableAdamW
 
     eng = get_engine(0)
     opts = {}
     for route, cls in (("fused", B200FusedOptimizer), ("stock", B200StockOptimizer)):
         torch.manual_seed(0)
         net = model_of(name).cuda()
-        opts[route] = cls(net, LAMB if kind == "lamb" else LARS, KWARGS[kind], engine=eng, lp_dtype=torch.bfloat16)
+        opt_cls = {"lamb": LAMB, "lars": LARS, "stable_adamw": StableAdamW}[kind]
+        opts[route] = cls(net, opt_cls, KWARGS[kind], engine=eng, lp_dtype=torch.bfloat16)
     path = opts["fused"].path
     grads = [synthetic.injected_grad(gv.numel(), 0, i, dtype=torch.bfloat16, scale=1e-3).view(gv.shape).cuda()
              for i, gv in enumerate(path.grad_views)]

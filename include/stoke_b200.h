@@ -39,8 +39,8 @@
  *                                    without `.item()`
  *   stk_adafactor_plan / _step       torch.optim.Adafactor's step (torch/optim/_adafactor.py _single_tensor_adafactor) plus
  *                                    the clip and the GradScaler.step gate, without its two .item() per parameter
- *   stk_layerwise_step               the step of the LAMB / LARS classes of stoke_b200.optim (per-parameter trust ratios;
- *                                    torch.optim has neither), plus the clip and the GradScaler.step gate
+ *   stk_layerwise_step               the step of the LAMB / LARS / StableAdamW classes of stoke_b200.optim (per-parameter
+ *                                    trust ratios or RMS; torch.optim has none), plus the clip and the GradScaler.step gate
  *   stk_adam8bit_step                the step of AdamW8bit / Adam8bit of stoke_b200.optim (bitsandbytes' 8-bit AdamW:
  *                                    block-wise quantized moments), plus the clip and the GradScaler.step gate
  *   stk_lion8bit_step / stk_ademamix8bit_step   the steps of Lion8bit / AdEMAMix8bit of stoke_b200.optim (bitsandbytes'
@@ -552,15 +552,22 @@ int stk_adafactor_step(stk_ctx* ctx, const stk_adafactor_args_t* args, void* str
  *         adapt: g = (g + wd w) trust
  *         momentum != 0: buf = t == 1 ? g : buf momentum + (1 - dampening) g;  g = nesterov ? g + momentum buf : buf
  *         w -= lr g
+ *   StableAdamW (stoke_b200.optim.StableAdamW; Wortsman et al. 2023, Algorithm 2): AdamW with debiased betas and the
+ *         learning rate scaled down per parameter by its RMS; every op one fp32 rounding (the betas in double):
+ *         b1 = beta1 (1 - beta1^(t-1)) / (1 - beta1^t);  b2 = beta2 (1 - beta2^(t-1)) / (1 - beta2^t)   (0 at t = 1)
+ *         m = lerp(m, g, 1 - b1);  v = v b2 + (1 - b2) g^2
+ *         rms = sqrt(mean(g^2 / max(v, eps^2)));  lr_t = (1 / max(rms, 1)) lr    (max propagates NaN, as torch.clamp)
+ *         weight_decay != 0: w = w (1 - lr_t wd);  w = w - lr_t (m / (sqrt(v) + eps))
  * A NaN norm fails the comparisons (trust 1), as torch.where does.  Three stream-ordered launches: a tile pass (per-tile
- * partial sums of w^2 and r^2 or g^2; LAMB also updates m, v and zeroes the raw bucket), a per-parameter fold (trust
- * ratio, step count), the update (fp32 master, low-precision copy; LARS: momentum buffer and bucket zeroing).  LAMB's
+ * partial sums of w^2 and r^2 or g^2, or StableAdamW's g^2 / max(v, eps^2); LAMB and StableAdamW also update m, v and
+ * zero the raw bucket), a per-parameter fold (trust ratio or lr_t, step count), the update (fp32 master, low-precision
+ * copy; LARS: momentum buffer and bucket zeroing).  LAMB's
  * update recomputes r from the stored m, v and w with the same fp32 operations as the tile pass, so the r it applies is
  * the r whose norm it took.  Deterministic: every sum adds in an order fixed by the shapes, no floating-point atomics.
  * found_inf skips every parameter and a set bit 7 of its group byte skips one: master, state and count are left as they
  * are (the raw bucket is still zeroed).  Nothing is synchronised. */
 #define STK_LW_TILE 8192   /* elements per tile of the tile passes */
-typedef enum { STK_LW_LAMB = 0, STK_LW_LARS = 1 } stk_layerwise_kind;
+typedef enum { STK_LW_LAMB = 0, STK_LW_LARS = 1, STK_LW_STABLE_ADAMW = 2 } stk_layerwise_kind;
 
 typedef struct {          /* one per parameter */
   uint64_t offset;        /* first element in the flat master / gradient / state / lp buffers: a multiple of 16 */
@@ -570,7 +577,7 @@ typedef struct {          /* one per parameter */
 
 typedef struct {          /* one per parameter group */
   double lr;
-  double beta1, beta2;    /* LAMB */
+  double beta1, beta2;    /* LAMB, StableAdamW */
   double eps, weight_decay;
   double momentum, dampening, trust_coefficient;  /* LARS */
   int bias_correction;    /* LAMB */
@@ -588,8 +595,8 @@ typedef struct {
   const uint8_t* param_group;  /* DEVICE, one per parameter: group index, bit 7 = no gradient this step (not stepped) */
   int32_t* steps;              /* DEVICE, one per parameter: steps taken; advanced here unless skipped or found_inf */
   float* master;               /* fp32 masters (flat indexing) */
-  float* exp_avg;              /* LAMB: exp_avg; LARS: momentum_buffer (may be NULL when no group has momentum) */
-  float* exp_avg_sq;           /* LAMB: exp_avg_sq; LARS: not used */
+  float* exp_avg;              /* LAMB, StableAdamW: exp_avg; LARS: momentum_buffer (may be NULL when no group has momentum) */
+  float* exp_avg_sq;           /* LAMB, StableAdamW: exp_avg_sq; LARS: not used */
   void* workspace;             /* 16 n_params + 8 n_tiles bytes, 16-byte aligned, no initialisation */
   const void* grad; int grad_dtype; int grad_raw;  /* raw = 1: model-dtype bucket (bf16 | f32) scaled by grad_mul and
                                                       1/loss_scale, ZEROED after the step (also when skipped);

@@ -112,7 +112,7 @@ class AdafactorArgs(C.Structure):
 
 
 LW_TILE = 8192
-LW_LAMB, LW_LARS = 0, 1
+LW_LAMB, LW_LARS, LW_STABLE_ADAMW = 0, 1, 2
 
 
 class LayerwiseParam(C.Structure):

@@ -40,7 +40,8 @@ parameters on one rank, so at world > 1 (``fairscale_oss=True`` included) it run
 every rank taking the same deterministic step on the same gradients, as the stock route is replicated too.
 ``LAMB`` and ``LARS`` (defined here; torch.optim has neither) take ``stk_layerwise_step``: per-parameter trust ratios from
 two whole-parameter norms, per-parameter step counts on the device, the classes' own state_dict layout, and the same
-replicated all-reduce route at world > 1.
+replicated all-reduce route at world > 1.  ``StableAdamW`` (defined here) is a third kind of that step: its per-parameter
+reduction is the RMS that scales its learning rate.
 ``AdamW8bit`` and ``Adam8bit`` (defined here, after bitsandbytes) take ``stk_adam8bit_step``: Adam's moments as 8-bit
 codes, block-wise quantized over 256 elements, with per-parameter step counts on the device, bitsandbytes' state keys
 and no fp32 moment buffers; replicated on the all-reduce route at world > 1 (the blocks do not follow shard boundaries).
@@ -209,6 +210,72 @@ class LARS(torch.optim.Optimizer):
                         buf.mul_(mom).add_(g, alpha=1 - damp)
                     g = g.add(buf, alpha=mom) if group["nesterov"] else buf
                 p.add_(g, alpha=-lr)
+        return loss
+
+
+class StableAdamW(torch.optim.Optimizer):
+    """StableAdamW (Wortsman et al., "Stable and low-precision training for large-scale vision-language models", 2023,
+    Algorithm 2): AdamW with debiased betas in place of bias correction, whose learning rate is scaled down per parameter
+    by max(1, RMS), RMS = sqrt(mean(g^2 / v)), so that a rare large gradient meeting a decayed second moment cannot make
+    a loss spike.  For one parameter w with gradient g and its own step count t (after the increment), exactly as this
+    ``step()`` runs it (b1, b2 are python floats, both 0 at t = 1; every tensor op is one fp32 rounding)::
+
+        b1 = beta1 * (1 - beta1 ** (t - 1)) / (1 - beta1 ** t)
+        b2 = beta2 * (1 - beta2 ** (t - 1)) / (1 - beta2 ** t)
+        m.lerp_(g, 1 - b1)                                         # exp_avg
+        v.mul_(b2).addcmul_(g, g, value=1 - b2)                    # exp_avg_sq
+        rms = (g * g).div_(v.clamp(min=eps * eps)).mean().sqrt()   # 0-dim on the parameter's device: no .item()
+        lr_t = rms.clamp(min=1.0).reciprocal() * lr
+        if weight_decay != 0:
+            w.mul_(1 - lr_t * weight_decay)
+        w.sub_(lr_t * (m / (v.sqrt() + eps)))
+
+    A NaN anywhere in g gives a NaN RMS, which ``clamp`` keeps: the whole parameter becomes NaN.  State per parameter,
+    created at its first step: ``step`` (0-dim fp32 tensor), ``exp_avg``, ``exp_avg_sq``.  This ``step()`` is plain
+    per-parameter torch: what runs outside the engine and on its stock route; inside ``Stoke`` the class runs on the
+    fused sm_90a step (``stk_layerwise_step``, kind ``STK_LW_STABLE_ADAMW``).  The defaults are this package's own."""
+
+    def __init__(self, params, lr: float = 1e-3, betas=(0.9, 0.99), eps: float = 1e-6, weight_decay: float = 1e-2):
+        if lr < 0.0:
+            raise ValueError(f"Invalid learning rate: {lr}")
+        if eps < 0.0:
+            raise ValueError(f"Invalid epsilon value: {eps}")
+        if not 0.0 <= betas[0] < 1.0 or not 0.0 <= betas[1] < 1.0:
+            raise ValueError(f"Invalid beta parameters: {betas}")
+        if weight_decay < 0.0:
+            raise ValueError(f"Invalid weight_decay value: {weight_decay}")
+        super().__init__(params, dict(lr=lr, betas=tuple(betas), eps=eps, weight_decay=weight_decay))
+
+    @torch.no_grad()
+    def step(self, closure=None):
+        loss = None
+        if closure is not None:
+            with torch.enable_grad():
+                loss = closure()
+        for group in self.param_groups:
+            beta1, beta2 = group["betas"]
+            lr, eps, wd = group["lr"], group["eps"], group["weight_decay"]
+            for p in group["params"]:
+                if p.grad is None:
+                    continue
+                g = p.grad
+                state = self.state[p]
+                if not state:
+                    state["step"] = torch.tensor(0.0, dtype=torch.float32)
+                    state["exp_avg"] = torch.zeros_like(p, memory_format=torch.preserve_format)
+                    state["exp_avg_sq"] = torch.zeros_like(p, memory_format=torch.preserve_format)
+                state["step"] += 1
+                t = float(state["step"])
+                b1 = beta1 * (1 - beta1 ** (t - 1)) / (1 - beta1 ** t)
+                b2 = beta2 * (1 - beta2 ** (t - 1)) / (1 - beta2 ** t)
+                m, v = state["exp_avg"], state["exp_avg_sq"]
+                m.lerp_(g, 1 - b1)
+                v.mul_(b2).addcmul_(g, g, value=1 - b2)
+                rms = (g * g).div_(v.clamp(min=eps * eps)).mean().sqrt()
+                lr_t = rms.clamp(min=1.0).reciprocal() * lr
+                if wd != 0:
+                    p.mul_(1 - lr_t * wd)
+                p.sub_(lr_t * (m / (v.sqrt() + eps)))
         return loss
 
 
@@ -1155,11 +1222,13 @@ _KINDS[Lion8bit] = _LION8BIT
 _KINDS[AdEMAMix8bit] = _ADEMAMIX8BIT
 _Q8_KINDS = {_ADAM8BIT: 2, _LION8BIT: 1, _ADEMAMIX8BIT: 3}   # kind -> quantized states per element
 
-# LAMB and LARS run on their own entry point, stk_layerwise_step (per-parameter trust ratios), not as kinds of K2
-_LAMB, _LARS = "lamb", "lars"
+# LAMB, LARS and StableAdamW run on their own entry point, stk_layerwise_step (per-parameter trust ratios or RMS), not
+# as kinds of K2
+_LAMB, _LARS, _STABLE_ADAMW = "lamb", "lars", "stable_adamw"
 _KINDS[LAMB] = _LAMB
 _KINDS[LARS] = _LARS
-_LAYERWISE = {_LAMB: _lib.LW_LAMB, _LARS: _lib.LW_LARS}
+_KINDS[StableAdamW] = _STABLE_ADAMW
+_LAYERWISE = {_LAMB: _lib.LW_LAMB, _LARS: _lib.LW_LARS, _STABLE_ADAMW: _lib.LW_STABLE_ADAMW}
 
 
 class StateTensor(NamedTuple):
@@ -1218,6 +1287,7 @@ _STATE_LAYOUT: Dict[object, StateLayout] = {
         StateTensor("neg_pre_grad", "M3")), ("step", "exp_avg")),
     _LAMB: StateLayout(True, (), "omit", _ADAM_STATE),
     _LARS: StateLayout(True, (), "omit", (StateTensor("momentum_buffer", "M", where=_momentum),)),
+    _STABLE_ADAMW: StateLayout(True, (), "omit", _ADAM_STATE),
     # row_var / col_var of a factored parameter, variance of the others: views of GradPath.af_state
     _ADAFACTOR: StateLayout(True, (), "omit", (StateTensor("row_var", "af"), StateTensor("col_var", "af"),
                                                StateTensor("variance", "af"))),
@@ -1310,6 +1380,13 @@ def _layerwise_hyper(g) -> _lib.LayerwiseHyper:
     return h
 
 
+def _stable_adamw_hyper(g) -> _lib.LayerwiseHyper:
+    h = _lib.LayerwiseHyper()
+    h.lr, h.eps, h.weight_decay = float(g["lr"]), float(g["eps"]), float(g["weight_decay"])
+    h.beta1, h.beta2 = (float(b) for b in g["betas"])
+    return h
+
+
 # The per-group struct each fused kind's step takes, built from one param group.  The K2 kinds pass it beside their
 # OptimHyper array (GradPath.optimizer_step chooses the prologues and the entry point by kind); a K2 kind without a row
 # passes OptimHyper alone.  Adafactor, LAMB, LARS and the 8-bit kinds pass it alone to their own entry points
@@ -1321,7 +1398,7 @@ _GROUP_HYPER: Dict[object, Callable[[Dict], object]] = {
     _lib.OPT_RMSPROP_TF: _rmsprop_tf_hyper,
     _lib.OPT_ADAN: _adan_hyper,
     _ADAFACTOR: _adafactor_hyper,
-    _LAMB: _layerwise_hyper, _LARS: _layerwise_hyper,
+    _LAMB: _layerwise_hyper, _LARS: _layerwise_hyper, _STABLE_ADAMW: _stable_adamw_hyper,
     _ADAM8BIT: _adam8bit_hyper, _LION8BIT: _adam8bit_hyper,
     _ADEMAMIX8BIT: _ademamix8bit_hyper,
 }
@@ -1501,7 +1578,7 @@ class B200FusedOptimizer(torch.optim.Optimizer):
                  bucket_mb: Optional[float] = None):
         if optim_cls not in _KINDS:
             raise NotImplementedError(
-                f"Stoke -- the fused step covers torch.optim.Adam, AdamW, SGD, NAdam, RAdam, Adamax, Adadelta, Rprop, ASGD and Adafactor and stoke_b200.optim.LAMB, LARS, Lion, AdamWScheduleFree, SGDScheduleFree, AdEMAMix, RMSpropTF, Adan, AdamW8bit, Adam8bit, Lion8bit and AdEMAMix8bit; got {getattr(optim_cls, '__name__', optim_cls)}"
+                f"Stoke -- the fused step covers torch.optim.Adam, AdamW, SGD, NAdam, RAdam, Adamax, Adadelta, Rprop, ASGD and Adafactor and stoke_b200.optim.LAMB, LARS, StableAdamW, Lion, AdamWScheduleFree, SGDScheduleFree, AdEMAMix, RMSpropTF, Adan, AdamW8bit, Adam8bit, Lion8bit and AdEMAMix8bit; got {getattr(optim_cls, '__name__', optim_cls)}"
                 f" (use B200StockOptimizer / build_optimizer, which routes other classes to the stock-optimizer path)")
         params, group_of, extra, kw = _group_layout(module, optim_kwargs)
         if len(extra) > _lib.MAX_GROUPS:
