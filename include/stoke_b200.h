@@ -45,6 +45,9 @@
  *                                    block-wise quantized moments), plus the clip and the GradScaler.step gate
  *   stk_lion8bit_step / stk_ademamix8bit_step   the steps of Lion8bit / AdEMAMix8bit of stoke_b200.optim (bitsandbytes'
  *                                    Lion8bit; AdEMAMix with 8-bit state), on the same quantized state and gate
+ *   stk_muon_step                    torch.optim.Muon's step (torch/optim/_muon.py _single_tensor_muon) and the Muon half
+ *                                    of stoke_b200.optim.MuonWithAuxAdamW: Newton-Schulz on tensor cores, batched over
+ *                                    every matrix of the step, plus the clip and the GradScaler.step gate
  *   stk_weight_avg                   torch.optim.swa_utils.AveragedModel.update_parameters (EMA / SWA) over the fp32
  *                                    master weights; the reference has no weight averaging
  */
@@ -683,6 +686,64 @@ int stk_adam8bit_step(stk_ctx* ctx, const stk_adam8bit_args_t* args, void* strea
 int stk_lion8bit_step(stk_ctx* ctx, const stk_adam8bit_args_t* args, void* stream);
 int stk_ademamix8bit_step(stk_ctx* ctx, const stk_adam8bit_args_t* args, const stk_ademamix_hyper_t* ademamix,
                           uint8_t* code3, float* absmax3, void* stream);
+
+/* ---- Muon: momentum, batched Newton-Schulz, update (torch.optim.Muon, the Muon half of MuonWithAuxAdamW) ----------
+ * Per matrix with a gradient (g after unscale, accumulation and clip; R x C the parameter as a row-major matrix over its
+ * flat elements), torch's _single_tensor_muon:
+ *   buf = lerp(buf, g, fp32(1 - momentum));  u = nesterov ? lerp(g, buf, fp32(momentum)) : buf   (fp32, torch's lerp)
+ *   X = bf16(u), transposed when R > C (so X is r x c with r = min(R, C), c = max(R, C))
+ *   X = bf16(X / n), n = bf16(||X||_F) clamped below at bf16(eps)
+ *   ns_steps times:  A = bf16(X X^T);  B = bf16(b A + c A A);  X = bf16(a X + B X)     (fp32 accumulation)
+ *   w = w fp32(1 - lr wd);  w = w + fp32(-(lr ratio)) float(X^T or X)                      (lr wd, lr ratio: double)
+ * ratio is torch's _adjust_lr factor of the parameter's shape, formed on the host in double.  The GEMMs are mma.sync
+ * bf16 tensor-core tiles of 64 x 64, one launch per sub-step for every matrix of the step; A and B are symmetric, so only
+ * their lower tile triangle is computed and mirrored.  Launches: a tile pass (momentum, X, per-tile partial sums of X^2,
+ * zeroes the raw bucket), a per-matrix fold (n, step count), the normalisation, 3 max(ns_steps) GEMM launches, the
+ * update (fp32 master, low-precision copy).  Deterministic: every sum adds in an order fixed by the shapes, no
+ * floating-point atomics.  found_inf skips every matrix and a set bit 7 of its group byte skips one: master, buf and count
+ * are left as they are (the raw bucket is still zeroed).  Nothing is synchronised. */
+#define STK_MUON_TILE 8192   /* elements per tile of the element-wise passes */
+#define STK_MUON_MMA_TILE 64 /* rows and columns of a GEMM output tile */
+
+typedef struct {          /* one per matrix, in ascending parameter order */
+  uint64_t offset;        /* first element in the flat master / gradient / buf / lp buffers: a multiple of 16 */
+  uint64_t x_offset;      /* first element of its X in both X buffers: a multiple of 8 */
+  uint64_t a_offset;      /* first element of its A and B: a multiple of 8 */
+  int32_t rows, cols;     /* r <= c after the transpose */
+  int32_t transposed;     /* 1: the parameter is c x r (R > C) */
+  int32_t param;          /* its index in param_group / steps */
+  int32_t tile0;          /* first element-wise tile: the sum of ceil(r c / STK_MUON_TILE) over the matrices before it */
+  int32_t tri0;           /* first triangle tile: the sum of t (t + 1) / 2, t = ceil(r / 64), over the matrices before it */
+  int32_t full0;          /* first full tile: the sum of ceil(r / 64) ceil(c / 64) over the matrices before it */
+  int32_t pad_;
+  double lr_ratio;        /* torch's _adjust_lr factor */
+} stk_muon_param_t;
+
+typedef struct {          /* one per parameter group */
+  double lr, weight_decay, momentum, eps;
+  double ns_a, ns_b, ns_c;
+  int nesterov, ns_steps;  /* ns_steps: 0 .. 99 */
+} stk_muon_hyper_t;
+
+typedef struct {
+  const stk_muon_hyper_t* hyper; int n_groups;   /* host array, <= STK_MAX_GROUPS */
+  int clip_kind; double clip_max_norm, clip_value;
+  const stk_muon_param_t* params;  /* DEVICE table */
+  int n_params, n_tiles, n_tri, n_full;  /* matrices; the totals of the tile counts above */
+  const uint8_t* param_group;  /* DEVICE, one per parameter: group index, bit 7 = no gradient this step (not stepped) */
+  int32_t* steps;              /* DEVICE, one per parameter: steps taken; advanced here unless skipped or found_inf */
+  float* master;               /* fp32 masters (flat indexing) */
+  float* momentum_buffer;      /* fp32 (flat indexing) */
+  void* x0; void* x1;          /* bf16 X ping-pong buffers; after the step a matrix's X is in x0 (ns_steps even) or x1 */
+  void* a; void* b;            /* bf16 A and B */
+  void* workspace;             /* 16 n_params + 4 n_tiles bytes, 16-byte aligned, no initialisation */
+  const void* grad; int grad_dtype; int grad_raw;  /* raw = 1: model-dtype bucket (bf16 | f32) scaled by grad_mul and
+                                                      1/loss_scale, ZEROED over the matrices (also when skipped);
+                                                      raw = 0: fp32 reduced main gradients */
+  const float* acc; double grad_mul;  /* raw route: optional fp32 accumulator, multiplier */
+  void* lp; int lp_dtype;      /* low-precision parameter copy written after the update (bf16 | f32), or NULL */
+} stk_muon_args_t;
+int stk_muon_step(stk_ctx* ctx, const stk_muon_args_t* args, void* stream);
 
 /* ---- small collectives on the signal pads -------------------------------------------------------------------------- */
 /* mean over ranks of *loss_dev (float32/bf16/f16 scalar) -> *out_host (pinned, mapped) ; synchronises `stream` */

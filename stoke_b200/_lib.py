@@ -158,6 +158,29 @@ class Adam8bitArgs(C.Structure):
                 ("lp", C.c_void_p), ("lp_dtype", C.c_int)]
 
 
+class MuonParam(C.Structure):
+    _fields_ = [("offset", C.c_uint64), ("x_offset", C.c_uint64), ("a_offset", C.c_uint64), ("rows", C.c_int32),
+                ("cols", C.c_int32), ("transposed", C.c_int32), ("param", C.c_int32), ("tile0", C.c_int32),
+                ("tri0", C.c_int32), ("full0", C.c_int32), ("pad_", C.c_int32), ("lr_ratio", C.c_double)]
+
+
+class MuonHyper(C.Structure):
+    _fields_ = [("lr", C.c_double), ("weight_decay", C.c_double), ("momentum", C.c_double), ("eps", C.c_double),
+                ("ns_a", C.c_double), ("ns_b", C.c_double), ("ns_c", C.c_double), ("nesterov", C.c_int),
+                ("ns_steps", C.c_int)]
+
+
+class MuonArgs(C.Structure):
+    _fields_ = [("hyper", C.POINTER(MuonHyper)), ("n_groups", C.c_int), ("clip_kind", C.c_int),
+                ("clip_max_norm", C.c_double), ("clip_value", C.c_double), ("params", C.c_void_p),
+                ("n_params", C.c_int), ("n_tiles", C.c_int), ("n_tri", C.c_int), ("n_full", C.c_int),
+                ("param_group", C.c_void_p), ("steps", C.c_void_p), ("master", C.c_void_p),
+                ("momentum_buffer", C.c_void_p), ("x0", C.c_void_p), ("x1", C.c_void_p), ("a", C.c_void_p),
+                ("b", C.c_void_p), ("workspace", C.c_void_p), ("grad", C.c_void_p), ("grad_dtype", C.c_int),
+                ("grad_raw", C.c_int), ("acc", C.c_void_p), ("grad_mul", C.c_double), ("lp", C.c_void_p),
+                ("lp_dtype", C.c_int)]
+
+
 class SamplerPlan(C.Structure):
     _fields_ = [("n", C.c_int64), ("buckets", C.c_int64), ("batch_size", C.c_int64), ("world", C.c_int64),
                 ("rank", C.c_int64), ("drop_last", C.c_int32), ("allow_bucket_overlap", C.c_int32),
@@ -222,6 +245,7 @@ _SIGNATURES = {
     "stk_adam8bit_step": (C.c_int, [_P, C.POINTER(Adam8bitArgs), _P]),
     "stk_lion8bit_step": (C.c_int, [_P, C.POINTER(Adam8bitArgs), _P]),
     "stk_ademamix8bit_step": (C.c_int, [_P, C.POINTER(Adam8bitArgs), C.POINTER(AdemamixHyper), _P, _P, _P]),
+    "stk_muon_step": (C.c_int, [_P, C.POINTER(MuonArgs), _P]),
     "stk_weight_avg": (C.c_int, [_P, _P, _P, C.c_size_t, C.c_int, C.c_float, _P]),
     "stk_loss_sync": (C.c_int, [_P, _P, C.c_int, C.POINTER(C.c_double), _P]),
     "stk_loss_sync_begin": (C.c_int, [_P, _P, C.c_int, C.POINTER(C.c_int64), _P]),

@@ -12,7 +12,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 PKG = os.path.dirname(HERE)
 LIB = os.path.join(PKG, "libstoke_b200.so")
 SOURCES = ["ctx.cu", "vmm.cu", "k1_reduce.cu", "k1_bulk.cu", "k1_nvls.cu", "k1_norm.cu", "k2_optim.cu", "k2_adafactor.cu",
-           "k2_layerwise.cu", "k2_optim8bit.cu", "collectives.cu", "sampler.cu", "bn_act.cu", "weight_avg.cu"]
+           "k2_layerwise.cu", "k2_optim8bit.cu", "k2_muon.cu", "collectives.cu", "sampler.cu", "bn_act.cu", "weight_avg.cu"]
 HEADERS = ["common.cuh", "ctx.cuh", "k1_common.cuh", "ademamix.cuh",os.path.join("..", "..", "include", "stoke_b200.h")]
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = ARCH + [

@@ -499,6 +499,8 @@ class GradPath:
              fp32 absmax per 256-element block of each,
              the maps, compact fp32 state of the
              parameters below min_8bit_size; no M / V
+      MUON   the Muon step's bf16 workspace (``muon``):        local          two X buffers (r x c per matrix, r <= c),
+             Newton-Schulz's X, A = X X^T and B                             A and B (r x r); the momentum buffer is in M
       AVG    fp32 weight average (EMA / SWA)                   local          indexed like MASTER; only when averaging is
                                                                               configured (``enable_weight_average``)
 
@@ -514,7 +516,8 @@ class GradPath:
                  state: Optional[Dict[str, object]] = None, bucket_mb: Optional[float] = None,
                  state_id: Optional[int] = None, route: Optional[str] = None, group_of: Optional[Sequence[int]] = None,
                  overlap: bool = True, scalar_state: int = 0, adafactor: bool = False, layerwise: bool = False,
-                 schedule_free: bool = False, adam8bit: Optional[Sequence[bool]] = None, q8_states: int = 2):
+                 schedule_free: bool = False, adam8bit: Optional[Sequence[bool]] = None, q8_states: int = 2,
+                 muon: Optional[Sequence[Optional[Tuple[int, int, float]]]] = None):
         self.engine = engine
         self.params = [p for p in params if p.requires_grad]
         if not self.params:
@@ -691,6 +694,9 @@ class GradPath:
         self.adam8bit = adam8bit is not None   # per parameter: 8-bit state (else fp32, below min_8bit_size)
         if self.adam8bit:
             self._adam8bit_setup(adam8bit, q8_states)
+        self.muon = muon is not None   # per parameter: (rows, cols, lr ratio) of its matrix, or None (AdamW groups)
+        if self.muon:
+            self._muon_setup(muon)
         self.avg_flat = None   # AVG, allocated by enable_weight_average
         self.avg_owner = None  # the WeightAverage over this path: its applied() refuses a schedule-free swap
         self.avg_due = None    # (mode, weight) of the weight-average update the next step carries, set by Stoke.step
@@ -784,6 +790,86 @@ class GradPath:
         self._q8_ws = torch.empty((32 if states == 3 else 16) * len(self.params), dtype=torch.uint8, device=dev)
         self._range_steps = torch.zeros(len(self.params), dtype=torch.int32, device=dev)
         self.adam8bit_reset()
+
+    def _muon_setup(self, mats: Sequence[Optional[Tuple[int, int, float]]]):
+        """Descriptor table, bf16 workspace and per-parameter step counts of the fused Muon step, built once.
+        ``mats``: per parameter the (rows, cols) of the matrix its flat elements form and torch's ``_adjust_lr`` factor
+        of that shape, or None for a parameter of an AdamW group, which the step hands to K2.  The table is
+        ``layout.muon_plan``'s.  The momentum buffer lives in M at the parameters' flat offsets.  Newton-Schulz needs
+        whole matrices on one rank, so there is no sharded route."""
+        if self.sharded:
+            raise ValueError("Stoke -- the fused Muon step needs whole matrices on one rank (no sharded route)")
+        dev = self._range_end.device
+        table, tot = layout.muon_plan([m[:2] if m is not None else None for m in mats], self.offsets)
+        if not table:
+            raise ValueError("Stoke -- the fused Muon step needs at least one Muon parameter")
+        self.mu_index = [t["param"] for t in table]
+        self.mu_descs = (_lib.MuonParam * len(table))()
+        for d, t in zip(self.mu_descs, table):
+            for k in ("offset", "x_offset", "a_offset", "rows", "cols", "param", "tile0", "tri0", "full0"):
+                setattr(d, k, t[k])
+            d.transposed = int(t["transposed"])
+        self.mu_shapes = [(t["rows"], t["cols"], t["transposed"]) for t in table]   # r <= c
+        self.mu_tiles, self.mu_tri, self.mu_full = tot["tiles"], tot["tri"], tot["full"]
+        xo, ao = tot["x_elems"], tot["a_elems"]
+        self._mu_desc = torch.empty(C.sizeof(self.mu_descs), dtype=torch.uint8, device=dev)
+        self._mu_ratios = None   # the lr ratios in the device table
+        self._mu_upload([float(mats[i][2]) for i in self.mu_index])
+        # zeroed once: the padding between matrices is never written, so two runs hold the same bytes
+        self.mu_x = torch.zeros(2, xo, dtype=torch.bfloat16, device=dev)
+        self._mu_ab = torch.zeros(2, max(ao, 8), dtype=torch.bfloat16, device=dev)
+        self._mu_ws = torch.empty(16 * len(self.mu_index) + 4 * self.mu_tiles, dtype=torch.uint8, device=dev)
+        # K2 steps the AdamW groups with every Muon parameter skipped: the group table with their bit 7 set
+        self._mu_k2_host = np.asarray(self.group_of, dtype=np.uint8)
+        self._mu_k2_host[self.mu_index] |= 0x80
+        self._mu_k2_group = torch.from_numpy(self._mu_k2_host).to(dev)
+        self.enable_per_param_steps([0] * len(self.params))
+
+    def _mu_upload(self, ratios: List[float]):
+        """The descriptor table to the device when its lr ratios changed (construction, or an edited adjust_lr_fn)."""
+        if ratios != self._mu_ratios:
+            for d, x in zip(self.mu_descs, ratios):
+                d.lr_ratio = x
+            self._mu_desc.copy_(torch.frombuffer(bytearray(C.string_at(self.mu_descs, C.sizeof(self.mu_descs))),
+                                                 dtype=torch.uint8))
+            self._mu_ratios = ratios
+
+    def muon_step(self, hypers: Sequence[_lib.MuonHyper], lr_ratios: Sequence[float],
+                  adamw: Optional[Sequence[_lib.OptimHyper]] = None):
+        """One fused Muon step (``stk_muon_step``), then -- for MuonWithAuxAdamW -- K2's AdamW over the other
+        parameters, then the epilogue.  ``hypers``: one ``MuonHyper`` per group; ``lr_ratios``: torch's ``_adjust_lr``
+        factor of every Muon matrix; ``adamw``: one AdamW ``OptimHyper`` per group, or None when every parameter is a
+        Muon parameter.  The Muon launches read the raw bucket before K2 zeroes it.  Parameters without a gradient in
+        this window are skipped through the skip bits of the range table; their step counts and state do not move."""
+        self._mu_upload([float(x) for x in lr_ratios])
+        a = _lib.MuonArgs()
+        e, _ = self._begin_step(a, _lib.MuonHyper, hypers)
+        a.params, a.n_params = self._mu_desc.data_ptr(), len(self.mu_index)
+        a.n_tiles, a.n_tri, a.n_full = self.mu_tiles, self.mu_tri, self.mu_full
+        a.momentum_buffer = self.M.ptr
+        a.x0, a.x1 = self.mu_x[0].data_ptr(), self.mu_x[1].data_ptr()
+        a.a, a.b = self._mu_ab[0].data_ptr(), self._mu_ab[1].data_ptr()
+        a.workspace = self._mu_ws.data_ptr()
+        self._per_param_args(a)
+        e._check(e.lib.stk_muon_step(e.ctx, C.byref(a), e._stream()))
+        e.launches += 4 + 3 * max(h.ns_steps for h in hypers)
+        if adamw is None:
+            self._end_step()
+            return
+        skip = self._track_touched and not bool(self._touched.all())
+        tab = np.asarray(self.group_of, dtype=np.uint8) | np.where(self._touched | (not skip), 0, 0x80).astype(np.uint8)
+        tab[self.mu_index] |= 0x80
+        if not np.array_equal(tab, self._mu_k2_host):   # the skip bits changed: pageable copy, staged before returning
+            self._mu_k2_group.copy_(torch.from_numpy(tab))
+            self._mu_k2_host = tab
+        self.optimizer_step(list(adamw), range_group=self._mu_k2_group.data_ptr())
+
+    def muon_x_views(self, ns_steps: Sequence[int]) -> List[torch.Tensor]:
+        """Per Muon matrix, in parameter order, its bf16 X after the last step's Newton-Schulz iterations: (r, c) with
+        r <= c, the parameter's matrix transposed when it has more rows than columns.  ``ns_steps``: every group's
+        count, whose parity chooses the buffer that holds a matrix's last X."""
+        return [self.mu_x[ns_steps[self.group_of[d.param]] & 1, d.x_offset: d.x_offset + r * c].view(r, c)
+                for d, (r, c, _) in zip(self.mu_descs, self.mu_shapes)]
 
     def adam8bit_reset(self):
         """The 8-bit state as before a first step: codes, absmax and fp32 state zero, the default maps."""
@@ -1011,7 +1097,7 @@ class GradPath:
         self._raw_has_acc = False
         e.comm_poll()  # a peer that went missing during this step surfaces here (no synchronisation)
 
-    def optimizer_step(self, hypers, ext=None):
+    def optimizer_step(self, hypers, ext=None, range_group: Optional[int] = None):
         """One fused K2 launch, its prologues and the one-thread epilogue.  ``hypers``: one ``OptimHyper`` or a list
         (one per group), all of one kind.  ``ext``: the kind's per-group struct beside them (one per group), or None.
         The kind chooses the launches::
@@ -1030,7 +1116,8 @@ class GradPath:
         kinds forms its own scalars.  The range-table prologues (stk_optim_step_prologue, or AdEMAMix's / Adan's own)
         form the per-step scalars and NAdam's / ASGD's scalar state on the device; stk_sf_step_prologue forms the
         schedule-free group scalars and advances lr_max / weight_sum.  M2 is the step's third state tensor (AdEMAMix's
-        exp_avg_slow, RMSpropTF's grad_avg, Adan's exp_avg_diff) and M3 Adan's neg_pre_grad."""
+        exp_avg_slow, RMSpropTF's grad_avg, Adan's exp_avg_diff) and M3 Adan's neg_pre_grad.  ``range_group``: a device
+        group table to use in place of the path's own (``muon_step``'s, which skips the Muon parameters)."""
         if isinstance(hypers, _lib.OptimHyper):
             hypers = [hypers]
         kind = hypers[0].kind
@@ -1059,6 +1146,8 @@ class GradPath:
         else:
             a.lp_ptrs, a.lp_world, a.lp_dtype = None, 0, _lib.F32
         nr, rend, rgrp = self._ranges_for_step()
+        if range_group is not None:
+            nr, rend, rgrp = len(self.params), self._range_end.data_ptr(), range_group
         a.n_ranges, a.range_end_vec, a.range_group = nr, rend, rgrp
         per_range = bool(nr) and self._range_steps is not None
         # AdEMAMix and Adan have range-table prologues of their own, which form their scalars
@@ -1333,6 +1422,8 @@ class GradPath:
         self.avg_flat = None
         self.af_state = self._af_ws = self._af_desc = None
         self._lw_ws = self._lw_desc = None
+        if getattr(self, "muon", False):
+            self.mu_x = self._mu_ab = self._mu_ws = self._mu_desc = self._mu_k2_group = None
         if getattr(self, "adam8bit", False):
             self.q8_code1 = self.q8_code2 = self.q8_absmax1 = self.q8_absmax2 = self.q8_small = None
             self.q8_codes = self.q8_absmaxes = self.q8_code3 = self.q8_absmax3 = None

@@ -6,7 +6,7 @@ shard of each bucket, concatenated by ascending element offset = the layout of t
 
 Kept separate from ``engine.GradPath`` so that the partition logic -- which must be identical on every rank, or the block
 barriers of the cross-rank kernels pair the wrong blocks -- is unit-tested on CPU (tests/test_layout.py)."""
-from typing import Callable, List, Sequence, Tuple
+from typing import Callable, List, Optional, Sequence, Tuple
 
 ALIGN_ELEMS = 16   # every parameter starts on a 16-element boundary (32 B of bf16 / 64 B of fp32)
 MAX_SEGMENTS = 64  # STK_MAX_SEGMENTS of the C ABI
@@ -96,3 +96,33 @@ def adafactor_layout(shape: Sequence[int], stride: Sequence[int]) -> dict:
     B, R, C = size4[0] * size4[1], size4[2], size4[3]
     return {"factored": factored, "size": size4, "stride": stride4, "numel": numel, "B": B, "R": R, "C": C,
             "state": B * R + B * C if factored else numel}
+
+
+MUON_TILE = 8192      # STK_MUON_TILE: elements per block of the Muon step's element-wise passes
+MUON_MMA_TILE = 64    # STK_MUON_MMA_TILE: rows and columns of one of its GEMM output tiles
+
+
+def muon_plan(mats: Sequence[Optional[Tuple[int, int]]], offsets: Sequence[int]) -> Tuple[List[dict], dict]:
+    """The descriptor table of the fused Muon step (``stk_muon_param_t``) and its totals.  ``mats``: per parameter the
+    (rows, cols) of its matrix, or None (not a Muon parameter).  Per matrix, in parameter order: ``param``, ``offset``,
+    ``rows`` r <= ``cols`` c after the transpose, ``transposed`` (more rows than columns), its X at ``x_offset`` in
+    both X buffers and its A / B at ``a_offset`` (each a multiple of 8 elements), and the first index of its
+    element-wise tiles (``tile0``: ceil(r c / MUON_TILE) of them), of its lower-triangle GEMM tiles (``tri0``: t (t + 1)
+    / 2, t = ceil(r / MUON_MMA_TILE)) and of its full GEMM tiles (``full0``: t ceil(c / MUON_MMA_TILE)).  Totals:
+    ``tiles``, ``tri``, ``full``, ``x_elems``, ``a_elems``."""
+    table = []
+    tot = dict(tiles=0, tri=0, full=0, x_elems=0, a_elems=0)
+    for i, m in enumerate(mats):
+        if m is None:
+            continue
+        rows, cols = m
+        r, c = min(rows, cols), max(rows, cols)
+        t = -(-r // MUON_MMA_TILE)
+        table.append(dict(param=i, offset=offsets[i], rows=r, cols=c, transposed=rows > cols, x_offset=tot["x_elems"],
+                          a_offset=tot["a_elems"], tile0=tot["tiles"], tri0=tot["tri"], full0=tot["full"]))
+        tot["tiles"] += -(-(r * c) // MUON_TILE)
+        tot["tri"] += t * (t + 1) // 2
+        tot["full"] += t * -(-c // MUON_MMA_TILE)
+        tot["x_elems"] += -(-(r * c) // 8) * 8
+        tot["a_elems"] += -(-(r * r) // 8) * 8
+    return table, tot

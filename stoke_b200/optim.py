@@ -47,6 +47,10 @@ codes, block-wise quantized over 256 elements, with per-parameter step counts on
 and no fp32 moment buffers; replicated on the all-reduce route at world > 1 (the blocks do not follow shard boundaries).
 ``Lion8bit`` and ``AdEMAMix8bit`` keep Lion's momentum and AdEMAMix's three moments the same way, on
 ``stk_lion8bit_step`` and ``stk_ademamix8bit_step`` (one and three quantized states per element), with the same routes.
+``torch.optim.Muon`` and ``MuonWithAuxAdamW`` (defined here) take ``stk_muon_step``: momentum, Newton-Schulz batched
+over every matrix on bf16 tensor cores, the update; ``momentum_buffer`` in M, per-parameter step counts on the device
+only to know which parameters have state.  MuonWithAuxAdamW's AdamW groups then take K2's AdamW with the Muon parameters
+skipped through the range table.  Newton-Schulz needs whole matrices: replicated on the all-reduce route at world > 1.
 Each fused kind's per-parameter state is one row of ``_STATE_LAYOUT``: torch's keys in order, the flat buffer that holds
 each tensor (M, V, M2 or Adafactor's own), its initial value, the groups it exists in, and what a never-stepped
 parameter exports.  The buffers ``GradPath`` allocates (``state_buffers``), ``state_dict`` (``export_state``) and
@@ -1231,6 +1235,186 @@ _KINDS[StableAdamW] = _STABLE_ADAMW
 _LAYERWISE = {_LAMB: _lib.LW_LAMB, _LARS: _lib.LW_LARS, _STABLE_ADAMW: _lib.LW_STABLE_ADAMW}
 
 
+def muon_lr_ratio(adjust_lr_fn: Optional[str], rows: int, cols: int) -> float:
+    """torch.optim.Muon's ``_adjust_lr`` factor for a rows x cols matrix: the step is ``lr`` times it (double)."""
+    if adjust_lr_fn is None or adjust_lr_fn == "original":
+        return math.sqrt(max(1, rows / cols))
+    if adjust_lr_fn == "match_rms_adamw":
+        return 0.2 * math.sqrt(max(rows, cols))
+    return 1.0
+
+
+_MUON_DEFAULTS = dict(lr=1e-3, weight_decay=0.1, momentum=0.95, nesterov=True, ns_coefficients=(3.4445, -4.7750, 2.0315),
+                      eps=1e-7, ns_steps=5, adjust_lr_fn=None)   # torch.optim.Muon's
+_AUX_ADAMW_DEFAULTS = dict(lr=1e-3, betas=(0.9, 0.999), eps=1e-8, weight_decay=1e-2)   # torch.optim.AdamW's
+
+
+class MuonWithAuxAdamW(torch.optim.Optimizer):
+    """Muon for the matrices of a model and AdamW for everything else, in one optimizer, so that a whole model (biases,
+    norms, embeddings, conv weights) can train with Muon.  Every parameter group carries ``use_muon``:
+
+    * ``use_muon=True``: torch.optim.Muon's keys and defaults (``lr``, ``weight_decay``, ``momentum``, ``nesterov``,
+      ``ns_coefficients``, ``eps``, ``ns_steps``, ``adjust_lr_fn``) and state (``momentum_buffer``, no ``step``).
+      Parameters of 2 or more dims, each treated as the ``(shape[0], numel / shape[0])`` matrix (a conv weight
+      ``(out, in, kh, kw)`` as ``(out, in kh kw)``).  For one parameter w with gradient g, as R x C matrices, this is
+      torch.optim.Muon's ``_single_tensor_muon``::
+
+          buf.lerp_(g, 1 - momentum)
+          u = g.lerp(buf, momentum) if nesterov else buf
+          X = u.bfloat16();  X = X.T if R > C
+          X.div_(X.norm().clamp(min=eps))
+          ns_steps times:  A = X @ X.T;  B = torch.addmm(A, A, A, beta=b, alpha=c);  X = torch.addmm(X, B, X, beta=a)
+          X = X.T if R > C
+          w.mul_(1 - lr * weight_decay)
+          w.add_(X, alpha=-(lr * ratio))        # ratio: muon_lr_ratio(adjust_lr_fn, R, C), torch's _adjust_lr
+
+    * ``use_muon=False``: torch.optim.AdamW's keys and defaults (``lr``, ``betas``, ``eps``, ``weight_decay``) and state
+      (``step`` as a 0-dim fp32 tensor, ``exp_avg``, ``exp_avg_sq``), in torch's single-tensor op order, t the
+      parameter's step count after the increment::
+
+          w.mul_(1 - lr * weight_decay)         # when weight_decay != 0
+          m.lerp_(g, 1 - beta1)
+          v.mul_(beta2).addcmul_(g, g, value=1 - beta2)
+          w.addcdiv_(m, (v.sqrt() / (1 - beta2 ** t) ** 0.5).add_(eps), value=-(lr / (1 - beta1 ** t)))
+
+    State is created at a parameter's first step; a parameter without a gradient is not touched.  ``step()`` is plain
+    per-parameter torch with no ``.item()``: what runs outside the engine and on its stock route; inside ``Stoke`` the
+    Muon groups run on the fused sm_90a Muon step (``stk_muon_step``) and the AdamW groups on the fused AdamW step.  No
+    parity with any third-party package is claimed."""
+
+    def __init__(self, params):
+        super().__init__(params, {})
+
+    def add_param_group(self, param_group):
+        if "use_muon" not in param_group:
+            raise ValueError("MuonWithAuxAdamW -- every parameter group needs use_muon=True or False")
+        muon = bool(param_group["use_muon"])
+        for k, v in (_MUON_DEFAULTS if muon else _AUX_ADAMW_DEFAULTS).items():
+            param_group.setdefault(k, v)
+        g = param_group
+        if not 0.0 <= g["lr"]:
+            raise ValueError(f"Invalid learning rate: {g['lr']}")
+        if not 0.0 <= g["weight_decay"]:
+            raise ValueError(f"Invalid weight_decay value: {g['weight_decay']}")
+        if not 0.0 <= g["eps"]:
+            raise ValueError(f"Invalid epsilon value: {g['eps']}")
+        if muon:
+            if not 0.0 <= g["momentum"]:
+                raise ValueError(f"Invalid momentum value: {g['momentum']}")
+            if g["adjust_lr_fn"] not in (None, "original", "match_rms_adamw"):
+                raise ValueError(f"Adjust learning rate function {g['adjust_lr_fn']} is not supported")
+            if len(g["ns_coefficients"]) != 3:
+                raise ValueError("ns_coefficients must be a tuple of exactly 3 values")
+            if not 0 <= int(g["ns_steps"]) < 100:
+                raise ValueError(f"ns_steps must be in [0, 100), got {g['ns_steps']}")
+        elif not 0.0 <= g["betas"][0] < 1.0 or not 0.0 <= g["betas"][1] < 1.0:
+            raise ValueError(f"Invalid beta parameters: {g['betas']}")
+        super().add_param_group(param_group)
+        if muon:
+            for p in self.param_groups[-1]["params"]:
+                if p.ndim < 2:
+                    raise ValueError(f"MuonWithAuxAdamW -- a use_muon group holds a parameter of size {tuple(p.shape)}; "
+                                     "Muon takes parameters of 2 or more dims")
+
+    @staticmethod
+    def _muon(p, g, state, group):
+        if "momentum_buffer" not in state:
+            state["momentum_buffer"] = torch.zeros_like(g, memory_format=torch.preserve_format)
+        rows = p.shape[0]
+        # views of contiguous tensors; copies (written back below) of strided ones, e.g. a channels-last conv weight
+        w, g2, buf = (t.reshape(rows, -1) for t in (p, g, state["momentum_buffer"]))
+        a, b, c = group["ns_coefficients"]
+        momentum = group["momentum"]
+        buf.lerp_(g2, 1 - momentum)
+        update = g2.lerp(buf, momentum) if group["nesterov"] else buf
+        x = update.bfloat16()
+        tall = x.size(0) > x.size(1)
+        if tall:
+            x = x.T
+        x.div_(x.norm().clamp(min=group["eps"]))
+        for _ in range(group["ns_steps"]):
+            gram = x @ x.T
+            gram_update = torch.addmm(gram, gram, gram, beta=b, alpha=c)
+            x = torch.addmm(x, gram_update, x, beta=a)
+        if tall:
+            x = x.T
+        lr = group["lr"]
+        w.mul_(1 - lr * group["weight_decay"])
+        w.add_(x, alpha=-(lr * muon_lr_ratio(group["adjust_lr_fn"], rows, w.size(1))))
+        for dst, src in ((p, w), (state["momentum_buffer"], buf)):
+            if dst.data_ptr() != src.data_ptr() or not dst.is_contiguous():
+                dst.copy_(src.reshape(dst.shape))
+
+    @staticmethod
+    def _adamw(p, g, state, group):
+        if not state:
+            state["step"] = torch.tensor(0.0, dtype=torch.float32)
+            state["exp_avg"] = torch.zeros_like(p, memory_format=torch.preserve_format)
+            state["exp_avg_sq"] = torch.zeros_like(p, memory_format=torch.preserve_format)
+        state["step"] += 1
+        t = float(state["step"])
+        beta1, beta2 = group["betas"]
+        lr, wd = group["lr"], group["weight_decay"]
+        m, v = state["exp_avg"], state["exp_avg_sq"]
+        if wd != 0:
+            p.mul_(1 - lr * wd)
+        m.lerp_(g, 1 - beta1)
+        v.mul_(beta2).addcmul_(g, g, value=1 - beta2)
+        denom = (v.sqrt() / (1 - beta2 ** t) ** 0.5).add_(group["eps"])
+        p.addcdiv_(m, denom, value=-(lr / (1 - beta1 ** t)))
+
+    @torch.no_grad()
+    def step(self, closure=None):
+        loss = None
+        if closure is not None:
+            with torch.enable_grad():
+                loss = closure()
+        for group in self.param_groups:
+            update = self._muon if group["use_muon"] else self._adamw
+            for p in group["params"]:
+                if p.grad is not None:
+                    update(p, p.grad, self.state[p], group)
+        return loss
+
+
+# torch.optim.Muon (torch >= 2.9) and MuonWithAuxAdamW run on their own entry point, stk_muon_step (batched
+# Newton-Schulz on tensor cores), not as kinds of K2; MuonWithAuxAdamW's AdamW groups then take K2's AdamW
+_MUON = "muon"
+if hasattr(torch.optim, "Muon"):
+    _KINDS[torch.optim.Muon] = _MUON
+_KINDS[MuonWithAuxAdamW] = _MUON
+
+
+def _use_muon(g) -> bool:
+    """A group of torch.optim.Muon (no ``use_muon`` key) or a Muon group of MuonWithAuxAdamW."""
+    return bool(g.get("use_muon", True))
+
+
+def muon_matrices(params, group_of: List[int], groups: List[Dict]) -> List[Optional[Tuple[int, int, float]]]:
+    """Per parameter, the (rows, cols) of its Muon matrix and torch's ``_adjust_lr`` factor of that shape, or None in
+    an AdamW group."""
+    out = []
+    for p, gi in zip(params, group_of):
+        g = groups[gi]
+        if not _use_muon(g):
+            out.append(None)
+            continue
+        rows = p.shape[0]
+        cols = p.numel() // rows
+        out.append((rows, cols, muon_lr_ratio(g["adjust_lr_fn"], rows, cols)))
+    return out
+
+
+def _muon_flat_matrix(p: torch.Tensor) -> bool:
+    """The fused Muon step reads a parameter's flat elements as its (shape[0], numel / shape[0]) matrix: every row one
+    contiguous run of the flat layout, dim 0 outermost and the tensor dense (contiguous or channels-last).  The column
+    order within a row may differ from the logical one (channels-last); Newton-Schulz commutes with that permutation."""
+    if p.ndim < 2 or p.numel() == 0:
+        return False
+    dense = p.is_contiguous() or (p.ndim == 4 and p.is_contiguous(memory_format=torch.channels_last))
+    return dense and p.stride(0) == p.numel() // p.shape[0]
+
+
 class StateTensor(NamedTuple):
     """One per-parameter state tensor of a fused kind."""
     key: str                                         # torch's state key
@@ -1299,6 +1483,12 @@ _STATE_LAYOUT: Dict[object, StateLayout] = {
     # state1 / absmax1 stack m1 and m2: shaped (2, *p.shape) / (2, n_blocks)
     _ADEMAMIX8BIT: StateLayout(True, (), "omit", tuple(StateTensor(k, "q8") for k in (
         "state1", "qmap1", "state2", "qmap2", "absmax1", "absmax2"))),
+    # Muon groups: momentum_buffer (no step: state_dict drops it from their entries); MuonWithAuxAdamW's AdamW groups:
+    # step, exp_avg, exp_avg_sq.  M holds both kinds of first tensor, each at its parameters' offsets.
+    _MUON: StateLayout(True, (), "omit", (
+        StateTensor("momentum_buffer", "M", where=_use_muon),
+        StateTensor("exp_avg", "M", where=lambda g: not _use_muon(g)),
+        StateTensor("exp_avg_sq", "V", where=lambda g: not _use_muon(g)))),
 }
 
 
@@ -1367,6 +1557,21 @@ def _ademamix8bit_hyper(g) -> Tuple[_lib.Adam8bitHyper, _lib.AdemamixHyper]:
     return _adam8bit_hyper(g), _ademamix_hyper(g)
 
 
+def _muon_hyper(g) -> Tuple[_lib.MuonHyper, _lib.OptimHyper]:
+    """(the Muon step's struct, K2's AdamW struct) of one group; the one its ``use_muon`` does not select is left
+    neutral (the step skips its parameters)."""
+    m, h = _lib.MuonHyper(), _lib.OptimHyper()
+    h.kind, h.beta1, h.beta2 = _lib.OPT_ADAMW, 0.9, 0.999
+    if _use_muon(g):
+        m.lr, m.weight_decay, m.momentum, m.eps = float(g["lr"]), float(g["weight_decay"]), float(g["momentum"]), float(g["eps"])
+        m.ns_a, m.ns_b, m.ns_c = (float(x) for x in g["ns_coefficients"])
+        m.nesterov, m.ns_steps = int(bool(g["nesterov"])), int(g["ns_steps"])
+    else:
+        h.lr, h.eps, h.weight_decay = float(g["lr"]), float(g["eps"]), float(g["weight_decay"])
+        h.beta1, h.beta2 = (float(b) for b in g["betas"])
+    return m, h
+
+
 def _layerwise_hyper(g) -> _lib.LayerwiseHyper:
     h = _lib.LayerwiseHyper()
     h.lr, h.eps, h.weight_decay = float(g["lr"]), float(g["eps"]), float(g["weight_decay"])
@@ -1390,7 +1595,7 @@ def _stable_adamw_hyper(g) -> _lib.LayerwiseHyper:
 # The per-group struct each fused kind's step takes, built from one param group.  The K2 kinds pass it beside their
 # OptimHyper array (GradPath.optimizer_step chooses the prologues and the entry point by kind); a K2 kind without a row
 # passes OptimHyper alone.  Adafactor, LAMB, LARS and the 8-bit kinds pass it alone to their own entry points
-# (AdEMAMix8bit: an (Adam8bitHyper, AdemamixHyper) pair).
+# (AdEMAMix8bit: an (Adam8bitHyper, AdemamixHyper) pair; Muon: a (MuonHyper, OptimHyper) pair).
 _GROUP_HYPER: Dict[object, Callable[[Dict], object]] = {
     **{k: _ext_hyper for k in _EXT_KINDS},
     _lib.OPT_SF_ADAMW: _sf_hyper, _lib.OPT_SF_SGD: _sf_hyper,
@@ -1401,6 +1606,7 @@ _GROUP_HYPER: Dict[object, Callable[[Dict], object]] = {
     _LAMB: _layerwise_hyper, _LARS: _layerwise_hyper, _STABLE_ADAMW: _stable_adamw_hyper,
     _ADAM8BIT: _adam8bit_hyper, _LION8BIT: _adam8bit_hyper,
     _ADEMAMIX8BIT: _ademamix8bit_hyper,
+    _MUON: _muon_hyper,
 }
 
 
@@ -1500,7 +1706,8 @@ def load_step_counts(kind, entries: List[Dict], group_of: List[int], opt_steps: 
     torch creates a parameter's state at its first step, so a parameter without an entry has taken 0 steps and has the
     initial scalar state (1.0).  torch's SGD keeps no ``step``: a parameter with a ``momentum_buffer`` has taken
     ``opt_steps`` steps (1 in a torch-written checkpoint), one without it 0; in a group without momentum the count has no
-    effect and is the optimizer-wide one.
+    effect and is the optimizer-wide one.  Muon keeps no ``step`` either: its parameters follow SGD's rule (a Muon group
+    always has the buffer), MuonWithAuxAdamW's AdamW parameters carry ``step``.
 
     Returns ``(opt_steps, steps, scalars)``: the optimizer-wide count, then either per-parameter counts and per-parameter
     scalar state (``steps`` a list) or ``steps = None`` and per-group scalar state.  Counts go per parameter when they
@@ -1524,6 +1731,8 @@ def load_step_counts(kind, entries: List[Dict], group_of: List[int], opt_steps: 
         return opt_steps, None, None
 
     def count(e, g):
+        if kind == _MUON and "step" not in e:
+            return 0 if e.get("momentum_buffer") is None else 1 if opt_steps is None else opt_steps
         if kind != _lib.OPT_SGD:
             return int(float(e["step"])) if "step" in e else 0
         if momentum[g] == 0:
@@ -1562,6 +1771,10 @@ def fused_supported(optim_cls, optim_kwargs: Dict, module: torch.nn.Module) -> b
         merged = dict(kw, **g)
         if any(merged.get(k) for k in _STOCK_ONLY_TRUE):
             return False
+    if _KINDS[optim_cls] == _MUON:   # every Muon parameter's flat elements must form its matrix
+        params, group_of, _, _ = _group_layout(module, optim_kwargs)
+        if not all(_muon_flat_matrix(p) for p, gi in zip(params, group_of) if _use_muon(extra[gi])):
+            return False
     if _KINDS[optim_cls] == _ADAFACTOR:
         try:   # up to four dims, dense (channels-last included)
             for p in _module_params(module):
@@ -1578,13 +1791,15 @@ class B200FusedOptimizer(torch.optim.Optimizer):
                  bucket_mb: Optional[float] = None):
         if optim_cls not in _KINDS:
             raise NotImplementedError(
-                f"Stoke -- the fused step covers torch.optim.Adam, AdamW, SGD, NAdam, RAdam, Adamax, Adadelta, Rprop, ASGD and Adafactor and stoke_b200.optim.LAMB, LARS, StableAdamW, Lion, AdamWScheduleFree, SGDScheduleFree, AdEMAMix, RMSpropTF, Adan, AdamW8bit, Adam8bit, Lion8bit and AdEMAMix8bit; got {getattr(optim_cls, '__name__', optim_cls)}"
+                f"Stoke -- the fused step covers torch.optim.Adam, AdamW, SGD, NAdam, RAdam, Adamax, Adadelta, Rprop, ASGD and Adafactor and stoke_b200.optim.LAMB, LARS, StableAdamW, Lion, AdamWScheduleFree, SGDScheduleFree, AdEMAMix, RMSpropTF, Adan, AdamW8bit, Adam8bit, Lion8bit, AdEMAMix8bit, torch.optim.Muon and MuonWithAuxAdamW; got {getattr(optim_cls, '__name__', optim_cls)}"
                 f" (use B200StockOptimizer / build_optimizer, which routes other classes to the stock-optimizer path)")
         params, group_of, extra, kw = _group_layout(module, optim_kwargs)
         if len(extra) > _lib.MAX_GROUPS:
             raise NotImplementedError(f"Stoke -- the fused step handles up to {_lib.MAX_GROUPS} parameter groups")
-        # let torch validate the kwargs exactly as the reference would (optimizer(params=..., **kwargs))
-        probe = optim_cls([dict(g, params=[torch.nn.Parameter(torch.zeros(1))]) for g in extra], **kw)
+        # let torch validate the kwargs exactly as the reference would (optimizer(params=..., **kwargs)); Muon takes
+        # matrices only
+        shape = (1, 1) if _KINDS[optim_cls] == _MUON else (1,)
+        probe = optim_cls([dict(g, params=[torch.nn.Parameter(torch.zeros(shape))]) for g in extra], **kw)
         for g in probe.param_groups:
             for k in _STOCK_ONLY_TRUE:
                 if g.get(k):
@@ -1602,16 +1817,28 @@ class B200FusedOptimizer(torch.optim.Optimizer):
         q8 = None
         if self._kind in _Q8_KINDS:   # which parameters keep 8-bit state (the others: fp32, below min_8bit_size)
             q8 = [p.numel() >= probe.param_groups[gi]["min_8bit_size"] for p, gi in zip(params, group_of)]
-        if (ada or lw or q8 is not None) and engine.world > 1:
-            # Adafactor's per-parameter reductions and LAMB's / LARS's trust ratios need whole parameters on one rank, and
-            # the 8-bit state's 256-element blocks do not follow the shard boundaries: their state is replicated (also
-            # under fairscale_oss) and every rank runs the same deterministic step on the same all-reduced fp32 gradients
+        muon = None
+        if self._kind == _MUON:
+            # MuonWithAuxAdamW has no optimizer-wide defaults: each group takes Muon's or AdamW's, as the probe filled them
+            extra = [{k: v for k, v in g.items() if k != "params"} for g in probe.param_groups]
+            # the class's own checks on the real parameters (torch.optim.Muon: 2-D only; MuonWithAuxAdamW: 2 or more dims)
+            optim_cls([dict(g, params=[p for p, gi in zip(params, group_of) if gi == k]) for k, g in enumerate(extra)],
+                      **kw)
+            if not all(_muon_flat_matrix(p) for p, gi in zip(params, group_of) if _use_muon(probe.param_groups[gi])):
+                raise NotImplementedError("Stoke -- the fused Muon step needs every Muon parameter dense with dim 0 "
+                                          "outermost (contiguous or channels-last)")
+            muon = muon_matrices(params, group_of, probe.param_groups)
+        if (ada or lw or q8 is not None or muon is not None) and engine.world > 1:
+            # Adafactor's per-parameter reductions, LAMB's / LARS's trust ratios and Muon's Newton-Schulz need whole
+            # parameters on one rank, and the 8-bit state's 256-element blocks do not follow the shard boundaries: their
+            # state is replicated (also under fairscale_oss) and every rank runs the same deterministic step on the same
+            # all-reduced fp32 gradients
             route = "allreduce"
         self.path = GradPath(engine, params, grad_accum=grad_accum, clip=clip, sharded=sharded, lp_dtype=lp_dtype,
                              module=module, state=self._buffers, state_id=state_id, route=route,
                              group_of=group_of, bucket_mb=bucket_mb, scalar_state=len(self._layout.scalars),
                              adafactor=ada, layerwise=lw, schedule_free=self._kind in _SF_KINDS, adam8bit=q8,
-                             q8_states=_Q8_KINDS.get(self._kind, 2))
+                             q8_states=_Q8_KINDS.get(self._kind, 2), muon=muon)
         by_group: List[List[torch.nn.Parameter]] = [[] for _ in extra]
         for p, gi in zip(params, group_of):
             by_group[gi].append(p)
@@ -1658,6 +1885,11 @@ class B200FusedOptimizer(torch.optim.Optimizer):
             self.path.lion8bit_step(per_group)
         elif self._kind == _ADEMAMIX8BIT:
             self.path.ademamix8bit_step(*zip(*per_group))
+        elif self._kind == _MUON:
+            muon, adamw = zip(*per_group)
+            mats = muon_matrices(self.path.params, self._group_of, self.param_groups)
+            aux = not all(_use_muon(g) for g in self.param_groups)
+            self.path.muon_step(muon, [m[2] for m in mats if m is not None], adamw if aux else None)
         else:
             self.path.optimizer_step([self._hyper_of(g) for g in self.param_groups], per_group)
 
@@ -1757,6 +1989,10 @@ class B200FusedOptimizer(torch.optim.Optimizer):
                             scheduled_lr=_sf_scheduled_lr(src, k - 1) if k > 0 else src["scheduled_lr"])
                 g.update(vals)
                 src.update(vals)   # param_groups as of this state_dict(); reading them every step would synchronise
+        if self._kind == _MUON:   # Muon keeps no step
+            for i, gi in enumerate(self._group_of):
+                if _use_muon(self.param_groups[gi]) and self._sd_index[i] in out["state"]:
+                    out["state"][self._sd_index[i]].pop("step", None)
         if self._kind == _lib.OPT_ADAN and out["b200_opt_steps"] > 0:   # the class creates group["step"] at its first step
             for g, src in zip(out["param_groups"], self.param_groups):
                 g["step"] = src["step"] = out["b200_opt_steps"]
